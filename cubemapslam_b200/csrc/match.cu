@@ -5,9 +5,13 @@
 // The all-pairs ("brute force") matcher of BASELINE config 3 has no reference function; DESIGN.md defines it as the
 // SearchByBoW acceptance rule + rotation histogram applied to the best/second-best column of every row of A.
 //
-// k_match_bruteforce  one CTA per pair; B is staged through shared memory in 128-descriptor tiles, every thread
-//                     owns one row of A (8 x u32 in registers), __popc per 32-bit lane; per-pair rotation histogram and
-//                     3-maxima filter in the same CTA. Bound by the integer/POPC issue rate, not by HBM (192 KB per pair).
+// k_match_bruteforce  binary tensor-core GEMM: dist(a, b) = popc(a) + popc(b) - 2 popc(a AND b), popc(a AND b) of a 16 x 8 tile of
+//                     (A row, B row) pairs over the whole 256-bit descriptor is one BMMA (mma m16n8k256 .b1 .and.popc). A CTA owns
+//                     256 rows of A (a warp keeps 4 m16 fragments in registers); B streams through shared memory in 128-descriptor
+//                     tiles (cp.async, double-buffered, ldmatrix with a 16-byte-chunk XOR swizzle). Best / second best per row are
+//                     exact integer minima of a key that packs (distance, column). The rows of a pair are split over CTAs; the
+//                     rotation histogram and 3-maxima filter run in the CTA of the pair that arrives last. Bound by the min/max
+//                     epilogue (4 integer instructions per distance) and the BMMA issue rate, not by HBM (192 KB per pair).
 // k_search_by_bow     one CTA per pair; both FeatureVectors are rebuilt on the fly by an in-CTA bitonic sort of
 //                     (node, index); one warp walks the KF features of a node in order (the reference's "already
 //                     matched" skip makes that order matter), lanes scan the F features of the node.
@@ -18,8 +22,13 @@
 namespace cslam {
 
 static const int HISTO_BINS = 30;      // ceil(360 / HISTO_LENGTH), HISTO_LENGTH = 12
-static const int BF_THREADS = 256;
-static const int BF_TILE = 128;
+static const int BF_WARPS = 4;
+static const int BF_THREADS = 32 * BF_WARPS;
+static const int BF_MT = 4;                          // m16 row fragments per warp
+static const int BF_ROWS = BF_WARPS * BF_MT * 16;    // rows of A per CTA
+static const int BF_TILE = 128;                      // descriptors of B per shared-memory stage (one per thread for the popcount)
+static const int BF_COL_BITS = 12;                   // column field of a selection key: columns < 4096 (max_features)
+static_assert(BF_TILE == BF_THREADS, "one thread per staged column");
 
 __device__ __forceinline__ int rot_bin(float a, float b) {
     const float factor = 1.0f / 12.0f;
@@ -49,6 +58,31 @@ __device__ __forceinline__ int hamming256(const uint32_t (&a)[8], const uint4 b0
            __popc(a[4] ^ b1.x) + __popc(a[5] ^ b1.y) + __popc(a[6] ^ b1.z) + __popc(a[7] ^ b1.w);
 }
 
+// popc(a AND b) for a 16 x 8 tile of 256-bit rows: A fragment a[0..3] = words (t, t of row g+8, 4+t, 4+t of row g+8) of row g = lane / 4,
+// t = lane % 4; B fragment b0 / b1 = words t / 4+t of column g; d[0..3] = (g, 2t), (g, 2t+1), (g+8, 2t), (g+8, 2t+1).
+__device__ __forceinline__ void bmma_and_popc(int (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};"
+        : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "r"(0));
+}
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {   // bytes < 16: the rest is zero-filled
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" :: "r"(dst), "l"(src), "r"(bytes) : "memory");
+}
+
+// Selection key of one distance: (popc(b) - 2 popc(a AND b)) << 12 | column; the row's popc(a) is added when the key is decoded. Smaller key =
+// smaller distance, then lower column ("first column wins"). best1 / best2 are the two smallest keys of the row (keys are distinct, so a
+// duplicate minimum distance gives dist(best2) == dist(best1)).
+__device__ __forceinline__ void bf_take(int& best1, int& best2, int key) {
+    best2 = min(best2, max(best1, key));
+    best1 = min(best1, key);
+}
+__device__ __forceinline__ void bf_merge(int& best1, int& best2, int o1, int o2) {
+    best2 = min(max(best1, o1), min(best2, o2));
+    best1 = min(best1, o1);
+}
+// Key -> distance (capped at 256, which also catches the key of a column past nB: its prefix is INT_MAX)
+__device__ __forceinline__ int bf_dist(int popcA, int key) { return min(256, popcA + (key >> BF_COL_BITS)); }
+
 // Layout: pair p reads rows [p*strideA, p*strideA + nA) of descA (and B likewise); angles are read with a stride of `angStride` floats
 // (1 for a plain float array, 7 for cv::KeyPoint records, whose `angle` field the pointer then addresses); when nAarr / nBarr are given they
 // hold per-pair row counts (the front end's n_out). Outputs are strided like A.
@@ -57,56 +91,127 @@ __global__ void __launch_bounds__(BF_THREADS) k_match_bruteforce(const uint8_t* 
                                                                  const uint8_t* __restrict__ descB, const float* __restrict__ angB, int nB_, float nnratio,
                                                                  int thLow, int checkOri, int32_t* __restrict__ match12, int32_t* __restrict__ dist12,
                                                                  int32_t* __restrict__ second12, int32_t* __restrict__ nmatches, BfLayout L, int* __restrict__ gHist) {
-    // gridDim.y > 1: the rows of A are dealt to several CTAs per pair (a batch of ~128 pairs would otherwise leave 132 SMs one CTA each, or none);
-    // the rotation histogram then goes through gHist[pair][32] (30 bins, total, arrival counter; zeroed by the launcher) and the CTA that arrives
-    // last applies the three-maxima filter to the whole pair.
-    __shared__ __align__(16) uint4 sB[2 * BF_TILE];
+    // CTA (pair, part) owns rows [part * BF_ROWS, +BF_ROWS) of A; gridDim.y covers the largest row count the launch allows, CTAs past the pair's
+    // own count exit at once. With more than one part the rotation histogram goes through gHist[pair][32] (30 bins, total, arrival counter;
+    // zeroed by the launcher) and the CTA that arrives last applies the three-maxima filter to the whole pair.
+    __shared__ __align__(128) uint4 sB[2][2 * BF_TILE];   // 32-byte rows; 16-byte chunk c of row r sits at chunk c ^ ((r >> 2) & 1)
+    __shared__ __align__(16) int sPre[BF_TILE];           // popc(b) << 12 | column, INT_MAX past nB
     __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total;
     __shared__ bool lastCta;
-    const int pair = blockIdx.x, tid = threadIdx.x, part = blockIdx.y, parts = gridDim.y;
+    const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int nA = L.nAarr ? min(L.nAarr[pair], L.strideA) : nA_, nB = L.nBarr ? min(L.nBarr[pair], L.strideB) : nB_;
-    const uint4* A4 = reinterpret_cast<const uint4*>(descA + (size_t)pair * L.strideA * 32);
+    const int parts = max(1, (nA + BF_ROWS - 1) / BF_ROWS), part = blockIdx.y;
+    if (part >= parts) return;
+    const uint32_t* Aw = reinterpret_cast<const uint32_t*>(descA + (size_t)pair * L.strideA * 32);
     const uint4* B4 = reinterpret_cast<const uint4*>(descB + (size_t)pair * L.strideB * 32);
     const float* aA = angA + (size_t)pair * L.strideA * L.angStride;
     const float* aB = angB + (size_t)pair * L.strideB * L.angStride;
     int32_t* m12 = match12 + (size_t)pair * L.strideA;
     if (tid < HISTO_BINS) hist[tid] = 0;
     if (tid == 0) total = 0;
-    __syncthreads();
-    for (int rbase = part * BF_THREADS; rbase < nA; rbase += parts * BF_THREADS) {
-        const int i = rbase + tid;
-        uint32_t a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        if (i < nA) {
-            const uint4 a0 = __ldg(A4 + 2 * i), a1 = __ldg(A4 + 2 * i + 1);
-            a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
+
+    // A fragments of this warp's 4 x 16 rows (zero past nA) and popc(a) of rows g / g+8 of each
+    const int row0 = part * BF_ROWS + warp * BF_MT * 16;
+    const int nmt = min(BF_MT, max(0, (nA - row0 + 15) >> 4));   // live m16 fragments of this warp
+    uint32_t a[BF_MT][4];
+    int popcA[BF_MT][2], best1[BF_MT][2], best2[BF_MT][2];
+#pragma unroll
+    for (int mt = 0; mt < BF_MT; mt++) {
+        const int r = row0 + mt * 16 + g;
+        a[mt][0] = r < nA ? __ldg(Aw + (size_t)r * 8 + t) : 0u;
+        a[mt][1] = r + 8 < nA ? __ldg(Aw + (size_t)(r + 8) * 8 + t) : 0u;
+        a[mt][2] = r < nA ? __ldg(Aw + (size_t)r * 8 + 4 + t) : 0u;
+        a[mt][3] = r + 8 < nA ? __ldg(Aw + (size_t)(r + 8) * 8 + 4 + t) : 0u;
+        int p0 = __popc(a[mt][0]) + __popc(a[mt][2]), p1 = __popc(a[mt][1]) + __popc(a[mt][3]);
+        p0 += __shfl_xor_sync(0xffffffffu, p0, 1); p1 += __shfl_xor_sync(0xffffffffu, p1, 1);
+        p0 += __shfl_xor_sync(0xffffffffu, p0, 2); p1 += __shfl_xor_sync(0xffffffffu, p1, 2);
+        popcA[mt][0] = p0; popcA[mt][1] = p1;
+        best1[mt][0] = best1[mt][1] = best2[mt][0] = best2[mt][1] = INT_MAX;
+    }
+
+    // B: stage k = descriptors [k * BF_TILE, +BF_TILE) into sB[k & 1]; rows past nB are zero-filled (their key prefix is INT_MAX anyway)
+    const uint32_t sBase = (uint32_t)__cvta_generic_to_shared(&sB[0][0]);
+    auto stage = [&](int k) {
+        const uint32_t dst = sBase + (uint32_t)(k & 1) * (2 * BF_TILE * 16);
+        for (int q = tid; q < 2 * BF_TILE; q += BF_THREADS) {
+            const int r = q >> 1, c = q & 1, col = k * BF_TILE + r;
+            const bool ok = col < nB;
+            cp_async16(dst + (uint32_t)(r * 32 + ((c ^ ((r >> 2) & 1)) << 4)), ok ? (const void*)(B4 + 2 * col + c) : (const void*)B4, ok ? 16 : 0);
         }
-        int best1 = 256, best2 = 256, bestIdx = -1;
-        for (int cb = 0; cb < nB; cb += BF_TILE) {
-            const int nt = min(BF_TILE, nB - cb);
-            __syncthreads();
-            for (int k = tid; k < 2 * nt; k += BF_THREADS) sB[k] = __ldg(B4 + 2 * cb + k);
-            __syncthreads();
-            if (i < nA) {
-#pragma unroll 4
-                for (int j = 0; j < nt; j++) {
-                    const int d = hamming256(a, sB[2 * j], sB[2 * j + 1]);
-                    if (d < best1) { best2 = best1; best1 = d; bestIdx = cb + j; }
-                    else if (d < best2) best2 = d;
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    // ldmatrix.x4 source row of this lane: matrices (cols 0-7, chunk 0), (0-7, 1), (8-15, 0), (8-15, 1) of a 16-column group -> b0, b1 of
+    // two n8 tiles
+    const int lr = ((lane >> 4) << 3) + (lane & 7), lc = (lane >> 3) & 1;
+    const uint32_t ldOff = (uint32_t)(lr * 32 + ((lc ^ ((lr >> 2) & 1)) << 4));
+    const int ntiles = (nB + BF_TILE - 1) / BF_TILE;
+    if (ntiles) stage(0);
+    __syncthreads();                         // hist / total are zeroed (nB may be 0)
+    for (int kt = 0; kt < ntiles; kt++) {
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        __syncthreads();                     // stage kt has landed; every warp is done with stage kt-1 and with sPre
+        if (kt + 1 < ntiles) stage(kt + 1);  // overlaps with this stage's MMAs
+        {
+            const int col = kt * BF_TILE + tid;
+            const uint4 u0 = sB[kt & 1][2 * tid], u1 = sB[kt & 1][2 * tid + 1];   // chunk order does not matter for the popcount
+            const int pb = __popc(u0.x) + __popc(u0.y) + __popc(u0.z) + __popc(u0.w) + __popc(u1.x) + __popc(u1.y) + __popc(u1.z) + __popc(u1.w);
+            sPre[tid] = col < nB ? (pb << BF_COL_BITS) | col : INT_MAX;
+        }
+        __syncthreads();
+        if (nmt > 0) {
+            const uint32_t sb = sBase + (uint32_t)(kt & 1) * (2 * BF_TILE * 16) + ldOff;
+#pragma unroll 2
+            for (int j = 0; j < BF_TILE / 16; j++) {
+                uint32_t b[4];
+                asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                             : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "r"(sb + (uint32_t)j * 512));
+                const int2 p0 = *reinterpret_cast<const int2*>(&sPre[16 * j + 2 * t]), p1 = *reinterpret_cast<const int2*>(&sPre[16 * j + 8 + 2 * t]);
+#pragma unroll
+                for (int mt = 0; mt < BF_MT; mt++) {
+                    if (mt < nmt) {
+                        int d[4], e[4];
+                        bmma_and_popc(d, a[mt], b[0], b[1]);
+                        bmma_and_popc(e, a[mt], b[2], b[3]);
+                        bf_take(best1[mt][0], best2[mt][0], d[0] * -(2 << BF_COL_BITS) + p0.x);
+                        bf_take(best1[mt][0], best2[mt][0], d[1] * -(2 << BF_COL_BITS) + p0.y);
+                        bf_take(best1[mt][1], best2[mt][1], d[2] * -(2 << BF_COL_BITS) + p0.x);
+                        bf_take(best1[mt][1], best2[mt][1], d[3] * -(2 << BF_COL_BITS) + p0.y);
+                        bf_take(best1[mt][0], best2[mt][0], e[0] * -(2 << BF_COL_BITS) + p1.x);
+                        bf_take(best1[mt][0], best2[mt][0], e[1] * -(2 << BF_COL_BITS) + p1.y);
+                        bf_take(best1[mt][1], best2[mt][1], e[2] * -(2 << BF_COL_BITS) + p1.x);
+                        bf_take(best1[mt][1], best2[mt][1], e[3] * -(2 << BF_COL_BITS) + p1.y);
+                    }
                 }
             }
         }
-        if (i < nA) {
+    }
+
+    // merge the 4 lanes of a quad (columns 2t, 2t+1 of every n8 tile); lane t then finishes row-sets (mt, h) with (2 mt + h) % 4 == t
+#pragma unroll
+    for (int mt = 0; mt < BF_MT; mt++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1)
+                bf_merge(best1[mt][h], best2[mt][h], __shfl_xor_sync(0xffffffffu, best1[mt][h], o), __shfl_xor_sync(0xffffffffu, best2[mt][h], o));
+#pragma unroll
+    for (int mt = 0; mt < BF_MT; mt++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int i = row0 + mt * 16 + h * 8 + g;
+            if (((2 * mt + h) & 3) != t || i >= nA) continue;
+            const int d1 = bf_dist(popcA[mt][h], best1[mt][h]), d2 = bf_dist(popcA[mt][h], best2[mt][h]);
+            const int bestIdx = d1 < 256 ? (best1[mt][h] & ((1 << BF_COL_BITS) - 1)) : -1;
             int m = -1;
-            if (bestIdx >= 0 && best1 <= thLow && (float)best1 < __fmul_rn(nnratio, (float)best2)) {
+            if (bestIdx >= 0 && d1 <= thLow && (float)d1 < __fmul_rn(nnratio, (float)d2)) {
                 m = bestIdx;
                 if (checkOri) atomicAdd(&hist[rot_bin(aA[(size_t)i * L.angStride], aB[(size_t)bestIdx * L.angStride])], 1);
                 atomicAdd(&total, 1);
             }
             m12[i] = m;
-            if (dist12) dist12[(size_t)pair * L.strideA + i] = best1;
-            if (second12) second12[(size_t)pair * L.strideA + i] = best2;
+            if (dist12) dist12[(size_t)pair * L.strideA + i] = d1;
+            if (second12) second12[(size_t)pair * L.strideA + i] = d2;
         }
-    }
     __syncthreads();
     if (parts > 1) {
         int* g = gHist + (size_t)pair * 32;
@@ -320,19 +425,16 @@ extern "C" int cslam_matcher_sync(cslam_matcher* m) {
     return CSLAM_OK;
 }
 
-// CTAs per pair of a brute-force launch: enough CTAs for ~2 per SM when the batch of pairs is small; the per-pair histogram buffer is zeroed here
-static int bf_split(cslam_matcher* m, int npairs, int** gHist) {
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-    int parts = 1;
-    if (npairs < 2 * sms) parts = std::min(4, (2 * sms + npairs - 1) / npairs);
+// CTAs per pair of a brute-force launch: one per BF_ROWS rows of the largest A a pair can have; the per-pair histogram buffer is zeroed here
+static int bf_split(cslam_matcher* m, int maxRowsA, int npairs, int* parts, int** gHist) {
+    *parts = std::max(1, cdiv(maxRowsA, BF_ROWS));
     *gHist = nullptr;
-    if (parts > 1) {
-        if (!m->dHist && cudaMalloc(&m->dHist, (size_t)2 * sms * 32 * sizeof(int)) != cudaSuccess) { cudaGetLastError(); return 1; }   // npairs < 2 * sms whenever parts > 1
-        if (cudaMemsetAsync(m->dHist, 0, (size_t)npairs * 32 * sizeof(int), m->stream) != cudaSuccess) return 1;
+    if (*parts > 1) {
+        if (!m->dHist) CSLAM_CUDA(cudaMalloc(&m->dHist, (size_t)m->maxPairs * 32 * sizeof(int)));
+        CSLAM_CUDA(cudaMemsetAsync(m->dHist, 0, (size_t)npairs * 32 * sizeof(int), m->stream));
         *gHist = m->dHist;
     }
-    return parts;
+    return CSLAM_OK;
 }
 
 static int check_sizes(cslam_matcher* m, int nA, int nB, int npairs) {
@@ -351,7 +453,9 @@ extern "C" int cslam_match_bruteforce_dev(cslam_matcher* m, const uint8_t* descA
     if (rc) return rc;
     if (nA == 0) { CSLAM_CUDA(cudaMemsetAsync(nmatches, 0, (size_t)npairs * 4, m->stream)); return CSLAM_OK; }
     const BfLayout L = {nA, nB, 1, nullptr, nullptr};
-    int* gHist; const int parts = bf_split(m, npairs, &gHist);
+    int parts, *gHist;
+    rc = bf_split(m, nA, npairs, &parts, &gHist);
+    if (rc) return rc;
     k_match_bruteforce<<<dim3(npairs, parts), BF_THREADS, 0, m->stream>>>(descA, angA, nA, descB, angB, nB, nnratio, th_low, check_ori, match12, dist12, second12, nmatches, L, gHist);
     m->launches++;
     CSLAM_CUDA(cudaGetLastError());
@@ -381,11 +485,16 @@ extern "C" int cslam_match_bruteforce(cslam_matcher* m, const uint8_t* descA, co
 // [f*kp_stride, f*kp_stride + n[f]) of kps / desc) is matched against frame f+1 for f = 0 .. nframes-2. match12: (nframes-1) x kp_stride.
 extern "C" int cslam_match_frames_dev(cslam_matcher* m, const cslam_keypoint* kps, const uint8_t* desc, const int32_t* n, int kp_stride, int nframes, float nnratio, int th_low,
                                       int check_ori, int32_t* match12, int32_t* nmatches) {
-    if (!m || !kps || !desc || !n || !match12 || !nmatches || nframes < 2 || kp_stride <= 0) { set_error("cslam_match_frames_dev: bad argument"); return CSLAM_E_BADARG; }
+    if (!m || !kps || !desc || !n || !match12 || !nmatches || nframes < 2 || nframes - 1 > m->maxPairs || kp_stride <= 0 || kp_stride > m->maxFeat) {
+        set_error("cslam_match_frames_dev: bad argument (frames %d, pairs <= %d, stride %d <= %d)", nframes, m ? m->maxPairs : 0, kp_stride, m ? m->maxFeat : 0);
+        return CSLAM_E_BADARG;
+    }
     CSLAM_CUDA(cudaSetDevice(m->device));
     const float* ang = &kps[0].angle;
     const BfLayout L = {kp_stride, kp_stride, (int)(sizeof(cslam_keypoint) / sizeof(float)), n, n + 1};
-    int* gHist; const int parts = bf_split(m, nframes - 1, &gHist);
+    int parts, *gHist;
+    const int rc = bf_split(m, kp_stride, nframes - 1, &parts, &gHist);
+    if (rc) return rc;
     k_match_bruteforce<<<dim3(nframes - 1, parts), BF_THREADS, 0, m->stream>>>(desc, ang, 0, desc + (size_t)kp_stride * 32, ang + (size_t)kp_stride * L.angStride, 0, nnratio, th_low,
                                                                                 check_ori, match12, nullptr, nullptr, nmatches, L, gHist);
     m->launches++;
@@ -444,6 +553,66 @@ extern "C" int cslam_ubench_popc(cslam_matcher* m, double* popc32_per_s) {
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     m->launches += 2;
     *popc32_per_s = (double)blocks * 256.0 * iters * 8.0 / (ms * 1e-3);
+    return CSLAM_OK;
+}
+
+// Tensor-core issue-rate micro-benchmark: every warp runs `iters` rounds of 8 independent accumulator chains of one MMA shape on registers.
+// BINARY: m16n8k256 .b1 AND.POPC (the matcher's BMMA); else m16n8k32 s8 IMMA (the same distance from +-1 int8 expansions of the bits).
+template <bool BINARY>
+__global__ void __launch_bounds__(256) k_ubench_mma(uint32_t* out, int iters, uint32_t seed) {
+    uint32_t a[4], b[2];
+#pragma unroll
+    for (int k = 0; k < 4; k++) a[k] = seed * (threadIdx.x + 1) + k * 0x9e3779b9u + blockIdx.x;
+    b[0] = a[0] ^ 0x5bd1e995u; b[1] = a[3] * 0x27d4eb2fu;
+    int acc[8][4];
+#pragma unroll
+    for (int c = 0; c < 8; c++) acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = c;
+    for (int i = 0; i < iters; i++) {
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+            if (BINARY)
+                asm volatile("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                             : "+r"(acc[c][0]), "+r"(acc[c][1]), "+r"(acc[c][2]), "+r"(acc[c][3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+            else
+                asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                             : "+r"(acc[c][0]), "+r"(acc[c][1]), "+r"(acc[c][2]), "+r"(acc[c][3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+        }
+    }
+    int s = 0;
+#pragma unroll
+    for (int c = 0; c < 8; c++) s += acc[c][0] + acc[c][1] + acc[c][2] + acc[c][3];
+    if (s == 0x7eadbeef) out[0] = (uint32_t)s;   // keeps the chains alive
+}
+template <bool BINARY>
+static int time_ubench_mma(cslam_matcher* m, double* ms_out, double* mma_count) {
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
+    const int blocks = sms * 8, iters = 4000;
+    cudaEvent_t e0, e1;
+    CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
+    k_ubench_mma<BINARY><<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), 100, 1u);   // warm-up
+    CSLAM_CUDA(cudaEventRecord(e0, m->stream));
+    k_ubench_mma<BINARY><<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), iters, 1u);
+    CSLAM_CUDA(cudaEventRecord(e1, m->stream));
+    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
+    float ms = 0;
+    CSLAM_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    m->launches += 2;
+    *ms_out = ms;
+    *mma_count = (double)blocks * 8.0 * iters * 8.0;   // warp-level MMA instructions
+    return CSLAM_OK;
+}
+extern "C" int cslam_ubench_bmma(cslam_matcher* m, double* bmma_products_per_s, double* imma_products_per_s) {
+    if (!m || !bmma_products_per_s || !imma_products_per_s) return CSLAM_E_BADARG;
+    CSLAM_CUDA(cudaSetDevice(m->device));
+    double ms, n;
+    int rc = time_ubench_mma<true>(m, &ms, &n);
+    if (rc) return rc;
+    *bmma_products_per_s = n * 128.0 / (ms * 1e-3);          // 16 x 8 256-bit products per BMMA
+    rc = time_ubench_mma<false>(m, &ms, &n);
+    if (rc) return rc;
+    *imma_products_per_s = n * 128.0 / 8.0 / (ms * 1e-3);    // 16 x 8 dot products of 32 bytes; a 256-bit product is 8 of them
     return CSLAM_OK;
 }
 

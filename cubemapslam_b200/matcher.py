@@ -88,6 +88,12 @@ class ORBMatcher:
         check(lib().cslam_ubench_popc(self._h, C.byref(v)))
         return v.value
 
+    def ubench_bmma(self):
+        """(BMMA, IMMA) rates in 256-bit products (= Hamming distances) per second, register-only chains."""
+        b = C.c_double(); i = C.c_double()
+        check(lib().cslam_ubench_bmma(self._h, C.byref(b), C.byref(i)))
+        return b.value, i.value
+
     def ubench_minmax3(self):
         v = C.c_double()
         check(lib().cslam_ubench_minmax3(self._h, C.byref(v)))

@@ -121,6 +121,9 @@ int cslam_match_frames(cslam_matcher* m, const cslam_keypoint* kps, const uint8_
 /* Measured POPC issue rate of this GPU (32-bit population counts per second with the XOR+POPC+ADD mix of the Hamming kernels, no memory traffic):
  * the ceiling the matcher's roofline fraction is quoted against (bench.py). */
 int cslam_ubench_popc(cslam_matcher* m, double* popc32_per_s);
+/* Measured tensor-core rates in 256-bit products per second (one product = one Hamming distance's worth of work), from register-only chains:
+ * BMMA m16n8k256 .b1 AND.POPC (what cslam_match_bruteforce runs on) and, for comparison, m16n8k32 s8 IMMA on +-1 int8 expansions. */
+int cslam_ubench_bmma(cslam_matcher* m, double* bmma_products_per_s, double* imma_products_per_s);
 /* Same for 3-input u16x2 min/max (VIMNMX3.U16x2), the instruction k_fast is bound by; out: thread-level operations per second. */
 int cslam_ubench_minmax3(cslam_matcher* m, double* ops_per_s);
 /* ORBMatcher::SearchByBoW(KeyFrame*, Frame&, vector<MapPoint*>&) (src/ORBMatcher.cpp:409-539) for npairs (KF,F) pairs.
