@@ -54,45 +54,123 @@ struct DevLevels {
     const uint16_t* yofs[MAX_LEVELS];
     const uint32_t* yab[MAX_LEVELS];
     const uint8_t* skip[MAX_LEVELS];   // per k_fast CTA: 1 = tile provably all-zero when level 0 came from k_warp (black corner tiles)
+    const uint8_t* pskip[MAX_LEVELS];  // per k_pyramid warp (PYR_WX x PYR_RY dst px), same meaning; levels >= 1
     int nlevels;
 };
 
 // ------------------------------------------------------------------------------------------------- k_warp
 // Map entry: sx | sy<<16 with sx=cvRound(u*32), sy=cvRound(v*32) (cv::remap's INTER_BITS=5 fixed point).
 // Weights are exact integers: (32-fy)(32-fx)*32 etc. (= cvRound of the fp32 table products * 32768).
-// One thread = one canvas pixel of one face row, looped over FPT frames so a map entry is read once per FPT frames.
-template <int FPT>
-__global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fisheye, int Iw, int Ih, const uint32_t* __restrict__ map, int W,
-                                              uint8_t* __restrict__ canvas, int cpitch, size_t cframe, int batch) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int row = blockIdx.y;
-    const int face = blockIdx.z % 5, fg = blockIdx.z / 5;
-    if (x >= W) return;
-    const int tcol = (face == 1) ? 0 : (face == 2) ? 2 : 1;
-    const int trow = (face == 3) ? 0 : (face == 4) ? 2 : 1;
-    const uint32_t m = __ldg(map + ((size_t)face * W + row) * W + x);
+// k_warp computes v = ((t00(32-fx) + t01 fx)(32-fy) + (t10(32-fx) + t11 fx) fy) * 32, rounded >> 15: the factored form is the
+// same integer as the four-weight sum, and (32 X + 2^14) >> 15 == (X + 2^9) >> 10.
+__device__ __forceinline__ uint32_t bilerp5(uint32_t t00, uint32_t t01, uint32_t t10, uint32_t t11, uint32_t fx, uint32_t fy) {
+    const uint32_t h0 = t00 * (32 - fx) + t01 * fx, h1 = t10 * (32 - fx) + t11 * fx;
+    return (h0 * (32 - fy) + h1 * fy + 512) >> 10;
+}
+// one pixel straight from global memory (tiles too large to stage); ix,iy >= 0 always (maps are >= 0); each tap outside the source reads 0 (BORDER_CONSTANT)
+__device__ __forceinline__ uint32_t gather_direct(const uint8_t* __restrict__ S, int Iw, int Ih, uint32_t m) {
     const int sx = m & 0xffff, sy = m >> 16;
-    const int ix = sx >> 5, iy = sy >> 5, fx = sx & 31, fy = sy & 31;
-    const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
-    // ix,iy >= 0 always (maps are >= 0); each tap outside the source reads 0 (BORDER_CONSTANT)
+    const int ix = sx >> 5, iy = sy >> 5;
     const bool x0ok = ix < Iw, x1ok = ix + 1 < Iw, y0ok = iy < Ih, y1ok = iy + 1 < Ih;
-    const size_t o00 = (size_t)iy * Iw + ix;
-    const size_t dst = (size_t)(trow * W + row) * cpitch + tcol * W + x;
+    const uint8_t* p = S + (size_t)iy * Iw + ix;
+    const uint32_t t00 = (y0ok && x0ok) ? __ldg(p) : 0u, t01 = (y0ok && x1ok) ? __ldg(p + 1) : 0u;
+    const uint32_t t10 = (y1ok && x0ok) ? __ldg(p + Iw) : 0u, t11 = (y1ok && x1ok) ? __ldg(p + Iw + 1) : 0u;
+    return bilerp5(t00, t01, t10, t11, sx & 31, sy & 31);
+}
+
+// Tiled warp. The map is fixed at create time, so each output tile's source footprint is known: a CTA stages the bounding box of
+// its tile's taps for FPT frames into shared memory with coalesced 4-byte cp.async (zero-filled outside the source = BORDER_CONSTANT;
+// byte loads when source rows are not word-aligned), then gathers the 4 taps of each pixel from there. All FPT boxes are loaded
+// before one barrier; several resident CTAs per SM overlap one CTA's loads with another's arithmetic. Tiles are WT_W canvas
+// columns (aligned to WT_W in canvas coordinates, so every thread stores its 4 pixels as one aligned u32) x WT_H face rows;
+// columns outside the face are masked, so only the five face ROIs are written. Table entry of a staged pixel: box offset | fx<<16 | fy<<21, or WE_ORIGIN for a pixel whose map is (0,0) (outside
+// the image circle: cv::remap reads S(0,0) with zero fractions). A tile whose box exceeds WARP_BOX_MAX is `direct`: its entries are
+// the raw map and its pixels gather from global memory.
+static const int WT_W = 32, WT_H = 32;
+static const int WARP_BOX_MAX = 6144;
+static const uint32_t WE_ORIGIN = 1u << 26;
+struct WarpTile {
+    int row0, xa;      // canvas row of the tile's first face row; canvas column of its first (aligned) column
+    int cx0, cx1, nr;  // face columns [cx0, cx1) in canvas coordinates; face rows in this tile
+    int bx0, by0;      // source box origin (bx0 a multiple of 4)
+    int bw, bh;        // source box width (bytes, a multiple of 4) and height
+    int direct;
+};
+
+__device__ __forceinline__ void cp_async4_zfill(void* smem, const void* gmem, int srcBytes) {
+    const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(s), "l"(gmem), "r"(srcBytes) : "memory");
+}
+
+template <int FPT>
+__global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fisheye, int Iw, int Ih, const WarpTile* __restrict__ tiles,
+                                              const uint32_t* __restrict__ ent, uint8_t* __restrict__ canvas, int cpitch, size_t cframe, int batch,
+                                              int slot, int words) {
+    extern __shared__ __align__(16) uint8_t wsm[];   // FPT boxes of `slot` bytes, then S(0,0) of each frame
+    uint8_t* origin = wsm + FPT * slot;
+    const WarpTile T = tiles[blockIdx.x];
+    const int f0 = blockIdx.y * FPT, nf = min(FPT, batch - f0), tid = threadIdx.x;
+    const size_t fsz = (size_t)Iw * Ih;
+    const uint8_t* S0 = fisheye + (size_t)f0 * fsz;
+    if (!T.direct) {
+        if (words) {   // Iw % 4 == 0 and a word-aligned frame pointer: a word is all inside or all outside the source row
+            const int bw4 = T.bw >> 2, nwords = bw4 * T.bh;
+            for (int i = tid; i < nwords; i += 256) {
+                const int r = i / bw4, x = T.bx0 + 4 * (i - r * bw4), y = T.by0 + r;
+                const bool ok = y < Ih && x < Iw;
+                const uint8_t* src = S0 + (ok ? (size_t)y * Iw + x : 0);
+                for (int k = 0; k < nf; k++) cp_async4_zfill(wsm + k * slot + 4 * i, src + k * fsz, ok ? 4 : 0);
+            }
+        } else {       // any other source width: byte loads, still coalesced along box rows
+            const int nb = T.bw * T.bh;
+            for (int i = tid; i < nb; i += 256) {
+                const int r = i / T.bw, x = T.bx0 + (i - r * T.bw), y = T.by0 + r;
+                const bool ok = y < Ih && x < Iw;
+                const uint8_t* src = S0 + (ok ? (size_t)y * Iw + x : 0);
+                for (int k = 0; k < nf; k++) wsm[k * slot + i] = ok ? __ldg(src + k * fsz) : (uint8_t)0;
+            }
+        }
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
+        if (tid < nf) origin[tid] = __ldg(S0 + tid * fsz);
+        asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+        __syncthreads();
+    }
+    const int r = tid >> 3, c = (tid & 7) * 4, x = T.xa + c;
+    if (r >= T.nr) return;
+    uint32_t lm = 0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) lm |= (x + j >= T.cx0 && x + j < T.cx1) ? 1u << j : 0u;
+    if (!lm) return;
+    const uint4 e4 = __ldg(reinterpret_cast<const uint4*>(ent) + (size_t)blockIdx.x * (WT_W * WT_H / 4) + tid);
+    const uint32_t e[4] = {e4.x, e4.y, e4.z, e4.w};
+    uint8_t* D = canvas + (size_t)f0 * cframe + (size_t)(T.row0 + r) * cpitch + x;
+    const int bw = T.bw;
 #pragma unroll
     for (int k = 0; k < FPT; k++) {
-        const int f = fg * FPT + k;
-        if (f >= batch) break;
-        const uint8_t* S = fisheye + (size_t)f * Iw * Ih;
-        int v = 0;
-        if (y0ok) {
-            if (x0ok) v += __ldg(S + o00) * w00;
-            if (x1ok) v += __ldg(S + o00 + 1) * w01;
+        if (k >= nf) break;
+        uint32_t out = 0;
+        if (T.direct) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) out |= gather_direct(S0 + k * fsz, Iw, Ih, e[j]) << (8 * j);
+        } else {
+            const uint8_t* B = wsm + k * slot;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                uint32_t v;
+                if (e[j] & WE_ORIGIN) v = origin[k];
+                else {
+                    const uint8_t* p = B + (e[j] & 0xffff);
+                    v = bilerp5(p[0], p[1], p[bw], p[bw + 1], (e[j] >> 16) & 31, (e[j] >> 21) & 31);
+                }
+                out |= v << (8 * j);
+            }
         }
-        if (y1ok) {
-            if (x0ok) v += __ldg(S + o00 + Iw) * w10;
-            if (x1ok) v += __ldg(S + o00 + Iw + 1) * w11;
+        uint8_t* d = D + k * cframe;
+        if (lm == 0xfu) *reinterpret_cast<uint32_t*>(d) = out;
+        else {
+#pragma unroll
+            for (int j = 0; j < 4; j++) if (lm & (1u << j)) d[j] = (uint8_t)(out >> (8 * j));
         }
-        canvas[(size_t)f * cframe + dst] = (uint8_t)((v + (1 << 14)) >> 15);
     }
 }
 
@@ -102,12 +180,17 @@ __global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fishey
 // the 8-byte source window of the 4 pixels is fetched with aligned 32-bit loads, the taps are gathered with PRMT and the
 // horizontal pass is two-tap IDP.2A (coefficient pair a0|a1<<16 straight from the table); a source row's H is reused by the
 // next dst row when it needs it again (1.2 source rows per dst row instead of 2).
+// `skip` (warp path only): one byte per warp-sized piece (128 dst px x PYR_RY rows), 1 = every pixel of the piece is provably 0
+// (the black cubemap corners, DevLevels::pskip). The buffer already holds those zeros, so the warp exits without reading or writing.
 static const int PYR_RY = 8;
+static const int PYR_WX = 32 * 4;   // dst columns per warp
 __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src, int sw, int sh, int spitch, uint8_t* __restrict__ dst, int dw, int dh,
                                                  int dpitch, const uint16_t* __restrict__ xofs, const uint32_t* __restrict__ xab,
-                                                 const uint16_t* __restrict__ yofs, const uint32_t* __restrict__ yab) {
+                                                 const uint16_t* __restrict__ yofs, const uint32_t* __restrict__ yab,
+                                                 const uint8_t* __restrict__ skip) {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x4 >= dw) return;
+    if (skip && skip[blockIdx.y * ((dw + PYR_WX - 1) / PYR_WX) + x4 / PYR_WX]) return;   // warp-uniform
     const uint8_t* S = src + (size_t)blockIdx.z * spitch * sh;
     uint8_t* D = dst + (size_t)blockIdx.z * dpitch * dh;
     int s0[4]; uint32_t ab[4];
@@ -790,7 +873,9 @@ struct cslam_frontend {
     DevLevels L;                     // host copy of the device-pointer table (passed by value to kernels)
     std::vector<float> scale, invScale, sigma2, invSigma2; std::vector<int> perLevel; int umax[16];
     std::vector<float> map1, map2;   // host float maps (3H x 3W), kept for cslam_frontend_get_maps
-    uint32_t* d_map = nullptr;       // 5 x W x W
+    const WarpTile* d_wtiles = nullptr; const uint32_t* d_went = nullptr;   // k_warp tiles and their WT_W x WT_H entry tables
+    int nWarpTiles = 0, warpSlot = 0;   // warpSlot: staged source box bytes per frame (largest staged box, rounded to 16)
+    int warpFpt = 8;                    // frames per k_warp CTA, 4 or 8 (env CSLAM_WARP_FPT)
     uint8_t* d_mask = nullptr; int maskPitch = 0;
     uint8_t* d_fisheye = nullptr;    // staging for host entry points: maxBatch x Ih x Iw
     uint32_t* d_candCount = nullptr; // maxBatch x nlevels
@@ -808,7 +893,7 @@ struct cslam_frontend {
     // optional per-kernel timing (cslam_frontend_set_timing): events between launches, accumulated per kernel kind
     bool timing = false; std::vector<cudaEvent_t> ev; std::vector<int> evKind; int evUsed = 0;
     double kindMs[8] = {0, 0, 0, 0, 0, 0, 0, 0}; int64_t kindCount[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    bool cornersDirty = false;   // level-0 buffer holds caller canvases (non-zero corner tiles) from cslam_orb_extract
+    bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     size_t distributeSmem = 0;
 };
 
@@ -1006,6 +1091,13 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
                     }
                 }
                 Z.swap(Zn);
+                // k_pyramid pieces inside Z_l: all four taps of every pixel are 0, so the piece is 0 and the kernel need not touch it
+                const int px = cdiv(g.w, PYR_WX), py = cdiv(g.h, PYR_RY);
+                std::vector<uint8_t> ps((size_t)px * py, 1);
+                for (int y = 0; y < g.h; y++)
+                    for (int x = 0; x < g.w; x++)
+                        if (!Z[(size_t)y * g.w + x]) ps[(size_t)(y / PYR_RY) * px + x / PYR_WX] = 0;
+                if ((rc = dev_upload(fe, &fe->L.pskip[l], ps))) return fail(rc);
             }
             const int gx = cdiv(g.nColsEff, CG), gy = g.nRowsEff;
             std::vector<uint8_t> sk((size_t)gx * gy, 0);
@@ -1050,9 +1142,58 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
                     const int sx = cv_round_f(fe->map1[src] * 32.f), sy = cv_round_f(fe->map2[src] * 32.f);
                     q[((size_t)f * W + y) * W + x] = (uint32_t)sx | ((uint32_t)sy << 16);
                 }
-        const uint32_t* dq = nullptr;
-        if ((rc = dev_upload(fe, &dq, q))) return fail(rc);
-        fe->d_map = const_cast<uint32_t*>(dq);
+        // k_warp tiles: per tile the source box of all its taps (ix..ix+1, iy..iy+1 of every pixel whose map is not (0,0)) and the
+        // per-pixel entries relative to it; a tile whose box exceeds WARP_BOX_MAX keeps the raw map and gathers from global memory
+        std::vector<WarpTile> tiles;
+        std::vector<uint32_t> ent;
+        int slot = 0;
+        for (int f = 0; f < 5; f++) {
+            const int cx0 = tc[f] * W, cx1 = cx0 + W;
+            for (int y0 = 0; y0 < W; y0 += WT_H)
+                for (int xa = cx0 / WT_W * WT_W; xa < cx1; xa += WT_W) {
+                    WarpTile t;
+                    t.row0 = tr[f] * W + y0; t.xa = xa; t.cx0 = cx0; t.cx1 = cx1; t.nr = std::min(WT_H, W - y0);
+                    int minX = 1 << 30, minY = 1 << 30, maxX = -1, maxY = -1;
+                    auto mapAt = [&](int r, int c) { return q[((size_t)f * W + y0 + r) * W + (xa + c - cx0)]; };
+                    auto inFace = [&](int r, int c) { return r < t.nr && xa + c >= cx0 && xa + c < cx1; };
+                    for (int r = 0; r < WT_H; r++)
+                        for (int c = 0; c < WT_W; c++) {
+                            if (!inFace(r, c)) continue;
+                            const uint32_t m = mapAt(r, c);
+                            if (m == 0) continue;
+                            const int ix = (m & 0xffff) >> 5, iy = (m >> 16) >> 5;
+                            minX = std::min(minX, ix); maxX = std::max(maxX, ix + 1); minY = std::min(minY, iy); maxY = std::max(maxY, iy + 1);
+                        }
+                    if (maxX < 0) { t.bx0 = t.by0 = 0; t.bw = t.bh = 0; }
+                    else { t.bx0 = minX & ~3; t.by0 = minY; t.bw = round_up(maxX + 1 - t.bx0, 4); t.bh = maxY + 1 - minY; }
+                    t.direct = t.bw * t.bh > WARP_BOX_MAX;
+                    if (!t.direct) slot = std::max(slot, t.bw * t.bh);
+                    for (int r = 0; r < WT_H; r++)
+                        for (int c = 0; c < WT_W; c++) {
+                            uint32_t e = 0;
+                            if (inFace(r, c)) {
+                                const uint32_t m = mapAt(r, c);
+                                const int sx = m & 0xffff, sy = m >> 16;
+                                if (t.direct) e = m;
+                                else if (m == 0) e = WE_ORIGIN;
+                                else e = (uint32_t)(((sy >> 5) - t.by0) * t.bw + (sx >> 5) - t.bx0) | ((uint32_t)(sx & 31) << 16) | ((uint32_t)(sy & 31) << 21);
+                            }
+                            ent.push_back(e);
+                        }
+                    tiles.push_back(t);
+                }
+        }
+        fe->nWarpTiles = (int)tiles.size();
+        fe->warpSlot = round_up(std::max(slot, 16), 16);
+        if (const char* e = getenv("CSLAM_WARP_FPT")) fe->warpFpt = atoi(e) == 4 ? 4 : 8;
+        const uint8_t* dt = nullptr;
+        std::vector<uint8_t> tb(tiles.size() * sizeof(WarpTile));
+        std::memcpy(tb.data(), tiles.data(), tb.size());
+        if ((rc = dev_upload(fe, &dt, tb)) || (rc = dev_upload(fe, &fe->d_went, ent))) return fail(rc);
+        fe->d_wtiles = reinterpret_cast<const WarpTile*>(dt);
+        const int smem8 = 8 * fe->warpSlot + 16;
+        if (cudaFuncSetAttribute(k_warp<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem8) != cudaSuccess ||
+            cudaFuncSetAttribute(k_warp<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem8) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
     }
     // ---- mask
     fe->maskPitch = round_up(fe->CW, 128);
@@ -1135,12 +1276,17 @@ static DevLevels shifted(const cslam_frontend* fe, int f0) {
 }
 
 static int launch_warp(cslam_frontend* fe, cudaStream_t st, const uint8_t* d_fisheye, int f0, int cnt) {
-    const int FPT = 4;
-    if (!fe->d_map) { set_error("this front end was created without fisheye geometry (Iw/Ih = 0): no warp"); return CSLAM_E_BADARG; }
+    if (!fe->d_wtiles) { set_error("this front end was created without fisheye geometry (Iw/Ih = 0): no warp"); return CSLAM_E_BADARG; }
     const size_t cframe = (size_t)fe->L.g[0].pitch * fe->CH;
-    dim3 grid(cdiv(fe->W, 256), fe->H, 5 * cdiv(cnt, FPT));
+    uint8_t* canvas = fe->L.img[0] + (size_t)f0 * cframe;
+    const int Iw = fe->cam.Iw, Ih = fe->cam.Ih, pitch = fe->L.g[0].pitch;
+    const int words = (Iw % 4 == 0 && ((uintptr_t)d_fisheye & 3) == 0) ? 1 : 0;   // 4-byte staging needs word-aligned source rows
+    const int fpt = fe->warpFpt;
+    dim3 grid(fe->nWarpTiles, cdiv(cnt, fpt));
+    const size_t smem = (size_t)fpt * fe->warpSlot + 16;
     mark(fe, st, KIND_WARP);
-    k_warp<FPT><<<grid, 256, 0, st>>>(d_fisheye, fe->cam.Iw, fe->cam.Ih, fe->d_map, fe->W, fe->L.img[0] + (size_t)f0 * cframe, fe->L.g[0].pitch, cframe, cnt);
+    if (fpt == 8) k_warp<8><<<grid, 256, smem, st>>>(d_fisheye, Iw, Ih, fe->d_wtiles, fe->d_went, canvas, pitch, cframe, cnt, fe->warpSlot, words);
+    else k_warp<4><<<grid, 256, smem, st>>>(d_fisheye, Iw, Ih, fe->d_wtiles, fe->d_went, canvas, pitch, cframe, cnt, fe->warpSlot, words);
     CSLAM_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1154,7 +1300,8 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         const LevelGeom& s = L.g[l - 1]; const LevelGeom& d = L.g[l];
         dim3 grid(cdiv(cdiv(d.w, 4), 128), cdiv(d.h, PYR_RY), cnt);
         mark(fe, st, KIND_PYRAMID);
-        k_pyramid<<<grid, 128, 0, st>>>(L.img[l - 1], s.w, s.h, s.pitch, L.img[l], d.w, d.h, d.pitch, L.xofs[l], L.xab[l], L.yofs[l], L.yab[l]);
+        k_pyramid<<<grid, 128, 0, st>>>(L.img[l - 1], s.w, s.h, s.pitch, L.img[l], d.w, d.h, d.pitch, L.xofs[l], L.xab[l], L.yofs[l], L.yab[l],
+                                        useSkip ? L.pskip[l] : nullptr);
     }
     for (int l = 0; l < nl; l++) {
         const LevelGeom& g = L.g[l];
@@ -1204,8 +1351,11 @@ static int join_lanes(cslam_frontend* fe, int nl) {
     return 0;
 }
 static int prepare_level0(cslam_frontend* fe, bool fromWarp) {
-    if (fromWarp && fe->cornersDirty) {   // the warp never writes the 4 corner tiles; they must read as the reference's zeroed canvas
-        CSLAM_CUDA(cudaMemsetAsync(fe->L.img[0], 0, (size_t)fe->maxBatch * fe->L.g[0].pitch * fe->CH, fe->stream));
+    // the warp never writes the 4 corner tiles; they must read as the reference's zeroed canvas. The warp path's k_pyramid does not
+    // write the corner regions of levels >= 1 either (DevLevels::pskip), so after a caller canvas every level is cleared once.
+    if (fromWarp && fe->cornersDirty) {
+        for (int l = 0; l < fe->L.nlevels; l++)
+            CSLAM_CUDA(cudaMemsetAsync(fe->L.img[l], 0, (size_t)fe->maxBatch * fe->L.g[l].pitch * fe->L.g[l].h, fe->stream));
         fe->cornersDirty = false;
     }
     if (!fromWarp) fe->cornersDirty = true;
