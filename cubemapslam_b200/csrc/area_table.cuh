@@ -9,6 +9,8 @@
 namespace cslam {
 
 enum { FACE_FRONT = 0, FACE_LEFT = 1, FACE_RIGHT = 2, FACE_UPPER = 3, FACE_LOWER = 4, FACE_NONE = 0xff };
+// canvas tile (column, row) of each face, in FACE_* order; the canvas is 3 x 3 faces and its four corner tiles belong to no face
+static const int FACE_TILE_COL[5] = {1, 0, 2, 1, 1}, FACE_TILE_ROW[5] = {1, 1, 1, 0, 2};
 static const int GRID_G = 50;   // CUBEFACE_GRID_COLS == CUBEFACE_GRID_ROWS (include/Frame.h:43-45)
 
 // symbols: cell index of a window edge, in the centre's face (a b c d) or shifted by one face width / negated (the neighbour's frame)
@@ -78,7 +80,9 @@ struct AreaRect { uint8_t face, x0, x1, y0, y1; };
 
 struct AreaQuery { int face; int caseRow; int sym[13]; };
 
-// FaceInCubemap<float>(x, y)  (include/CamModelGeneral.h:458-470)
+// FaceInCubemap (include/CamModelGeneral.h:458-470), the one definition of the face a canvas pixel lies on; -1: a corner tile or outside.
+// It also stands for the cv::Point2f overload, which widens the float quotient to double: the quotients are IEEE-rounded here (nvcc's
+// default -prec-div=true, plain IEEE float on the host) and compared with the exact constants 0..3, which widening does not change.
 __host__ __device__ inline int face_of_pixel_f(float x, float y, int W, int H) {
     const float i = x / (float)W, j = y / (float)H;
     if (i >= 0 && i < 1 && j >= 1 && j < 2) return FACE_LEFT;
@@ -88,6 +92,8 @@ __host__ __device__ inline int face_of_pixel_f(float x, float y, int W, int H) {
     if (i >= 2 && i < 3 && j >= 1 && j < 2) return FACE_RIGHT;
     return -1;
 }
+// GetPosInFace<double>: the position of canvas coordinate x inside its face of width W
+__host__ __device__ inline double pos_in_face(float x, int W) { return (double)x - floor((double)x / W) * W; }
 
 // classifies the search window [x-r, x+r] x [y-r, y+r] (src/Frame.cpp:256-286) and evaluates the thirteen symbols; false: centre on no face
 __host__ __device__ inline bool area_query(float x, float y, float r, int W, int H, float inv, AreaQuery& q) {

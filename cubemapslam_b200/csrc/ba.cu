@@ -25,7 +25,6 @@
 #include <dlfcn.h>
 #include <algorithm>
 #include <cfloat>
-#include <chrono>
 #include <cstring>
 #include <vector>
 #include "optimizer.cuh"
@@ -443,6 +442,7 @@ __global__ void __launch_bounds__(SCHUR_T) k_ba_schur(BADev D, int addLambda) {
 // was parked in L2 scratch by (2)) instead of a 32-step triangular solve, then the rows above take y -= L_b^T x_b. scal[3] = 1 on a zero / non-finite pivot (LinearSolverEigen's failure): the LM trial is rejected.
 static const int LD_NB = 32;
 static const int SOLVE_T = 256;
+static const int SOLVE_CLUSTER = 8;   // CTAs per solver cluster: the largest portable cluster size
 
 // 1 / d to within an ulp: MUFU.RCP64H seed (~20 bits) and two Newton steps, instead of the ~127 clk IEEE divide on the critical path
 __device__ __forceinline__ double fast_rcp(double d) {
@@ -453,7 +453,7 @@ __device__ __forceinline__ double fast_rcp(double d) {
     return r;
 }
 
-__global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restrict__ Lt, double* __restrict__ LDt, double* __restrict__ Mg, int ldp, int stage, long long* prof) {
+__global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restrict__ Lt, double* __restrict__ LDt, double* __restrict__ Mg, int ldp, int stage) {
     extern __shared__ double dsm[];                 // [stage ? 2 * NB * ldp : 0] panels, then y[n] for the back substitution
     __shared__ double Pd[LD_NB][LD_NB + 1];         // L of the diagonal block (strictly lower part)
     __shared__ double Msm[LD_NB][LD_NB + 1];        // M = L^-1 of the diagonal block (zeros above the diagonal)
@@ -467,10 +467,6 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
     double* sL = dsm; double* sLD = dsm + (size_t)LD_NB * ldp;
     if (tid == 0) fail = 0;
     __syncthreads();
-    long long tprev = 0, tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const bool doProf = prof && crank == 0 && tid == 0;
-#define SOLVE_MARK(k) do { if (doProf) { const long long tn = clock64(); tacc[k] += tn - tprev; tprev = tn; } } while (0)
-    if (doProf) tprev = clock64();
     for (int jb = 0; jb < n; jb += LD_NB) {
         const int nb = min(LD_NB, n - jb), rows = n + 1 - jb;
         // (1) diagonal block: thread (r, g) owns (r, 4g .. 4g+3)
@@ -480,7 +476,6 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
         for (int k = 0; k < 4; k++) { const int c = g4 + k; a[k] = (r < nb && c <= r) ? __ldcg(A + (size_t)(jb + r) * n + jb + c) : 0.0; }
         if (g4 == 0) colbuf[0][r] = a[0];
         __syncthreads();
-        SOLVE_MARK(0);
 #pragma unroll
         for (int c = 0; c < LD_NB; c++) {
             if (c < nb) {   // block-uniform
@@ -525,7 +520,6 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
         __syncthreads();
         if (tid < nb) { const double iv = dinvv[tid]; if (!isfinite(iv) || iv == 0.0) fail = 1; }   // zero / non-finite pivot <=> its reciprocal is not a finite non-zero number
         __syncthreads();
-        SOLVE_MARK(1);
         if (fail) break;   // block-uniform and identical in every CTA of the cluster (same data)
         // (2) rows below the diagonal block (including the rhs row): a contiguous chunk of rows per CTA, 4 lanes per row, 8 columns per lane.
         // Per element the subtractions run over c2 = 0, 1, ... in the order of the plain forward substitution.
@@ -563,9 +557,7 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
         // M of this panel to the scratch the back substitution reads (cluster rank 0)
         if (crank == 0)
             for (int i = tid; i < LD_NB * LD_NB; i += SOLVE_T) { const int rr = i / LD_NB, c = i - rr * LD_NB; __stcg(Mg + (size_t)(jb / LD_NB) * LD_NB * LD_NB + i, (rr < nb && c < nb) ? Msm[rr][c] : 0.0); }
-        SOLVE_MARK(2);
         cluster.sync();
-        SOLVE_MARK(3);
         // (3) trailing update A[i][k] -= sum_c (L d)[i][c] L[k][c], rows i include the rhs row, columns k < trC, k <= i
         const int trC = n - jb - nb;
         if (trC > 0) {
@@ -598,7 +590,6 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
                     for (int c = half; c < nb; c += 2) { hL[c * st2 + q] = __ldcg(gL + c * st2 + q); hD[c * st2 + q] = __ldcg(gD + c * st2 + q); }
                 __syncthreads();
             }
-            SOLVE_MARK(4);
             const int tR = (trR + 3) >> 2, tC = (trC + 1) >> 1;
             // tile row br (4 rows) holds the tile columns bc with 2 bc <= 4 br + 3, i.e. bc <= 2 br + 1: 2 br + 2 tiles, br (br + 1) before it
             const int nTiles = tR * (tR + 1);
@@ -647,9 +638,7 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
                 }
             }
         }
-        SOLVE_MARK(5);
         cluster.sync();
-        SOLVE_MARK(6);
     }
     if (fail) { if (crank == 0 && tid == 0) D.scal[3] = 1.0; return; }
     if (crank != 0) return;
@@ -693,9 +682,6 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
         __syncthreads();
     }
     for (int i = tid; i < n; i += SOLVE_T) D.xp[i] = y[i];
-    SOLVE_MARK(7);
-    if (doProf) for (int k = 0; k < 8; k++) prof[k] += tacc[k];
-#undef SOLVE_MARK
 }
 
 // xl = Dinv (bl - Hpl^T xp)   (block_solver.hpp:461-481)
@@ -871,24 +857,19 @@ static NcclApi* nccl_api() {
     return &api;
 }
 enum { NCCL_U8 = 1, NCCL_I32 = 2, NCCL_F64 = 8, NCCL_SUM = 0, NCCL_MAX = 2 };
-enum { BK_ERRORS = 0, BK_LIN_POINTS, BK_LIN_POSES, BK_DINV, BK_SCHUR, BK_XCHG, BK_SOLVE, BK_BACKSUB, BK_UPDATE, BK_SCALE, BK_END, BK_COUNT };
-static const char* kBaKindNames[BK_COUNT] = {"k_ba_errors", "k_ba_lin_points", "k_ba_lin_poses", "k_ba_dinv", "k_ba_schur", "exchange", "k_ba_solve", "k_ba_backsub", "k_ba_update", "k_ba_scale", "end"};
+enum { BK_ERRORS = 0, BK_LIN_POINTS, BK_LIN_POSES, BK_DINV, BK_SCHUR, BK_XCHG, BK_SOLVE, BK_BACKSUB, BK_UPDATE, BK_SCALE, BK_COUNT, BK_END = KernelTimer::END };
+static const char* kBaKindNames[BK_COUNT] = {"k_ba_errors", "k_ba_lin_points", "k_ba_lin_poses", "k_ba_dinv", "k_ba_schur", "exchange", "k_ba_solve", "k_ba_backsub", "k_ba_update", "k_ba_scale"};
 
 
 extern "C" int cslam_optimizer_create(cslam_optimizer** out, int device) {
     if (!out) return CSLAM_E_BADARG;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
+    const int rc = check_device(device);
+    if (rc) return rc;
     cslam_optimizer* o = new cslam_optimizer; o->device = device;
     if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMallocHost(&o->h_scal, 16 * sizeof(double)) != cudaSuccess) {
         set_error("optimizer: stream / pinned allocation failed"); delete o; return CSLAM_E_CUDA;
     }
-    if (const char* e = getenv("CSLAM_SOLVE_CLUSTER")) o->clusterSize = std::max(1, std::min(atoi(e), 16));
-    if (o->clusterSize > 8) cudaFuncSetAttribute(k_ba_solve, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     cudaFuncSetAttribute(k_ba_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
-    if (const char* e = getenv("CSLAM_BA_GRAPH")) o->useGraphs = atoi(e) != 0;
     *out = o;
     return CSLAM_OK;
 }
@@ -908,15 +889,10 @@ extern "C" int64_t cslam_optimizer_launches(const cslam_optimizer* o) { return o
 extern "C" int cslam_optimizer_set_timing(cslam_optimizer* o, int enable) {
     if (!o) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(o->device));
-    if (enable && o->ev.empty()) { o->ev.resize(64); o->evKind.resize(64); for (auto& e : o->ev) CSLAM_CUDA(cudaEventCreate(&e)); }
-    o->timing = enable != 0; o->evUsed = 0;
-    for (int i = 0; i < 16; i++) { o->kindMs[i] = 0; o->kindCount[i] = 0; }
-    return CSLAM_OK;
+    return o->timer.enable(enable != 0, 64);
 }
 extern "C" int cslam_optimizer_get_timing(const cslam_optimizer* o, int kind, const char** name, double* ms, int64_t* count) {
-    if (!o || kind < 0 || kind >= BK_END) return CSLAM_E_BADARG;
-    *name = kBaKindNames[kind]; *ms = o->kindMs[kind]; *count = o->kindCount[kind];
-    return CSLAM_OK;
+    return o ? o->timer.get(kind, BK_COUNT, kBaKindNames, name, ms, count) : CSLAM_E_BADARG;
 }
 
 extern "C" int cslam_nccl_unique_id(uint8_t id128[128]) {
@@ -993,17 +969,11 @@ __global__ void __launch_bounds__(256) k_ba_prep_edges(int nE, const int* __rest
     if (s >= nE) return;
     const int e = perm ? perm[s] : s;
     const float2 k = kp[e];
-    const float fi = __fdiv_rn(k.x, (float)faceW), fj = __fdiv_rn(k.y, (float)faceH);
-    int f = -1;
-    if (fi >= 0 && fi < 1 && fj >= 1 && fj < 2) f = 1;
-    else if (fi >= 1 && fi < 2 && fj >= 0 && fj < 1) f = 3;
-    else if (fi >= 1 && fi < 2 && fj >= 1 && fj < 2) f = 0;
-    else if (fi >= 1 && fi < 2 && fj >= 2 && fj < 3) f = 4;
-    else if (fi >= 2 && fi < 3 && fj >= 1 && fj < 2) f = 2;
+    const int f = face_of_pixel_f(k.x, k.y, faceW, faceH);
     if (f < 0) atomicMin(bad, e);
     face[s] = (int8_t)f;
-    obs[3 * s] = (double)k.x - floor((double)k.x / faceW) * faceW;
-    obs[3 * s + 1] = (double)k.y - floor((double)k.y / faceH) * faceH;
+    obs[3 * s] = pos_in_face(k.x, faceW);
+    obs[3 * s + 1] = pos_in_face(k.y, faceH);
     obs[3 * s + 2] = (double)isig[e];
 }
 __global__ void __launch_bounds__(256) k_ba_prep_points(int n3, const float* __restrict__ in, double* __restrict__ out) {
@@ -1022,7 +992,6 @@ struct BAHost {
     double* HppFull = nullptr;        // multi-GPU: all-reduced copy of the pose blocks for computeLambdaInit
     size_t xstride = 0;               // one-shot path: doubles between the two payload buffers of an exchange region
     int* d_xerr = nullptr;
-    long long* d_prof = nullptr;      // CSLAM_BA_PROFILE=1: clock64 per solver phase (debug)
     double lambda = -1, ni = 2; int nBad = 0; int iterations = 0, trials = 0;
     bool errorsCurrent = false; double lastChi = 0;   // D.err / chi2 belong to the current state (set by an accepted trial)
     const volatile uint8_t* stop = nullptr;
@@ -1117,18 +1086,7 @@ struct BAHost {
         *lam = 1e-5 * o->h_scal[2];
         return 0;
     }
-    // ---- optional per-kernel timing (cslam_optimizer_set_timing): CUDA events between launches, accumulated per kernel kind
-    void tick(int kind) {
-        if (!o->timing || o->evUsed >= (int)o->ev.size()) return;
-        cudaEventRecord(o->ev[o->evUsed], o->stream); o->evKind[o->evUsed++] = kind;
-    }
-    void collect() {
-        for (int i = 0; i + 1 < o->evUsed; i++) {
-            float ms = 0;
-            if (o->evKind[i] != BK_END && cudaEventElapsedTime(&ms, o->ev[i], o->ev[i + 1]) == cudaSuccess) { o->kindMs[o->evKind[i]] += ms; o->kindCount[o->evKind[i]]++; }
-        }
-        o->evUsed = 0;
-    }
+    void tick(int kind) { o->timer.record(o->stream, kind); }
     // One LM trial on the stream: lambda -> device, BlockSolver::solve (Dinv, Schur, [exchange], reduced solve, back substitution), push + oplus,
     // computeActiveErrors + activeRobustChi2, computeScale, the four scalars -> pinned host memory. Single-GPU trials are replayed as ONE CUDA graph.
     int enqueue_trial() {
@@ -1165,11 +1123,11 @@ struct BAHost {
             const size_t panel = 2 * (size_t)LD_NB * ldp * 8, ybytes = (size_t)D.n * 8;
             const int stage = panel + ybytes <= 200 * 1024 ? 1 : 0;
             cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(o->clusterSize); cfg.blockDim = dim3(SOLVE_T); cfg.dynamicSmemBytes = (stage ? panel : 0) + ybytes; cfg.stream = o->stream;
+            cfg.gridDim = dim3(SOLVE_CLUSTER); cfg.blockDim = dim3(SOLVE_T); cfg.dynamicSmemBytes = (stage ? panel : 0) + ybytes; cfg.stream = o->stream;
             cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = o->clusterSize; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+            at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = SOLVE_CLUSTER; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
             cfg.attrs = at; cfg.numAttrs = 1;
-            CSLAM_CUDA(cudaLaunchKernelEx(&cfg, k_ba_solve, R, Lt, LDt, Minv, ldp, stage, d_prof)); o->launches++;
+            CSLAM_CUDA(cudaLaunchKernelEx(&cfg, k_ba_solve, R, Lt, LDt, Minv, ldp, stage)); o->launches++;
         }
         tick(BK_BACKSUB);
         k_ba_backsub<<<grid(D.nMP * LM_LANES, 128), 128, 0, o->stream>>>(D); o->launches++;
@@ -1190,7 +1148,7 @@ struct BAHost {
     int run_trial() {
         int rc;
         o->h_scal[8] = lambda;
-        const bool useGraph = o->nranks == 1 && !o->timing && o->useGraphs;
+        const bool useGraph = o->nranks == 1 && !o->timer.on();
         if (useGraph) {
             if (!trialGraph) {
                 cudaGraph_t g = nullptr;
@@ -1208,7 +1166,7 @@ struct BAHost {
             o->launches += launchesPerTrial;
         } else if ((rc = enqueue_trial())) return rc;
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-        if (o->timing) collect();
+        o->timer.collect();
         return 0;
     }
     int64_t launchesPerTrial = 0;
@@ -1297,10 +1255,6 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     if (p->face_w != p->face_h || p->face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(o->device));
     free_pool(o);
-    const bool hostProf = getenv("CSLAM_BA_PROFILE") != nullptr;
-    auto tNow = []() { return std::chrono::steady_clock::now(); };
-    auto tMs = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-    const auto tp0 = tNow();
     const int nKF = p->n_kf, nMP = p->n_mp, nEg = p->n_edges;   // nEg: the caller's edges; nE below: the edges this rank works on
     if (r) { r->iterations = 0; r->trials = 0; if (r->outlier) std::memset(r->outlier, 0, nEg); }
     if (stop_flag && *stop_flag) return CSLAM_OK;   // src/Optimizer.cpp:359-361
@@ -1348,7 +1302,6 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     D.nQ = nQ;
     int rc;
     const int nmax = 6 * nQ;
-    const auto tp1 = tNow();
     const Pose* cpose = nullptr; double* cX = nullptr;
     int* d_eMP = nullptr; int* d_eKF = nullptr; int* d_perm = nullptr; float2* d_kp = nullptr; float* d_isig = nullptr; float* d_pts32 = nullptr; int* d_bad = nullptr;
     double* d_obs = nullptr; int8_t* d_face = nullptr;
@@ -1382,14 +1335,16 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         (rc = dalloc(o, &H.Lt, (size_t)LD_NB * H.ldp)) || (rc = dalloc(o, &H.LDt, (size_t)LD_NB * H.ldp)) || (rc = dalloc(o, &H.Minv, (size_t)(nmax / LD_NB + 1) * LD_NB * LD_NB)) || (rc = dalloc(o, &pairCnt, (size_t)nQ * nQ + 1)) ||
         (rc = dalloc(o, &H.d_xerr, 1, true))) return rc;
     D.poseIdx = H.d_poseIdx; D.ptAct = H.d_ptAct;
-    if (getenv("CSLAM_BA_PROFILE")) { if ((rc = dalloc(o, &H.d_prof, 8, true))) return rc; }
     // ---- multi-GPU exchange path
     if (o->nranks > 1) {
-        if (!getenv("CSLAM_BA_NCCL_ONLY") && (!o->oneShot || o->xchgBytes < payloadMax * 8)) {
+        // The one-shot path falls back to ncclAllReduce by itself where CUDA IPC is unavailable; CSLAM_BA_NCCL_ONLY forces that
+        // fallback, the only way to exercise it on a machine where IPC works.
+        const bool ncclOnly = getenv("CSLAM_BA_NCCL_ONLY") != nullptr;
+        if (!ncclOnly && (!o->oneShot || o->xchgBytes < payloadMax * 8)) {
             const int xr = setup_xchg(o, payloadMax * 8);
             if (xr < 0) return xr;
         }
-        H.useOneShot = o->oneShot && o->xchgBytes >= payloadMax * 8 && !getenv("CSLAM_BA_NCCL_ONLY");
+        H.useOneShot = o->oneShot && o->xchgBytes >= payloadMax * 8 && !ncclOnly;
         H.xstride = ((o->xchgBytes + 255) & ~(size_t)255) / 8;
         if ((rc = dalloc(o, &H.HppFull, (size_t)std::max(nQ, 1) * 36))) return rc;
     }
@@ -1414,8 +1369,6 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
         if (badEdge < nEg) { set_error("edge %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", badEdge, p->kp_xy[2 * badEdge], p->kp_xy[2 * badEdge + 1]); return CSLAM_E_BADARG; }
     }
-    if (hostProf) cudaStreamSynchronize(o->stream);
-    const auto tp2 = tNow();
     // ---- src/Optimizer.cpp:363-395
     if ((rc = H.initialize())) return rc;
     if ((rc = H.optimize(its1))) return rc;
@@ -1439,13 +1392,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         CSLAM_CUDA(cudaMemcpyAsync(gflags.data(), d_gflag, nEg, cudaMemcpyDeviceToHost, o->stream));
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
     }
-    const auto tp3 = tNow();
     H.drop_graph();
-    if (H.d_prof) {
-        long long hp[8]; cudaMemcpyAsync(hp, H.d_prof, sizeof(hp), cudaMemcpyDeviceToHost, o->stream); cudaStreamSynchronize(o->stream);
-        static const char* nm[8] = {"load diag", "factor diag", "trsm", "cluster sync 1", "stage panel", "trailing update", "cluster sync 2", "back substitution"};
-        for (int k = 0; k < 8; k++) std::fprintf(stderr, "[k_ba_solve] %-18s %10.1f kclk total, %7.2f us per trial\n", nm[k], hp[k] / 1e3, hp[k] / 1.9e3 / std::max(H.trials, 1));
-    }
     // ---- write back (src/Optimizer.cpp:432-450): float32 poses / points; with landmark sharding every rank holds its own points
     if (o->nranks > 1) {
         k_ba_mask_points<<<H.grid(nMP), 256, 0, o->stream>>>(D); o->launches++;
@@ -1466,6 +1413,5 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         r->iterations = H.iterations; r->trials = H.trials;
     }
     free_pool(o);
-    if (hostProf) std::fprintf(stderr, "[cslam_local_ba] host prep %.3f ms, upload + co-observation lists %.3f ms, LM schedule %.3f ms (%d trials), write-back %.3f ms\n", tMs(tp0, tp1), tMs(tp1, tp2), tMs(tp2, tp3), H.trials, tMs(tp3, tNow()));
     return CSLAM_OK;
 }

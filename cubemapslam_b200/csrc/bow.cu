@@ -112,8 +112,6 @@ struct cslam_vocabulary {
     uint8_t* dFeat = nullptr; int32_t *dN = nullptr, *dWord = nullptr, *dLeaf = nullptr, *dNode = nullptr, *dBowWord = nullptr, *dBowCount = nullptr; double* dBowVal = nullptr;
 };
 
-template <class T> static int valloc(cslam_vocabulary* v, T** p, size_t n) { void* q = nullptr; CSLAM_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T))); v->owned.push_back(q); *p = (T*)q; return 0; }
-
 extern "C" void cslam_vocabulary_destroy(cslam_vocabulary* v) {
     if (!v) return;
     cudaSetDevice(v->device);
@@ -126,10 +124,8 @@ extern "C" void cslam_vocabulary_destroy(cslam_vocabulary* v) {
 extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k, int L, int n_nodes, const int32_t* parent, const uint8_t* is_leaf, const uint8_t* desc,
                                        const double* weight, int max_frames, int max_features) {
     if (!out || k < 2 || L < 1 || n_nodes <= 0 || !parent || !is_leaf || !desc || !weight || max_frames <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_vocabulary_create: bad argument"); return CSLAM_E_BADARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
+    int rc = check_device(device);
+    if (rc) return rc;
     const int N = n_nodes + 1;
     std::vector<int> cnt(N + 1, 0), wordId(N, -1);
     int words = 0;
@@ -146,13 +142,14 @@ extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k
     std::memcpy(d.data() + 32, desc, (size_t)n_nodes * 32);
     std::memcpy(w.data() + 1, weight, (size_t)n_nodes * 8);
     cslam_vocabulary* v = new cslam_vocabulary; v->device = device; v->maxFrames = max_frames; v->maxFeat = max_features;
-    int *dStart, *dList, *dWid; uint4* dDesc; double* dW; int rc;
+    int *dStart, *dList, *dWid; uint4* dDesc; double* dW;
     auto fail = [&](int code) { cslam_vocabulary_destroy(v); return code; };
     if (cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); return fail(CSLAM_E_CUDA); }
     const size_t nf = (size_t)max_frames * max_features;
-    if ((rc = valloc(v, &dStart, N + 1)) || (rc = valloc(v, &dList, n_nodes)) || (rc = valloc(v, &dWid, N)) || (rc = valloc(v, &dDesc, (size_t)N * 2)) || (rc = valloc(v, &dW, N)) ||
-        (rc = valloc(v, &v->dFeat, nf * 32)) || (rc = valloc(v, &v->dN, max_frames)) || (rc = valloc(v, &v->dWord, nf)) || (rc = valloc(v, &v->dLeaf, nf)) || (rc = valloc(v, &v->dNode, nf)) ||
-        (rc = valloc(v, &v->dBowWord, nf)) || (rc = valloc(v, &v->dBowVal, nf)) || (rc = valloc(v, &v->dBowCount, max_frames))) return fail(rc);
+    auto valloc = [&](auto** p, size_t n) { return dev_alloc(v->owned, p, n, false); };
+    if ((rc = valloc(&dStart, N + 1)) || (rc = valloc(&dList, n_nodes)) || (rc = valloc(&dWid, N)) || (rc = valloc(&dDesc, (size_t)N * 2)) || (rc = valloc(&dW, N)) ||
+        (rc = valloc(&v->dFeat, nf * 32)) || (rc = valloc(&v->dN, max_frames)) || (rc = valloc(&v->dWord, nf)) || (rc = valloc(&v->dLeaf, nf)) || (rc = valloc(&v->dNode, nf)) ||
+        (rc = valloc(&v->dBowWord, nf)) || (rc = valloc(&v->dBowVal, nf)) || (rc = valloc(&v->dBowCount, max_frames))) return fail(rc);
     if (cudaMemcpy(dStart, start.data(), (N + 1) * 4, cudaMemcpyHostToDevice) != cudaSuccess || cudaMemcpy(dList, list.data(), (size_t)n_nodes * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(dWid, wordId.data(), N * 4, cudaMemcpyHostToDevice) != cudaSuccess || cudaMemcpy(dDesc, d.data(), (size_t)N * 32, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(dW, w.data(), (size_t)N * 8, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("vocabulary upload failed"); return fail(CSLAM_E_CUDA); }

@@ -1,14 +1,18 @@
 // Shared helpers for the sm_90a kernels of libcubemap_b200.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <vector>
 #include "../../include/cubemap_b200.h"
 
 namespace cslam {
 
 void set_error(const char* fmt, ...);   // thread-local message behind cslam_last_error()
+// every handle constructor: CSLAM_E_NODEVICE without a CUDA device (no CPU fallback), CSLAM_E_BADARG for a device out of range, else cudaSetDevice
+int check_device(int device);
 
 #define CSLAM_CUDA(expr)                                                                        \
     do {                                                                                        \
@@ -21,6 +25,62 @@ void set_error(const char* fmt, ...);   // thread-local message behind cslam_las
 
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// Device buffer of `count` elements (at least one) owned by a handle: it goes onto `owned`, which the handle's destroy frees. zero: cleared once.
+template <class T>
+static int dev_alloc(std::vector<void*>& owned, T** p, size_t count, bool zero) {
+    void* q = nullptr;
+    const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
+    CSLAM_CUDA(cudaMalloc(&q, bytes));
+    owned.push_back(q);
+    if (zero) CSLAM_CUDA(cudaMemset(q, 0, bytes));
+    *p = (T*)q;
+    return 0;
+}
+
+// Optional per-kernel timing of a handle (cslam_*_set_timing / cslam_*_get_timing): record() puts an event on the stream before each
+// launch, and collect() adds the time from every event to the next one to the kind of the earlier event. A handle records END after its
+// last launch; the interval that starts there (up to the next call's first launch) belongs to no kernel and is not counted.
+struct KernelTimer {
+    static const int END = -1, MAX_KINDS = 16;
+    KernelTimer() = default;
+    KernelTimer(const KernelTimer&) = delete;
+    KernelTimer& operator=(const KernelTimer&) = delete;
+    ~KernelTimer() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
+    bool on() const { return enabled; }
+    // the first enable creates `capacity` events on the current device (records beyond them are dropped); every call clears the totals
+    int enable(bool en, int capacity) {
+        if (en && ev.empty()) {
+            ev.resize(capacity); evKind.resize(capacity);
+            for (auto& e : ev) CSLAM_CUDA(cudaEventCreate(&e));
+        }
+        enabled = en; used = 0;
+        for (int i = 0; i < MAX_KINDS; i++) { ms[i] = 0; count[i] = 0; }
+        return CSLAM_OK;
+    }
+    void record(cudaStream_t st, int kind) {
+        if (!enabled || used >= (int)ev.size()) return;
+        cudaEventRecord(ev[used], st);
+        evKind[used++] = kind;
+    }
+    void collect() {   // after the stream has been synchronised
+        for (int i = 0; i + 1 < used; i++) {
+            float t = 0;
+            if (evKind[i] != END && cudaEventElapsedTime(&t, ev[i], ev[i + 1]) == cudaSuccess) { ms[evKind[i]] += t; count[evKind[i]]++; }
+        }
+        used = 0;
+    }
+    int get(int kind, int nkinds, const char* const* names, const char** name, double* msOut, int64_t* countOut) const {
+        if (kind < 0 || kind >= nkinds) return CSLAM_E_BADARG;
+        *name = names[kind]; *msOut = ms[kind]; *countOut = count[kind];
+        return CSLAM_OK;
+    }
+
+  private:
+    bool enabled = false;
+    std::vector<cudaEvent_t> ev; std::vector<int> evKind; int used = 0;
+    double ms[MAX_KINDS] = {0}; int64_t count[MAX_KINDS] = {0};
+};
 
 // ---------------------------------------------------------------------------------------------------------
 // Device math with pinned rounding. The CPU path these must match bit-for-bit is specified without FMA

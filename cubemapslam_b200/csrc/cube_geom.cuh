@@ -4,17 +4,6 @@
 
 namespace cslam {
 
-// FaceInCubemap(const cv::Point2f&): `double i = pixel.x / mWCubeFace` (float quotient widened)
-__device__ __forceinline__ int face_of_pixel_d(float px, float py, int W, int H) {
-    const double i = (double)__fdiv_rn(px, (float)W), j = (double)__fdiv_rn(py, (float)H);
-    if (i >= 0 && i < 1 && j >= 1 && j < 2) return FACE_LEFT;
-    if (i >= 1 && i < 2 && j >= 0 && j < 1) return FACE_UPPER;
-    if (i >= 1 && i < 2 && j >= 1 && j < 2) return FACE_FRONT;
-    if (i >= 1 && i < 2 && j >= 2 && j < 3) return FACE_LOWER;
-    if (i >= 2 && i < 3 && j >= 1 && j < 2) return FACE_RIGHT;
-    return -1;
-}
-
 // TransformRaysToCubemap (src/CamModelGeneral.cpp:95-154): ordered face tests, double pinhole, float result, in-face bounds, tile offset
 __device__ __forceinline__ bool ray_to_cubemap(float x, float y, float z, int W, int H, float& up, float& vp) {
     int face; float lx, ly, lz;

@@ -17,6 +17,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <vector>
+#include "area_table.cuh"
 #include "common.cuh"
 
 namespace cslam {
@@ -79,14 +80,15 @@ __device__ __forceinline__ uint32_t gather_direct(const uint8_t* __restrict__ S,
 }
 
 // Tiled warp. The map is fixed at create time, so each output tile's source footprint is known: a CTA stages the bounding box of
-// its tile's taps for FPT frames into shared memory with coalesced 4-byte cp.async (zero-filled outside the source = BORDER_CONSTANT;
-// byte loads when source rows are not word-aligned), then gathers the 4 taps of each pixel from there. All FPT boxes are loaded
+// its tile's taps for WARP_FPT frames into shared memory with coalesced 4-byte cp.async (zero-filled outside the source = BORDER_CONSTANT;
+// byte loads when source rows are not word-aligned), then gathers the 4 taps of each pixel from there. All WARP_FPT boxes are loaded
 // before one barrier; several resident CTAs per SM overlap one CTA's loads with another's arithmetic. Tiles are WT_W canvas
 // columns (aligned to WT_W in canvas coordinates, so every thread stores its 4 pixels as one aligned u32) x WT_H face rows;
 // columns outside the face are masked, so only the five face ROIs are written. Table entry of a staged pixel: box offset | fx<<16 | fy<<21, or WE_ORIGIN for a pixel whose map is (0,0) (outside
 // the image circle: cv::remap reads S(0,0) with zero fractions). A tile whose box exceeds WARP_BOX_MAX is `direct`: its entries are
 // the raw map and its pixels gather from global memory.
 static const int WT_W = 32, WT_H = 32;
+static const int WARP_FPT = 8;   // frames per CTA
 static const int WARP_BOX_MAX = 6144;
 static const uint32_t WE_ORIGIN = 1u << 26;
 struct WarpTile {
@@ -102,14 +104,13 @@ __device__ __forceinline__ void cp_async4_zfill(void* smem, const void* gmem, in
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(s), "l"(gmem), "r"(srcBytes) : "memory");
 }
 
-template <int FPT>
 __global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fisheye, int Iw, int Ih, const WarpTile* __restrict__ tiles,
                                               const uint32_t* __restrict__ ent, uint8_t* __restrict__ canvas, int cpitch, size_t cframe, int batch,
                                               int slot, int words) {
-    extern __shared__ __align__(16) uint8_t wsm[];   // FPT boxes of `slot` bytes, then S(0,0) of each frame
-    uint8_t* origin = wsm + FPT * slot;
+    extern __shared__ __align__(16) uint8_t wsm[];   // WARP_FPT boxes of `slot` bytes, then S(0,0) of each frame
+    uint8_t* origin = wsm + WARP_FPT * slot;
     const WarpTile T = tiles[blockIdx.x];
-    const int f0 = blockIdx.y * FPT, nf = min(FPT, batch - f0), tid = threadIdx.x;
+    const int f0 = blockIdx.y * WARP_FPT, nf = min(WARP_FPT, batch - f0), tid = threadIdx.x;
     const size_t fsz = (size_t)Iw * Ih;
     const uint8_t* S0 = fisheye + (size_t)f0 * fsz;
     if (!T.direct) {
@@ -146,7 +147,7 @@ __global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fishey
     uint8_t* D = canvas + (size_t)f0 * cframe + (size_t)(T.row0 + r) * cpitch + x;
     const int bw = T.bw;
 #pragma unroll
-    for (int k = 0; k < FPT; k++) {
+    for (int k = 0; k < WARP_FPT; k++) {
         if (k >= nf) break;
         uint32_t out = 0;
         if (T.direct) {
@@ -706,8 +707,7 @@ __global__ void __launch_bounds__(256) k_distribute(DistributeArgs A) {
             const uint32_t x = key & 0xfff, y = (key >> 12) & 0xfff, r = (uint32_t)(b >> 40) - 1;
             const uint32_t lx = x + g.minB, ly = y + g.minB;
             const float ptx = __fmul_rn((float)lx, g.scale), pty = __fmul_rn((float)ly, g.scale);
-            const float fi = __fdiv_rn(ptx, (float)A.faceW), fj = __fdiv_rn(pty, (float)A.faceH);
-            const bool face = (fi >= 0 && fi < 1 && fj >= 1 && fj < 2) || (fi >= 1 && fi < 2 && fj >= 0 && fj < 3) || (fi >= 2 && fi < 3 && fj >= 1 && fj < 2);
+            const bool face = face_of_pixel_f(ptx, pty, A.faceW, A.faceH) >= 0;
             const int mxI = (int)__fadd_rn(ptx, 0.5f), myI = (int)__fadd_rn(pty, 0.5f);
             keep = face && !(ptx < 0 || mxI >= A.imgW || pty < 0 || myI >= A.imgH);
             if (keep) keep = A.mask[(size_t)myI * A.maskPitch + mxI] != 0;
@@ -864,6 +864,9 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
 // =================================================================================================== host side
 using namespace cslam;
 
+enum { KIND_WARP = 0, KIND_PYRAMID, KIND_FAST, KIND_DISTRIBUTE, KIND_DESCRIBE, KIND_COUNT, KIND_END = KernelTimer::END };
+static const char* kKindNames[KIND_COUNT] = {"k_warp", "k_pyramid", "k_fast", "k_distribute", "k_describe"};
+
 struct cslam_frontend {
     int device = 0;
     cslam_cam_params cam;
@@ -875,7 +878,6 @@ struct cslam_frontend {
     std::vector<float> map1, map2;   // host float maps (3H x 3W), kept for cslam_frontend_get_maps
     const WarpTile* d_wtiles = nullptr; const uint32_t* d_went = nullptr;   // k_warp tiles and their WT_W x WT_H entry tables
     int nWarpTiles = 0, warpSlot = 0;   // warpSlot: staged source box bytes per frame (largest staged box, rounded to 16)
-    int warpFpt = 8;                    // frames per k_warp CTA, 4 or 8 (env CSLAM_WARP_FPT)
     uint8_t* d_mask = nullptr; int maskPitch = 0;
     uint8_t* d_fisheye = nullptr;    // staging for host entry points: maxBatch x Ih x Iw
     uint32_t* d_candCount = nullptr; // maxBatch x nlevels
@@ -886,31 +888,18 @@ struct cslam_frontend {
     std::vector<void*> owned;
     static const int MAX_LANES = 4;
     cudaStream_t lane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evLane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evFork = nullptr;
-    int devLanes = 2;                // lanes used by cslam_frontend_run_dev (env CSLAM_DEV_LANES)
-    int hostChunks = 8;              // chunks a host-buffer batch is cut into (env CSLAM_HOST_CHUNKS)
+    static constexpr int DEV_LANES = 2;     // lanes used by cslam_frontend_run_dev
+    static constexpr int HOST_CHUNKS = 8;   // most chunks a host-buffer batch is cut into
     int64_t launches = 0;
     int lastBatch = 0;
-    // optional per-kernel timing (cslam_frontend_set_timing): events between launches, accumulated per kernel kind
-    bool timing = false; std::vector<cudaEvent_t> ev; std::vector<int> evKind; int evUsed = 0;
-    double kindMs[8] = {0, 0, 0, 0, 0, 0, 0, 0}; int64_t kindCount[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     size_t distributeSmem = 0;
 };
 
-enum { KIND_WARP = 0, KIND_PYRAMID, KIND_FAST, KIND_DISTRIBUTE, KIND_DESCRIBE, KIND_END, KIND_COUNT };
-static const char* kKindNames[KIND_COUNT] = {"k_warp", "k_pyramid", "k_fast", "k_distribute", "k_describe", "end"};
 static inline void mark(cslam_frontend* fe, cudaStream_t st, int kind) {
     if (kind != KIND_END) fe->launches++;
-    if (!fe->timing || fe->evUsed >= (int)fe->ev.size()) return;
-    cudaEventRecord(fe->ev[fe->evUsed], st);
-    fe->evKind[fe->evUsed++] = kind;
-}
-static void collect_timing(cslam_frontend* fe) {
-    for (int i = 0; i + 1 < fe->evUsed; i++) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, fe->ev[i], fe->ev[i + 1]) == cudaSuccess) { fe->kindMs[fe->evKind[i]] += ms; fe->kindCount[fe->evKind[i]]++; }
-    }
-    fe->evUsed = 0;
+    fe->timer.record(st, kind);
 }
 
 static inline int cv_round_f(float v) { return (int)lrintf(v); }
@@ -921,13 +910,7 @@ static inline int cv_round_d(double v) { return (int)lrint(v); }
 static void host_cubemap_to_fisheye(const cslam_cam_params& cp, double up, double vp, double& uf, double& vf) {
     float i = (float)up, j = (float)vp;
     uf = -1; vf = -1;
-    const float fi = i / (float)cp.face_w, fj = j / (float)cp.face_h;
-    int face = -1;   // 0 front 1 left 2 right 3 upper 4 lower
-    if (fi >= 0 && fi < 1 && fj >= 1 && fj < 2) face = 1;
-    else if (fi >= 1 && fi < 2 && fj >= 0 && fj < 1) face = 3;
-    else if (fi >= 1 && fi < 2 && fj >= 1 && fj < 2) face = 0;
-    else if (fi >= 1 && fi < 2 && fj >= 2 && fj < 3) face = 4;
-    else if (fi >= 2 && fi < 3 && fj >= 1 && fj < 2) face = 2;
+    const int face = face_of_pixel_f(i, j, cp.face_w, cp.face_h);
     if (face < 0) return;
     const double fx = cp.face_w / 2.0, fy = cp.face_h / 2.0;
     i = i - static_cast<int>(i / cp.face_w) * cp.face_w;
@@ -935,10 +918,10 @@ static void host_cubemap_to_fisheye(const cslam_cam_params& cp, double up, doubl
     const double lz = 1.0, lx = (i - fx) * lz / fx, ly = (j - fy) * lz / fy;
     double X, Y, Z;
     switch (face) {
-        case 0: X = lx; Y = ly; Z = lz; break;
-        case 1: X = -lz; Y = ly; Z = lx; break;
-        case 2: X = lz; Y = ly; Z = -lx; break;
-        case 4: X = lx; Y = lz; Z = -ly; break;
+        case FACE_FRONT: X = lx; Y = ly; Z = lz; break;
+        case FACE_LEFT: X = -lz; Y = ly; Z = lx; break;
+        case FACE_RIGHT: X = lz; Y = ly; Z = -lx; break;
+        case FACE_LOWER: X = lx; Y = lz; Z = -ly; break;
         default: X = lx; Y = -lz; Z = ly; break;
     }
     double norm = std::sqrt(X * X + Y * Y);
@@ -953,19 +936,9 @@ static void host_cubemap_to_fisheye(const cslam_cam_params& cp, double up, doubl
 }
 
 template <class T>
-static int dev_alloc(cslam_frontend* fe, T** p, size_t count, bool zero = true) {
-    void* q = nullptr;
-    if (count == 0) count = 1;
-    CSLAM_CUDA(cudaMalloc(&q, count * sizeof(T)));
-    if (zero) CSLAM_CUDA(cudaMemset(q, 0, count * sizeof(T)));
-    fe->owned.push_back(q);
-    *p = (T*)q;
-    return 0;
-}
-template <class T>
 static int dev_upload(cslam_frontend* fe, const T** p, const std::vector<T>& v) {
     T* q = nullptr;
-    int rc = dev_alloc(fe, &q, v.size(), false);
+    int rc = dev_alloc(fe->owned, &q, v.size(), false);
     if (rc) return rc;
     CSLAM_CUDA(cudaMemcpy(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
     *p = q;
@@ -989,13 +962,11 @@ static void build_resize_tables(int sn, int dn, std::vector<uint16_t>& ofs, std:
 extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const cslam_cam_params* cam, const cslam_orb_params* orb,
                                      const uint8_t* mask, int mask_pitch, int max_batch) {
     if (!out || !cam || !orb || !mask || max_batch <= 0) { set_error("cslam_frontend_create: null/invalid argument"); return CSLAM_E_BADARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range (%d devices)", device, ndev); return CSLAM_E_BADARG; }
+    int rc = check_device(device);
+    if (rc) return rc;
     if (cam->face_w != cam->face_h || cam->face_w <= 0) { set_error("cube faces must be square (got %dx%d)", cam->face_w, cam->face_h); return CSLAM_E_BADARG; }
     if (3 * cam->face_w > 4095 || cam->Iw * 32 > 65535 || cam->Ih * 32 > 65535) { set_error("image too large for the packed coordinate formats"); return CSLAM_E_BADARG; }
     if (orb->nlevels < 1 || orb->nlevels > MAX_LEVELS || orb->nfeatures < 1 || orb->scale_factor <= 1.f || orb->scale_factor > 2.f) { set_error("bad ORB parameters (need 1 < scaleFactor <= 2)"); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
     cslam_frontend* fe = new cslam_frontend;
     fe->device = device; fe->cam = *cam; fe->orb = *orb; fe->maxBatch = max_batch;
     fe->W = cam->face_w; fe->H = cam->face_h; fe->CW = 3 * fe->W; fe->CH = 3 * fe->H;
@@ -1016,14 +987,11 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         for (v = 0; v <= vmax; ++v) fe->umax[v] = cv_round_d(std::sqrt(hp2 - v * v));
         for (v = HALF_PATCH, v0 = 0; v >= vmin; --v) { while (fe->umax[v0] == fe->umax[v0 + 1]) ++v0; fe->umax[v] = v0; ++v0; }
     }
-    int rc = 0;
     auto fail = [&](int code) { cslam_frontend_destroy(fe); return code; };
     if (cudaStreamCreateWithFlags(&fe->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("cudaStreamCreate failed"); return fail(CSLAM_E_CUDA); }
     for (int i = 0; i < cslam_frontend::MAX_LANES; i++)
         if (cudaStreamCreateWithFlags(&fe->lane[i], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&fe->evLane[i], cudaEventDisableTiming) != cudaSuccess) { set_error("lane stream creation failed"); return fail(CSLAM_E_CUDA); }
     if (cudaEventCreateWithFlags(&fe->evFork, cudaEventDisableTiming) != cudaSuccess) { set_error("event creation failed"); return fail(CSLAM_E_CUDA); }
-    if (const char* e = getenv("CSLAM_DEV_LANES")) fe->devLanes = std::max(1, std::min(atoi(e), (int)cslam_frontend::MAX_LANES));
-    if (const char* e = getenv("CSLAM_HOST_CHUNKS")) fe->hostChunks = std::max(1, std::min(atoi(e), 64));
     if (cudaMemcpyToSymbol(c_umax, fe->umax, sizeof(fe->umax)) != cudaSuccess) { set_error("cudaMemcpyToSymbol failed"); return fail(CSLAM_E_CUDA); }
     {
         static const signed char hostPattern[1024] = {
@@ -1057,9 +1025,9 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         g.quota = fe->perLevel[l]; maxQuota = std::max(maxQuota, g.quota);
         g.candCap = std::max(4096, g.nColsEff * g.nRowsEff * 32);
         g.scale = fe->scale[l]; g.sizeF = (float)(int)(PATCH_SIZE * fe->scale[l]);
-        if ((rc = dev_alloc(fe, &fe->L.img[l], (size_t)max_batch * g.pitch * g.h + 256))) return fail(rc);   // slack: word loads may run a few bytes past the last row
-        if ((rc = dev_alloc(fe, &fe->L.cand[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
-        if ((rc = dev_alloc(fe, &fe->L.pnode[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
+        if ((rc = dev_alloc(fe->owned, &fe->L.img[l], (size_t)max_batch * g.pitch * g.h + 256, true))) return fail(rc);   // slack: word loads may run a few bytes past the last row; zeroed: the black corners are never written on the warp path
+        if ((rc = dev_alloc(fe->owned, &fe->L.cand[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
+        if ((rc = dev_alloc(fe->owned, &fe->L.pnode[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
         if (l > 0) {
             std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
             build_resize_tables(fe->L.g[l - 1].w, g.w, xo, xa); build_resize_tables(fe->L.g[l - 1].h, g.h, yo, ya);
@@ -1134,11 +1102,10 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
                 fe->map1[(size_t)y * CW + x] = (float)u; fe->map2[(size_t)y * CW + x] = (float)v;
             }
         std::vector<uint32_t> q((size_t)5 * W * W);
-        const int tc[5] = {1, 0, 2, 1, 1}, tr[5] = {1, 1, 1, 0, 2};
         for (int f = 0; f < 5; f++)
             for (int y = 0; y < W; y++)
                 for (int x = 0; x < W; x++) {
-                    const size_t src = (size_t)(tr[f] * W + y) * CW + tc[f] * W + x;
+                    const size_t src = (size_t)(FACE_TILE_ROW[f] * W + y) * CW + FACE_TILE_COL[f] * W + x;
                     const int sx = cv_round_f(fe->map1[src] * 32.f), sy = cv_round_f(fe->map2[src] * 32.f);
                     q[((size_t)f * W + y) * W + x] = (uint32_t)sx | ((uint32_t)sy << 16);
                 }
@@ -1148,11 +1115,11 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         std::vector<uint32_t> ent;
         int slot = 0;
         for (int f = 0; f < 5; f++) {
-            const int cx0 = tc[f] * W, cx1 = cx0 + W;
+            const int cx0 = FACE_TILE_COL[f] * W, cx1 = cx0 + W;
             for (int y0 = 0; y0 < W; y0 += WT_H)
                 for (int xa = cx0 / WT_W * WT_W; xa < cx1; xa += WT_W) {
                     WarpTile t;
-                    t.row0 = tr[f] * W + y0; t.xa = xa; t.cx0 = cx0; t.cx1 = cx1; t.nr = std::min(WT_H, W - y0);
+                    t.row0 = FACE_TILE_ROW[f] * W + y0; t.xa = xa; t.cx0 = cx0; t.cx1 = cx1; t.nr = std::min(WT_H, W - y0);
                     int minX = 1 << 30, minY = 1 << 30, maxX = -1, maxY = -1;
                     auto mapAt = [&](int r, int c) { return q[((size_t)f * W + y0 + r) * W + (xa + c - cx0)]; };
                     auto inFace = [&](int r, int c) { return r < t.nr && xa + c >= cx0 && xa + c < cx1; };
@@ -1185,26 +1152,23 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         }
         fe->nWarpTiles = (int)tiles.size();
         fe->warpSlot = round_up(std::max(slot, 16), 16);
-        if (const char* e = getenv("CSLAM_WARP_FPT")) fe->warpFpt = atoi(e) == 4 ? 4 : 8;
         const uint8_t* dt = nullptr;
         std::vector<uint8_t> tb(tiles.size() * sizeof(WarpTile));
         std::memcpy(tb.data(), tiles.data(), tb.size());
         if ((rc = dev_upload(fe, &dt, tb)) || (rc = dev_upload(fe, &fe->d_went, ent))) return fail(rc);
         fe->d_wtiles = reinterpret_cast<const WarpTile*>(dt);
-        const int smem8 = 8 * fe->warpSlot + 16;
-        if (cudaFuncSetAttribute(k_warp<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem8) != cudaSuccess ||
-            cudaFuncSetAttribute(k_warp<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem8) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
+        if (cudaFuncSetAttribute(k_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, WARP_FPT * fe->warpSlot + 16) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
     }
     // ---- mask
     fe->maskPitch = round_up(fe->CW, 128);
-    if ((rc = dev_alloc(fe, &fe->d_mask, (size_t)fe->maskPitch * fe->CH))) return fail(rc);
+    if ((rc = dev_alloc(fe->owned, &fe->d_mask, (size_t)fe->maskPitch * fe->CH, true))) return fail(rc);
     if (cudaMemcpy2D(fe->d_mask, fe->maskPitch, mask, mask_pitch, fe->CW, fe->CH, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("mask upload failed"); return fail(CSLAM_E_CUDA); }
     // ---- batch buffers
     const size_t B = max_batch;
-    if ((rc = dev_alloc(fe, &fe->d_fisheye, B * cam->Iw * cam->Ih)) || (rc = dev_alloc(fe, &fe->d_candCount, B * nl)) ||
-        (rc = dev_alloc(fe, &fe->d_kept, B * nl * fe->keptCap)) || (rc = dev_alloc(fe, &fe->d_keptCount, B * nl)) ||
-        (rc = dev_alloc(fe, &fe->d_kps, B * fe->kpCap)) || (rc = dev_alloc(fe, &fe->d_desc, B * fe->kpCap * 32)) ||
-        (rc = dev_alloc(fe, &fe->d_nout, B)) || (rc = dev_alloc(fe, &fe->d_err, 1))) return fail(rc);
+    if ((rc = dev_alloc(fe->owned, &fe->d_fisheye, B * cam->Iw * cam->Ih, true)) || (rc = dev_alloc(fe->owned, &fe->d_candCount, B * nl, true)) ||
+        (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->keptCap, true)) || (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) ||
+        (rc = dev_alloc(fe->owned, &fe->d_kps, B * fe->kpCap, true)) || (rc = dev_alloc(fe->owned, &fe->d_desc, B * fe->kpCap * 32, true)) ||
+        (rc = dev_alloc(fe->owned, &fe->d_nout, B, true)) || (rc = dev_alloc(fe->owned, &fe->d_err, 1, true))) return fail(rc);
     const size_t inBytes = std::max((size_t)cam->Iw * cam->Ih, (size_t)fe->L.g[0].pitch * fe->CH) * B;
     if (cudaMallocHost(&fe->h_pin_in, inBytes) != cudaSuccess || cudaMallocHost(&fe->h_pin_kps, B * fe->kpCap * sizeof(cslam_keypoint)) != cudaSuccess ||
         cudaMallocHost(&fe->h_pin_desc, B * fe->kpCap * 32) != cudaSuccess || cudaMallocHost(&fe->h_pin_n, B * sizeof(int32_t)) != cudaSuccess ||
@@ -1221,7 +1185,6 @@ extern "C" void cslam_frontend_destroy(cslam_frontend* fe) {
     if (fe->evFork) cudaEventDestroy(fe->evFork);
     if (fe->stream) cudaStreamDestroy(fe->stream);
     for (void* p : fe->owned) cudaFree(p);
-    for (auto& e : fe->ev) cudaEventDestroy(e);
     if (fe->h_pin_in) cudaFreeHost(fe->h_pin_in);
     if (fe->h_pin_kps) cudaFreeHost(fe->h_pin_kps);
     if (fe->h_pin_desc) cudaFreeHost(fe->h_pin_desc);
@@ -1233,18 +1196,10 @@ extern "C" void cslam_frontend_destroy(cslam_frontend* fe) {
 extern "C" int cslam_frontend_set_timing(cslam_frontend* fe, int enable) {
     if (!fe) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(fe->device));
-    if (enable && fe->ev.empty()) {
-        fe->ev.resize(256); fe->evKind.resize(256);
-        for (auto& e : fe->ev) CSLAM_CUDA(cudaEventCreate(&e));
-    }
-    fe->timing = enable != 0; fe->evUsed = 0;
-    for (int i = 0; i < 8; i++) { fe->kindMs[i] = 0; fe->kindCount[i] = 0; }
-    return CSLAM_OK;
+    return fe->timer.enable(enable != 0, 256);
 }
 extern "C" int cslam_frontend_get_timing(const cslam_frontend* fe, int kind, const char** name, double* ms, int64_t* count) {
-    if (!fe || kind < 0 || kind >= KIND_END) return CSLAM_E_BADARG;
-    *name = kKindNames[kind]; *ms = fe->kindMs[kind]; *count = fe->kindCount[kind];
-    return CSLAM_OK;
+    return fe ? fe->timer.get(kind, KIND_COUNT, kKindNames, name, ms, count) : CSLAM_E_BADARG;
 }
 extern "C" int cslam_frontend_kp_capacity(const cslam_frontend* fe) { return fe ? fe->kpCap : 0; }
 extern "C" void* cslam_frontend_stream(const cslam_frontend* fe) { return fe ? (void*)fe->stream : nullptr; }
@@ -1255,7 +1210,7 @@ extern "C" int cslam_frontend_sync(cslam_frontend* fe) {
     CSLAM_CUDA(cudaSetDevice(fe->device));
     CSLAM_CUDA(cudaMemcpyAsync(fe->h_pin_err, fe->d_err, sizeof(int), cudaMemcpyDeviceToHost, fe->stream));
     CSLAM_CUDA(cudaStreamSynchronize(fe->stream));
-    if (fe->timing) collect_timing(fe);
+    fe->timer.collect();
     if (*fe->h_pin_err != 0) {
         const int code = *fe->h_pin_err;
         cudaMemsetAsync(fe->d_err, 0, sizeof(int), fe->stream);
@@ -1281,12 +1236,10 @@ static int launch_warp(cslam_frontend* fe, cudaStream_t st, const uint8_t* d_fis
     uint8_t* canvas = fe->L.img[0] + (size_t)f0 * cframe;
     const int Iw = fe->cam.Iw, Ih = fe->cam.Ih, pitch = fe->L.g[0].pitch;
     const int words = (Iw % 4 == 0 && ((uintptr_t)d_fisheye & 3) == 0) ? 1 : 0;   // 4-byte staging needs word-aligned source rows
-    const int fpt = fe->warpFpt;
-    dim3 grid(fe->nWarpTiles, cdiv(cnt, fpt));
-    const size_t smem = (size_t)fpt * fe->warpSlot + 16;
+    dim3 grid(fe->nWarpTiles, cdiv(cnt, WARP_FPT));
+    const size_t smem = (size_t)WARP_FPT * fe->warpSlot + 16;
     mark(fe, st, KIND_WARP);
-    if (fpt == 8) k_warp<8><<<grid, 256, smem, st>>>(d_fisheye, Iw, Ih, fe->d_wtiles, fe->d_went, canvas, pitch, cframe, cnt, fe->warpSlot, words);
-    else k_warp<4><<<grid, 256, smem, st>>>(d_fisheye, Iw, Ih, fe->d_wtiles, fe->d_went, canvas, pitch, cframe, cnt, fe->warpSlot, words);
+    k_warp<<<grid, 256, smem, st>>>(d_fisheye, Iw, Ih, fe->d_wtiles, fe->d_went, canvas, pitch, cframe, cnt, fe->warpSlot, words);
     CSLAM_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1362,7 +1315,7 @@ static int prepare_level0(cslam_frontend* fe, bool fromWarp) {
     return 0;
 }
 static int lanes_for(const cslam_frontend* fe, int batch, int want) {
-    if (fe->timing) return 1;
+    if (fe->timer.on()) return 1;
     return std::max(1, std::min(std::min(want, cslam_frontend::MAX_LANES), batch));
 }
 
@@ -1377,11 +1330,12 @@ extern "C" int cslam_warp(cslam_frontend* fe, const uint8_t* fisheye, int batch,
     if ((rc = launch_warp(fe, fe->stream, fe->d_fisheye, 0, batch))) return rc;
     // the reference writes only the five face ROIs; corner tiles of the caller's canvas are left untouched
     const int W = fe->W, pitch = fe->L.g[0].pitch;
-    const int tc[5] = {1, 0, 2, 1, 1}, tr[5] = {1, 1, 1, 0, 2};
     for (int f = 0; f < batch; f++)
-        for (int t = 0; t < 5; t++)
-            CSLAM_CUDA(cudaMemcpy2DAsync(canvas + (size_t)f * canvas_pitch * fe->CH + (size_t)tr[t] * W * canvas_pitch + tc[t] * W, canvas_pitch,
-                                         fe->L.img[0] + (size_t)f * pitch * fe->CH + (size_t)tr[t] * W * pitch + tc[t] * W, pitch, W, W, cudaMemcpyDeviceToHost, fe->stream));
+        for (int t = 0; t < 5; t++) {
+            const size_t row = (size_t)FACE_TILE_ROW[t] * W, col = (size_t)FACE_TILE_COL[t] * W;
+            CSLAM_CUDA(cudaMemcpy2DAsync(canvas + (size_t)f * canvas_pitch * fe->CH + row * canvas_pitch + col, canvas_pitch,
+                                         fe->L.img[0] + (size_t)f * pitch * fe->CH + row * pitch + col, pitch, W, W, cudaMemcpyDeviceToHost, fe->stream));
+        }
     return cslam_frontend_sync(fe);
 }
 
@@ -1392,7 +1346,7 @@ static int run_host(cslam_frontend* fe, const uint8_t* in, size_t inFrameBytes, 
     const int nlanes = lanes_for(fe, batch, 4);
     // the batch is cut into more chunks than there are streams (chunk c runs on stream c % nlanes): the first upload - the only one nothing overlaps -
     // is then 1/8 of the batch instead of 1/4, and the copy engines stay busy behind the kernels of earlier chunks
-    const int nchunks = fe->timing ? 1 : std::max(nlanes, std::min(fe->hostChunks, std::max(1, batch / 8)));
+    const int nchunks = fe->timer.on() ? 1 : std::max(nlanes, std::min(cslam_frontend::HOST_CHUNKS, std::max(1, batch / 8)));
     const bool pinIn = is_pinned(in), pinK = is_pinned(kps), pinD = is_pinned(desc), pinN = is_pinned(n_out);
     const size_t nk = (size_t)fe->kpCap;
     if ((rc = fork_lanes(fe, nlanes))) return rc;
@@ -1452,7 +1406,7 @@ extern "C" int cslam_frontend_run_dev(cslam_frontend* fe, const uint8_t* fisheye
     if (rc) return rc;
     if (!desc_dev || !n_out_dev) { set_error("cslam_frontend_run_dev: null output"); return CSLAM_E_BADARG; }
     if ((rc = prepare_level0(fe, true))) return rc;
-    const int nlanes = lanes_for(fe, batch, fe->devLanes);
+    const int nlanes = lanes_for(fe, batch, cslam_frontend::DEV_LANES);
     const size_t nk = (size_t)fe->kpCap, fsz = (size_t)fe->cam.Iw * fe->cam.Ih;
     if ((rc = fork_lanes(fe, nlanes))) return rc;
     int erc = 0;

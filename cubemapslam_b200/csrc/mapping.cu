@@ -179,7 +179,7 @@ __device__ __forceinline__ float dot3_f(float a0, float a1, float a2, float b0, 
 __device__ float vector_sigma_d(float kx, float ky, float nx, float ny, float nz, int W, int H) {
     const double fx = W / 2.0, cx = W / 2.0, cy = H / 2.0;
     float c0, c1;   // normalCam(0), normalCam(1)  (cvtRigToFaces<float>)
-    switch (face_of_pixel_d(kx, ky, W, H)) {
+    switch (face_of_pixel_f(kx, ky, W, H)) {
         case FACE_FRONT: c0 = nx; c1 = ny; break;
         case FACE_LEFT: c0 = nz; c1 = ny; break;
         case FACE_RIGHT: c0 = -nz; c1 = ny; break;
@@ -339,12 +339,10 @@ template <class T> static int mbuf(cslam_mapper* m, int slot, size_t count, T** 
 
 extern "C" int cslam_mapper_create(cslam_mapper** out, int device) {
     if (!out) return CSLAM_E_BADARG;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
+    int rc = check_device(device);
+    if (rc) return rc;
     cslam_mapper* m = new cslam_mapper; m->device = device;
-    int rc = cslam_tracker_create(&m->trk, device, 1, 4096);
+    rc = cslam_tracker_create(&m->trk, device, 1, 4096);
     if (rc) { delete m; return rc; }
     m->stream = (cudaStream_t)cslam_tracker_stream(m->trk);   // one stream: the frame index and the searches are ordered
     cudaFuncSetAttribute(k_triangulation, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 4);

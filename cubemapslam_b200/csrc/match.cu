@@ -383,25 +383,25 @@ struct cslam_matcher {
     int32_t *nodeA = nullptr, *nodeB = nullptr, *dMatch = nullptr, *dDist = nullptr, *dSecond = nullptr, *dN = nullptr;
     cslam_keypoint* dKps = nullptr;   // staging of cslam_match_frames (lazily allocated)
     int* dHist = nullptr;             // per-pair rotation histogram of the row-split brute-force launches (lazily allocated)
+    std::vector<void*> owned;
     int64_t launches = 0;
 };
 
 extern "C" int cslam_matcher_create(cslam_matcher** out, int device, int max_pairs, int max_features) {
     if (!out || max_pairs <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_matcher_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
+    int rc = check_device(device);
+    if (rc) return rc;
     cslam_matcher* m = new cslam_matcher;
     m->device = device; m->maxPairs = max_pairs; m->maxFeat = max_features;
     const size_t nf = (size_t)max_pairs * max_features;
-    if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMalloc(&m->dA, nf * 32) != cudaSuccess || cudaMalloc(&m->dB, nf * 32) != cudaSuccess ||
-        cudaMalloc(&m->dValid, nf) != cudaSuccess || cudaMalloc(&m->aA, nf * 4) != cudaSuccess || cudaMalloc(&m->aB, nf * 4) != cudaSuccess ||
-        cudaMalloc(&m->nodeA, nf * 4) != cudaSuccess || cudaMalloc(&m->nodeB, nf * 4) != cudaSuccess || cudaMalloc(&m->dMatch, nf * 4) != cudaSuccess ||
-        cudaMalloc(&m->dDist, nf * 4) != cudaSuccess || cudaMalloc(&m->dSecond, nf * 4) != cudaSuccess || cudaMalloc(&m->dN, (size_t)max_pairs * 4) != cudaSuccess) {
-        set_error("matcher: device allocation failed");
+    if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); cslam_matcher_destroy(m); return CSLAM_E_CUDA; }
+    std::vector<void*>& o = m->owned;
+    if ((rc = dev_alloc(o, &m->dA, nf * 32, false)) || (rc = dev_alloc(o, &m->dB, nf * 32, false)) || (rc = dev_alloc(o, &m->dValid, nf, false)) ||
+        (rc = dev_alloc(o, &m->aA, nf, false)) || (rc = dev_alloc(o, &m->aB, nf, false)) || (rc = dev_alloc(o, &m->nodeA, nf, false)) || (rc = dev_alloc(o, &m->nodeB, nf, false)) ||
+        (rc = dev_alloc(o, &m->dMatch, nf, false)) || (rc = dev_alloc(o, &m->dDist, nf, false)) || (rc = dev_alloc(o, &m->dSecond, nf, false)) ||
+        (rc = dev_alloc(o, &m->dN, max_pairs, false))) {
         cslam_matcher_destroy(m);
-        return CSLAM_E_CUDA;
+        return rc;
     }
     cudaFuncSetAttribute(k_search_by_bow, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
     *out = m;
@@ -412,8 +412,7 @@ extern "C" void cslam_matcher_destroy(cslam_matcher* m) {
     if (!m) return;
     cudaSetDevice(m->device);
     if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-    void* ptrs[] = {m->dA, m->dB, m->dValid, m->aA, m->aB, m->nodeA, m->nodeB, m->dMatch, m->dDist, m->dSecond, m->dN, m->dKps, m->dHist};
-    for (void* p : ptrs) if (p) cudaFree(p);
+    for (void* p : m->owned) cudaFree(p);
     delete m;
 }
 extern "C" void* cslam_matcher_stream(const cslam_matcher* m) { return m ? (void*)m->stream : nullptr; }
@@ -430,7 +429,7 @@ static int bf_split(cslam_matcher* m, int maxRowsA, int npairs, int* parts, int*
     *parts = std::max(1, cdiv(maxRowsA, BF_ROWS));
     *gHist = nullptr;
     if (*parts > 1) {
-        if (!m->dHist) CSLAM_CUDA(cudaMalloc(&m->dHist, (size_t)m->maxPairs * 32 * sizeof(int)));
+        if (!m->dHist) { const int rc = dev_alloc(m->owned, &m->dHist, (size_t)m->maxPairs * 32, false); if (rc) return rc; }
         CSLAM_CUDA(cudaMemsetAsync(m->dHist, 0, (size_t)npairs * 32 * sizeof(int), m->stream));
         *gHist = m->dHist;
     }
@@ -508,7 +507,7 @@ extern "C" int cslam_match_frames(cslam_matcher* m, const cslam_keypoint* kps, c
     if (!m || nframes < 2 || nframes > m->maxPairs || kp_stride <= 0 || kp_stride > m->maxFeat) { set_error("cslam_match_frames: sizes out of range (frames %d/%d, stride %d/%d)", nframes, m ? m->maxPairs : 0, kp_stride, m ? m->maxFeat : 0); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(m->device));
     const size_t nf = (size_t)nframes * kp_stride;
-    if (!m->dKps) CSLAM_CUDA(cudaMalloc(&m->dKps, (size_t)m->maxPairs * m->maxFeat * sizeof(cslam_keypoint)));
+    if (!m->dKps) { const int rc = dev_alloc(m->owned, &m->dKps, (size_t)m->maxPairs * m->maxFeat, false); if (rc) return rc; }
     CSLAM_CUDA(cudaMemcpyAsync(m->dKps, kps, nf * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(m->dA, desc, nf * 32, cudaMemcpyHostToDevice, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(m->nodeA, n, (size_t)nframes * 4, cudaMemcpyHostToDevice, m->stream));
@@ -517,6 +516,27 @@ extern "C" int cslam_match_frames(cslam_matcher* m, const cslam_keypoint* kps, c
     CSLAM_CUDA(cudaMemcpyAsync(match12, m->dMatch, (size_t)(nframes - 1) * kp_stride * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, m->dN, (size_t)(nframes - 1) * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
+    return CSLAM_OK;
+}
+
+// Harness of the register-only issue-rate micro-benchmarks below: 8 CTAs per SM, a warm-up launch of 100 iterations, then the timed
+// launch of `iters`. launch(blocks, iters, out) enqueues the kernel on m->stream; *blocks is the grid it was given, *ms the timed launch.
+template <class Launch>
+static int time_ubench(cslam_matcher* m, int iters, Launch launch, int* blocks, float* ms) {
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
+    *blocks = sms * 8;
+    uint32_t* out = reinterpret_cast<uint32_t*>(m->dN);
+    cudaEvent_t e0, e1;
+    CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
+    launch(*blocks, 100, out);   // warm-up
+    CSLAM_CUDA(cudaEventRecord(e0, m->stream));
+    launch(*blocks, iters, out);
+    CSLAM_CUDA(cudaEventRecord(e1, m->stream));
+    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
+    CSLAM_CUDA(cudaEventElapsedTime(ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    m->launches += 2;
     return CSLAM_OK;
 }
 
@@ -538,20 +558,10 @@ __global__ void __launch_bounds__(256) k_ubench_popc(uint32_t* out, int iters, u
 extern "C" int cslam_ubench_popc(cslam_matcher* m, double* popc32_per_s) {
     if (!m || !popc32_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-    const int blocks = sms * 8, iters = 20000;
-    cudaEvent_t e0, e1;
-    CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
-    k_ubench_popc<<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), 100, 1u);   // warm-up
-    CSLAM_CUDA(cudaEventRecord(e0, m->stream));
-    k_ubench_popc<<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), iters, 1u);
-    CSLAM_CUDA(cudaEventRecord(e1, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    float ms = 0;
-    CSLAM_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    m->launches += 2;
+    const int iters = 20000;
+    int blocks; float ms;
+    const int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_popc<<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
+    if (rc) return rc;
     *popc32_per_s = (double)blocks * 256.0 * iters * 8.0 / (ms * 1e-3);
     return CSLAM_OK;
 }
@@ -583,34 +593,16 @@ __global__ void __launch_bounds__(256) k_ubench_mma(uint32_t* out, int iters, ui
     for (int c = 0; c < 8; c++) s += acc[c][0] + acc[c][1] + acc[c][2] + acc[c][3];
     if (s == 0x7eadbeef) out[0] = (uint32_t)s;   // keeps the chains alive
 }
-template <bool BINARY>
-static int time_ubench_mma(cslam_matcher* m, double* ms_out, double* mma_count) {
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-    const int blocks = sms * 8, iters = 4000;
-    cudaEvent_t e0, e1;
-    CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
-    k_ubench_mma<BINARY><<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), 100, 1u);   // warm-up
-    CSLAM_CUDA(cudaEventRecord(e0, m->stream));
-    k_ubench_mma<BINARY><<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), iters, 1u);
-    CSLAM_CUDA(cudaEventRecord(e1, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    float ms = 0;
-    CSLAM_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    m->launches += 2;
-    *ms_out = ms;
-    *mma_count = (double)blocks * 8.0 * iters * 8.0;   // warp-level MMA instructions
-    return CSLAM_OK;
-}
 extern "C" int cslam_ubench_bmma(cslam_matcher* m, double* bmma_products_per_s, double* imma_products_per_s) {
     if (!m || !bmma_products_per_s || !imma_products_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
-    double ms, n;
-    int rc = time_ubench_mma<true>(m, &ms, &n);
+    const int iters = 4000;
+    int blocks; float ms;
+    int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_mma<true><<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
     if (rc) return rc;
+    const double n = (double)blocks * 8.0 * iters * 8.0;     // warp-level MMA instructions
     *bmma_products_per_s = n * 128.0 / (ms * 1e-3);          // 16 x 8 256-bit products per BMMA
-    rc = time_ubench_mma<false>(m, &ms, &n);
+    rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_mma<false><<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
     if (rc) return rc;
     *imma_products_per_s = n * 128.0 / 8.0 / (ms * 1e-3);    // 16 x 8 dot products of 32 bytes; a 256-bit product is 8 of them
     return CSLAM_OK;
@@ -636,20 +628,10 @@ __global__ void __launch_bounds__(256) k_ubench_minmax3(uint32_t* out, int iters
 extern "C" int cslam_ubench_minmax3(cslam_matcher* m, double* ops_per_s) {
     if (!m || !ops_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-    const int blocks = sms * 8, iters = 20000;
-    cudaEvent_t e0, e1;
-    CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
-    k_ubench_minmax3<<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), 100, 1u);   // warm-up
-    CSLAM_CUDA(cudaEventRecord(e0, m->stream));
-    k_ubench_minmax3<<<blocks, 256, 0, m->stream>>>(reinterpret_cast<uint32_t*>(m->dN), iters, 1u);
-    CSLAM_CUDA(cudaEventRecord(e1, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    float ms = 0;
-    CSLAM_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    m->launches += 2;
+    const int iters = 20000;
+    int blocks; float ms;
+    const int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_minmax3<<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
+    if (rc) return rc;
     *ops_per_s = (double)blocks * 256.0 * iters * 8.0 / (ms * 1e-3);   // warp-lane u16x2 3-input min/max per second
     return CSLAM_OK;
 }

@@ -2,6 +2,7 @@
 #pragma once
 #include <algorithm>
 #include <vector>
+#include "area_table.cuh"
 #include "ba_math.cuh"
 #include "common.cuh"
 
@@ -16,12 +17,9 @@ struct cslam_optimizer {
     struct Chunk { char* p; size_t size, used; };
     std::vector<Chunk> chunks;
     double* h_scal = nullptr;   // pinned, 16 doubles
-    int clusterSize = 8;        // CTAs of the reduced-camera-system solver cluster
-    bool useGraphs = true;      // single-GPU LM trials are replayed as one CUDA graph (CSLAM_BA_GRAPH=0 disables)
     // host scratch of cslam_local_ba, kept across calls (fresh multi-megabyte vectors cost page faults on every call)
     struct HostScratch { std::vector<int> lmStart, perm, eMP, eKF, fill, peStart, peList; std::vector<double> X; } hs;
-    // optional per-kernel timing (cslam_optimizer_set_timing)
-    bool timing = false; std::vector<cudaEvent_t> ev; std::vector<int> evKind; int evUsed = 0; double kindMs[16] = {0}; int64_t kindCount[16] = {0};
+    cslam::KernelTimer timer;   // optional per-kernel timing (cslam_optimizer_set_timing); LM trials then run eagerly instead of as a graph
     // one-shot NVLink all-reduce of the reduced camera system (multi-GPU LocalBA): peer views of every rank's exchange buffer
     struct Peer { void* base = nullptr; bool mine = false; };
     std::vector<Peer> peers; size_t xchgBytes = 0; uint32_t epoch = 0, epoch2 = 0; bool oneShot = false;

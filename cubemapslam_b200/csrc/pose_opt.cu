@@ -26,14 +26,8 @@ struct PoShared { double sh[32]; double Hs[27]; double red[8][27]; Pose pose, po
 
 __device__ __forceinline__ int po_obs_face(const PoFrame& F, int e, double& mx, double& my, double& w) {
     const float kx = F.kpxy[2 * e], ky = F.kpxy[2 * e + 1];
-    const float fi = kx / (float)F.faceW, fj = ky / (float)F.faceH;
-    int face = -1;
-    if (fi >= 0 && fi < 1 && fj >= 1 && fj < 2) face = 1;
-    else if (fi >= 1 && fi < 2 && fj >= 0 && fj < 1) face = 3;
-    else if (fi >= 1 && fi < 2 && fj >= 1 && fj < 2) face = 0;
-    else if (fi >= 1 && fi < 2 && fj >= 2 && fj < 3) face = 4;
-    else if (fi >= 2 && fi < 3 && fj >= 1 && fj < 2) face = 2;
-    mx = (double)kx - floor((double)kx / F.faceW) * F.faceW; my = (double)ky - floor((double)ky / F.faceH) * F.faceH;
+    const int face = face_of_pixel_f(kx, ky, F.faceW, F.faceH);
+    mx = pos_in_face(kx, F.faceW); my = pos_in_face(ky, F.faceH);
     w = (double)F.invSigma2[e];
     return face;
 }

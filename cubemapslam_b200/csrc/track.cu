@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(256) k_frame_index(const cslam_keypoint* __res
     const float inv = __fdiv_rn((float)(3 * GRID_G), (float)(3 * W));   // mfGridElementLengthInv
     for (int i = tid; i < n; i += 256) {
         const float px = K[i].x, py = K[i].y;
-        const int face = face_of_pixel_d(px, py, W, H);
+        const int face = face_of_pixel_f(px, py, W, H);
         if (R) {   // TransformCubemapToRays
             float r0 = 0, r1 = 0, r2 = 0;
             if (face >= 0) {
@@ -96,7 +96,7 @@ __global__ void __launch_bounds__(256) k_frame_index(const cslam_keypoint* __res
     __syncthreads();
     for (int i = tid; i < n; i += 256) {
         const float px = K[i].x, py = K[i].y;
-        const int face = face_of_pixel_d(px, py, W, H);
+        const int face = face_of_pixel_f(px, py, W, H);
         if (face < 0) continue;
         const int posX = (int)__fmul_rn(px, inv) % GRID_G, posY = (int)__fmul_rn(py, inv) % GRID_G;
         CI[atomicAdd(&cnt[(face * GRID_G + posX) * GRID_G + posY], 1u)] = (uint16_t)i;
@@ -350,26 +350,19 @@ struct cslam_tracker {
     int64_t launches = 0;
 };
 
-template <class T> static int talloc(cslam_tracker* t, T** p, size_t n) {
-    void* q = nullptr; CSLAM_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T))); CSLAM_CUDA(cudaMemset(q, 0, std::max<size_t>(n, 1) * sizeof(T)));
-    t->owned.push_back(q); *p = (T*)q; return 0;
-}
-
 extern "C" int cslam_tracker_create(cslam_tracker** out, int device, int max_frames, int max_features) {
     if (!out || max_frames <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_tracker_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { set_error("no CUDA device (this library has no CPU fallback)"); return CSLAM_E_NODEVICE; }
-    if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(device));
+    int rc = check_device(device);
+    if (rc) return rc;
     cslam_tracker* t = new cslam_tracker; t->device = device; t->maxFrames = max_frames; t->maxFeat = max_features;
     const size_t nf = (size_t)max_frames * max_features;
-    int rc;
     if (cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); delete t; return CSLAM_E_CUDA; }
-    if ((rc = talloc(t, &t->kCur, nf)) || (rc = talloc(t, &t->kLast, nf)) || (rc = talloc(t, &t->dCur, nf * 32)) || (rc = talloc(t, &t->dQ, nf * 32)) || (rc = talloc(t, &t->valid, nf)) ||
-        (rc = talloc(t, &t->obs, nf)) || (rc = talloc(t, &t->taken, nf)) || (rc = talloc(t, &t->nCur, max_frames)) || (rc = talloc(t, &t->nQ, max_frames)) ||
-        (rc = talloc(t, &t->level, nf)) || (rc = talloc(t, &t->match, nf)) || (rc = talloc(t, &t->nm, max_frames)) || (rc = talloc(t, &t->Xw, nf * 3)) ||
-        (rc = talloc(t, &t->Tcw, (size_t)max_frames * 16)) || (rc = talloc(t, &t->proj, nf * 2)) || (rc = talloc(t, &t->vcos, nf)) || (rc = talloc(t, &t->rays, nf * 3)) ||
-        (rc = talloc(t, &t->cellStart, (size_t)max_frames * (NCELLS + 1))) || (rc = talloc(t, &t->cellIdx, nf)) || (rc = talloc(t, &t->err, 1))) { cslam_tracker_destroy(t); return rc; }
+    auto talloc = [&](auto** p, size_t n) { return dev_alloc(t->owned, p, n, true); };   // every staging buffer starts zeroed
+    if ((rc = talloc(&t->kCur, nf)) || (rc = talloc(&t->kLast, nf)) || (rc = talloc(&t->dCur, nf * 32)) || (rc = talloc(&t->dQ, nf * 32)) || (rc = talloc(&t->valid, nf)) ||
+        (rc = talloc(&t->obs, nf)) || (rc = talloc(&t->taken, nf)) || (rc = talloc(&t->nCur, max_frames)) || (rc = talloc(&t->nQ, max_frames)) ||
+        (rc = talloc(&t->level, nf)) || (rc = talloc(&t->match, nf)) || (rc = talloc(&t->nm, max_frames)) || (rc = talloc(&t->Xw, nf * 3)) ||
+        (rc = talloc(&t->Tcw, (size_t)max_frames * 16)) || (rc = talloc(&t->proj, nf * 2)) || (rc = talloc(&t->vcos, nf)) || (rc = talloc(&t->rays, nf * 3)) ||
+        (rc = talloc(&t->cellStart, (size_t)max_frames * (NCELLS + 1))) || (rc = talloc(&t->cellIdx, nf)) || (rc = talloc(&t->err, 1))) { cslam_tracker_destroy(t); return rc; }
     cudaFuncSetAttribute(k_frame_index, cudaFuncAttributeMaxDynamicSharedMemorySize, NCELLS * 4);
     *out = t;
     return CSLAM_OK;

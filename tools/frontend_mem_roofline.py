@@ -2,14 +2,14 @@
 """Memory roofline of the front end's byte kernels, k_warp and k_pyramid, at bench.py's headline shape (front camera, 1280x1024 frames,
 650-px faces, batches of 128 on one stream). One JSON line on stdout:
 
-  ms_per_batch        per-kernel time from the front end's own CUDA events between launches (cslam_frontend_set_timing), over --batches
-                      batches after a warm-up, for each --fpt (frames per k_warp CTA)
+  run                 the one timed run: per kernel ms_per_batch, the time from the front end's own CUDA events between launches
+                      (cslam_frontend_set_timing) over --batches batches after a warm-up, and the frac_* below
   bytes_live          bytes the algorithm needs per frame: k_warp reads every fisheye pixel some face pixel taps once and writes the five
                       faces; k_pyramid reads and writes only the pixels outside the provably black cubemap corners (Z_l, frontend.cu)
   bytes_full          bench.py's accounting: the whole fisheye frame + 5 faces, and every level of the pyramid in full
   frac_*              those bytes per second over 3.35 TB/s (H100 SXM HBM3 data sheet)
 
-  python tools/frontend_mem_roofline.py [--batches 16] [--fpt 8 4]
+  python tools/frontend_mem_roofline.py [--batches 16]
 """
 import argparse
 import json
@@ -64,7 +64,6 @@ def live_bytes(cfg, sizes):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batches", type=int, default=16)
-    ap.add_argument("--fpt", type=int, nargs="+", default=[8, 4])
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -80,33 +79,30 @@ def main():
     side = [int(round(s ** 0.5)) for s in gb["levels_px"]]
     warp_live, pyr_live = live_bytes(cfg, side)
     out = {"card": card(), "batch": B, "bytes_full": {"k_warp": gb["k_warp"], "k_pyramid": gb["k_pyramid"]},
-           "bytes_live": {"k_warp": warp_live, "k_pyramid": pyr_live}, "runs": {}}
+           "bytes_live": {"k_warp": warp_live, "k_pyramid": pyr_live}}
     fish, _ = bench.make_frames_device(torch, cfg, B, dev)
-    for fpt in args.fpt:
-        os.environ["CSLAM_WARP_FPT"] = str(fpt)
-        fe = FrontEnd(cfg, bench.load_mask(), max_batch=B)
-        cap = fe.kp_cap
-        kps = torch.empty((B, cap, 28), dtype=torch.uint8, device=dev); desc = torch.empty((B, cap, 32), dtype=torch.uint8, device=dev)
-        n = torch.zeros(B, dtype=torch.int32, device=dev)
-        torch.cuda.synchronize()
-        run = lambda: fe.run_dev(fish.data_ptr(), B, kps.data_ptr(), desc.data_ptr(), n.data_ptr())
-        for _ in range(3):
-            run()
-        fe.sync()
-        fe.set_timing(True)
-        for _ in range(args.batches):
-            run(); fe.sync()
-        tm = fe.timing(); fe.set_timing(False)
-        r = {}
-        for k in ("k_warp", "k_pyramid"):
-            sec = tm[k][0] / args.batches / 1e3
-            r[k] = {"ms_per_batch": round(sec * 1e3, 4),
-                    "frac_of_hbm_live": round(out["bytes_live"][k] * B / sec / HBM, 4),
-                    "frac_of_hbm_full": round(out["bytes_full"][k] * B / sec / HBM, 4)}
-        r["all_kernels_ms_per_batch"] = {k: round(v[0] / args.batches, 4) for k, v in tm.items()}
-        out["runs"]["fpt%d" % fpt] = r
-        fe.close()
-    os.environ.pop("CSLAM_WARP_FPT", None)
+    fe = FrontEnd(cfg, bench.load_mask(), max_batch=B)
+    cap = fe.kp_cap
+    kps = torch.empty((B, cap, 28), dtype=torch.uint8, device=dev); desc = torch.empty((B, cap, 32), dtype=torch.uint8, device=dev)
+    n = torch.zeros(B, dtype=torch.int32, device=dev)
+    torch.cuda.synchronize()
+    run = lambda: fe.run_dev(fish.data_ptr(), B, kps.data_ptr(), desc.data_ptr(), n.data_ptr())
+    for _ in range(3):
+        run()
+    fe.sync()
+    fe.set_timing(True)
+    for _ in range(args.batches):
+        run(); fe.sync()
+    tm = fe.timing(); fe.set_timing(False)
+    r = {}
+    for k in ("k_warp", "k_pyramid"):
+        sec = tm[k][0] / args.batches / 1e3
+        r[k] = {"ms_per_batch": round(sec * 1e3, 4),
+                "frac_of_hbm_live": round(out["bytes_live"][k] * B / sec / HBM, 4),
+                "frac_of_hbm_full": round(out["bytes_full"][k] * B / sec / HBM, 4)}
+    r["all_kernels_ms_per_batch"] = {k: round(v[0] / args.batches, 4) for k, v in tm.items()}
+    out["run"] = r
+    fe.close()
     print(json.dumps(out))
 
 
