@@ -54,8 +54,10 @@ struct DevLevels {
     const uint32_t* xab[MAX_LEVELS];   // a0 | a1<<16
     const uint16_t* yofs[MAX_LEVELS];
     const uint32_t* yab[MAX_LEVELS];
-    const uint8_t* skip[MAX_LEVELS];   // per k_fast CTA: 1 = tile provably all-zero when level 0 came from k_warp (black corner tiles)
-    const uint8_t* pskip[MAX_LEVELS];  // per k_pyramid warp (PYR_WX x PYR_RY dst px), same meaning; levels >= 1
+    const uint8_t* skip[MAX_LEVELS];   // per k_fast CTA: 1 = tile provably corner-free when level 0 came from k_warp (no live work item)
+    const uint8_t* pskip[MAX_LEVELS];  // per k_pyramid warp (PYR_WX x PYR_RY dst px): 1 = every pixel provably 0 (black corner tiles); levels >= 1
+    const uint16_t* live[MAX_LEVELS];     // k_fast phase-A work items that can score above 0 on the warp path: y<<6 | (wi - w0), per CTA tile
+    const uint32_t* liveOff[MAX_LEVELS];  // per CTA tile [liveOff[t], liveOff[t+1]) into live
     int nlevels;
 };
 
@@ -270,16 +272,20 @@ __device__ __forceinline__ int fdiv_small(int i, uint32_t magic) { return (int)(
 __device__ __forceinline__ uint32_t fdiv_magic(int d) { return ((1u << 20) + d - 1) / d; }
 
 // Layout of one CTA: CG cells of one cell row. Phases:
-//  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u8, 0 where s <= minTh)
+//  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, 0 where s <= minTh). On the warp path
+//     (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant (DevLevels::live), so
+//     its scores are 0, which the zeroed S already holds
 //  B  3x3 NMS at minTh inside each cell -> shared list; a keypoint at iniTh is exactly an NMS survivor with s > iniTh
 //     (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
 //  C  compaction of the selected entries into the global candidate list (one global atomic per 256 entries)
 static const int FAST_KMAX = CG * (CELL_MAX / 2) * (CELL_MAX / 2);   // NMS survivors are pairwise non-adjacent
 static const int FAST_SW = FAST_TS / 2;                              // pair-words per score row
+static_assert((CG * CELL_MAX + 9) / 4 < 64 && CELL_MAX < 1024, "a live work item packs y<<6 | (wi - w0) into 16 bits");
 
 __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, LevelGeom g, int iniTh, int minTh, uint32_t* __restrict__ cand,
                                               uint32_t* __restrict__ candCount, int countStride, int* __restrict__ errFlag,
-                                              const uint8_t* __restrict__ skip) {
+                                              const uint8_t* __restrict__ skip, const uint16_t* __restrict__ live,
+                                              const uint32_t* __restrict__ liveOff) {
     __shared__ __align__(16) uint8_t tile[FAST_TH * FAST_TS];
     // score map, one u16 per pixel as u16x2 pair-words: word 2*wi (+1) of row y+1 holds tile columns 4*wi..4*wi+1 (+2..+3)
     __shared__ __align__(16) uint32_t S2[(CELL_MAX + 2) * FAST_SW];
@@ -291,7 +297,8 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
     __shared__ int warpCnt[8];
     const int frame = blockIdx.z, cellRow = blockIdx.y, j0 = blockIdx.x * CG;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (skip && skip[cellRow * gridDim.x + blockIdx.x]) return;   // tile provably all-zero (black cubemap corner)
+    const int tileIdx = cellRow * gridDim.x + blockIdx.x;
+    if (skip && skip[tileIdx]) return;   // tile provably corner-free (no live work item)
     const uint8_t* I = img + (size_t)frame * g.pitch * g.h;
     const int iniY = g.minB + cellRow * g.hCell, maxY = min(iniY + g.hCell + 6, g.maxBY);
     const int ncell = min(CG, g.nColsEff - j0);
@@ -316,12 +323,8 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
         }
     }
     if (acc) anyNonZero = 1;
-    // S2 must read 0 around the scored area: rows 0 and ny+1, and the pair-words left/right of [2*w0, 2*w1) in every row
-    for (int i = tid; i < 2 * FAST_SW; i += 256) S2[(i >= FAST_SW ? (ny + 1) * FAST_SW : 0) + (i % FAST_SW)] = 0;
-    for (int i = tid; i < 2 * ny; i += 256) {
-        const int r = (i >> 1) + 1, psel = (i & 1) ? 2 * w1 : 2 * w0 - 1;
-        if (psel >= 0 && psel < FAST_SW) S2[r * FAST_SW + psel] = 0;
-    }
+    // S2 must read 0 around the scored area (rows 0 and ny+1, the pair-words left/right of [2*w0, 2*w1)) and wherever phase A skips an item
+    for (int i = tid; i < (ny + 2) * (FAST_SW / 4); i += 256) reinterpret_cast<uint4*>(S2)[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int pw = tid; pw < FAST_SW; pw += 256) {
         uint32_t v = 0, l = 0, r = 0;
         for (int h = 0; h < 2; h++) {
@@ -342,11 +345,8 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
     __syncthreads();
     if (!anyNonZero) return;   // an all-zero tile has no corners at any threshold
     // ---- A
-    const uint32_t mgw = fdiv_magic(nw);
     {
-        const int nitems = nw * ny;
-        for (int it = tid; it < nitems; it += 256) {
-            const int y = fdiv_small(it, mgw), wi = w0 + (it - y * nw);
+        auto score_item = [&](int y, int wi) {
             const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + y * FAST_TS) + wi;   // row y-3 relative to the centre row
             const int RS = FAST_TS / 4;
             uint32_t V[16];
@@ -392,6 +392,13 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
             uint32_t oB = ((sB & 0xffffu) > thr ? (sB & 0xffffu) : 0u) | ((sB >> 16) > thr ? (sB & 0xffff0000u) : 0u);
             uint32_t* Srow = S2 + (y + 1) * FAST_SW + 2 * wi;
             Srow[0] = oA & mskV[2 * wi]; Srow[1] = oB & mskV[2 * wi + 1];
+        };
+        if (live) {
+            const uint32_t i0 = liveOff[tileIdx], i1 = liveOff[tileIdx + 1];
+            for (uint32_t it = i0 + tid; it < i1; it += 256) { const int e = live[it]; score_item(e >> 6, w0 + (e & 63)); }
+        } else {
+            const uint32_t mgw = fdiv_magic(nw);
+            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgw); score_item(y, w0 + (it - y * nw)); }
         }
     }
     __syncthreads();
@@ -959,6 +966,96 @@ static void build_resize_tables(int sn, int dn, std::vector<uint16_t>& ofs, std:
     }
 }
 
+// Static pixel classes of the warp path, fixed by the geometry alone. K_0: Z = the canvas corner tiles (never written by k_warp, zeroed at
+// allocation, so 0); C = face pixels whose quantised map is (0,0) (outside the image circle: k_warp writes S(0,0), one constant per frame);
+// live = the rest. K_l(x,y): Z if all four resize taps of (x,y) are in Z_{l-1}; C if all four are in C_{l-1} and both tap-weight pairs sum to
+// 2048 (k_pyramid then returns the constant itself: (((b0 128c) >> 16) + ((b1 128c) >> 16) + 2) >> 2 = c); live otherwise.
+// From them: k_pyramid pieces inside Z_l (pskip); and, per k_fast CTA tile, the phase-A work items holding a pixel whose 7x7 window is not
+// all Z or all C (live / liveOff). Every other pixel's ring and centre are equal, so its arc score is 0 at any threshold and for any frame.
+// A tile without live items has no corner: its skip byte is set and its CTA exits before loading the tile.
+static int build_static_classes(cslam_frontend* fe) {
+    enum : uint8_t { K_LIVE = 0, K_Z = 1, K_C = 2 };
+    int rc;
+    std::vector<uint8_t> K((size_t)fe->CW * fe->CH), Kn;
+    for (int y = 0; y < fe->CH; y++)
+        for (int x = 0; x < fe->CW; x++) {
+            const size_t i = (size_t)y * fe->CW + x;
+            const bool corner = x / fe->W != 1 && y / fe->H != 1;
+            K[i] = corner ? K_Z : (cv_round_f(fe->map1[i] * 32.f) == 0 && cv_round_f(fe->map2[i] * 32.f) == 0) ? K_C : K_LIVE;
+        }
+    for (int l = 0; l < fe->L.nlevels; l++) {
+        const LevelGeom& g = fe->L.g[l];
+        const int w = g.w, h = g.h;
+        if (l > 0) {
+            const LevelGeom& sg = fe->L.g[l - 1];
+            std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
+            build_resize_tables(sg.w, w, xo, xa); build_resize_tables(sg.h, h, yo, ya);
+            Kn.assign((size_t)w * h, K_LIVE);
+            for (int y = 0; y < h; y++) {
+                const int y0 = yo[y], y1 = std::min(y0 + 1, sg.h - 1);
+                const bool unitY = (ya[y] & 0xffff) + (ya[y] >> 16) == 2048;
+                for (int x = 0; x < w; x++) {
+                    const int x0 = xo[x], x1 = std::min(x0 + 1, sg.w - 1);
+                    const uint8_t k = K[(size_t)y0 * sg.w + x0];
+                    if (k == K_LIVE || K[(size_t)y0 * sg.w + x1] != k || K[(size_t)y1 * sg.w + x0] != k || K[(size_t)y1 * sg.w + x1] != k) continue;
+                    if (k == K_Z || (unitY && (xa[x] & 0xffff) + (xa[x] >> 16) == 2048)) Kn[(size_t)y * w + x] = k;
+                }
+            }
+            K.swap(Kn);
+            const int px = cdiv(w, PYR_WX), py = cdiv(h, PYR_RY);
+            std::vector<uint8_t> ps((size_t)px * py, 1);
+            for (int y = 0; y < h; y++)
+                for (int x = 0; x < w; x++)
+                    if (K[(size_t)y * w + x] != K_Z) ps[(size_t)(y / PYR_RY) * px + x / PYR_WX] = 0;
+            if ((rc = dev_upload(fe, &fe->L.pskip[l], ps))) return rc;
+        }
+        // U(x,y) = k if the 7x7 window centred on (x,y) is all class k (separably: rows of 7, then columns of 7 such rows), else K_LIVE
+        std::vector<uint8_t> Hr((size_t)w * h, K_LIVE), U((size_t)w * h, K_LIVE);
+        for (int y = 0; y < h; y++)
+            for (int x = 3; x < w - 3; x++) {
+                const uint8_t* r = &K[(size_t)y * w + x];
+                bool same = true;
+                for (int d = -3; d <= 3 && same; d++) same = r[d] == r[0];
+                if (same) Hr[(size_t)y * w + x] = r[0];
+            }
+        for (int y = 3; y < h - 3; y++)
+            for (int x = 0; x < w; x++) {
+                const uint8_t k = Hr[(size_t)y * w + x];
+                bool same = k != K_LIVE;
+                for (int d = -3; d <= 3 && same; d++) same = Hr[(size_t)(y + d) * w + x] == k;
+                if (same) U[(size_t)y * w + x] = k;
+            }
+        // work items in k_fast's order and geometry (tile rows iniY.., tile columns from a0 = tx0 & ~3, item = tile word wi of detection row y)
+        const int gx = cdiv(g.nColsEff, CG), gy = g.nRowsEff;
+        std::vector<uint8_t> sk((size_t)gx * gy);
+        std::vector<uint32_t> off((size_t)gx * gy + 1);
+        std::vector<uint16_t> items;
+        for (int cy = 0; cy < gy; cy++)
+            for (int cxg = 0; cxg < gx; cxg++) {
+                const size_t t = (size_t)cy * gx + cxg;
+                off[t] = (uint32_t)items.size();
+                const int iniY = g.minB + cy * g.hCell, maxY = std::min(iniY + g.hCell + 6, g.maxBY);
+                const int ncell = std::min(CG, g.nColsEff - cxg * CG);
+                const int tx0 = g.minB + cxg * CG * g.wCell, tx1 = std::min(tx0 + ncell * g.wCell + 6, g.maxBX);
+                const int a0 = tx0 & ~3, nx = tx1 - tx0 - 6, ny = maxY - iniY - 6, xoff = tx0 - a0 + 3;
+                const int w0 = xoff >> 2, w1 = (xoff + nx + 3) >> 2;
+                for (int y = 0; y < ny; y++)
+                    for (int wi = w0; wi < w1; wi++) {
+                        bool any = false;
+                        for (int j = 0; j < 4; j++) {
+                            const int x = 4 * wi + j - xoff;   // detection x; the kernel masks the lanes outside [0, nx)
+                            if (x >= 0 && x < nx && U[(size_t)(iniY + 3 + y) * w + a0 + 4 * wi + j] == K_LIVE) any = true;
+                        }
+                        if (any) items.push_back((uint16_t)(y << 6 | (wi - w0)));
+                    }
+                sk[t] = items.size() == off[t];
+            }
+        off[(size_t)gx * gy] = (uint32_t)items.size();
+        if ((rc = dev_upload(fe, &fe->L.skip[l], sk)) || (rc = dev_upload(fe, &fe->L.live[l], items)) || (rc = dev_upload(fe, &fe->L.liveOff[l], off))) return rc;
+    }
+    return 0;
+}
+
 extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const cslam_cam_params* cam, const cslam_orb_params* orb,
                                      const uint8_t* mask, int mask_pitch, int max_batch) {
     if (!out || !cam || !orb || !mask || max_batch <= 0) { set_error("cslam_frontend_create: null/invalid argument"); return CSLAM_E_BADARG; }
@@ -1033,53 +1130,6 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
             build_resize_tables(fe->L.g[l - 1].w, g.w, xo, xa); build_resize_tables(fe->L.g[l - 1].h, g.h, yo, ya);
             if ((rc = dev_upload(fe, &fe->L.xofs[l], xo)) || (rc = dev_upload(fe, &fe->L.xab[l], xa)) || (rc = dev_upload(fe, &fe->L.yofs[l], yo)) ||
                 (rc = dev_upload(fe, &fe->L.yab[l], ya))) return fail(rc);
-        }
-    }
-    // ---- static zero map: Z_0 = corner tiles of the canvas (never written by k_warp, zeroed at allocation); Z_l(x,y) = all four
-    // resize taps of (x,y) are in Z_{l-1}. A k_fast tile inside Z_l is all-zero, hence corner-free: its CTA exits at once.
-    {
-        std::vector<uint8_t> Z((size_t)fe->CW * fe->CH, 0), Zn;
-        for (int y = 0; y < fe->CH; y++)
-            for (int x = 0; x < fe->CW; x++) {
-                const int tc = x / fe->W, tr = y / fe->H;
-                Z[(size_t)y * fe->CW + x] = (tc != 1 && tr != 1) ? 1 : 0;
-            }
-        for (int l = 0; l < nl; l++) {
-            const LevelGeom& g = fe->L.g[l];
-            if (l > 0) {
-                const LevelGeom& sg = fe->L.g[l - 1];
-                std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
-                build_resize_tables(sg.w, g.w, xo, xa); build_resize_tables(sg.h, g.h, yo, ya);
-                Zn.assign((size_t)g.w * g.h, 0);
-                for (int y = 0; y < g.h; y++) {
-                    const int y0 = yo[y], y1 = std::min(y0 + 1, sg.h - 1);
-                    for (int x = 0; x < g.w; x++) {
-                        const int x0 = xo[x], x1 = std::min(x0 + 1, sg.w - 1);
-                        Zn[(size_t)y * g.w + x] = Z[(size_t)y0 * sg.w + x0] & Z[(size_t)y0 * sg.w + x1] & Z[(size_t)y1 * sg.w + x0] & Z[(size_t)y1 * sg.w + x1];
-                    }
-                }
-                Z.swap(Zn);
-                // k_pyramid pieces inside Z_l: all four taps of every pixel are 0, so the piece is 0 and the kernel need not touch it
-                const int px = cdiv(g.w, PYR_WX), py = cdiv(g.h, PYR_RY);
-                std::vector<uint8_t> ps((size_t)px * py, 1);
-                for (int y = 0; y < g.h; y++)
-                    for (int x = 0; x < g.w; x++)
-                        if (!Z[(size_t)y * g.w + x]) ps[(size_t)(y / PYR_RY) * px + x / PYR_WX] = 0;
-                if ((rc = dev_upload(fe, &fe->L.pskip[l], ps))) return fail(rc);
-            }
-            const int gx = cdiv(g.nColsEff, CG), gy = g.nRowsEff;
-            std::vector<uint8_t> sk((size_t)gx * gy, 0);
-            for (int cy = 0; cy < gy; cy++)
-                for (int cxg = 0; cxg < gx; cxg++) {
-                    const int iniY = g.minB + cy * g.hCell, maxY = std::min(iniY + g.hCell + 6, g.maxBY);
-                    const int ncell = std::min(CG, g.nColsEff - cxg * CG);
-                    const int tx0 = g.minB + cxg * CG * g.wCell, tx1 = std::min(tx0 + ncell * g.wCell + 6, g.maxBX);
-                    uint8_t all = 1;
-                    for (int y = iniY; y < maxY && all; y++)
-                        for (int x = tx0; x < tx1; x++) if (!Z[(size_t)y * g.w + x]) { all = 0; break; }
-                    sk[(size_t)cy * gx + cxg] = all;
-                }
-            if ((rc = dev_upload(fe, &fe->L.skip[l], sk))) return fail(rc);
         }
     }
     fe->M = round_up(std::max(maxQuota + 4, 16), 32);
@@ -1158,6 +1208,7 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         if ((rc = dev_upload(fe, &dt, tb)) || (rc = dev_upload(fe, &fe->d_went, ent))) return fail(rc);
         fe->d_wtiles = reinterpret_cast<const WarpTile*>(dt);
         if (cudaFuncSetAttribute(k_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, WARP_FPT * fe->warpSlot + 16) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
+        if ((rc = build_static_classes(fe))) return fail(rc);
     }
     // ---- mask
     fe->maskPitch = round_up(fe->CW, 128);
@@ -1260,7 +1311,8 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         const LevelGeom& g = L.g[l];
         dim3 grid(cdiv(g.nColsEff, CG), g.nRowsEff, cnt);
         mark(fe, st, KIND_FAST);
-        k_fast<<<grid, 256, 0, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err, useSkip ? L.skip[l] : nullptr);
+        k_fast<<<grid, 256, 0, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err,
+                                     useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
     }
     CSLAM_CUDA(cudaGetLastError());
     DistributeArgs da;
