@@ -58,6 +58,7 @@ struct DevLevels {
     const uint8_t* pskip[MAX_LEVELS];  // per k_pyramid warp (PYR_WX x PYR_RY dst px): 1 = every pixel provably 0 (black corner tiles); levels >= 1
     const uint16_t* live[MAX_LEVELS];     // k_fast phase-A work items that can score above 0 on the warp path: y<<6 | (wi - w0), per CTA tile
     const uint32_t* liveOff[MAX_LEVELS];  // per CTA tile [liveOff[t], liveOff[t+1]) into live
+    const struct FastCols* fcols[MAX_LEVELS];   // per k_fast tile column: lane masks, cells and division magics (build_fast_cols)
     int nlevels;
 };
 
@@ -240,83 +241,136 @@ __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src
 // corner(thr) <=> s > thr; OpenCV response = s-1. The reference runs cv::FAST per cell ROI [ini, ini+cell+6):
 // detection areas of neighbouring cells tile the level without overlap, NMS only sees scores of the same cell,
 // and the 20->7 fallback is decided per cell on "no keypoint survived NMS" (src/ORBExtractor.cpp:763-803).
-// Exact arc score of 2 horizontally adjacent pixels at once in u16x2 lanes (sm_90a VIMNMX3.U16x2):
+// Exact arc score of 2 pixels at once in u16x2 lanes (sm_90a VIMNMX3.U16x2):
 //   s = max(0, A - c, c - B),  A = max_k min(R[k..k+8]),  B = min_k max(R[k..k+8])   (R = ring intensities, c = centre)
 // min/max over 9 contiguous ring pixels = min3 of three min3's. No data-dependent branch, no per-pixel early-out:
 // on textured input almost every pixel passes the cheap antipodal tests, so the branch-free full score is cheaper
 // than queueing.
-__device__ __forceinline__ uint32_t arc_score_x2(const uint32_t (&R)[16], uint32_t c) {
+// The intensities sit in the high bytes of the lanes, the low bytes hold anything (the neighbouring pixels of a raw image word): u16
+// min/max orders by the high byte first, so the high byte of every min/max is the min/max of the high bytes. Only A, B and c are
+// masked, before the subtractions. Returned per lane: (max(s, t) - t) << 8 for the threshold t, given as T = t << 8 in each lane, i.e.
+// 0 where s <= t and order-preserving above it.
+__device__ __forceinline__ uint32_t arc_score_x2(const uint32_t (&R)[16], uint32_t c, uint32_t T) {
     uint32_t mn[16], mx[16];
 #pragma unroll
     for (int k = 0; k < 16; k++) {
         mn[k] = __vimin3_u16x2(R[k], R[(k + 1) & 15], R[(k + 2) & 15]);
         mx[k] = __vimax3_u16x2(R[k], R[(k + 1) & 15], R[(k + 2) & 15]);
     }
-    uint32_t A = 0u, Bm = 0xffffffffu;
+    uint32_t A, Bm;
 #pragma unroll
     for (int k = 0; k < 16; k += 2) {
         const uint32_t a0 = __vimin3_u16x2(mn[k], mn[(k + 3) & 15], mn[(k + 6) & 15]);
         const uint32_t a1 = __vimin3_u16x2(mn[k + 1], mn[(k + 4) & 15], mn[(k + 7) & 15]);
         const uint32_t b0 = __vimax3_u16x2(mx[k], mx[(k + 3) & 15], mx[(k + 6) & 15]);
         const uint32_t b1 = __vimax3_u16x2(mx[k + 1], mx[(k + 4) & 15], mx[(k + 7) & 15]);
-        A = __vimax3_u16x2(A, a0, a1);
-        Bm = __vimin3_u16x2(Bm, b0, b1);
+        A = k ? __vimax3_u16x2(A, a0, a1) : __vmaxu2(a0, a1);
+        Bm = k ? __vimin3_u16x2(Bm, b0, b1) : __vminu2(b0, b1);
     }
+    const uint32_t HI = 0xff00ff00u;
+    A &= HI; Bm &= HI; c &= HI;
     const uint32_t t1 = __vmaxu2(A, c) - c;      // lanes never borrow: max(A,c) >= c
     const uint32_t t2 = c - __vminu2(Bm, c);
-    return __vmaxu2(t1, t2);
+    return __vimax3_u16x2(t1, t2, T) - T;
 }
 
 // q = i / d for 0 <= i < 65536/..: d-uniform fast division (tile loops have i < 8192, d <= 64)
 __device__ __forceinline__ int fdiv_small(int i, uint32_t magic) { return (int)(((uint32_t)i * magic) >> 20); }
-__device__ __forceinline__ uint32_t fdiv_magic(int d) { return ((1u << 20) + d - 1) / d; }
+__host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d - 1) / d; }
 
 // Layout of one CTA: CG cells of one cell row. Phases:
-//  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, 0 where s <= minTh). On the warp path
-//     (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant (DevLevels::live), so
-//     its scores are 0, which the zeroed S already holds
-//  B  3x3 NMS at minTh inside each cell -> shared list; a keypoint at iniTh is exactly an NMS survivor with s > iniTh
-//     (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
+//  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, (s - mt) << 8, 0 where s <= mt; mt = minTh clamped to
+//     1..255, see below).
+//     On the warp path (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant
+//     (DevLevels::live), so its scores are 0, which the zeroed S already holds
+//  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the same items as A -> shared list; a keypoint at
+//     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
 //  C  compaction of the selected entries into the global candidate list (one global atomic per 256 entries)
 static const int FAST_KMAX = CG * (CELL_MAX / 2) * (CELL_MAX / 2);   // NMS survivors are pairwise non-adjacent
 static const int FAST_SW = FAST_TS / 2;                              // pair-words per score row
 static_assert((CG * CELL_MAX + 9) / 4 < 64 && CELL_MAX < 1024, "a live work item packs y<<6 | (wi - w0) into 16 bits");
+static_assert(CG <= 4, "FastItem packs a pixel's cell index into 2 bits");
+
+// Column geometry of the k_fast CTA tile in tile column cx (blockIdx.x) of a level. The tile's rows start at a0 = tx0 & ~3 (word-aligned
+// loads); work item wi covers tile columns 4*wi..4*wi+3, and detection x = tile column - xoff.
+struct FastTileX {
+    int tx0, a0, nwords;   // first ROI column, first loaded column, loaded words per row
+    int nx, xoff;          // detection width, tile column of detection x = 0
+    int w0, w1;            // work items [w0, w1) cover the detection columns
+    int q0, q1;            // uint4 columns [q0, q1) of an S2 row cover the pair-words phase B reads, [2*w0 - 1, 2*w1 + 1)
+};
+__host__ __device__ inline FastTileX fast_tile_x(const LevelGeom& g, int cx) {
+    FastTileX t;
+    const int j0 = cx * CG, ncell = min(CG, g.nColsEff - j0);
+    t.tx0 = g.minB + j0 * g.wCell;
+    const int tx1 = min(t.tx0 + ncell * g.wCell + 6, g.maxBX);
+    t.a0 = t.tx0 & ~3; t.nwords = (tx1 - t.a0 + 3) >> 2;
+    t.nx = tx1 - t.tx0 - 6; t.xoff = t.tx0 - t.a0 + 3;
+    t.w0 = t.xoff >> 2; t.w1 = (t.xoff + t.nx + 3) >> 2;
+    t.q0 = max(2 * t.w0 - 1, 0) >> 2; t.q1 = (t.w1 + 2) >> 1;
+    return t;
+}
+// Per work item wi of a tile column: lane masks of pair-words 2*wi and 2*wi+1 (a lane is 0xffff or 0) and the cell of each pixel
+struct FastItem {
+    uint32_t valid[2];    // column inside the detection area
+    uint32_t cells;       // cell index within the tile of pixel j (tile column 4*wi + j) in bits 2j..2j+1
+    uint32_t pad;
+    uint32_t left[2], right[2];   // has a left / right neighbour in its cell
+};
+// Everything k_fast needs that depends on the tile column alone; built once per level at create time (build_fast_cols)
+struct FastCols {
+    uint32_t mgWords, mgItems, mgZero, pad;   // fdiv_magic of nwords, w1 - w0 and q1 - q0
+    FastItem item[FAST_SW / 2];
+};
+
+// Neighbourhood maximum of pair-word `cur` over its 8 same-cell neighbours: a*, b*, c* = the pair-words left of, at and right of it in the
+// row above (0), its own row (1) and the row below (2); ml / mr mask the lanes without a left / right neighbour in their cell
+__device__ __forceinline__ uint32_t nms_max(uint32_t a0, uint32_t b0, uint32_t c0, uint32_t a1, uint32_t cur, uint32_t c1, uint32_t a2, uint32_t b2,
+                                            uint32_t c2, uint32_t ml, uint32_t mr) {
+    const uint32_t upL = __funnelshift_r(a0, b0, 16) & ml, upR = __funnelshift_r(b0, c0, 16) & mr;
+    const uint32_t cuL = __funnelshift_r(a1, cur, 16) & ml, cuR = __funnelshift_r(cur, c1, 16) & mr;
+    const uint32_t dnL = __funnelshift_r(a2, b2, 16) & ml, dnR = __funnelshift_r(b2, c2, 16) & mr;
+    return __vimax3_u16x2(__vimax3_u16x2(upL, b0, upR), __vimax3_u16x2(cuL, cuR, b2), __vmaxu2(dnL, dnR));
+}
 
 __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, LevelGeom g, int iniTh, int minTh, uint32_t* __restrict__ cand,
                                               uint32_t* __restrict__ candCount, int countStride, int* __restrict__ errFlag,
-                                              const uint8_t* __restrict__ skip, const uint16_t* __restrict__ live,
-                                              const uint32_t* __restrict__ liveOff) {
-    __shared__ __align__(16) uint8_t tile[FAST_TH * FAST_TS];
+                                              const FastCols* __restrict__ cols, const uint8_t* __restrict__ skip,
+                                              const uint16_t* __restrict__ live, const uint32_t* __restrict__ liveOff) {
+    // tile rows; 16 bytes in front so that the word left of row 0's first word is addressable (phase A reads it unguarded)
+    __shared__ __align__(16) uint8_t tileBuf[16 + FAST_TH * FAST_TS];
+    uint8_t* const tile = tileBuf + 16;
     // score map, one u16 per pixel as u16x2 pair-words: word 2*wi (+1) of row y+1 holds tile columns 4*wi..4*wi+1 (+2..+3)
     __shared__ __align__(16) uint32_t S2[(CELL_MAX + 2) * FAST_SW];
     __shared__ uint32_t klist[FAST_KMAX];                            // x | y<<8 | s<<16 | cell<<24
-    __shared__ uint8_t cellInfo[FAST_TS];   // per detection column: cell index | 0x40 first column of its cell | 0x80 last
-    __shared__ uint32_t mskV[FAST_SW], mskL[FAST_SW], mskR[FAST_SW];  // per pair-word lane masks: valid column / has left / has right neighbour in its cell
     __shared__ int cnt20[CG];
     __shared__ int anyNonZero, nK, chunkBase;
     __shared__ int warpCnt[8];
-    const int frame = blockIdx.z, cellRow = blockIdx.y, j0 = blockIdx.x * CG;
+    const int frame = blockIdx.z, cellRow = blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tileIdx = cellRow * gridDim.x + blockIdx.x;
     if (skip && skip[tileIdx]) return;   // tile provably corner-free (no live work item)
     const uint8_t* I = img + (size_t)frame * g.pitch * g.h;
     const int iniY = g.minB + cellRow * g.hCell, maxY = min(iniY + g.hCell + 6, g.maxBY);
-    const int ncell = min(CG, g.nColsEff - j0);
-    const int tx0 = g.minB + j0 * g.wCell, tx1 = min(tx0 + ncell * g.wCell + 6, g.maxBX);
-    const int a0 = tx0 & ~3, nwords = (tx1 - a0 + 3) >> 2, nrows = maxY - iniY;
-    const int nx = tx1 - tx0 - 6, ny = nrows - 6;   // detection area
-    const int xoff = tx0 - a0 + 3;                   // tile column of detection x = 0
-    const int w0 = xoff >> 2, w1 = (xoff + nx + 3) >> 2, nw = w1 - w0;   // S/tile words covering the detection columns
+    const FastTileX X = fast_tile_x(g, blockIdx.x);
+    const int nrows = maxY - iniY, ny = nrows - 6;   // detection rows
+    const int nx = X.nx, xoff = X.xoff, w0 = X.w0, nw = X.w1 - X.w0;
     if (nx <= 0 || ny <= 0) return;   // block-uniform: a ROI with fewer than 7 rows / columns has no detection area (cv::FAST returns nothing)
+    const FastCols* C = cols + blockIdx.x;
+    const uint4 mg = __ldg(reinterpret_cast<const uint4*>(C));
+    // cv::FAST clamps its threshold to 0..255 and ranks corners by s - 1, with 0 for "no corner": at threshold 0 a corner with s = 1 ties
+    // with its non-corner neighbours and never survives NMS, exactly as if the threshold were 1
+    const int mt = min(max(minTh, 1), 255);
+    const uint32_t T = (uint32_t)mt * 0x01000100u;
     if (tid < CG) cnt20[tid] = 0;
     if (tid == 0) { anyNonZero = 0; nK = 0; }
     __syncthreads();
     uint32_t acc = 0;
     {
-        const uint32_t mg = fdiv_magic(nwords);
-        const uint8_t* base = I + (size_t)iniY * g.pitch + a0;
+        const int nwords = X.nwords;
+        const uint8_t* base = I + (size_t)iniY * g.pitch + X.a0;
         for (int i = tid; i < nwords * nrows; i += 256) {
-            const int r = fdiv_small(i, mg), wd = i - r * nwords;
+            const int r = fdiv_small(i, mg.x), wd = i - r * nwords;
             const uint32_t v = __ldg(reinterpret_cast<const uint32_t*>(base + (size_t)r * g.pitch) + wd);
             reinterpret_cast<uint32_t*>(tile + r * FAST_TS)[wd] = v;
             acc |= v;
@@ -324,113 +378,114 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
     }
     if (acc) anyNonZero = 1;
     // S2 must read 0 around the scored area (rows 0 and ny+1, the pair-words left/right of [2*w0, 2*w1)) and wherever phase A skips an item
-    for (int i = tid; i < (ny + 2) * (FAST_SW / 4); i += 256) reinterpret_cast<uint4*>(S2)[i] = make_uint4(0u, 0u, 0u, 0u);
-    for (int pw = tid; pw < FAST_SW; pw += 256) {
-        uint32_t v = 0, l = 0, r = 0;
-        for (int h = 0; h < 2; h++) {
-            const int x = 2 * pw + h - xoff;   // detection x of this lane
-            if (x >= 0 && x < nx) {
-                const int xl = x % g.wCell;
-                v |= 0xffffu << (16 * h);
-                if (xl != 0) l |= 0xffffu << (16 * h);
-                if (xl != g.wCell - 1 && x != nx - 1) r |= 0xffffu << (16 * h);
-            }
+    {
+        const int q0 = X.q0, nq = X.q1 - X.q0;
+        for (int i = tid; i < (ny + 2) * nq; i += 256) {
+            const int r = fdiv_small(i, mg.z);
+            reinterpret_cast<uint4*>(S2 + r * FAST_SW)[q0 + i - r * nq] = make_uint4(0u, 0u, 0u, 0u);
         }
-        mskV[pw] = v; mskL[pw] = l; mskR[pw] = r;
-    }
-    for (int x = tid; x < nx; x += 256) {
-        const int c = x / g.wCell, xl = x - c * g.wCell;
-        cellInfo[x] = (uint8_t)(c | (xl == 0 ? 0x40 : 0) | ((xl == g.wCell - 1 || x == nx - 1) ? 0x80 : 0));
     }
     __syncthreads();
     if (!anyNonZero) return;   // an all-zero tile has no corners at any threshold
     // ---- A
     {
         auto score_item = [&](int y, int wi) {
-            const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + y * FAST_TS) + wi;   // row y-3 relative to the centre row
+            const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
+            const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
             const int RS = FAST_TS / 4;
-            uint32_t V[16];
+            // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
+            // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
+            // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle
+            uint32_t V[16], U[16], Cv, Cu;
             {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
-                const uint32_t m = wi > 0 ? r0[-1] : 0u, c = r0[0], p = r0[1];
+                const uint32_t m = r0[-1], c = r0[0], p = r0[1];
                 V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
+                U[15] = __funnelshift_r(m, c, 16); U[0] = V[15]; U[1] = c;
             }
             {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
-                const uint32_t* r = r0 + RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
+                const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                 V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
+                U[14] = __funnelshift_r(m, c, 8); U[2] = __funnelshift_r(c, p, 8);
             }
             {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
-                const uint32_t* r = r0 + 2 * RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
+                const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                 V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
+                U[13] = m; U[3] = __funnelshift_r(c, p, 16);
             }
-            uint32_t C;
             {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
-                const uint32_t* r = r0 + 3 * RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
-                V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); C = c;
+                const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
+                U[12] = m; U[4] = __funnelshift_r(c, p, 16); Cu = __funnelshift_r(m, c, 24);
             }
             {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
-                const uint32_t* r = r0 + 4 * RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
+                const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                 V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
+                U[11] = m; U[5] = __funnelshift_r(c, p, 16);
             }
             {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
-                const uint32_t* r = r0 + 5 * RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
+                const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                 V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
+                U[10] = __funnelshift_r(m, c, 8); U[6] = __funnelshift_r(c, p, 8);
             }
             {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
-                const uint32_t* r = r0 + 6 * RS; const uint32_t m = wi > 0 ? r[-1] : 0u, c = r[0], p = r[1];
+                const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                 V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
+                U[9] = __funnelshift_r(m, c, 16); U[8] = V[9]; U[7] = c;
             }
-            uint32_t R[16];
-#pragma unroll
-            for (int k = 0; k < 16; k++) R[k] = __byte_perm(V[k], 0u, 0x4140);
-            const uint32_t sA = arc_score_x2(R, __byte_perm(C, 0u, 0x4140));
-#pragma unroll
-            for (int k = 0; k < 16; k++) R[k] = __byte_perm(V[k], 0u, 0x4342);
-            const uint32_t sB = arc_score_x2(R, __byte_perm(C, 0u, 0x4342));
-            // scores <= minTh and columns outside the detection area read as 0
-            const uint32_t thr = (uint32_t)minTh;
-            uint32_t oA = ((sA & 0xffffu) > thr ? (sA & 0xffffu) : 0u) | ((sA >> 16) > thr ? (sA & 0xffff0000u) : 0u);
-            uint32_t oB = ((sB & 0xffffu) > thr ? (sB & 0xffffu) : 0u) | ((sB >> 16) > thr ? (sB & 0xffff0000u) : 0u);
-            uint32_t* Srow = S2 + (y + 1) * FAST_SW + 2 * wi;
-            Srow[0] = oA & mskV[2 * wi]; Srow[1] = oB & mskV[2 * wi + 1];
+            const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
+            // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
+            // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset)
+            *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
+                make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
         };
         if (live) {
             const uint32_t i0 = liveOff[tileIdx], i1 = liveOff[tileIdx + 1];
             for (uint32_t it = i0 + tid; it < i1; it += 256) { const int e = live[it]; score_item(e >> 6, w0 + (e & 63)); }
         } else {
-            const uint32_t mgw = fdiv_magic(nw);
-            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgw); score_item(y, w0 + (it - y * nw)); }
+            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); score_item(y, w0 + (it - y * nw)); }
         }
     }
     __syncthreads();
-    // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh)
+    // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
+    // non-zero only inside an item phase A scored, so B walks the same items; one thread reads the item's 3 x 4 pair-word neighbourhood once.
+    // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
+    // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
     {
-        const int np = 2 * nw, nitems = np * ny;
-        const uint32_t mgp = fdiv_magic(np);
-        for (int it = tid; it < nitems; it += 256) {
-            const int y = fdiv_small(it, mgp), pw = 2 * w0 + (it - y * np);
-            const uint32_t* r1 = S2 + (y + 1) * FAST_SW + pw;
-            const uint32_t cur = r1[0];
-            if (cur == 0) continue;
+        auto nms_item = [&](int y, int wi) {
+            const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
+            const uint4 hd = __ldg(reinterpret_cast<const uint4*>(&C->item[wi]));
+            uint2 cu = *reinterpret_cast<const uint2*>(r1);
+            cu.x &= hd.x; cu.y &= hd.y;
+            if ((cu.x | cu.y) == 0) return;
             const uint32_t* r0 = r1 - FAST_SW; const uint32_t* r2 = r1 + FAST_SW;
-            const uint32_t ml = mskL[pw], mr = mskR[pw];
-            const uint32_t a0 = pw > 0 ? r0[-1] : 0u, b0 = r0[0], c0 = r0[1];
-            const uint32_t a1 = pw > 0 ? r1[-1] : 0u, c1 = r1[1];
-            const uint32_t a2 = pw > 0 ? r2[-1] : 0u, b2 = r2[0], c2 = r2[1];
-            const uint32_t upL = __funnelshift_r(a0, b0, 16) & ml, upR = __funnelshift_r(b0, c0, 16) & mr;
-            const uint32_t cuL = __funnelshift_r(a1, cur, 16) & ml, cuR = __funnelshift_r(cur, c1, 16) & mr;
-            const uint32_t dnL = __funnelshift_r(a2, b2, 16) & ml, dnR = __funnelshift_r(b2, c2, 16) & mr;
-            const uint32_t M = __vimax3_u16x2(__vimax3_u16x2(upL, b0, upR), __vimax3_u16x2(cuL, cuR, b2), __vmaxu2(dnL, dnR));
+            const uint2 up = *reinterpret_cast<const uint2*>(r0), dn = *reinterpret_cast<const uint2*>(r2);
+            const uint32_t uL = wi > 0 ? r0[-1] : 0u, cL = wi > 0 ? r1[-1] : 0u, dL = wi > 0 ? r2[-1] : 0u;
+            const uint32_t uR = r0[2], cR = r1[2], dR = r2[2];
+            const uint4 lr = __ldg(reinterpret_cast<const uint4*>(&C->item[wi]) + 1);
+            const uint32_t M0 = nms_max(uL, up.x, up.y, cL, cu.x, cu.y, dL, dn.x, dn.y, lr.x, lr.z);
+            const uint32_t M1 = nms_max(up.x, up.y, uR, cu.x, cu.y, cR, dn.x, dn.y, dR, lr.y, lr.w);
+            uint32_t keep = 0;   // bit j: pixel j of the item survives
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int sv = (cur >> (16 * h)) & 0xffff, mv = (M >> (16 * h)) & 0xffff;
-                if (sv > mv) {
-                    const int x = 2 * pw + h - xoff, cell = cellInfo[x] & 0x3f;
-                    const int pos = atomicAdd(&nK, 1);
-                    if (pos >= FAST_KMAX) *errFlag = CSLAM_E_CAPACITY;
-                    else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)sv << 16) | ((uint32_t)cell << 24);
-                    if (sv > iniTh) atomicAdd(&cnt20[cell], 1);
-                }
+            for (int j = 0; j < 4; j++) {
+                const uint32_t c = j < 2 ? cu.x : cu.y, m = j < 2 ? M0 : M1, h = 16 * (j & 1);
+                keep |= (((c >> h) & 0xffff) > ((m >> h) & 0xffff)) ? 1u << j : 0u;
             }
+            while (keep) {
+                const int j = __ffs(keep) - 1;
+                keep &= keep - 1;
+                const uint32_t sv = ((j < 2 ? cu.x : cu.y) >> (16 * (j & 1))) & 0xffff;
+                const int x = 4 * wi + j - xoff, cell = (hd.z >> (2 * j)) & 3, s = (int)(sv >> 8) + mt;
+                const int pos = atomicAdd(&nK, 1);
+                if (pos >= FAST_KMAX) *errFlag = CSLAM_E_CAPACITY;
+                else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)s << 16) | ((uint32_t)cell << 24);
+                if (s > iniTh) atomicAdd(&cnt20[cell], 1);
+            }
+        };
+        if (live) {
+            const uint32_t i0 = liveOff[tileIdx], i1 = liveOff[tileIdx + 1];
+            for (uint32_t it = i0 + tid; it < i1; it += 256) { const int e = live[it]; nms_item(e >> 6, w0 + (e & 63)); }
+        } else {
+            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); nms_item(y, w0 + (it - y * nw)); }
         }
     }
     __syncthreads();
@@ -458,8 +513,8 @@ __global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, L
         if (sel) {
             const uint32_t pos = (uint32_t)chunkBase + warpCnt[warp] + __popc(ball & ((1u << lane) - 1));
             if (pos < (uint32_t)g.candCap) {
-                const uint32_t X = tx0 + 3 + (e & 0xff) - g.minB, Y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
-                out[pos] = X | (Y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
+                const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
+                out[pos] = x | (y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
             } else {
                 *errFlag = CSLAM_E_CAPACITY;
             }
@@ -1027,6 +1082,8 @@ static int build_static_classes(cslam_frontend* fe) {
             }
         // work items in k_fast's order and geometry (tile rows iniY.., tile columns from a0 = tx0 & ~3, item = tile word wi of detection row y)
         const int gx = cdiv(g.nColsEff, CG), gy = g.nRowsEff;
+        std::vector<FastTileX> tx(gx);
+        for (int cxg = 0; cxg < gx; cxg++) tx[cxg] = fast_tile_x(g, cxg);
         std::vector<uint8_t> sk((size_t)gx * gy);
         std::vector<uint32_t> off((size_t)gx * gy + 1);
         std::vector<uint16_t> items;
@@ -1035,10 +1092,7 @@ static int build_static_classes(cslam_frontend* fe) {
                 const size_t t = (size_t)cy * gx + cxg;
                 off[t] = (uint32_t)items.size();
                 const int iniY = g.minB + cy * g.hCell, maxY = std::min(iniY + g.hCell + 6, g.maxBY);
-                const int ncell = std::min(CG, g.nColsEff - cxg * CG);
-                const int tx0 = g.minB + cxg * CG * g.wCell, tx1 = std::min(tx0 + ncell * g.wCell + 6, g.maxBX);
-                const int a0 = tx0 & ~3, nx = tx1 - tx0 - 6, ny = maxY - iniY - 6, xoff = tx0 - a0 + 3;
-                const int w0 = xoff >> 2, w1 = (xoff + nx + 3) >> 2;
+                const int a0 = tx[cxg].a0, nx = tx[cxg].nx, ny = maxY - iniY - 6, xoff = tx[cxg].xoff, w0 = tx[cxg].w0, w1 = tx[cxg].w1;
                 for (int y = 0; y < ny; y++)
                     for (int wi = w0; wi < w1; wi++) {
                         bool any = false;
@@ -1054,6 +1108,31 @@ static int build_static_classes(cslam_frontend* fe) {
         if ((rc = dev_upload(fe, &fe->L.skip[l], sk)) || (rc = dev_upload(fe, &fe->L.live[l], items)) || (rc = dev_upload(fe, &fe->L.liveOff[l], off))) return rc;
     }
     return 0;
+}
+
+// k_fast's per-tile-column table of one level (FastCols): the same for every frame, cell row and image, caller canvases included
+static std::vector<FastCols> build_fast_cols(const LevelGeom& g) {
+    std::vector<FastCols> cols(cdiv(g.nColsEff, CG));
+    std::memset(cols.data(), 0, cols.size() * sizeof(FastCols));
+    for (size_t cx = 0; cx < cols.size(); cx++) {
+        const FastTileX t = fast_tile_x(g, (int)cx);
+        FastCols& c = cols[cx];
+        if (t.nx <= 0) continue;   // k_fast exits before reading the table
+        c.mgWords = fdiv_magic(t.nwords); c.mgItems = fdiv_magic(t.w1 - t.w0); c.mgZero = fdiv_magic(t.q1 - t.q0);
+        for (int wi = 0; wi < FAST_SW / 2; wi++)
+            for (int j = 0; j < 4; j++) {
+                const int x = 4 * wi + j - t.xoff;   // detection x of tile column 4*wi + j
+                if (x < 0 || x >= t.nx) continue;
+                const int cell = x / g.wCell, xl = x - cell * g.wCell;
+                const uint32_t lane = 0xffffu << (16 * (j & 1));
+                FastItem& it = c.item[wi];
+                it.valid[j >> 1] |= lane;
+                if (xl != 0) it.left[j >> 1] |= lane;
+                if (xl != g.wCell - 1 && x != t.nx - 1) it.right[j >> 1] |= lane;
+                it.cells |= (uint32_t)cell << (2 * j);
+            }
+    }
+    return cols;
 }
 
 extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const cslam_cam_params* cam, const cslam_orb_params* orb,
@@ -1125,6 +1204,7 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         if ((rc = dev_alloc(fe->owned, &fe->L.img[l], (size_t)max_batch * g.pitch * g.h + 256, true))) return fail(rc);   // slack: word loads may run a few bytes past the last row; zeroed: the black corners are never written on the warp path
         if ((rc = dev_alloc(fe->owned, &fe->L.cand[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
         if ((rc = dev_alloc(fe->owned, &fe->L.pnode[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
+        if ((rc = dev_upload(fe, &fe->L.fcols[l], build_fast_cols(g)))) return fail(rc);
         if (l > 0) {
             std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
             build_resize_tables(fe->L.g[l - 1].w, g.w, xo, xa); build_resize_tables(fe->L.g[l - 1].h, g.h, yo, ya);
@@ -1312,7 +1392,7 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         dim3 grid(cdiv(g.nColsEff, CG), g.nRowsEff, cnt);
         mark(fe, st, KIND_FAST);
         k_fast<<<grid, 256, 0, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err,
-                                     useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
+                                     L.fcols[l], useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
     }
     CSLAM_CUDA(cudaGetLastError());
     DistributeArgs da;
