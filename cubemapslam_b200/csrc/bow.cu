@@ -1,7 +1,7 @@
 // DBoW2 vocabulary-tree transform of libcubemap_b200.so (SURVEY 8(f) row 2), sm_90a.
 //
 // Reference (CPU): Frame::ComputeBoW / KeyFrame::ComputeBoW (src/Frame.cpp:719-726) -> TemplatedVocabulary::transform(features, BowVector&, FeatureVector&, 4)
-//   ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1193 (per feature :1218-1262: greedy descent, first minimum wins; FORB::distance FORB.cpp:81-101),
+//   ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1193 (per feature :1218-1262: greedy descent, first minimum wins; FORB::distance is hamming256 in orb_match.cuh),
 //   BowVector::addWeight / normalize(L1) BowVector.cpp:31-45,62-85. ORBvoc.txt is k = 10, L = 6, L1_NORM scoring, TF_IDF weighting.
 //
 // k_bow_descend   thread per feature: L levels x k children, 256-bit Hamming against node descriptors (35 MB for the full vocabulary: L2-resident);
@@ -11,6 +11,7 @@
 #include <cstring>
 #include <vector>
 #include "common.cuh"
+#include "orb_match.cuh"
 
 namespace cslam {
 
@@ -31,8 +32,7 @@ __global__ void __launch_bounds__(128) k_bow_descend(VocDev V, const uint8_t* __
         for (int c = s; c < e; c++) {
             const int id = V.childList[c];
             const uint4 b0 = __ldg(V.desc + 2 * (size_t)id), b1 = __ldg(V.desc + 2 * (size_t)id + 1);
-            const int d = __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) +
-                          __popc(a1.w ^ b1.w);
+            const int d = hamming256(a0, a1, b0, b1);
             if (d < best) { best = d; bestId = id; }
         }
         fin = bestId;
@@ -40,17 +40,6 @@ __global__ void __launch_bounds__(128) k_bow_descend(VocDev V, const uint8_t* __
     } while (V.childStart[fin + 1] > V.childStart[fin]);
     const size_t o = (size_t)f * stride + i;
     word[o] = V.wordId[fin]; leaf[o] = fin; node[o] = V.weight[fin] > 0 ? nid : -1;   // stopped words (weight 0) join neither vector
-}
-
-__device__ void bitonic_sort_u32(uint32_t* key, int n2) {
-    for (int k = 2; k <= n2; k <<= 1)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = threadIdx.x; t < n2; t += blockDim.x) {
-                const int ixj = t ^ j;
-                if (ixj > t) { const uint32_t a = key[t], b = key[ixj]; const bool up = (t & k) == 0; if ((a > b) == up) { key[t] = b; key[ixj] = a; } }
-            }
-            __syncthreads();
-        }
 }
 
 // keys: word << 12 | feature index (index < 4096, word < 2^20)
@@ -64,7 +53,7 @@ __global__ void __launch_bounds__(256) k_bow_vector(VocDev V, const int32_t* __r
     const size_t o = (size_t)f * stride;
     for (int i = tid; i < n2; i += 256) key[i] = (i < nf && node[o + i] >= 0) ? ((uint32_t)word[o + i] << 12) | (uint32_t)i : 0xffffffffu;
     __syncthreads();
-    bitonic_sort_u32(key, n2);
+    block_bitonic_sort(key, n2);
     // segment starts -> output rank (exclusive scan of the start flags)
     if (tid == 0) carry = 0;
     __syncthreads();
@@ -161,14 +150,12 @@ extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k
 extern "C" void* cslam_vocabulary_stream(const cslam_vocabulary* v) { return v ? (void*)v->stream : nullptr; }
 extern "C" int cslam_vocabulary_sync(cslam_vocabulary* v) { if (!v) return CSLAM_E_BADARG; CSLAM_CUDA(cudaSetDevice(v->device)); CSLAM_CUDA(cudaStreamSynchronize(v->stream)); return CSLAM_OK; }
 
-static int pow2_ge(int n) { int p = 1; while (p < n) p <<= 1; return p; }
-
 extern "C" int cslam_bow_transform_dev(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* word, int32_t* leaf, int32_t* node,
                                        int32_t* bow_word, double* bow_val, int32_t* bow_count) {
     if (!v || !desc || !n || !word || !leaf || !node || !bow_word || !bow_val || !bow_count || nframes <= 0 || stride <= 0 || stride > 4096) { set_error("cslam_bow_transform_dev: bad argument"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(v->device));
     k_bow_descend<<<dim3(cdiv(stride, 128), nframes), 128, 0, v->stream>>>(v->V, desc, n, stride, levelsup, word, leaf, node);
-    const int n2 = pow2_ge(stride);
+    const int n2 = pow2_at_least(stride);
     k_bow_vector<<<nframes, 256, (size_t)2 * n2 * 4, v->stream>>>(v->V, n, stride, n2, word, leaf, node, bow_word, bow_val, bow_count);
     v->launches += 2;
     CSLAM_CUDA(cudaGetLastError());

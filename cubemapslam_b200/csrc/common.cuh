@@ -25,6 +25,7 @@ int check_device(int device);
 
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+static inline int pow2_at_least(int n) { int p = 1; while (p < n) p <<= 1; return p; }   // sizes of the block-wide bitonic sorts
 
 // Device buffer of `count` elements (at least one) owned by a handle: it goes onto `owned`, which the handle's destroy frees. zero: cleared once.
 template <class T>

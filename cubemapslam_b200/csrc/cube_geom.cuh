@@ -4,6 +4,38 @@
 
 namespace cslam {
 
+// The GetFeaturesInArea window table in constant memory (without -rdc every translation unit that includes this holds its own copy)
+static __constant__ AreaRect c_area[5][9][3] = AREA_TABLE_INIT;
+
+// `Rcw * x + tcw` on CV_32F Mats: float products summed left to right, then (float)((double)t + (double)tcw). T: the top 3 x 4 of a
+// row-major 4 x 4 Tcw.
+__device__ __forceinline__ void transform_cw(const float* T, const float* x, float (&xc)[3]) {
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        float t = __fmul_rn(T[4 * i], x[0]);
+        t = __fadd_rn(t, __fmul_rn(T[4 * i + 1], x[1]));
+        t = __fadd_rn(t, __fmul_rn(T[4 * i + 2], x[2]));
+        xc[i] = (float)((double)t + (double)T[4 * i + 3]);
+    }
+}
+
+// Rectangle k of a GetFeaturesInArea window, clamped to its face: n cells (0 if the clamp leaves none); the ci-th in the reference's
+// visiting order (ix major, iy minor) is cell(ci) of the 5 x 50 x 50 grid.
+struct AreaCells {
+    int face, x0, y0, ny, n;
+    __device__ int cell(int ci) const { return (face * GRID_G + x0 + ci / ny) * GRID_G + y0 + ci % ny; }
+};
+// false: the window has no rectangle k (the table lists the used ones first)
+__device__ __forceinline__ bool area_cells(const AreaQuery& aq, int k, AreaCells& r) {
+    const AreaRect rc = c_area[aq.face][aq.caseRow][k];
+    if (rc.face == FACE_NONE) return false;
+    const int x0 = max(0, area_sym(aq, rc.x0)), x1 = min(GRID_G - 1, area_sym(aq, rc.x1));
+    const int y0 = max(0, area_sym(aq, rc.y0)), y1 = min(GRID_G - 1, area_sym(aq, rc.y1));
+    r.face = rc.face; r.x0 = x0; r.y0 = y0; r.ny = y1 - y0 + 1;
+    r.n = (x0 > x1 || y0 > y1) ? 0 : (x1 - x0 + 1) * r.ny;
+    return true;
+}
+
 // TransformRaysToCubemap (src/CamModelGeneral.cpp:95-154): ordered face tests, double pinhole, float result, in-face bounds, tile offset
 __device__ __forceinline__ bool ray_to_cubemap(float x, float y, float z, int W, int H, float& up, float& vp) {
     int face; float lx, ly, lz;

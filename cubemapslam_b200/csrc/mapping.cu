@@ -8,27 +8,23 @@
 //
 // k_distinctive      one CTA per MapPoint: thread i owns observation i; its median distance to the others is the k-th order statistic found by a
 //                    9-step bisection on the distance value (distances are integers in [0, 256]; no N x N matrix, no sort); first least median wins.
-// k_fuse_search      one warp per MapPoint: projection into the key frame, the GetFeaturesInArea window (area_table.cuh) walked in the
+// k_fuse_search      one warp per MapPoint: projection into the key frame, the GetFeaturesInArea window (cube_geom.cuh) walked in the
 //                    reference's order, level / chi2 gates, Hamming; the winner is the FIRST least distance in that order (the loop uses <).
 //                    MapPoints are independent here: the order-dependent part of Fuse (Replace / AddObservation) stays on the host objects.
 // k_triangulation    one CTA per key-frame pair: KF2's FeatureVector is rebuilt by an in-CTA bitonic sort of (node, index); one thread per KF1
 //                    feature scans its node's KF2 features in list order with the reference's `<=` update rule, epipole and epipolar-line tests
 //                    in the reference's float arithmetic (no FMA contraction); rotation histogram + three maxima per pair.
+// The ORB-matching rules (Hamming distance, rotation bin, three maxima, bitonic sort, FeatureVector lookup) are orb_match.cuh's.
 #include <cstring>
 #include <vector>
 #include "area_table.cuh"
 #include "common.cuh"
 #include "cube_geom.cuh"
+#include "orb_match.cuh"
 
 namespace cslam {
 
-__constant__ AreaRect c_area_m[5][9][3] = AREA_TABLE_INIT;
 static const int MAP_NCELLS = 5 * GRID_G * GRID_G;
-
-__device__ __forceinline__ int hamming_u4(const uint4 a0, const uint4 a1, const uint4 b0, const uint4 b1) {
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) +
-           __popc(a1.w ^ b1.w);
-}
 
 // ------------------------------------------------------------------------------------------------- ComputeDistinctiveDescriptors
 static const int DD_THREADS = 128;
@@ -54,7 +50,7 @@ __global__ void __launch_bounds__(DD_THREADS) k_distinctive(const uint8_t* __res
             int cnt = 0;
             for (int j = 0; j < N; j++) {
                 const uint4 b0 = staged ? sd[2 * j] : __ldg(D + 2 * j), b1 = staged ? sd[2 * j + 1] : __ldg(D + 2 * j + 1);
-                cnt += hamming_u4(a0, a1, b0, b1) <= mid;
+                cnt += hamming256(a0, a1, b0, b1) <= mid;
             }
             if (cnt >= k + 1) hi = mid; else lo = mid + 1;
         }
@@ -86,15 +82,8 @@ __global__ void __launch_bounds__(256) k_fuse_search(FuseArgs A) {
     unsigned best = 0xffffffffu;   // dist << 20 | position in the visiting order
     int bestI = -1;
     if (A.valid[m]) {
-        const float* X = A.Xw + 3 * (size_t)m;
         float xc[3];
-#pragma unroll
-        for (int i = 0; i < 3; i++) {   // `Rcw*p3Dw + tcw` on CV_32F Mats
-            float t = __fmul_rn(A.Tcw[4 * i], X[0]);
-            t = __fadd_rn(t, __fmul_rn(A.Tcw[4 * i + 1], X[1]));
-            t = __fadd_rn(t, __fmul_rn(A.Tcw[4 * i + 2], X[2]));
-            xc[i] = (float)((double)t + (double)A.Tcw[4 * i + 3]);
-        }
+        transform_cw(A.Tcw, A.Xw + 3 * (size_t)m, xc);   // `Rcw*p3Dw + tcw`
         float u, v;
         ray_to_cubemap(xc[0], xc[1], xc[2], A.W, A.H, u, v);   // the face result is not used: KeyFrame::IsInImage decides
         if (u >= 0.0f && u < (float)(3 * A.W) && v >= 0.0f && v < (float)(3 * A.H)) {
@@ -108,16 +97,12 @@ __global__ void __launch_bounds__(256) k_fuse_search(FuseArgs A) {
                 const uint4* dC = reinterpret_cast<const uint4*>(A.dKF);
                 int posBase = 0;
                 for (int k = 0; k < 3; k++) {
-                    const AreaRect rc = c_area_m[aq.face][aq.caseRow][k];
-                    if (rc.face == FACE_NONE) break;
-                    const int x0 = max(0, area_sym(aq, rc.x0)), x1 = min(GRID_G - 1, area_sym(aq, rc.x1));
-                    const int y0 = max(0, area_sym(aq, rc.y0)), y1 = min(GRID_G - 1, area_sym(aq, rc.y1));
-                    if (x0 > x1 || y0 > y1) continue;
-                    const int ny = y1 - y0 + 1, ncell = (x1 - x0 + 1) * ny;
-                    for (int cb = 0; cb < ncell; cb += 32) {   // lanes = consecutive cells (ix major, iy minor) = the reference's cell order
+                    AreaCells rc;
+                    if (!area_cells(aq, k, rc)) break;
+                    for (int cb = 0; cb < rc.n; cb += 32) {   // lanes = consecutive cells (ix major, iy minor) = the reference's cell order
                         const int ci = cb + lane;
                         int s = 0, e = 0;
-                        if (ci < ncell) { const int cell = (rc.face * GRID_G + x0 + ci / ny) * GRID_G + y0 + ci % ny; s = A.cellStart[cell]; e = A.cellStart[cell + 1]; }
+                        if (ci < rc.n) { const int cell = rc.cell(ci); s = A.cellStart[cell]; e = A.cellStart[cell + 1]; }
                         // position of this lane's first entry in the visiting order = entries of the earlier cells
                         int pre = e - s;
 #pragma unroll
@@ -132,7 +117,7 @@ __global__ void __launch_bounds__(256) k_fuse_search(FuseArgs A) {
                             const float ex = __fsub_rn(u, kp.x), ey = __fsub_rn(v, kp.y);
                             const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
                             if ((double)__fmul_rn(e2, A.invSigma2[kp.octave]) > 5.99) continue;
-                            const unsigned d = (unsigned)hamming_u4(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
+                            const unsigned d = (unsigned)hamming256(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
                             const unsigned key = (d << 20) | (unsigned)min(posBase + pre + (a - s), 0xfffff);
                             if (key < best) { best = key; bestI = idx; }
                         }
@@ -153,21 +138,6 @@ __global__ void __launch_bounds__(256) k_fuse_search(FuseArgs A) {
 
 // ------------------------------------------------------------------------------------------------- SearchForTriangulation
 static const int TRI_THREADS = 256;
-static const int TRI_BINS = 30;
-__device__ void bitonic_sort_m(uint32_t* key, int n2) {   // ascending, n2 power of two
-    for (int k = 2; k <= n2; k <<= 1)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = threadIdx.x; t < n2; t += blockDim.x) {
-                const int ixj = t ^ j;
-                if (ixj > t) {
-                    const uint32_t a = key[t], b = key[ixj];
-                    const bool up = (t & k) == 0;
-                    if ((a > b) == up) { key[t] = b; key[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-}
 // cv::norm(Vec3f) / cv::Vec3f::dot as OpenCV evaluates them (double accumulation + double sqrt / float accumulation)
 __device__ __forceinline__ double norm3_d(float a, float b, float c) {
     return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn((double)a, (double)a), __dmul_rn((double)b, (double)b)), __dmul_rn((double)c, (double)c)));
@@ -209,7 +179,7 @@ struct TriArgs {
 };
 __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
     extern __shared__ uint32_t key2[];   // (node << 12 | index) of KF2, sorted
-    __shared__ int hist[TRI_BINS], keep[TRI_BINS], total;
+    __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total;
     __shared__ float E[9], epi[2];
     const int p = blockIdx.x, tid = threadIdx.x;
     const int n1 = min(A.n1[p], A.s1), n2 = min(A.n2[p], A.s2);
@@ -220,31 +190,23 @@ __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
     const int32_t* N1 = A.node1 + (size_t)p * A.s1; const int32_t* N2 = A.node2 + (size_t)p * A.s2;
     int32_t* out = A.match12 + (size_t)p * A.s1;
     for (int i = tid; i < A.n2pow; i += TRI_THREADS) key2[i] = i < n2 ? ((uint32_t)N2[i] << 12) | (uint32_t)i : 0xffffffffu;
-    if (tid < TRI_BINS) hist[tid] = 0;
+    if (tid < HISTO_BINS) hist[tid] = 0;
     if (tid < 9) E[tid] = A.E12[(size_t)p * 9 + tid];
     if (tid == 0) {
         total = 0;
-        const float* T = A.Tcw2 + (size_t)p * 16; const float* O = A.Ow1 + (size_t)p * 3;
         float c[3];
-        for (int i = 0; i < 3; i++) {   // C2 = R2w*Cw + t2w
-            float t = __fmul_rn(T[4 * i], O[0]);
-            t = __fadd_rn(t, __fmul_rn(T[4 * i + 1], O[1]));
-            t = __fadd_rn(t, __fmul_rn(T[4 * i + 2], O[2]));
-            c[i] = (float)((double)t + (double)T[4 * i + 3]);
-        }
+        transform_cw(A.Tcw2 + (size_t)p * 16, A.Ow1 + (size_t)p * 3, c);   // C2 = R2w*Cw + t2w
         float ex, ey;
         ray_to_cubemap(c[0], c[1], c[2], A.W, A.H, ex, ey);
         epi[0] = ex; epi[1] = ey;
     }
     __syncthreads();
-    bitonic_sort_m(key2, A.n2pow);
+    block_bitonic_sort(key2, A.n2pow);
     const float ex = epi[0], ey = epi[1];
     for (int i1 = tid; i1 < n1; i1 += TRI_THREADS) {
         int bestIdx2 = -1;
         if (!M1[i1]) {
-            const uint32_t target = (uint32_t)N1[i1] << 12;
-            int lo = 0, hi = n2;
-            while (lo < hi) { const int mid = (lo + hi) >> 1; if (key2[mid] < target) lo = mid + 1; else hi = mid; }
+            const int lo = node_lower_bound(key2, n2, (uint32_t)N1[i1]);
             const uint4 a0 = __ldg(D1 + 2 * i1), a1 = __ldg(D1 + 2 * i1 + 1);
             const float r0 = R1[3 * i1], r1 = R1[3 * i1 + 1], r2 = R1[3 * i1 + 2];
             // epipolar plane normal in the frame of KF2: [a b c] = ray1^T E12 (columns of E12)
@@ -256,7 +218,7 @@ __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
             for (int q = lo; q < n2 && (key2[q] >> 12) == (uint32_t)N1[i1]; q++) {
                 const int i2 = key2[q] & 0xfff;
                 if (M2[i2]) continue;
-                const int dist = hamming_u4(a0, a1, __ldg(D2 + 2 * i2), __ldg(D2 + 2 * i2 + 1));
+                const int dist = hamming256(a0, a1, __ldg(D2 + 2 * i2), __ldg(D2 + 2 * i2 + 1));
                 if (dist > 50 || dist > bestDist) continue;
                 const cslam_keypoint kp2 = K2[i2];
                 const float dx = __fsub_rn(ex, kp2.x), dy = __fsub_rn(ey, kp2.y);
@@ -273,38 +235,17 @@ __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
         out[i1] = bestIdx2;
         if (bestIdx2 >= 0) {
             atomicAdd(&total, 1);
-            if (A.checkOri) {
-                float rot = __fsub_rn(K1[i1].angle, K2[bestIdx2].angle);
-                if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-                int bin = (int)roundf(__fmul_rn(rot, 1.0f / 12.0f));
-                if (bin == TRI_BINS) bin = 0;
-                atomicAdd(&hist[bin], 1);
-            }
+            if (A.checkOri) atomicAdd(&hist[rot_bin(K1[i1].angle, K2[bestIdx2].angle)], 1);
         }
     }
     __syncthreads();
     if (A.checkOri) {
-        if (tid == 0) {
-            int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-            for (int i = 0; i < TRI_BINS; i++) {
-                const int s = hist[i];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-                else if (s > max3) { max3 = s; ind3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-            for (int i = 0; i < TRI_BINS; i++) keep[i] = (i == ind1 || i == ind2 || i == ind3);
-        }
+        if (tid == 0) three_maxima(hist, keep);
         __syncthreads();
         for (int i1 = tid; i1 < n1; i1 += TRI_THREADS) {
             const int m = out[i1];
             if (m < 0) continue;
-            float rot = __fsub_rn(K1[i1].angle, K2[m].angle);
-            if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-            int bin = (int)roundf(__fmul_rn(rot, 1.0f / 12.0f));
-            if (bin == TRI_BINS) bin = 0;
-            if (!keep[bin]) { out[i1] = -1; atomicSub(&total, 1); }
+            if (!keep[rot_bin(K1[i1].angle, K2[m].angle)]) { out[i1] = -1; atomicSub(&total, 1); }
         }
         __syncthreads();
     }
@@ -447,7 +388,7 @@ extern "C" int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const
     A.k2 = dK2; A.d2 = dD2; A.rays2 = dR2; A.hasMP2 = dM2; A.node2 = dN2; A.n2 = dC2; A.s2 = stride2;
     A.Ow1 = dO; A.Tcw2 = dT; A.E12 = dE; A.W = face_w; A.H = face_h; A.checkOri = check_orientation ? 1 : 0;
     for (int i = 0; i < 16; i++) { A.scale[i] = scale_factors[std::min(i, nlevels - 1)]; A.sigma2[i] = level_sigma2[std::min(i, nlevels - 1)]; }
-    int p2 = 1; while (p2 < stride2) p2 <<= 1;
+    const int p2 = pow2_at_least(stride2);
     A.n2pow = p2; A.match12 = dOut; A.nmatches = dNm;
     k_triangulation<<<npairs, TRI_THREADS, (size_t)p2 * 4, st>>>(A); m->launches++;
     CSLAM_CUDA(cudaGetLastError());

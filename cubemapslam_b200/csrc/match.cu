@@ -1,7 +1,7 @@
 // 256-bit Hamming matching of libcubemap_b200.so, sm_90a.
 //
-// Reference (CPU): ORBMatcher::DescriptorDistance src/ORBMatcher.cpp:951-967 (SWAR popcount of 8 x 32-bit XOR),
-//   SearchByBoW(KeyFrame*,Frame&,...) :409-539, ComputeThreeMaxima :905-946, thresholds :42-45.
+// Reference (CPU): SearchByBoW(KeyFrame*,Frame&,...) src/ORBMatcher.cpp:409-539, thresholds :42-45; DescriptorDistance, the rotation bin
+//   and ComputeThreeMaxima are restated once in orb_match.cuh.
 // The all-pairs ("brute force") matcher of BASELINE config 3 has no reference function; DESIGN.md defines it as the
 // SearchByBoW acceptance rule + rotation histogram applied to the best/second-best column of every row of A.
 //
@@ -18,10 +18,10 @@
 #include <cstring>
 #include <vector>
 #include "common.cuh"
+#include "orb_match.cuh"
 
 namespace cslam {
 
-static const int HISTO_BINS = 30;      // ceil(360 / HISTO_LENGTH), HISTO_LENGTH = 12
 static const int BF_WARPS = 4;
 static const int BF_THREADS = 32 * BF_WARPS;
 static const int BF_MT = 4;                          // m16 row fragments per warp
@@ -29,34 +29,6 @@ static const int BF_ROWS = BF_WARPS * BF_MT * 16;    // rows of A per CTA
 static const int BF_TILE = 128;                      // descriptors of B per shared-memory stage (one per thread for the popcount)
 static const int BF_COL_BITS = 12;                   // column field of a selection key: columns < 4096 (max_features)
 static_assert(BF_TILE == BF_THREADS, "one thread per staged column");
-
-__device__ __forceinline__ int rot_bin(float a, float b) {
-    const float factor = 1.0f / 12.0f;
-    float rot = __fsub_rn(a, b);
-    if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-    int bin = (int)roundf(__fmul_rn(rot, factor));   // C round(): half away from zero
-    if (bin == HISTO_BINS) bin = 0;
-    return bin;
-}
-
-// ComputeThreeMaxima on bin counts (thread 0 only); keep[] = 1 for the bins that survive
-__device__ void three_maxima(const int* hist, int* keep) {
-    int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-    for (int i = 0; i < HISTO_BINS; i++) {
-        const int s = hist[i];
-        if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-        else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-        else if (s > max3) { max3 = s; ind3 = i; }
-    }
-    if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-    else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-    for (int i = 0; i < HISTO_BINS; i++) keep[i] = (i == ind1 || i == ind2 || i == ind3);
-}
-
-__device__ __forceinline__ int hamming256(const uint32_t (&a)[8], const uint4 b0, const uint4 b1) {
-    return __popc(a[0] ^ b0.x) + __popc(a[1] ^ b0.y) + __popc(a[2] ^ b0.z) + __popc(a[3] ^ b0.w) +
-           __popc(a[4] ^ b1.x) + __popc(a[5] ^ b1.y) + __popc(a[6] ^ b1.z) + __popc(a[7] ^ b1.w);
-}
 
 // popc(a AND b) for a 16 x 8 tile of 256-bit rows: A fragment a[0..3] = words (t, t of row g+8, 4+t, 4+t of row g+8) of row g = lane / 4,
 // t = lane % 4; B fragment b0 / b1 = words t / 4+t of column g; d[0..3] = (g, 2t), (g, 2t+1), (g+8, 2t), (g+8, 2t+1).
@@ -242,21 +214,6 @@ __global__ void __launch_bounds__(BF_THREADS) k_match_bruteforce(const uint8_t* 
 // ------------------------------------------------------------------------------------------------- SearchByBoW
 static const int BOW_THREADS = 256;
 
-__device__ void bitonic_sort(uint32_t* key, int n2) {   // ascending, n2 power of two
-    for (int k = 2; k <= n2; k <<= 1)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = threadIdx.x; t < n2; t += blockDim.x) {
-                const int ixj = t ^ j;
-                if (ixj > t) {
-                    const uint32_t a = key[t], b = key[ixj];
-                    const bool up = (t & k) == 0;
-                    if ((a > b) == up) { key[t] = b; key[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-}
-
 // keys: node << 12 | index (index < 4096, node < 2^20). Shared memory: keyKF[n2K], keyF[n2F], takenF[nF] bytes.
 __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __restrict__ descKF, const float* __restrict__ angKF,
                                                                const uint8_t* __restrict__ kfValid, const int32_t* __restrict__ nodeKF, int nKF,
@@ -286,8 +243,8 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
     if (tid < HISTO_BINS) hist[tid] = 0;
     if (tid == 0) total = 0;
     __syncthreads();
-    bitonic_sort(keyKF, n2K);
-    bitonic_sort(keyF, n2F);
+    block_bitonic_sort(keyKF, n2K);
+    block_bitonic_sort(keyF, n2F);
     // one warp per KF node group: a group starts where the node id changes
     for (int s = warp; s < nKF; s += nwarps) {
         // warps take candidate group starts round-robin: position s is a start iff s==0 or node differs from s-1
@@ -298,10 +255,7 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
         int e = s + 1;
         while (e < nKF && (keyKF[e] >> 12) == node) e++;
         // F group by binary search of node << 12
-        int lo = 0, hi = nF;
-        const uint32_t target = node << 12;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (keyF[mid] < target) lo = mid + 1; else hi = mid; }
-        const int fs = lo;
+        const int fs = node_lower_bound(keyF, nF, node);
         int fe = fs;
         while (fe < nF && (keyF[fe] >> 12) == node) fe++;
         if (fe == fs) continue;
@@ -309,14 +263,13 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
             const int iK = keyKF[q] & 0xfff;
             if (!val[iK]) continue;
             const uint4 k0 = __ldg(K4 + 2 * iK), k1 = __ldg(K4 + 2 * iK + 1);
-            const uint32_t a[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
             // lanes scan the F features of the node in list order; (best1, pos, best2) with first-position ties
             int best1 = 256, best2 = 256, bpos = 0x7fffffff;
             for (int p = fs + lane; p < fe; p += 32) {
                 const int iF = keyF[p] & 0xfff;
                 if (mF[iF] >= 0) continue;
                 if (kfkfMode && !fValid[(size_t)pair * nF + iF]) continue;
-                const int d = hamming256(a, __ldg(F4 + 2 * iF), __ldg(F4 + 2 * iF + 1));
+                const int d = hamming256(k0, k1, __ldg(F4 + 2 * iF), __ldg(F4 + 2 * iF + 1));
                 if (d < best1) { best2 = best1; best1 = d; bpos = p; }
                 else if (d < best2) best2 = d;
             }
@@ -367,8 +320,7 @@ __global__ void k_hamming(const uint8_t* __restrict__ a, const uint8_t* __restri
     const uint4* A4 = reinterpret_cast<const uint4*>(a) + 2 * (size_t)i;
     const uint4* B4 = reinterpret_cast<const uint4*>(b) + 2 * (size_t)i;
     const uint4 a0 = __ldg(A4), a1 = __ldg(A4 + 1);
-    const uint32_t av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-    dist[i] = hamming256(av, __ldg(B4), __ldg(B4 + 1));
+    dist[i] = hamming256(a0, a1, __ldg(B4), __ldg(B4 + 1));
 }
 
 }  // namespace cslam
@@ -541,7 +493,7 @@ static int time_ubench(cslam_matcher* m, int iters, Launch launch, int* blocks, 
 }
 
 // POPC issue-rate micro-benchmark (SURVEY 8d: "measure the real rate with a micro-benchmark on the box before quoting a fraction"): every thread
-// runs `iters` rounds of 8 independent XOR+POPC+ADD chains on registers - the exact instruction mix of hamming256 without any memory traffic.
+// runs `iters` rounds of 8 independent XOR+POPC+ADD chains on registers - the exact instruction mix of hamming256 (orb_match.cuh) without any memory traffic.
 __global__ void __launch_bounds__(256) k_ubench_popc(uint32_t* out, int iters, uint32_t seed) {
     uint32_t a[8], acc[8];
 #pragma unroll
@@ -635,8 +587,6 @@ extern "C" int cslam_ubench_minmax3(cslam_matcher* m, double* ops_per_s) {
     *ops_per_s = (double)blocks * 256.0 * iters * 8.0 / (ms * 1e-3);   // warp-lane u16x2 3-input min/max per second
     return CSLAM_OK;
 }
-
-static int pow2_at_least(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 
 extern "C" int cslam_search_by_bow_dev(cslam_matcher* m, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid, const int32_t* node_kf, int nKF,
                                        const uint8_t* descF, const float* angF, const int32_t* node_f, int nF, int npairs, float nnratio, int check_ori,

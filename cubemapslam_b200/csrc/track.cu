@@ -3,7 +3,7 @@
 // Reference (CPU):
 //   Frame::ComputeKeyPointRays  src/Frame.cpp:746-760 -> CamModelGeneral::TransformCubemapToRays include/CamModelGeneral.h:494-513
 //   Frame::AssignFeaturesToGrid src/Frame.cpp:158-176 (5 x 50 x 50 cells)          -> k_frame_index (one CTA per frame)
-//   Frame::GetFeaturesInArea    src/Frame.cpp:251-716 (cube-face wrap-around)      -> area_table.cuh, used inside the matcher kernels
+//   Frame::GetFeaturesInArea    src/Frame.cpp:251-716 (cube-face wrap-around)      -> area_table.cuh, walked through cube_geom.cuh's area_cells
 //   ORBMatcher::SearchByProjection(Frame&, const Frame&, th, mono)   src/ORBMatcher.cpp:130-251 (Tracking::TrackWithMotionModel :634)
 //   ORBMatcher::SearchByProjection(Frame&, vector<MapPoint*>&, th)   src/ORBMatcher.cpp:51-128  (Tracking::SearchLocalPoints :841)
 //
@@ -11,22 +11,22 @@
 // an earlier MapPoint (with observations) is invisible to later ones - so the kernel works in rounds of 8 MapPoints: (A) each warp projects
 // its MapPoint, walks the window's cells in the reference's visiting order and stores the (feature, Hamming distance) candidates in shared
 // memory; (B) one thread commits the 8 MapPoints in order with the reference's scalar best / second-best rule against the `taken` flags.
-// Distances dominate the work and stay parallel; the commit touches a few dozen shorts per MapPoint.
+// Distances dominate the work and stay parallel; the commit touches a few dozen shorts per MapPoint. Hamming distance, rotation bin and
+// three-maxima filter: orb_match.cuh.
 #include <cstring>
 #include <vector>
 #include "area_table.cuh"
 #include "common.cuh"
 #include "cube_geom.cuh"
+#include "orb_match.cuh"
 
 namespace cslam {
 
-__constant__ AreaRect c_area[5][9][3] = AREA_TABLE_INIT;
 static const AreaRect h_area[5][9][3] = AREA_TABLE_INIT;
 
 static const int NCELLS = 5 * GRID_G * GRID_G;
 static const int TRK_WARPS = 8;
 static const int TRK_CAND = 256;          // candidate capacity per MapPoint (window cells are walked until it is full -> CSLAM_E_CAPACITY)
-static const int HISTO_BINS_T = 30;
 
 // ------------------------------------------------------------------------------------------------- k_frame_index
 // rays: n x 3 float; cellStart: NCELLS+1 u16 (CSR over cells in (face, col, row) order); cellIdx: n u16, ascending inside a cell
@@ -124,24 +124,12 @@ struct TrackArgs {
     int32_t* match; int32_t* nmatches; int* errFlag;
 };
 
-__device__ __forceinline__ int hamming_row(const uint4 a0, const uint4 a1, const uint4 b0, const uint4 b1) {
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) +
-           __popc(a1.w ^ b1.w);
-}
-__device__ __forceinline__ int rot_bin_t(float a, float b) {
-    float rot = __fsub_rn(a, b);
-    if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-    int bin = (int)roundf(__fmul_rn(rot, 1.0f / 12.0f));
-    if (bin == HISTO_BINS_T) bin = 0;
-    return bin;
-}
-
 __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackArgs A) {
     __shared__ uint16_t candIdx[TRK_WARPS][TRK_CAND];
     __shared__ uint16_t candDist[TRK_WARPS][TRK_CAND];
     __shared__ int candN[TRK_WARPS];
     __shared__ uint8_t slotObs[4096];
-    __shared__ int hist[HISTO_BINS_T], keep[HISTO_BINS_T], total, logN;
+    __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total, logN;
     __shared__ uint16_t logIdx[4096];   // mode 0: every accepted assignment (current slot, rotation bin), replayed by the orientation filter
     __shared__ uint8_t logBin[4096];
     const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -153,7 +141,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
     const uint4* dQ = reinterpret_cast<const uint4*>(A.qDesc + (size_t)p * A.qStride * 32);
     int32_t* M = A.match + (size_t)p * A.curStride;
     for (int i = tid; i < nCur; i += blockDim.x) { M[i] = -1; slotObs[i] = A.curTaken ? A.curTaken[(size_t)p * A.curStride + i] : 0; }
-    if (tid < HISTO_BINS_T) hist[tid] = 0;
+    if (tid < HISTO_BINS) hist[tid] = 0;
     if (tid == 0) { total = 0; logN = 0; }
     __syncthreads();
     const float inv = __fdiv_rn((float)(3 * GRID_G), (float)(3 * A.W));
@@ -166,15 +154,8 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
         if (q < nQ && A.qValid[(size_t)p * A.qStride + q]) {
             float u = 0, v = 0, radius = 0; int minL = 0, maxL = 0; bool ok = true;
             if (A.mode == 0) {
-                const float* X = A.qXw + ((size_t)p * A.qStride + q) * 3;
                 float xc[3];
-#pragma unroll
-                for (int i = 0; i < 3; i++) {   // `Rcw*x3Dw+tcw`: float inner product left to right, then (float)((double)t + (double)c)
-                    float t = __fmul_rn(Tc[4 * i], X[0]);
-                    t = __fadd_rn(t, __fmul_rn(Tc[4 * i + 1], X[1]));
-                    t = __fadd_rn(t, __fmul_rn(Tc[4 * i + 2], X[2]));
-                    xc[i] = (float)((double)t + (double)Tc[4 * i + 3]);
-                }
+                transform_cw(Tc, A.qXw + ((size_t)p * A.qStride + q) * 3, xc);   // `Rcw*x3Dw+tcw`
                 if (xc[2] < A.cosFovTh) ok = false;
                 if (ok) ok = ray_to_cubemap(xc[0], xc[1], xc[2], A.W, A.H, u, v);
                 const int oct = A.kLast[(size_t)p * A.qStride + q].octave;
@@ -191,16 +172,12 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
                 const bool checkLevels = (minL > 0) || (maxL >= 0);
                 const uint4 a0 = __ldg(dQ + 2 * q), a1 = __ldg(dQ + 2 * q + 1);
                 for (int k = 0; k < 3; k++) {
-                    const AreaRect rc = c_area[aq.face][aq.caseRow][k];
-                    if (rc.face == FACE_NONE) break;
-                    const int x0 = max(0, area_sym(aq, rc.x0)), x1 = min(GRID_G - 1, area_sym(aq, rc.x1));
-                    const int y0 = max(0, area_sym(aq, rc.y0)), y1 = min(GRID_G - 1, area_sym(aq, rc.y1));
-                    if (x0 > x1 || y0 > y1) continue;
-                    const int ny = y1 - y0 + 1, ncell = (x1 - x0 + 1) * ny;
-                    for (int cb = 0; cb < ncell; cb += 32) {   // lanes = consecutive cells (ix major, iy minor), entries kept in cell order
+                    AreaCells rc;
+                    if (!area_cells(aq, k, rc)) break;
+                    for (int cb = 0; cb < rc.n; cb += 32) {   // lanes = consecutive cells (ix major, iy minor), entries kept in cell order
                         const int ci = cb + lane;
                         int s = 0, e = 0;
-                        if (ci < ncell) { const int cell = (rc.face * GRID_G + x0 + ci / ny) * GRID_G + y0 + ci % ny; s = CS[cell]; e = CS[cell + 1]; }
+                        if (ci < rc.n) { const int cell = rc.cell(ci); s = CS[cell]; e = CS[cell + 1]; }
                         // walk the (few) entries of the 32 cells in order
                         const int maxLen = __reduce_max_sync(0xffffffffu, e - s);
                         if (maxLen == 0) continue;
@@ -224,7 +201,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
                             if (pos < TRK_CAND) {
                                 const int idx = keepIdx[j];
                                 candIdx[warp][pos] = (uint16_t)idx;
-                                candDist[warp][pos] = (uint16_t)hamming_row(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
+                                candDist[warp][pos] = (uint16_t)hamming256(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
                             } else *A.errFlag = CSLAM_E_CAPACITY;
                         }
                         ncand = min(ncand + tot, TRK_CAND);
@@ -252,7 +229,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
                 M[bestIdx] = qq; slotObs[bestIdx] = A.qObs[(size_t)p * A.qStride + qq];
                 total++;
                 if (A.mode == 0 && A.checkOri) {
-                    const int bin = rot_bin_t(A.kLast[(size_t)p * A.qStride + qq].angle, kC[bestIdx].angle);
+                    const int bin = rot_bin(A.kLast[(size_t)p * A.qStride + qq].angle, kC[bestIdx].angle);
                     hist[bin]++;
                     if (logN < 4096) { logIdx[logN] = (uint16_t)bestIdx; logBin[logN] = (uint8_t)bin; logN++; } else *A.errFlag = CSLAM_E_CAPACITY;
                 }
@@ -263,18 +240,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
     if (A.mode == 0 && A.checkOri) {
         // the reference keeps per-bin lists of CURRENT feature indices (a slot overwritten by a later, observation-less MapPoint is listed twice)
         // and clears every slot listed in a non-dominant bin, decrementing nmatches per list entry: the assignment log is replayed.
-        if (tid == 0) {
-            int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-            for (int i = 0; i < HISTO_BINS_T; i++) {
-                const int s = hist[i];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; ind3 = ind2; ind2 = ind1; ind1 = i; }
-                else if (s > max2) { max3 = max2; max2 = s; ind3 = ind2; ind2 = i; }
-                else if (s > max3) { max3 = s; ind3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { ind2 = -1; ind3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) { ind3 = -1; }
-            for (int i = 0; i < HISTO_BINS_T; i++) keep[i] = (i == ind1 || i == ind2 || i == ind3);
-        }
+        if (tid == 0) three_maxima(hist, keep);
         __syncthreads();
         for (int i = tid; i < logN; i += blockDim.x)
             if (!keep[logBin[i]]) { M[logIdx[i]] = -2; atomicSub(&total, 1); }   // -2: assigned, then cleared (the reference NULLs the slot)
