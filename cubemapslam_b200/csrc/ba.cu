@@ -869,17 +869,16 @@ extern "C" int cslam_optimizer_create(cslam_optimizer** out, int device) {
     if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMallocHost(&o->h_scal, 16 * sizeof(double)) != cudaSuccess) {
         set_error("optimizer: stream / pinned allocation failed"); delete o; return CSLAM_E_CUDA;
     }
+    o->arena.bind(o->stream, (size_t)64 << 20);
     cudaFuncSetAttribute(k_ba_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
     *out = o;
     return CSLAM_OK;
 }
-static void release_pool(cslam_optimizer* o) { for (auto& c : o->chunks) cudaFree(c.p); o->chunks.clear(); }
 extern "C" void cslam_optimizer_destroy(cslam_optimizer* o) {
     if (!o) return;
     cudaSetDevice(o->device);
     if (o->stream) cudaStreamSynchronize(o->stream);
     for (auto& p : o->peers) { if (p.base && !p.mine) cudaIpcCloseMemHandle(p.base); else if (p.base) cudaFree(p.base); }
-    release_pool(o);
     if (o->comm && nccl_api()) nccl_api()->CommDestroy(o->comm);
     if (o->stream) cudaStreamDestroy(o->stream);
     if (o->h_scal) cudaFreeHost(o->h_scal);
@@ -1254,7 +1253,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     if (!o || !p || p->n_kf <= 0 || p->n_mp < 0 || p->n_edges < 0 || !p->Tcw || !p->kf_fixed || (p->n_mp && !p->points)) { set_error("cslam_local_ba: bad problem"); return CSLAM_E_BADARG; }
     if (p->face_w != p->face_h || p->face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(o->device));
-    free_pool(o);
+    o->arena.reset();
     const int nKF = p->n_kf, nMP = p->n_mp, nEg = p->n_edges;   // nEg: the caller's edges; nE below: the edges this rank works on
     if (r) { r->iterations = 0; r->trials = 0; if (r->outlier) std::memset(r->outlier, 0, nEg); }
     if (stop_flag && *stop_flag) return CSLAM_OK;   // src/Optimizer.cpp:359-361
@@ -1305,10 +1304,10 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     const Pose* cpose = nullptr; double* cX = nullptr;
     int* d_eMP = nullptr; int* d_eKF = nullptr; int* d_perm = nullptr; float2* d_kp = nullptr; float* d_isig = nullptr; float* d_pts32 = nullptr; int* d_bad = nullptr;
     double* d_obs = nullptr; int8_t* d_face = nullptr;
-    if ((rc = dupload(o, &cpose, poses)) || (rc = dupload(o, &D.lmStart, hs.lmStart)) || (rc = dupload(o, &D.peStart, hs.peStart)) || (rc = dupload(o, &D.peList, hs.peList)) ||
-        (rc = dupload(o, &D.kfOfQ, kfOfQ)) || (rc = dalloc(o, &d_eMP, nE)) || (rc = dalloc(o, &d_eKF, nE)) || (rc = dalloc(o, &d_kp, nEg)) || (rc = dalloc(o, &d_isig, nEg)) ||
-        (rc = dalloc(o, &d_pts32, (size_t)nMP * 3)) || (rc = dalloc(o, &cX, (size_t)nMP * 3)) || (rc = dalloc(o, &d_obs, (size_t)nE * 3)) || (rc = dalloc(o, &d_face, nE)) ||
-        (rc = dalloc(o, &d_bad, 1)) || (!grouped && (rc = dalloc(o, &d_perm, nE)))) return rc;
+    if ((rc = o->arena.upload(&cpose, poses.data(), poses.size())) || (rc = o->arena.upload(&D.lmStart, hs.lmStart.data(), hs.lmStart.size())) || (rc = o->arena.upload(&D.peStart, hs.peStart.data(), hs.peStart.size())) || (rc = o->arena.upload(&D.peList, hs.peList.data(), hs.peList.size())) ||
+        (rc = o->arena.upload(&D.kfOfQ, kfOfQ.data(), kfOfQ.size())) || (rc = o->arena.take(&d_eMP, nE)) || (rc = o->arena.take(&d_eKF, nE)) || (rc = o->arena.take(&d_kp, nEg)) || (rc = o->arena.take(&d_isig, nEg)) ||
+        (rc = o->arena.take(&d_pts32, (size_t)nMP * 3)) || (rc = o->arena.take(&cX, (size_t)nMP * 3)) || (rc = o->arena.take(&d_obs, (size_t)nE * 3)) || (rc = o->arena.take(&d_face, nE)) ||
+        (rc = o->arena.take(&d_bad, 1)) || (!grouped && (rc = o->arena.take(&d_perm, nE)))) return rc;
     if (nE > 0) {
         CSLAM_CUDA(cudaMemcpyAsync(d_eMP, H.h_eMP, (size_t)nE * 4, cudaMemcpyHostToDevice, o->stream));
         CSLAM_CUDA(cudaMemcpyAsync(d_eKF, H.h_eKF, (size_t)nE * 4, cudaMemcpyHostToDevice, o->stream));
@@ -1326,14 +1325,14 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     const size_t payloadMax = (size_t)nmax * nmax + 2 * (size_t)nmax + 4;
     const int maxBlocks = std::max({cdiv(nE, 256), cdiv(nmax + 3 * nMP, 256), 1});
     long long* pairCnt = nullptr;
-    if ((rc = dalloc(o, &D.poseBak, nKF)) || (rc = dalloc(o, &D.Xbak, (size_t)nMP * 3)) || (rc = dalloc(o, &D.err, (size_t)nE * 2, true)) || (rc = dalloc(o, &D.level, nE, true)) ||
-        (rc = dalloc(o, &H.d_poseIdx, nKF)) || (rc = dalloc(o, &H.d_pact, nKF + 1)) || (rc = dalloc(o, &H.d_ptAct, nMP)) || (rc = dalloc(o, &H.d_flag, nE)) || (rc = dalloc(o, &D.Hpp, (size_t)std::max(nQ, 1) * 36)) ||
-        (rc = dalloc(o, &D.bp, (size_t)std::max(nQ, 1) * 6)) || (rc = dalloc(o, &D.Hll, (size_t)nMP * 9)) || (rc = dalloc(o, &D.bl, (size_t)nMP * 3)) ||
-        (rc = dalloc(o, &D.Hpl, (size_t)nE * 18)) || (rc = dalloc(o, &D.Dinv, (size_t)nMP * DINV_LD)) || (rc = dalloc(o, &D.db, (size_t)nMP * 3)) ||
-        (rc = dalloc(o, &H.red, payloadMax)) || (rc = dalloc(o, &D.xp, std::max(nmax, 1), true)) || (rc = dalloc(o, &D.xl, (size_t)nMP * 3, true)) ||
-        (rc = dalloc(o, &D.scal, 8, true)) || (rc = dalloc(o, &D.part, maxBlocks)) || (rc = dalloc(o, &D.ticket, 4, true)) || (rc = dalloc(o, &D.posePart, (size_t)std::max(nQ, 1) * POSE_SPLIT * 27)) || (rc = dalloc(o, &D.poseTicket, std::max(nQ, 1), true)) ||
-        (rc = dalloc(o, &H.Lt, (size_t)LD_NB * H.ldp)) || (rc = dalloc(o, &H.LDt, (size_t)LD_NB * H.ldp)) || (rc = dalloc(o, &H.Minv, (size_t)(nmax / LD_NB + 1) * LD_NB * LD_NB)) || (rc = dalloc(o, &pairCnt, (size_t)nQ * nQ + 1)) ||
-        (rc = dalloc(o, &H.d_xerr, 1, true))) return rc;
+    if ((rc = o->arena.take(&D.poseBak, nKF)) || (rc = o->arena.take(&D.Xbak, (size_t)nMP * 3)) || (rc = o->arena.take(&D.err, (size_t)nE * 2, true)) || (rc = o->arena.take(&D.level, nE, true)) ||
+        (rc = o->arena.take(&H.d_poseIdx, nKF)) || (rc = o->arena.take(&H.d_pact, nKF + 1)) || (rc = o->arena.take(&H.d_ptAct, nMP)) || (rc = o->arena.take(&H.d_flag, nE)) || (rc = o->arena.take(&D.Hpp, (size_t)std::max(nQ, 1) * 36)) ||
+        (rc = o->arena.take(&D.bp, (size_t)std::max(nQ, 1) * 6)) || (rc = o->arena.take(&D.Hll, (size_t)nMP * 9)) || (rc = o->arena.take(&D.bl, (size_t)nMP * 3)) ||
+        (rc = o->arena.take(&D.Hpl, (size_t)nE * 18)) || (rc = o->arena.take(&D.Dinv, (size_t)nMP * DINV_LD)) || (rc = o->arena.take(&D.db, (size_t)nMP * 3)) ||
+        (rc = o->arena.take(&H.red, payloadMax)) || (rc = o->arena.take(&D.xp, std::max(nmax, 1), true)) || (rc = o->arena.take(&D.xl, (size_t)nMP * 3, true)) ||
+        (rc = o->arena.take(&D.scal, 8, true)) || (rc = o->arena.take(&D.part, maxBlocks)) || (rc = o->arena.take(&D.ticket, 4, true)) || (rc = o->arena.take(&D.posePart, (size_t)std::max(nQ, 1) * POSE_SPLIT * 27)) || (rc = o->arena.take(&D.poseTicket, std::max(nQ, 1), true)) ||
+        (rc = o->arena.take(&H.Lt, (size_t)LD_NB * H.ldp)) || (rc = o->arena.take(&H.LDt, (size_t)LD_NB * H.ldp)) || (rc = o->arena.take(&H.Minv, (size_t)(nmax / LD_NB + 1) * LD_NB * LD_NB)) || (rc = o->arena.take(&pairCnt, (size_t)nQ * nQ + 1)) ||
+        (rc = o->arena.take(&H.d_xerr, 1, true))) return rc;
     D.poseIdx = H.d_poseIdx; D.ptAct = H.d_ptAct;
     // ---- multi-GPU exchange path
     if (o->nranks > 1) {
@@ -1346,7 +1345,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         }
         H.useOneShot = o->oneShot && o->xchgBytes >= payloadMax * 8 && !ncclOnly;
         H.xstride = ((o->xchgBytes + 255) & ~(size_t)255) / 8;
-        if ((rc = dalloc(o, &H.HppFull, (size_t)std::max(nQ, 1) * 36))) return rc;
+        if ((rc = o->arena.take(&H.HppFull, (size_t)std::max(nQ, 1) * 36))) return rc;
     }
     // ---- co-observation lists (once per call, all edges)
     int badEdge = 0x7f7f7f7f;
@@ -1359,7 +1358,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
         if (badEdge < nEg) { set_error("edge %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", badEdge, p->kp_xy[2 * badEdge], p->kp_xy[2 * badEdge + 1]); return CSLAM_E_BADARG; }
         int4* tuples = nullptr;
-        if ((rc = dalloc(o, &tuples, (size_t)std::max<long long>(total, 1)))) return rc;
+        if ((rc = o->arena.take(&tuples, (size_t)std::max<long long>(total, 1)))) return rc;
         k_ba_pairs_fill<<<dim3(nQ, nQ), 128, 0, o->stream>>>(D, pairCnt, tuples); o->launches++;
         CSLAM_CUDA(cudaGetLastError());
         D.pairStart = pairCnt; D.tuples = tuples;
@@ -1384,7 +1383,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     std::vector<uint8_t> gflags;   // multi-GPU: every rank returns the flags of ALL edges (max over the owners' flags, in the caller's order)
     if (multi) {
         uint8_t* d_gflag = nullptr;
-        if ((rc = dalloc(o, &d_gflag, std::max(nEg, 1), true))) return rc;
+        if ((rc = o->arena.take(&d_gflag, std::max(nEg, 1), true))) return rc;
         if (nE > 0) { k_ba_scatter_flags<<<cdiv(nE, 256), 256, 0, o->stream>>>(nE, d_perm, H.d_flag, d_gflag); o->launches++; }
         rc = nccl_api()->AllReduce(d_gflag, d_gflag, nEg, NCCL_U8, NCCL_MAX, o->comm, o->stream);
         if (rc) { set_error("ncclAllReduce (flags) failed (%d)", rc); return CSLAM_E_NCCL; }
@@ -1412,6 +1411,5 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
         if (r->outlier) { if (multi) std::memcpy(r->outlier, gflags.data(), nEg); else for (int s = 0; s < nE; s++) r->outlier[H.perm ? H.perm[s] : s] = flags[s]; }
         r->iterations = H.iterations; r->trials = H.trials;
     }
-    free_pool(o);
     return CSLAM_OK;
 }

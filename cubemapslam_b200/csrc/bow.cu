@@ -98,7 +98,7 @@ using namespace cslam;
 struct cslam_vocabulary {
     int device = 0; VocDev V; cudaStream_t stream = nullptr; std::vector<void*> owned; int64_t launches = 0;
     int maxFrames = 0, maxFeat = 0;
-    uint8_t* dFeat = nullptr; int32_t *dN = nullptr, *dWord = nullptr, *dLeaf = nullptr, *dNode = nullptr, *dBowWord = nullptr, *dBowCount = nullptr; double* dBowVal = nullptr;
+    DevArena arena;   // staging of cslam_bow_transform
 };
 
 extern "C" void cslam_vocabulary_destroy(cslam_vocabulary* v) {
@@ -134,11 +134,10 @@ extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k
     int *dStart, *dList, *dWid; uint4* dDesc; double* dW;
     auto fail = [&](int code) { cslam_vocabulary_destroy(v); return code; };
     if (cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); return fail(CSLAM_E_CUDA); }
-    const size_t nf = (size_t)max_frames * max_features;
+    // chunks: room for the descriptors, four int32 arrays and the double weights of a call at the handle's limits, at most 64 MB
+    v->arena.bind(v->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * (32 + 4 * 4 + 8) + (size_t)max_frames * 8));
     auto valloc = [&](auto** p, size_t n) { return dev_alloc(v->owned, p, n, false); };
-    if ((rc = valloc(&dStart, N + 1)) || (rc = valloc(&dList, n_nodes)) || (rc = valloc(&dWid, N)) || (rc = valloc(&dDesc, (size_t)N * 2)) || (rc = valloc(&dW, N)) ||
-        (rc = valloc(&v->dFeat, nf * 32)) || (rc = valloc(&v->dN, max_frames)) || (rc = valloc(&v->dWord, nf)) || (rc = valloc(&v->dLeaf, nf)) || (rc = valloc(&v->dNode, nf)) ||
-        (rc = valloc(&v->dBowWord, nf)) || (rc = valloc(&v->dBowVal, nf)) || (rc = valloc(&v->dBowCount, max_frames))) return fail(rc);
+    if ((rc = valloc(&dStart, N + 1)) || (rc = valloc(&dList, n_nodes)) || (rc = valloc(&dWid, N)) || (rc = valloc(&dDesc, (size_t)N * 2)) || (rc = valloc(&dW, N))) return fail(rc);
     if (cudaMemcpy(dStart, start.data(), (N + 1) * 4, cudaMemcpyHostToDevice) != cudaSuccess || cudaMemcpy(dList, list.data(), (size_t)n_nodes * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(dWid, wordId.data(), N * 4, cudaMemcpyHostToDevice) != cudaSuccess || cudaMemcpy(dDesc, d.data(), (size_t)N * 32, cudaMemcpyHostToDevice) != cudaSuccess ||
         cudaMemcpy(dW, w.data(), (size_t)N * 8, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("vocabulary upload failed"); return fail(CSLAM_E_CUDA); }
@@ -166,16 +165,17 @@ extern "C" int cslam_bow_transform(cslam_vocabulary* v, const uint8_t* desc, con
                                    double* bow_val, int32_t* bow_count) {
     if (!v || nframes <= 0 || nframes > v->maxFrames || stride <= 0 || stride > v->maxFeat) { set_error("cslam_bow_transform: sizes out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(v->device));
+    v->arena.reset();
     const size_t nf = (size_t)nframes * stride;
-    CSLAM_CUDA(cudaMemcpyAsync(v->dFeat, desc, nf * 32, cudaMemcpyHostToDevice, v->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(v->dN, n, (size_t)nframes * 4, cudaMemcpyHostToDevice, v->stream));
-    int rc = cslam_bow_transform_dev(v, v->dFeat, v->dN, stride, nframes, levelsup, v->dWord, v->dLeaf, v->dNode, v->dBowWord, v->dBowVal, v->dBowCount);
-    if (rc) return rc;
-    if (word) CSLAM_CUDA(cudaMemcpyAsync(word, v->dWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(node, v->dNode, nf * 4, cudaMemcpyDeviceToHost, v->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(bow_word, v->dBowWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(bow_val, v->dBowVal, nf * 8, cudaMemcpyDeviceToHost, v->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(bow_count, v->dBowCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
+    const uint8_t* dFeat; const int32_t* dN; int32_t *dWord, *dLeaf, *dNode, *dBowWord, *dBowCount; double* dBowVal; int rc;
+    if ((rc = v->arena.upload(&dFeat, desc, nf * 32)) || (rc = v->arena.upload(&dN, n, nframes)) || (rc = v->arena.take(&dWord, nf)) || (rc = v->arena.take(&dLeaf, nf)) ||
+        (rc = v->arena.take(&dNode, nf)) || (rc = v->arena.take(&dBowWord, nf)) || (rc = v->arena.take(&dBowVal, nf)) || (rc = v->arena.take(&dBowCount, nframes)) ||
+        (rc = cslam_bow_transform_dev(v, dFeat, dN, stride, nframes, levelsup, dWord, dLeaf, dNode, dBowWord, dBowVal, dBowCount))) return rc;
+    if (word) CSLAM_CUDA(cudaMemcpyAsync(word, dWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(node, dNode, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(bow_word, dBowWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(bow_val, dBowVal, nf * 8, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(bow_count, dBowCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
     CSLAM_CUDA(cudaStreamSynchronize(v->stream));
     return CSLAM_OK;
 }

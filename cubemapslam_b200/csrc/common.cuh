@@ -39,6 +39,58 @@ static int dev_alloc(std::vector<void*>& owned, T** p, size_t count, bool zero) 
     return 0;
 }
 
+// Device memory of a handle's single calls (staged inputs, outputs, scratch), carved from chunks the handle keeps across calls: cudaMalloc /
+// cudaFree per call would cost more than many of the calls themselves. Pieces are 256-byte aligned and go to the first chunk with room; a new
+// chunk is max(request, minimum) bytes, so a call sequence of fixed shape lands on the same pieces every time and stops allocating after its
+// first call. Rules:
+// - Only public entry points call reset(), and only on entry, before anything is taken. All of a handle's work runs on its one stream, so a
+//   piece is reused only by work enqueued after the work that last used it.
+// - A function that another entry point calls never resets: a host form that called a resetting _dev form would give its staged inputs
+//   away to the _dev form's scratch.
+// - Every fill or copy into arena memory is cudaMemsetAsync / cudaMemcpyAsync on the handle's stream. A legacy-stream cudaMemset /
+//   cudaMemcpy does not order against a non-blocking stream.
+// - Chunks are freed only by the destructor: cudaFree synchronises the device, and a _dev call may still be in flight.
+class DevArena {
+  public:
+    DevArena() = default;
+    DevArena(const DevArena&) = delete;
+    DevArena& operator=(const DevArena&) = delete;
+    ~DevArena() { for (auto& c : chunks) cudaFree(c.p); }
+    void bind(cudaStream_t s, size_t minChunk) { stream = s; minBytes = minChunk; }   // once, when the handle's stream exists
+    void reset() { for (auto& c : chunks) c.used = 0; }
+    // `count` elements (at least one); zero: cleared on the stream
+    template <class T>
+    int take(T** p, size_t count, bool zero = false) {
+        const size_t bytes = (std::max<size_t>(count, 1) * sizeof(T) + 255) & ~(size_t)255;
+        char* q = nullptr;
+        for (auto& c : chunks) if (c.size - c.used >= bytes) { q = c.p + c.used; c.used += bytes; break; }
+        if (!q) {
+            Chunk c; c.size = std::max(bytes, minBytes); c.used = bytes;
+            CSLAM_CUDA(cudaMalloc((void**)&c.p, c.size));
+            chunks.push_back(c); q = c.p;
+        }
+        if (zero) CSLAM_CUDA(cudaMemsetAsync(q, 0, bytes, stream));
+        *p = (T*)q;
+        return 0;
+    }
+    // take + one host-to-device copy of `count` elements
+    template <class T>
+    int upload(const T** p, const T* host, size_t count) {
+        T* q = nullptr;
+        const int rc = take(&q, count);
+        if (rc) return rc;
+        if (count) CSLAM_CUDA(cudaMemcpyAsync(q, host, count * sizeof(T), cudaMemcpyHostToDevice, stream));
+        *p = q;
+        return 0;
+    }
+
+  private:
+    struct Chunk { char* p; size_t size, used; };
+    std::vector<Chunk> chunks;
+    cudaStream_t stream = nullptr;
+    size_t minBytes = 0;
+};
+
 // Optional per-kernel timing of a handle (cslam_*_set_timing / cslam_*_get_timing): record() puts an event on the stream before each
 // launch, and collect() adds the time from every event to the next one to the kind of the earlier event. A handle records END after its
 // last launch; the interval that starts there (up to the next call's first launch) belongs to no kernel and is not counted.

@@ -260,23 +260,9 @@ struct cslam_mapper {
     int device = 0;
     cudaStream_t stream = nullptr;
     cslam_tracker* trk = nullptr;   // for the frame index of the key frame (k_frame_index)
-    // growable device scratch for the host entry points
-    struct Buf { void* p = nullptr; size_t cap = 0; };
-    Buf b[16];
+    DevArena arena;                 // staging of the host entry points
     int64_t launches = 0;
 };
-template <class T> static int mbuf(cslam_mapper* m, int slot, size_t count, T** out) {
-    const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
-    cslam_mapper::Buf& B = m->b[slot];
-    if (B.cap < bytes) {
-        if (B.p) cudaFree(B.p);
-        B.p = nullptr; B.cap = 0;
-        CSLAM_CUDA(cudaMalloc(&B.p, bytes * 2));
-        B.cap = bytes * 2;
-    }
-    *out = (T*)B.p;
-    return 0;
-}
 
 extern "C" int cslam_mapper_create(cslam_mapper** out, int device) {
     if (!out) return CSLAM_E_BADARG;
@@ -286,6 +272,7 @@ extern "C" int cslam_mapper_create(cslam_mapper** out, int device) {
     rc = cslam_tracker_create(&m->trk, device, 1, 4096);
     if (rc) { delete m; return rc; }
     m->stream = (cudaStream_t)cslam_tracker_stream(m->trk);   // one stream: the frame index and the searches are ordered
+    m->arena.bind(m->stream, (size_t)1 << 20);
     cudaFuncSetAttribute(k_triangulation, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 4);
     *out = m;
     return CSLAM_OK;
@@ -294,7 +281,6 @@ extern "C" void cslam_mapper_destroy(cslam_mapper* m) {
     if (!m) return;
     cudaSetDevice(m->device);
     if (m->stream) cudaStreamSynchronize(m->stream);
-    for (auto& B : m->b) if (B.p) cudaFree(B.p);
     cslam_tracker_destroy(m->trk);
     delete m;
 }
@@ -305,11 +291,11 @@ extern "C" int cslam_distinctive_descriptors(cslam_mapper* m, const uint8_t* des
     if (n_points == 0) return CSLAM_OK;
     for (int p = 0; p < n_points; p++) if (offset[p + 1] < offset[p] || offset[p] < 0) { set_error("cslam_distinctive_descriptors: offsets must be non-decreasing"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(m->device));
+    m->arena.reset();
     const size_t total = (size_t)offset[n_points];
-    uint8_t* dD; int32_t* dO; int32_t* dB; int rc;
-    if ((rc = mbuf(m, 0, total * 32 + 32, &dD)) || (rc = mbuf(m, 1, (size_t)n_points + 1, &dO)) || (rc = mbuf(m, 2, (size_t)n_points, &dB))) return rc;
+    uint8_t* dD; const int32_t* dO; int32_t* dB; int rc;
+    if ((rc = m->arena.take(&dD, total * 32 + 32)) || (rc = m->arena.upload(&dO, offset, (size_t)n_points + 1)) || (rc = m->arena.take(&dB, n_points))) return rc;
     if (total) CSLAM_CUDA(cudaMemcpyAsync(dD, desc, total * 32, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(dO, offset, ((size_t)n_points + 1) * 4, cudaMemcpyHostToDevice, m->stream));
     k_distinctive<<<n_points, DD_THREADS, 0, m->stream>>>(dD, dO, dB); m->launches++;
     CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(best, dB, (size_t)n_points * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -325,21 +311,14 @@ extern "C" int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, co
     if (n_mp == 0) return CSLAM_OK;
     for (int i = 0; i < n_mp; i++) if (mp_valid[i] && (mp_level[i] < 0 || mp_level[i] >= nlevels)) { set_error("cslam_fuse_search: predicted level out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(m->device));
-    cslam_keypoint* dK; uint8_t* dD; int32_t* dN; uint16_t* dCS; uint16_t* dCI; uint8_t* dV; float* dX; int32_t* dL; uint8_t* dM; int32_t* dBI; int32_t* dBD; int rc;
+    m->arena.reset();
+    DevArena& a = m->arena;
     const int cap = std::max(n_kf, 1);
-    if ((rc = mbuf(m, 0, (size_t)cap, &dK)) || (rc = mbuf(m, 1, (size_t)cap * 32, &dD)) || (rc = mbuf(m, 2, 1, &dN)) || (rc = mbuf(m, 3, (size_t)MAP_NCELLS + 1, &dCS)) ||
-        (rc = mbuf(m, 4, (size_t)cap, &dCI)) || (rc = mbuf(m, 5, (size_t)n_mp, &dV)) || (rc = mbuf(m, 6, (size_t)n_mp * 3, &dX)) || (rc = mbuf(m, 7, (size_t)n_mp, &dL)) ||
-        (rc = mbuf(m, 8, (size_t)n_mp * 32, &dM)) || (rc = mbuf(m, 9, (size_t)n_mp, &dBI)) || (rc = mbuf(m, 10, (size_t)n_mp, &dBD))) return rc;
-    if (n_kf) {
-        CSLAM_CUDA(cudaMemcpyAsync(dK, k_kf, (size_t)n_kf * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, m->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(dD, d_kf, (size_t)n_kf * 32, cudaMemcpyHostToDevice, m->stream));
-    }
-    CSLAM_CUDA(cudaMemcpyAsync(dN, &n_kf, 4, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(dV, mp_valid, (size_t)n_mp, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(dX, mp_xw, (size_t)n_mp * 12, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(dL, mp_level, (size_t)n_mp * 4, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(dM, mp_desc, (size_t)n_mp * 32, cudaMemcpyHostToDevice, m->stream));
-    if ((rc = cslam_frame_index_dev(m->trk, dK, dN, 1, cap, face_w, face_h, nullptr, dCS, dCI))) return rc;
+    const cslam_keypoint* dK; const uint8_t *dD, *dV, *dM; const int32_t *dN, *dL; const float* dX; uint16_t *dCS, *dCI; int32_t *dBI, *dBD; int rc;
+    if ((rc = a.upload(&dK, k_kf, n_kf)) || (rc = a.upload(&dD, d_kf, (size_t)n_kf * 32)) || (rc = a.upload(&dN, &n_kf, 1)) || (rc = a.take(&dCS, MAP_NCELLS + 1)) ||
+        (rc = a.take(&dCI, cap)) || (rc = a.upload(&dV, mp_valid, n_mp)) || (rc = a.upload(&dX, mp_xw, (size_t)n_mp * 3)) || (rc = a.upload(&dL, mp_level, n_mp)) ||
+        (rc = a.upload(&dM, mp_desc, (size_t)n_mp * 32)) || (rc = a.take(&dBI, n_mp)) || (rc = a.take(&dBD, n_mp)) ||
+        (rc = cslam_frame_index_dev(m->trk, dK, dN, 1, cap, face_w, face_h, nullptr, dCS, dCI))) return rc;
     FuseArgs A;
     A.kKF = dK; A.dKF = dD; A.cellStart = dCS; A.cellIdx = dCI; A.nKF = n_kf;
     for (int i = 0; i < 12; i++) A.Tcw[i] = Tcw[i];
@@ -368,22 +347,15 @@ extern "C" int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const
     for (size_t i = 0; i < t1; i++) if (node1[i] < 0 || node1[i] >= (1 << 20) - 1) { set_error("cslam_search_for_triangulation: node ids must be in [0, 2^20 - 1)"); return CSLAM_E_BADARG; }
     for (size_t i = 0; i < t2; i++) if (node2[i] < 0 || node2[i] >= (1 << 20) - 1) { set_error("cslam_search_for_triangulation: node ids must be in [0, 2^20 - 1)"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(m->device));
-    TriArgs A; int rc;
-    cslam_keypoint *dK1, *dK2; uint8_t *dD1, *dD2, *dM1, *dM2; float *dR1, *dR2, *dO, *dT, *dE; int32_t *dN1, *dN2, *dC1, *dC2, *dOut, *dNm;
-    if ((rc = mbuf(m, 0, t1, &dK1)) || (rc = mbuf(m, 1, t1 * 32, &dD1)) || (rc = mbuf(m, 2, t1 * 3, &dR1)) || (rc = mbuf(m, 3, t1, &dM1)) || (rc = mbuf(m, 4, t1, &dN1)) ||
-        (rc = mbuf(m, 5, t2, &dK2)) || (rc = mbuf(m, 6, t2 * 32, &dD2)) || (rc = mbuf(m, 7, t2 * 3, &dR2)) || (rc = mbuf(m, 8, t2, &dM2)) || (rc = mbuf(m, 9, t2, &dN2)) ||
-        (rc = mbuf(m, 10, (size_t)npairs * 2, &dC1)) || (rc = mbuf(m, 11, (size_t)npairs * 28, &dO)) || (rc = mbuf(m, 12, t1, &dOut)) || (rc = mbuf(m, 13, (size_t)npairs, &dNm))) return rc;
-    dC2 = dC1 + npairs; dT = dO + (size_t)npairs * 3; dE = dT + (size_t)npairs * 16;
+    m->arena.reset();
+    DevArena& a = m->arena;
+    const cslam_keypoint *dK1, *dK2; const uint8_t *dD1, *dD2, *dM1, *dM2; const float *dR1, *dR2, *dO, *dT, *dE; const int32_t *dN1, *dN2, *dC1, *dC2; int32_t *dOut, *dNm; int rc;
+    if ((rc = a.upload(&dK1, k1, t1)) || (rc = a.upload(&dD1, d1, t1 * 32)) || (rc = a.upload(&dR1, rays1, t1 * 3)) || (rc = a.upload(&dM1, has_mp1, t1)) || (rc = a.upload(&dN1, node1, t1)) ||
+        (rc = a.upload(&dK2, k2, t2)) || (rc = a.upload(&dD2, d2, t2 * 32)) || (rc = a.upload(&dR2, rays2, t2 * 3)) || (rc = a.upload(&dM2, has_mp2, t2)) || (rc = a.upload(&dN2, node2, t2)) ||
+        (rc = a.upload(&dC1, n1, npairs)) || (rc = a.upload(&dC2, n2, npairs)) || (rc = a.upload(&dO, Ow1, (size_t)npairs * 3)) || (rc = a.upload(&dT, Tcw2, (size_t)npairs * 16)) ||
+        (rc = a.upload(&dE, E12, (size_t)npairs * 9)) || (rc = a.take(&dOut, t1)) || (rc = a.take(&dNm, npairs))) return rc;
     const cudaStream_t st = m->stream;
-    CSLAM_CUDA(cudaMemcpyAsync(dK1, k1, t1 * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dD1, d1, t1 * 32, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dR1, rays1, t1 * 12, cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dM1, has_mp1, t1, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dN1, node1, t1 * 4, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dK2, k2, t2 * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dD2, d2, t2 * 32, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dR2, rays2, t2 * 12, cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dM2, has_mp2, t2, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dN2, node2, t2 * 4, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dC1, n1, (size_t)npairs * 4, cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dC2, n2, (size_t)npairs * 4, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dO, Ow1, (size_t)npairs * 12, cudaMemcpyHostToDevice, st)); CSLAM_CUDA(cudaMemcpyAsync(dT, Tcw2, (size_t)npairs * 64, cudaMemcpyHostToDevice, st));
-    CSLAM_CUDA(cudaMemcpyAsync(dE, E12, (size_t)npairs * 36, cudaMemcpyHostToDevice, st));
+    TriArgs A;
     A.k1 = dK1; A.d1 = dD1; A.rays1 = dR1; A.hasMP1 = dM1; A.node1 = dN1; A.n1 = dC1; A.s1 = stride1;
     A.k2 = dK2; A.d2 = dD2; A.rays2 = dR2; A.hasMP2 = dM2; A.node2 = dN2; A.n2 = dC2; A.s2 = stride2;
     A.Ow1 = dO; A.Tcw2 = dT; A.E12 = dE; A.W = face_w; A.H = face_h; A.checkOri = check_orientation ? 1 : 0;

@@ -330,31 +330,19 @@ using namespace cslam;
 struct cslam_matcher {
     int device = 0, maxPairs = 0, maxFeat = 0;
     cudaStream_t stream = nullptr;
-    uint8_t *dA = nullptr, *dB = nullptr, *dValid = nullptr;
-    float *aA = nullptr, *aB = nullptr;
-    int32_t *nodeA = nullptr, *nodeB = nullptr, *dMatch = nullptr, *dDist = nullptr, *dSecond = nullptr, *dN = nullptr;
-    cslam_keypoint* dKps = nullptr;   // staging of cslam_match_frames (lazily allocated)
-    int* dHist = nullptr;             // per-pair rotation histogram of the row-split brute-force launches (lazily allocated)
-    std::vector<void*> owned;
+    DevArena arena;   // staging of the host entry points, the row-split histogram and the micro-benchmarks' output sink
     int64_t launches = 0;
 };
 
 extern "C" int cslam_matcher_create(cslam_matcher** out, int device, int max_pairs, int max_features) {
     if (!out || max_pairs <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_matcher_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
-    int rc = check_device(device);
+    const int rc = check_device(device);
     if (rc) return rc;
     cslam_matcher* m = new cslam_matcher;
     m->device = device; m->maxPairs = max_pairs; m->maxFeat = max_features;
-    const size_t nf = (size_t)max_pairs * max_features;
     if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); cslam_matcher_destroy(m); return CSLAM_E_CUDA; }
-    std::vector<void*>& o = m->owned;
-    if ((rc = dev_alloc(o, &m->dA, nf * 32, false)) || (rc = dev_alloc(o, &m->dB, nf * 32, false)) || (rc = dev_alloc(o, &m->dValid, nf, false)) ||
-        (rc = dev_alloc(o, &m->aA, nf, false)) || (rc = dev_alloc(o, &m->aB, nf, false)) || (rc = dev_alloc(o, &m->nodeA, nf, false)) || (rc = dev_alloc(o, &m->nodeB, nf, false)) ||
-        (rc = dev_alloc(o, &m->dMatch, nf, false)) || (rc = dev_alloc(o, &m->dDist, nf, false)) || (rc = dev_alloc(o, &m->dSecond, nf, false)) ||
-        (rc = dev_alloc(o, &m->dN, max_pairs, false))) {
-        cslam_matcher_destroy(m);
-        return rc;
-    }
+    // chunks: room for both descriptor sets, a flag and seven 4-byte arrays per feature at the handle's limits, at most 64 MB
+    m->arena.bind(m->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_pairs * max_features * (2 * 32 + 1 + 7 * 4) + (size_t)max_pairs * 4));
     cudaFuncSetAttribute(k_search_by_bow, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
     *out = m;
     return CSLAM_OK;
@@ -364,7 +352,6 @@ extern "C" void cslam_matcher_destroy(cslam_matcher* m) {
     if (!m) return;
     cudaSetDevice(m->device);
     if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-    for (void* p : m->owned) cudaFree(p);
     delete m;
 }
 extern "C" void* cslam_matcher_stream(const cslam_matcher* m) { return m ? (void*)m->stream : nullptr; }
@@ -376,16 +363,25 @@ extern "C" int cslam_matcher_sync(cslam_matcher* m) {
     return CSLAM_OK;
 }
 
-// CTAs per pair of a brute-force launch: one per BF_ROWS rows of the largest A a pair can have; the per-pair histogram buffer is zeroed here
-static int bf_split(cslam_matcher* m, int maxRowsA, int npairs, int* parts, int** gHist) {
-    *parts = std::max(1, cdiv(maxRowsA, BF_ROWS));
-    *gHist = nullptr;
-    if (*parts > 1) {
-        if (!m->dHist) { const int rc = dev_alloc(m->owned, &m->dHist, (size_t)m->maxPairs * 32, false); if (rc) return rc; }
-        CSLAM_CUDA(cudaMemsetAsync(m->dHist, 0, (size_t)npairs * 32 * sizeof(int), m->stream));
-        *gHist = m->dHist;
-    }
+// The brute-force launch of every entry point: one CTA per BF_ROWS rows of the largest A a pair can have (L.strideA); with more than one, the
+// per-pair rotation histogram is a zeroed arena piece.
+static int bf_launch(cslam_matcher* m, int npairs, const uint8_t* descA, const float* angA, int nA, const uint8_t* descB, const float* angB, int nB, float nnratio,
+                     int th_low, int check_ori, int32_t* match12, int32_t* dist12, int32_t* second12, int32_t* nmatches, const BfLayout& L) {
+    const int parts = std::max(1, cdiv(L.strideA, BF_ROWS));
+    int* gHist = nullptr;
+    if (parts > 1) { const int rc = m->arena.take(&gHist, (size_t)npairs * 32, true); if (rc) return rc; }
+    k_match_bruteforce<<<dim3(npairs, parts), BF_THREADS, 0, m->stream>>>(descA, angA, nA, descB, angB, nB, nnratio, th_low, check_ori, match12, dist12, second12, nmatches, L, gHist);
+    m->launches++;
+    CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;
+}
+// frame f of a front-end batch (rows [f*kp_stride, f*kp_stride + n[f]) of kps / desc) against frame f+1, for f = 0 .. nframes-2
+static int frames_launch(cslam_matcher* m, const cslam_keypoint* kps, const uint8_t* desc, const int32_t* n, int kp_stride, int nframes, float nnratio, int th_low,
+                         int check_ori, int32_t* match12, int32_t* nmatches) {
+    const float* ang = &kps[0].angle;
+    const BfLayout L = {kp_stride, kp_stride, (int)(sizeof(cslam_keypoint) / sizeof(float)), n, n + 1};
+    return bf_launch(m, nframes - 1, desc, ang, 0, desc + (size_t)kp_stride * 32, ang + (size_t)kp_stride * L.angStride, 0, nnratio, th_low, check_ori, match12, nullptr,
+                     nullptr, nmatches, L);
 }
 
 static int check_sizes(cslam_matcher* m, int nA, int nB, int npairs) {
@@ -403,31 +399,27 @@ extern "C" int cslam_match_bruteforce_dev(cslam_matcher* m, const uint8_t* descA
     int rc = check_sizes(m, nA, nB, npairs);
     if (rc) return rc;
     if (nA == 0) { CSLAM_CUDA(cudaMemsetAsync(nmatches, 0, (size_t)npairs * 4, m->stream)); return CSLAM_OK; }
-    const BfLayout L = {nA, nB, 1, nullptr, nullptr};
-    int parts, *gHist;
-    rc = bf_split(m, nA, npairs, &parts, &gHist);
-    if (rc) return rc;
-    k_match_bruteforce<<<dim3(npairs, parts), BF_THREADS, 0, m->stream>>>(descA, angA, nA, descB, angB, nB, nnratio, th_low, check_ori, match12, dist12, second12, nmatches, L, gHist);
-    m->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    return CSLAM_OK;
+    m->arena.reset();
+    return bf_launch(m, npairs, descA, angA, nA, descB, angB, nB, nnratio, th_low, check_ori, match12, dist12, second12, nmatches, {nA, nB, 1, nullptr, nullptr});
 }
 
 extern "C" int cslam_match_bruteforce(cslam_matcher* m, const uint8_t* descA, const float* angA, int nA, const uint8_t* descB, const float* angB, int nB, int npairs,
                                       float nnratio, int th_low, int check_ori, int32_t* match12, int32_t* dist12, int32_t* second12, int32_t* nmatches) {
     int rc = check_sizes(m, nA, nB, npairs);
     if (rc) return rc;
+    m->arena.reset();
     const size_t na = (size_t)npairs * nA, nb = (size_t)npairs * nB;
-    if (na) { CSLAM_CUDA(cudaMemcpyAsync(m->dA, descA, na * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aA, angA, na * 4, cudaMemcpyHostToDevice, m->stream)); }
-    if (nb) { CSLAM_CUDA(cudaMemcpyAsync(m->dB, descB, nb * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aB, angB, nb * 4, cudaMemcpyHostToDevice, m->stream)); }
-    rc = cslam_match_bruteforce_dev(m, m->dA, m->aA, nA, m->dB, m->aB, nB, npairs, nnratio, th_low, check_ori, m->dMatch, m->dDist, m->dSecond, m->dN);
-    if (rc) return rc;
+    const uint8_t *dA, *dB; const float *aA, *aB; int32_t *dMatch, *dDist, *dSecond, *dN;
+    if ((rc = m->arena.upload(&dA, descA, na * 32)) || (rc = m->arena.upload(&aA, angA, na)) || (rc = m->arena.upload(&dB, descB, nb * 32)) || (rc = m->arena.upload(&aB, angB, nb)) ||
+        (rc = m->arena.take(&dMatch, na)) || (rc = m->arena.take(&dDist, na)) || (rc = m->arena.take(&dSecond, na)) || (rc = m->arena.take(&dN, npairs))) return rc;
+    if (nA == 0) CSLAM_CUDA(cudaMemsetAsync(dN, 0, (size_t)npairs * 4, m->stream));
+    else if ((rc = bf_launch(m, npairs, dA, aA, nA, dB, aB, nB, nnratio, th_low, check_ori, dMatch, dDist, dSecond, dN, {nA, nB, 1, nullptr, nullptr}))) return rc;
     if (na) {
-        CSLAM_CUDA(cudaMemcpyAsync(match12, m->dMatch, na * 4, cudaMemcpyDeviceToHost, m->stream));
-        if (dist12) CSLAM_CUDA(cudaMemcpyAsync(dist12, m->dDist, na * 4, cudaMemcpyDeviceToHost, m->stream));
-        if (second12) CSLAM_CUDA(cudaMemcpyAsync(second12, m->dSecond, na * 4, cudaMemcpyDeviceToHost, m->stream));
+        CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, na * 4, cudaMemcpyDeviceToHost, m->stream));
+        if (dist12) CSLAM_CUDA(cudaMemcpyAsync(dist12, dDist, na * 4, cudaMemcpyDeviceToHost, m->stream));
+        if (second12) CSLAM_CUDA(cudaMemcpyAsync(second12, dSecond, na * 4, cudaMemcpyDeviceToHost, m->stream));
     }
-    CSLAM_CUDA(cudaMemcpyAsync(nmatches, m->dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(nmatches, dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
     return CSLAM_OK;
 }
@@ -441,16 +433,8 @@ extern "C" int cslam_match_frames_dev(cslam_matcher* m, const cslam_keypoint* kp
         return CSLAM_E_BADARG;
     }
     CSLAM_CUDA(cudaSetDevice(m->device));
-    const float* ang = &kps[0].angle;
-    const BfLayout L = {kp_stride, kp_stride, (int)(sizeof(cslam_keypoint) / sizeof(float)), n, n + 1};
-    int parts, *gHist;
-    const int rc = bf_split(m, kp_stride, nframes - 1, &parts, &gHist);
-    if (rc) return rc;
-    k_match_bruteforce<<<dim3(nframes - 1, parts), BF_THREADS, 0, m->stream>>>(desc, ang, 0, desc + (size_t)kp_stride * 32, ang + (size_t)kp_stride * L.angStride, 0, nnratio, th_low,
-                                                                                check_ori, match12, nullptr, nullptr, nmatches, L, gHist);
-    m->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    return CSLAM_OK;
+    m->arena.reset();
+    return frames_launch(m, kps, desc, n, kp_stride, nframes, nnratio, th_low, check_ori, match12, nmatches);
 }
 
 // host buffers in / out (copies inside, synchronous): kps / desc / n as cslam_frontend_run returns them
@@ -458,15 +442,13 @@ extern "C" int cslam_match_frames(cslam_matcher* m, const cslam_keypoint* kps, c
                                   int check_ori, int32_t* match12, int32_t* nmatches) {
     if (!m || nframes < 2 || nframes > m->maxPairs || kp_stride <= 0 || kp_stride > m->maxFeat) { set_error("cslam_match_frames: sizes out of range (frames %d/%d, stride %d/%d)", nframes, m ? m->maxPairs : 0, kp_stride, m ? m->maxFeat : 0); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(m->device));
-    const size_t nf = (size_t)nframes * kp_stride;
-    if (!m->dKps) { const int rc = dev_alloc(m->owned, &m->dKps, (size_t)m->maxPairs * m->maxFeat, false); if (rc) return rc; }
-    CSLAM_CUDA(cudaMemcpyAsync(m->dKps, kps, nf * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->dA, desc, nf * 32, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->nodeA, n, (size_t)nframes * 4, cudaMemcpyHostToDevice, m->stream));
-    int rc = cslam_match_frames_dev(m, m->dKps, m->dA, m->nodeA, kp_stride, nframes, nnratio, th_low, check_ori, m->dMatch, m->dN);
-    if (rc) return rc;
-    CSLAM_CUDA(cudaMemcpyAsync(match12, m->dMatch, (size_t)(nframes - 1) * kp_stride * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(nmatches, m->dN, (size_t)(nframes - 1) * 4, cudaMemcpyDeviceToHost, m->stream));
+    m->arena.reset();
+    const size_t nf = (size_t)nframes * kp_stride, nm = (size_t)(nframes - 1) * kp_stride;
+    const cslam_keypoint* dK; const uint8_t* dD; const int32_t* dN; int32_t *dMatch, *dNm; int rc;
+    if ((rc = m->arena.upload(&dK, kps, nf)) || (rc = m->arena.upload(&dD, desc, nf * 32)) || (rc = m->arena.upload(&dN, n, nframes)) || (rc = m->arena.take(&dMatch, nm)) ||
+        (rc = m->arena.take(&dNm, nframes - 1)) || (rc = frames_launch(m, dK, dD, dN, kp_stride, nframes, nnratio, th_low, check_ori, dMatch, dNm))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, nm * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)(nframes - 1) * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
     return CSLAM_OK;
 }
@@ -478,7 +460,9 @@ static int time_ubench(cslam_matcher* m, int iters, Launch launch, int* blocks, 
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
     *blocks = sms * 8;
-    uint32_t* out = reinterpret_cast<uint32_t*>(m->dN);
+    uint32_t* out;
+    const int rc = m->arena.take(&out, 1);
+    if (rc) return rc;
     cudaEvent_t e0, e1;
     CSLAM_CUDA(cudaEventCreate(&e0)); CSLAM_CUDA(cudaEventCreate(&e1));
     launch(*blocks, 100, out);   // warm-up
@@ -510,6 +494,7 @@ __global__ void __launch_bounds__(256) k_ubench_popc(uint32_t* out, int iters, u
 extern "C" int cslam_ubench_popc(cslam_matcher* m, double* popc32_per_s) {
     if (!m || !popc32_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
+    m->arena.reset();
     const int iters = 20000;
     int blocks; float ms;
     const int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_popc<<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
@@ -548,6 +533,7 @@ __global__ void __launch_bounds__(256) k_ubench_mma(uint32_t* out, int iters, ui
 extern "C" int cslam_ubench_bmma(cslam_matcher* m, double* bmma_products_per_s, double* imma_products_per_s) {
     if (!m || !bmma_products_per_s || !imma_products_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
+    m->arena.reset();
     const int iters = 4000;
     int blocks; float ms;
     int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_mma<true><<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
@@ -580,11 +566,25 @@ __global__ void __launch_bounds__(256) k_ubench_minmax3(uint32_t* out, int iters
 extern "C" int cslam_ubench_minmax3(cslam_matcher* m, double* ops_per_s) {
     if (!m || !ops_per_s) return CSLAM_E_BADARG;
     CSLAM_CUDA(cudaSetDevice(m->device));
+    m->arena.reset();
     const int iters = 20000;
     int blocks; float ms;
     const int rc = time_ubench(m, iters, [&](int b, int it, uint32_t* out) { k_ubench_minmax3<<<b, 256, 0, m->stream>>>(out, it, 1u); }, &blocks, &ms);
     if (rc) return rc;
     *ops_per_s = (double)blocks * 256.0 * iters * 8.0 / (ms * 1e-3);   // warp-lane u16x2 3-input min/max per second
+    return CSLAM_OK;
+}
+
+// SearchByBoW launch of both forms. valid_f == nullptr: (KeyFrame, Frame), output per F feature; else (KeyFrame, KeyFrame) with the second
+// key frame's valid flags, output per KF feature.
+static int bow_launch(cslam_matcher* m, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid, const int32_t* node_kf, int nKF, const uint8_t* descF,
+                      const float* angF, const int32_t* node_f, int nF, const uint8_t* valid_f, int npairs, float nnratio, int check_ori, int32_t* match, int32_t* nmatches) {
+    const int n2K = pow2_at_least(nKF), n2F = pow2_at_least(nF);
+    const size_t smem = (size_t)(n2K + n2F + nF) * 4;
+    k_search_by_bow<<<npairs, BOW_THREADS, smem, m->stream>>>(descKF, angKF, kf_valid, node_kf, nKF, descF, angF, node_f, nF, n2K, n2F, nnratio, check_ori, match, nmatches,
+                                                              valid_f, valid_f ? 1 : 0);
+    m->launches++;
+    CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;
 }
 
@@ -598,12 +598,7 @@ extern "C" int cslam_search_by_bow_dev(cslam_matcher* m, const uint8_t* descKF, 
         if (nF) CSLAM_CUDA(cudaMemsetAsync(match_f, 0xff, (size_t)npairs * nF * 4, m->stream));
         return CSLAM_OK;
     }
-    const int n2K = pow2_at_least(nKF), n2F = pow2_at_least(nF);
-    const size_t smem = (size_t)(n2K + n2F + nF) * 4;
-    k_search_by_bow<<<npairs, BOW_THREADS, smem, m->stream>>>(descKF, angKF, kf_valid, node_kf, nKF, descF, angF, node_f, nF, n2K, n2F, nnratio, check_ori, match_f, nmatches, nullptr, 0);
-    m->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    return CSLAM_OK;
+    return bow_launch(m, descKF, angKF, kf_valid, node_kf, nKF, descF, angF, node_f, nF, nullptr, npairs, nnratio, check_ori, match_f, nmatches);
 }
 
 extern "C" int cslam_search_by_bow(cslam_matcher* m, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid, const int32_t* node_kf, int nKF,
@@ -611,19 +606,15 @@ extern "C" int cslam_search_by_bow(cslam_matcher* m, const uint8_t* descKF, cons
                                    int32_t* nmatches) {
     int rc = check_sizes(m, nKF, nF, npairs);
     if (rc) return rc;
+    m->arena.reset();
     const size_t nk = (size_t)npairs * nKF, nf = (size_t)npairs * nF;
-    if (nk) {
-        CSLAM_CUDA(cudaMemcpyAsync(m->dA, descKF, nk * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aA, angKF, nk * 4, cudaMemcpyHostToDevice, m->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(m->dValid, kf_valid, nk, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->nodeA, node_kf, nk * 4, cudaMemcpyHostToDevice, m->stream));
-    }
-    if (nf) {
-        CSLAM_CUDA(cudaMemcpyAsync(m->dB, descF, nf * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aB, angF, nf * 4, cudaMemcpyHostToDevice, m->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(m->nodeB, node_f, nf * 4, cudaMemcpyHostToDevice, m->stream));
-    }
-    rc = cslam_search_by_bow_dev(m, m->dA, m->aA, m->dValid, m->nodeA, nKF, m->dB, m->aB, m->nodeB, nF, npairs, nnratio, check_ori, m->dMatch, m->dN);
-    if (rc) return rc;
-    if (nf) CSLAM_CUDA(cudaMemcpyAsync(match_f, m->dMatch, nf * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(nmatches, m->dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
+    const uint8_t *dK, *dValid, *dF; const float *aK, *aF; const int32_t *nodeK, *nodeF; int32_t *dMatch, *dN;
+    if ((rc = m->arena.upload(&dK, descKF, nk * 32)) || (rc = m->arena.upload(&aK, angKF, nk)) || (rc = m->arena.upload(&dValid, kf_valid, nk)) ||
+        (rc = m->arena.upload(&nodeK, node_kf, nk)) || (rc = m->arena.upload(&dF, descF, nf * 32)) || (rc = m->arena.upload(&aF, angF, nf)) ||
+        (rc = m->arena.upload(&nodeF, node_f, nf)) || (rc = m->arena.take(&dMatch, nf)) || (rc = m->arena.take(&dN, npairs)) ||
+        (rc = cslam_search_by_bow_dev(m, dK, aK, dValid, nodeK, nKF, dF, aF, nodeF, nF, npairs, nnratio, check_ori, dMatch, dN))) return rc;
+    if (nf) CSLAM_CUDA(cudaMemcpyAsync(match_f, dMatch, nf * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(nmatches, dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
     return CSLAM_OK;
 }
@@ -632,11 +623,12 @@ extern "C" int cslam_hamming(cslam_matcher* m, const uint8_t* a, const uint8_t* 
     if (!m || n < 0 || (size_t)n > (size_t)m->maxPairs * m->maxFeat) { set_error("cslam_hamming: n out of range"); return CSLAM_E_BADARG; }
     if (n == 0) return CSLAM_OK;
     CSLAM_CUDA(cudaSetDevice(m->device));
-    CSLAM_CUDA(cudaMemcpyAsync(m->dA, a, (size_t)n * 32, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->dB, b, (size_t)n * 32, cudaMemcpyHostToDevice, m->stream));
-    k_hamming<<<cdiv(n, 256), 256, 0, m->stream>>>(m->dA, m->dB, n, m->dDist);
+    m->arena.reset();
+    const uint8_t *dA, *dB; int32_t* dDist; int rc;
+    if ((rc = m->arena.upload(&dA, a, (size_t)n * 32)) || (rc = m->arena.upload(&dB, b, (size_t)n * 32)) || (rc = m->arena.take(&dDist, n))) return rc;
+    k_hamming<<<cdiv(n, 256), 256, 0, m->stream>>>(dA, dB, n, dDist);
     m->launches++;
-    CSLAM_CUDA(cudaMemcpyAsync(dist, m->dDist, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(dist, dDist, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
     return CSLAM_OK;
 }
@@ -648,21 +640,15 @@ extern "C" int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, co
     int rc = check_sizes(m, n1, n2, npairs);
     if (rc) return rc;
     if (n1 == 0 || n2 == 0) { for (size_t i = 0; i < (size_t)npairs * n1; i++) match12[i] = -1; for (int p = 0; p < npairs; p++) nmatches[p] = 0; return CSLAM_OK; }
+    m->arena.reset();
     const size_t k1 = (size_t)npairs * n1, k2 = (size_t)npairs * n2;
-    CSLAM_CUDA(cudaMemcpyAsync(m->dA, desc1, k1 * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aA, ang1, k1 * 4, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->dValid, valid1, k1, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->nodeA, node1, k1 * 4, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->dB, desc2, k2 * 32, cudaMemcpyHostToDevice, m->stream)); CSLAM_CUDA(cudaMemcpyAsync(m->aB, ang2, k2 * 4, cudaMemcpyHostToDevice, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(m->nodeB, node2, k2 * 4, cudaMemcpyHostToDevice, m->stream));
-    uint8_t* dValid2 = reinterpret_cast<uint8_t*>(m->dSecond);   // scratch: second12 is unused by this entry point
-    CSLAM_CUDA(cudaMemcpyAsync(dValid2, valid2, k2, cudaMemcpyHostToDevice, m->stream));
-    const int n2K = pow2_at_least(n1), n2F = pow2_at_least(n2);
-    const size_t smem = (size_t)(n2K + n2F + n2) * 4;
-    k_search_by_bow<<<npairs, BOW_THREADS, smem, m->stream>>>(m->dA, m->aA, m->dValid, m->nodeA, n1, m->dB, m->aB, m->nodeB, n2, n2K, n2F, nnratio, check_ori, m->dMatch, m->dN,
-                                                              dValid2, 1);
-    m->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    CSLAM_CUDA(cudaMemcpyAsync(match12, m->dMatch, k1 * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(nmatches, m->dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
+    const uint8_t *dD1, *dV1, *dD2, *dV2; const float *dA1, *dA2; const int32_t *dN1, *dN2; int32_t *dMatch, *dNm;
+    if ((rc = m->arena.upload(&dD1, desc1, k1 * 32)) || (rc = m->arena.upload(&dA1, ang1, k1)) || (rc = m->arena.upload(&dV1, valid1, k1)) ||
+        (rc = m->arena.upload(&dN1, node1, k1)) || (rc = m->arena.upload(&dD2, desc2, k2 * 32)) || (rc = m->arena.upload(&dA2, ang2, k2)) ||
+        (rc = m->arena.upload(&dN2, node2, k2)) || (rc = m->arena.upload(&dV2, valid2, k2)) || (rc = m->arena.take(&dMatch, k1)) || (rc = m->arena.take(&dNm, npairs)) ||
+        (rc = bow_launch(m, dD1, dA1, dV1, dN1, n1, dD2, dA2, dN2, n2, dV2, npairs, nnratio, check_ori, dMatch, dNm))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, k1 * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaStreamSynchronize(m->stream));
     return CSLAM_OK;
 }

@@ -13,9 +13,7 @@ struct cslam_optimizer {
     cudaStream_t stream = nullptr;
     nccl_comm_t comm = nullptr; int rank = 0, nranks = 1;
     int64_t launches = 0;
-    // device arena: chunks are kept across calls (cudaMalloc/cudaFree per BA call cost more than the solve itself)
-    struct Chunk { char* p; size_t size, used; };
-    std::vector<Chunk> chunks;
+    cslam::DevArena arena;      // 64 MB chunks
     double* h_scal = nullptr;   // pinned, 16 doubles
     // host scratch of cslam_local_ba, kept across calls (fresh multi-megabyte vectors cost page faults on every call)
     struct HostScratch { std::vector<int> lmStart, perm, eMP, eKF, fill, peStart, peList; std::vector<double> X; } hs;
@@ -26,30 +24,6 @@ struct cslam_optimizer {
 };
 
 namespace cslam {
-
-template <class T>
-static int dalloc(cslam_optimizer* o, T** p, size_t count, bool zero = false) {
-    const size_t bytes = (std::max<size_t>(count, 1) * sizeof(T) + 255) & ~(size_t)255;
-    char* q = nullptr;
-    for (auto& c : o->chunks) if (c.size - c.used >= bytes) { q = c.p + c.used; c.used += bytes; break; }
-    if (!q) {
-        cslam_optimizer::Chunk c; c.size = std::max<size_t>(bytes, (size_t)64 << 20); c.used = bytes;
-        CSLAM_CUDA(cudaMalloc((void**)&c.p, c.size));
-        o->chunks.push_back(c); q = c.p;
-    }
-    if (zero) CSLAM_CUDA(cudaMemsetAsync(q, 0, bytes, o->stream));
-    *p = (T*)q;
-    return 0;
-}
-template <class T>
-static int dupload(cslam_optimizer* o, const T** p, const std::vector<T>& v) {
-    T* q = nullptr; int rc = dalloc(o, &q, v.size());
-    if (rc) return rc;
-    if (!v.empty()) CSLAM_CUDA(cudaMemcpyAsync(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, o->stream));
-    *p = q;
-    return 0;
-}
-static inline void free_pool(cslam_optimizer* o) { for (auto& c : o->chunks) c.used = 0; }
 
 #ifdef __CUDACC__
 // fixed-shape (deterministic) block sum; result valid in thread 0. sh: >= 32 doubles

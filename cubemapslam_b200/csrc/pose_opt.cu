@@ -211,14 +211,14 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
     if (!o || nframes <= 0 || !offset || !Tcw || !inliers) { set_error("cslam_pose_optimization: bad argument"); return CSLAM_E_BADARG; }
     if (face_w != face_h || face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(o->device));
-    free_pool(o);
+    o->arena.reset();
     const int n = offset[nframes];
     PoseOptArgs A; std::memset(&A, 0, sizeof(A));
     int* d_off; float *d_T, *d_X, *d_kp, *d_w; uint8_t *d_out, *d_lvl; int32_t* d_inl; double *d_p64, *d_err;
     int rc;
-    if ((rc = dalloc(o, &d_off, nframes + 1)) || (rc = dalloc(o, &d_T, (size_t)nframes * 16)) || (rc = dalloc(o, &d_X, (size_t)n * 3)) || (rc = dalloc(o, &d_kp, (size_t)n * 2)) ||
-        (rc = dalloc(o, &d_w, n)) || (rc = dalloc(o, &d_out, n)) || (rc = dalloc(o, &d_lvl, n)) || (rc = dalloc(o, &d_inl, nframes)) || (rc = dalloc(o, &d_p64, (size_t)nframes * 7)) ||
-        (rc = dalloc(o, &d_err, (size_t)n * 2))) return rc;
+    if ((rc = o->arena.take(&d_off, nframes + 1)) || (rc = o->arena.take(&d_T, (size_t)nframes * 16)) || (rc = o->arena.take(&d_X, (size_t)n * 3)) || (rc = o->arena.take(&d_kp, (size_t)n * 2)) ||
+        (rc = o->arena.take(&d_w, n)) || (rc = o->arena.take(&d_out, n)) || (rc = o->arena.take(&d_lvl, n)) || (rc = o->arena.take(&d_inl, nframes)) || (rc = o->arena.take(&d_p64, (size_t)nframes * 7)) ||
+        (rc = o->arena.take(&d_err, (size_t)n * 2))) return rc;
     CSLAM_CUDA(cudaMemcpyAsync(d_off, offset, (nframes + 1) * 4, cudaMemcpyHostToDevice, o->stream));
     CSLAM_CUDA(cudaMemcpyAsync(d_T, Tcw, (size_t)nframes * 64, cudaMemcpyHostToDevice, o->stream));
     if (n) {
@@ -238,7 +238,6 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
     if (pose_fp64) CSLAM_CUDA(cudaMemcpyAsync(pose_fp64, d_p64, (size_t)nframes * 56, cudaMemcpyDeviceToHost, o->stream));
     CSLAM_CUDA(cudaStreamSynchronize(o->stream));
     for (int f = 0; f < nframes; f++) if (offset[f + 1] - offset[f] >= 3) std::memcpy(Tcw + 16 * f, Tout.data() + 16 * f, 64);
-    free_pool(o);
     return CSLAM_OK;
 }
 
@@ -248,11 +247,11 @@ extern "C" int cslam_pose_optimization_dev(cslam_optimizer* o, int nframes, int 
     if (!o || nframes <= 0 || stride <= 0 || !count || !Tcw || !Xw || !kp_xy || !inv_sigma2 || !outlier || !inliers) { set_error("cslam_pose_optimization_dev: bad argument"); return CSLAM_E_BADARG; }
     if (face_w != face_h || face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(o->device));
-    free_pool(o);
+    o->arena.reset();
     PoseOptArgs A; std::memset(&A, 0, sizeof(A));
     double* d_err; uint8_t* d_lvl; int rc;
     const size_t n = (size_t)nframes * stride;
-    if ((rc = dalloc(o, &d_err, n * 2)) || (rc = dalloc(o, &d_lvl, n))) return rc;
+    if ((rc = o->arena.take(&d_err, n * 2)) || (rc = o->arena.take(&d_lvl, n))) return rc;
     A.offset = nullptr; A.count = count; A.stride = stride; A.Tcw = Tcw; A.Xw = Xw; A.kpxy = kp_xy; A.invSigma2 = inv_sigma2; A.faceW = face_w; A.faceH = face_h;
     A.outlier = outlier; A.inliers = inliers; A.pose64 = nullptr; A.err = d_err; A.level = d_lvl;
     k_pose_opt<<<nframes, 256, 0, o->stream>>>(A); o->launches++;

@@ -308,11 +308,9 @@ extern "C" int cslam_area_rects(float x, float y, float r, int face_w, int face_
 struct cslam_tracker {
     int device = 0, maxFrames = 0, maxFeat = 0;
     cudaStream_t stream = nullptr;
-    // staging for the host entry points
-    cslam_keypoint *kCur = nullptr, *kLast = nullptr; uint8_t *dCur = nullptr, *dQ = nullptr, *valid = nullptr, *obs = nullptr, *taken = nullptr;
-    int32_t *nCur = nullptr, *nQ = nullptr, *level = nullptr, *match = nullptr, *nm = nullptr; float *Xw = nullptr, *Tcw = nullptr, *proj = nullptr, *vcos = nullptr, *rays = nullptr;
-    uint16_t *cellStart = nullptr, *cellIdx = nullptr; int* err = nullptr;
+    int* err = nullptr;   // CSLAM_E_CAPACITY once a search window overflowed; read and cleared by cslam_tracker_sync
     std::vector<void*> owned;
+    DevArena arena;       // staging of the host entry points
     int64_t launches = 0;
 };
 
@@ -321,14 +319,11 @@ extern "C" int cslam_tracker_create(cslam_tracker** out, int device, int max_fra
     int rc = check_device(device);
     if (rc) return rc;
     cslam_tracker* t = new cslam_tracker; t->device = device; t->maxFrames = max_frames; t->maxFeat = max_features;
-    const size_t nf = (size_t)max_frames * max_features;
     if (cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); delete t; return CSLAM_E_CUDA; }
-    auto talloc = [&](auto** p, size_t n) { return dev_alloc(t->owned, p, n, true); };   // every staging buffer starts zeroed
-    if ((rc = talloc(&t->kCur, nf)) || (rc = talloc(&t->kLast, nf)) || (rc = talloc(&t->dCur, nf * 32)) || (rc = talloc(&t->dQ, nf * 32)) || (rc = talloc(&t->valid, nf)) ||
-        (rc = talloc(&t->obs, nf)) || (rc = talloc(&t->taken, nf)) || (rc = talloc(&t->nCur, max_frames)) || (rc = talloc(&t->nQ, max_frames)) ||
-        (rc = talloc(&t->level, nf)) || (rc = talloc(&t->match, nf)) || (rc = talloc(&t->nm, max_frames)) || (rc = talloc(&t->Xw, nf * 3)) ||
-        (rc = talloc(&t->Tcw, (size_t)max_frames * 16)) || (rc = talloc(&t->proj, nf * 2)) || (rc = talloc(&t->vcos, nf)) || (rc = talloc(&t->rays, nf * 3)) ||
-        (rc = talloc(&t->cellStart, (size_t)max_frames * (NCELLS + 1))) || (rc = talloc(&t->cellIdx, nf)) || (rc = talloc(&t->err, 1))) { cslam_tracker_destroy(t); return rc; }
+    if ((rc = dev_alloc(t->owned, &t->err, 1, true))) { cslam_tracker_destroy(t); return rc; }
+    // chunks: room for every array the host calls stage at the handle's limits, at most 64 MB
+    const size_t perFeature = 2 * sizeof(cslam_keypoint) + 2 * 32 + 3 + 2 * 4 + 3 * 4 + 2 * 4 + 4 + 3 * 4 + 2, perFrame = 3 * 4 + 16 * 4 + (NCELLS + 1) * 2;
+    t->arena.bind(t->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * perFeature + (size_t)max_frames * perFrame));
     cudaFuncSetAttribute(k_frame_index, cudaFuncAttributeMaxDynamicSharedMemorySize, NCELLS * 4);
     *out = t;
     return CSLAM_OK;
@@ -376,14 +371,15 @@ extern "C" int cslam_frame_index(cslam_tracker* t, const cslam_keypoint* kps, co
                                  uint16_t* cell_idx) {
     if (!t || nframes <= 0 || nframes > t->maxFrames || kp_stride > t->maxFeat) { set_error("cslam_frame_index: sizes out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
+    t->arena.reset();
     const size_t nf = (size_t)nframes * kp_stride;
-    CSLAM_CUDA(cudaMemcpyAsync(t->kCur, kps, nf * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, t->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(t->nCur, n, nframes * 4, cudaMemcpyHostToDevice, t->stream));
-    int rc = cslam_frame_index_dev(t, t->kCur, t->nCur, nframes, kp_stride, face_w, face_h, t->rays, t->cellStart, t->cellIdx);
-    if (rc) return rc;
-    if (rays) CSLAM_CUDA(cudaMemcpyAsync(rays, t->rays, nf * 12, cudaMemcpyDeviceToHost, t->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(cell_start, t->cellStart, (size_t)nframes * (NCELLS + 1) * 2, cudaMemcpyDeviceToHost, t->stream));
-    CSLAM_CUDA(cudaMemcpyAsync(cell_idx, t->cellIdx, nf * 2, cudaMemcpyDeviceToHost, t->stream));
+    const cslam_keypoint* dK; const int32_t* dN; float* dR; uint16_t *dCS, *dCI; int rc;
+    if ((rc = t->arena.upload(&dK, kps, nf)) || (rc = t->arena.upload(&dN, n, nframes)) || (rc = t->arena.take(&dR, nf * 3)) ||
+        (rc = t->arena.take(&dCS, (size_t)nframes * (NCELLS + 1))) || (rc = t->arena.take(&dCI, nf)) ||
+        (rc = cslam_frame_index_dev(t, dK, dN, nframes, kp_stride, face_w, face_h, dR, dCS, dCI))) return rc;
+    if (rays) CSLAM_CUDA(cudaMemcpyAsync(rays, dR, nf * 12, cudaMemcpyDeviceToHost, t->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(cell_start, dCS, (size_t)nframes * (NCELLS + 1) * 2, cudaMemcpyDeviceToHost, t->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(cell_idx, dCI, nf * 2, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }
 
@@ -426,27 +422,26 @@ extern "C" int cslam_search_by_projection_local_dev(cslam_tracker* t, int nframe
     return CSLAM_OK;
 }
 
-// host entry points (one pair / frame per call batch; staging inside): what the drop-in ORBMatcher::SearchByProjection definitions call
+// host entry points (one pair / frame per call batch; staging inside): what the drop-in ORBMatcher::SearchByProjection definitions call. Every
+// array is uploaded at its exact size: the kernels read no row past a frame's count.
 extern "C" int cslam_search_by_projection_last(cslam_tracker* t, int npairs, const cslam_keypoint* k_cur, const uint8_t* d_cur, const int32_t* n_cur, int cur_stride,
                                                const uint8_t* cur_taken, const float* Tcw_cur, const cslam_keypoint* k_last, const int32_t* n_last, int last_stride,
                                                const uint8_t* has_mp, const float* Xw, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float cos_fov_th, float th,
                                                int check_ori, float scale_factor, int nlevels, int32_t* match_cur, int32_t* nmatches) {
     if (!t || npairs <= 0 || npairs > t->maxFrames || cur_stride > t->maxFeat || last_stride > t->maxFeat) { set_error("cslam_search_by_projection_last: sizes out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
+    t->arena.reset();
     const size_t nc = (size_t)npairs * cur_stride, nl = (size_t)npairs * last_stride;
-    cudaStream_t s = t->stream;
-    CSLAM_CUDA(cudaMemcpyAsync(t->kCur, k_cur, nc * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->dCur, d_cur, nc * 32, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->nCur, n_cur, npairs * 4, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->taken, cur_taken, nc, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->Tcw, Tcw_cur, (size_t)npairs * 64, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->kLast, k_last, nl * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->nQ, n_last, npairs * 4, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->valid, has_mp, nl, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->Xw, Xw, nl * 12, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->dQ, d_mp, nl * 32, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->obs, mp_obs, nl, cudaMemcpyHostToDevice, s));
-    int rc = cslam_frame_index_dev(t, t->kCur, t->nCur, npairs, cur_stride, face_w, face_h, nullptr, t->cellStart, t->cellIdx);
-    if (rc) return rc;
-    rc = cslam_search_by_projection_last_dev(t, npairs, t->kCur, t->dCur, t->nCur, cur_stride, t->cellStart, t->cellIdx, t->taken, t->Tcw, t->kLast, t->nQ, last_stride, t->valid, t->Xw, t->dQ,
-                                             t->obs, face_w, face_h, cos_fov_th, th, check_ori, scale_factor, nlevels, t->match, t->nm);
-    if (rc) return rc;
-    CSLAM_CUDA(cudaMemcpyAsync(match_cur, t->match, nc * 4, cudaMemcpyDeviceToHost, s)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, t->nm, npairs * 4, cudaMemcpyDeviceToHost, s));
+    DevArena& a = t->arena;
+    const cslam_keypoint *kC, *kL; const uint8_t *dC, *taken, *valid, *dQ, *obs; const int32_t *nC, *nL; const float *Tcw, *dXw; uint16_t *cs, *ci; int32_t *match, *nm; int rc;
+    if ((rc = a.upload(&kC, k_cur, nc)) || (rc = a.upload(&dC, d_cur, nc * 32)) || (rc = a.upload(&nC, n_cur, npairs)) || (rc = a.upload(&taken, cur_taken, nc)) ||
+        (rc = a.upload(&Tcw, Tcw_cur, (size_t)npairs * 16)) || (rc = a.upload(&kL, k_last, nl)) || (rc = a.upload(&nL, n_last, npairs)) || (rc = a.upload(&valid, has_mp, nl)) ||
+        (rc = a.upload(&dXw, Xw, nl * 3)) || (rc = a.upload(&dQ, d_mp, nl * 32)) || (rc = a.upload(&obs, mp_obs, nl)) || (rc = a.take(&cs, (size_t)npairs * (NCELLS + 1))) ||
+        (rc = a.take(&ci, nc)) || (rc = a.take(&match, nc)) || (rc = a.take(&nm, npairs)) ||
+        (rc = cslam_frame_index_dev(t, kC, nC, npairs, cur_stride, face_w, face_h, nullptr, cs, ci)) ||
+        (rc = cslam_search_by_projection_last_dev(t, npairs, kC, dC, nC, cur_stride, cs, ci, taken, Tcw, kL, nL, last_stride, valid, dXw, dQ, obs, face_w, face_h, cos_fov_th, th,
+                                                  check_ori, scale_factor, nlevels, match, nm))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match_cur, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nm, npairs * 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }
 
@@ -456,19 +451,17 @@ extern "C" int cslam_search_by_projection_local(cslam_tracker* t, int nframes, c
                                                 int32_t* match_f, int32_t* nmatches) {
     if (!t || nframes <= 0 || nframes > t->maxFrames || f_stride > t->maxFeat || mp_stride > t->maxFeat) { set_error("cslam_search_by_projection_local: sizes out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
+    t->arena.reset();
     const size_t nc = (size_t)nframes * f_stride, nm = (size_t)nframes * mp_stride;
-    cudaStream_t s = t->stream;
-    CSLAM_CUDA(cudaMemcpyAsync(t->kCur, k_f, nc * sizeof(cslam_keypoint), cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->dCur, d_f, nc * 32, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->nCur, n_f, nframes * 4, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->taken, f_taken, nc, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->nQ, n_mp, nframes * 4, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->valid, in_view, nm, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->proj, proj_xy, nm * 8, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->level, level, nm * 4, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->vcos, view_cos, nm * 4, cudaMemcpyHostToDevice, s)); CSLAM_CUDA(cudaMemcpyAsync(t->dQ, d_mp, nm * 32, cudaMemcpyHostToDevice, s));
-    CSLAM_CUDA(cudaMemcpyAsync(t->obs, mp_obs, nm, cudaMemcpyHostToDevice, s));
-    int rc = cslam_frame_index_dev(t, t->kCur, t->nCur, nframes, f_stride, face_w, face_h, nullptr, t->cellStart, t->cellIdx);
-    if (rc) return rc;
-    rc = cslam_search_by_projection_local_dev(t, nframes, t->kCur, t->dCur, t->nCur, f_stride, t->cellStart, t->cellIdx, t->taken, t->nQ, mp_stride, t->valid, t->proj, t->level, t->vcos, t->dQ,
-                                              t->obs, face_w, face_h, th, nnratio, scale_factor, nlevels, t->match, t->nm);
-    if (rc) return rc;
-    CSLAM_CUDA(cudaMemcpyAsync(match_f, t->match, nc * 4, cudaMemcpyDeviceToHost, s)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, t->nm, nframes * 4, cudaMemcpyDeviceToHost, s));
+    DevArena& a = t->arena;
+    const cslam_keypoint* kF; const uint8_t *dF, *taken, *valid, *dQ, *obs; const int32_t *nF, *nQ, *lvl; const float *proj, *vcos; uint16_t *cs, *ci; int32_t *match, *nmOut; int rc;
+    if ((rc = a.upload(&kF, k_f, nc)) || (rc = a.upload(&dF, d_f, nc * 32)) || (rc = a.upload(&nF, n_f, nframes)) || (rc = a.upload(&taken, f_taken, nc)) ||
+        (rc = a.upload(&nQ, n_mp, nframes)) || (rc = a.upload(&valid, in_view, nm)) || (rc = a.upload(&proj, proj_xy, nm * 2)) || (rc = a.upload(&lvl, level, nm)) ||
+        (rc = a.upload(&vcos, view_cos, nm)) || (rc = a.upload(&dQ, d_mp, nm * 32)) || (rc = a.upload(&obs, mp_obs, nm)) || (rc = a.take(&cs, (size_t)nframes * (NCELLS + 1))) ||
+        (rc = a.take(&ci, nc)) || (rc = a.take(&match, nc)) || (rc = a.take(&nmOut, nframes)) ||
+        (rc = cslam_frame_index_dev(t, kF, nF, nframes, f_stride, face_w, face_h, nullptr, cs, ci)) ||
+        (rc = cslam_search_by_projection_local_dev(t, nframes, kF, dF, nF, f_stride, cs, ci, taken, nQ, mp_stride, valid, proj, lvl, vcos, dQ, obs, face_w, face_h, th, nnratio,
+                                                   scale_factor, nlevels, match, nmOut))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }

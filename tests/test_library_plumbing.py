@@ -22,6 +22,25 @@ def test_only_the_nccl_fallback_reads_the_environment():
     assert calls and all(arg == '"CSLAM_BA_NCCL_ONLY"' for _, arg in calls), calls
 
 
+def test_device_memory_comes_from_dev_alloc_or_the_arena():
+    """Persistent per-handle state is allocated by dev_alloc, everything a single call needs comes from the handle's DevArena (common.cuh).
+    The one other device allocation is the multi-GPU optimizer's exchange set-up (CUDA IPC buffers and the NCCL handshake)."""
+    regions = {"common.cuh": [r"static int dev_alloc\(", r"class DevArena \{"], "ba.cu": [r"static int setup_xchg\("]}
+    found = {}
+    for path in glob.glob(os.path.join(ROOT, "cubemapslam_b200", "csrc", "*.cu*")):
+        name = os.path.basename(path)
+        src = open(path).read()
+        spans = []
+        for start in regions.get(name, []):
+            b = re.search(start, src).start()
+            spans.append((start, b, re.compile(r"\n\}").search(src, b).end()))
+        for m in re.finditer(r"\bcudaMalloc(?!Host)\w*\s*\(", src):
+            inside = [s for s, b, e in spans if b <= m.start() < e]
+            assert inside, "%s:%d allocates device memory outside dev_alloc / DevArena" % (name, src.count("\n", 0, m.start()) + 1)
+            found[inside[0]] = found.get(inside[0], 0) + 1
+    assert set(found) == {s for v in regions.values() for s in v}, found
+
+
 def test_every_handle_needs_a_device():
     import torch
     if torch.cuda.is_available():
