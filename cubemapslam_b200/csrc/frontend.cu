@@ -27,7 +27,6 @@ static const int MAX_LEVELS = 16;
 static const int CG = 4;            // cells per CTA (x) in k_fast
 static const int CELL_MAX = 48;     // largest supported cell edge
 static const int FAST_TS = 208;     // smem tile stride (bytes), >= CG*CELL_MAX+6+3 rounded
-static const int FAST_TH = CELL_MAX + 6;
 static const int DESC_WARPS = 4;
 
 __constant__ int c_umax[16];
@@ -41,6 +40,7 @@ struct LevelGeom {
     int wCell, hCell, nColsEff, nRowsEff;
     int quota;                // mnFeaturesPerLevel
     int candCap;
+    int liveCap;              // longest k_fast live list of one tile (DevLevels::live; 0 without warp geometry)
     float scale;              // mvScaleFactor
     float sizeF;              // (int)(PATCH_SIZE*scale)
 };
@@ -243,7 +243,7 @@ __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src
 // and the 20->7 fallback is decided per cell on "no keypoint survived NMS" (src/ORBExtractor.cpp:763-803).
 // Exact arc score of 2 pixels at once in u16x2 lanes (sm_90a VIMNMX3.U16x2):
 //   s = max(0, A - c, c - B),  A = max_k min(R[k..k+8]),  B = min_k max(R[k..k+8])   (R = ring intensities, c = centre)
-// min/max over 9 contiguous ring pixels = min3 of three min3's. No data-dependent branch, no per-pixel early-out:
+// A and B take 32 min/max each, windows paired as described in the function. No data-dependent branch, no per-pixel early-out:
 // on textured input almost every pixel passes the cheap antipodal tests, so the branch-free full score is cheaper
 // than queueing.
 // The intensities sit in the high bytes of the lanes, the low bytes hold anything (the neighbouring pixels of a raw image word): u16
@@ -251,22 +251,30 @@ __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src
 // masked, before the subtractions. Returned per lane: (max(s, t) - t) << 8 for the threshold t, given as T = t << 8 in each lane, i.e.
 // 0 where s <= t and order-preserving above it.
 __device__ __forceinline__ uint32_t arc_score_x2(const uint32_t (&R)[16], uint32_t c, uint32_t T) {
-    uint32_t mn[16], mx[16];
+    // Windows k and k+1 (k even) share ring pixels k+1..k+8. By distributivity max(min(R[k], s), min(s, R[k+9])) = min(s, max(R[k], R[k+9])),
+    // so the pair's larger minimum is min(R[k+1..k+8], max(R[k], R[k+9])). For k = 4g and k = 4g + 2 the shared runs are P[k+1] + S[g] and
+    // S[g] + P[k+9], with P[j] = min(R[j], R[j+1]) (j odd) and S[g] = R[4g+3..4g+8] = min3 of three P: 8 + 4 + 16 + 4 = 32 min/max per side
+    // instead of 40 (B: the same with min and max swapped)
+    uint32_t pn[8], px[8];   // P at index (j - 1) / 2
 #pragma unroll
-    for (int k = 0; k < 16; k++) {
-        mn[k] = __vimin3_u16x2(R[k], R[(k + 1) & 15], R[(k + 2) & 15]);
-        mx[k] = __vimax3_u16x2(R[k], R[(k + 1) & 15], R[(k + 2) & 15]);
+    for (int i = 0; i < 8; i++) {
+        const int j = 2 * i + 1;
+        pn[i] = __vminu2(R[j], R[(j + 1) & 15]);
+        px[i] = __vmaxu2(R[j], R[(j + 1) & 15]);
     }
-    uint32_t A, Bm;
+    uint32_t tA[8], tB[8];
 #pragma unroll
-    for (int k = 0; k < 16; k += 2) {
-        const uint32_t a0 = __vimin3_u16x2(mn[k], mn[(k + 3) & 15], mn[(k + 6) & 15]);
-        const uint32_t a1 = __vimin3_u16x2(mn[k + 1], mn[(k + 4) & 15], mn[(k + 7) & 15]);
-        const uint32_t b0 = __vimax3_u16x2(mx[k], mx[(k + 3) & 15], mx[(k + 6) & 15]);
-        const uint32_t b1 = __vimax3_u16x2(mx[k + 1], mx[(k + 4) & 15], mx[(k + 7) & 15]);
-        A = k ? __vimax3_u16x2(A, a0, a1) : __vmaxu2(a0, a1);
-        Bm = k ? __vimin3_u16x2(Bm, b0, b1) : __vminu2(b0, b1);
+    for (int g = 0; g < 4; g++) {
+        const int k = 4 * g;
+        const uint32_t sn = __vimin3_u16x2(pn[2 * g + 1], pn[(2 * g + 2) & 7], pn[(2 * g + 3) & 7]);
+        const uint32_t sx = __vimax3_u16x2(px[2 * g + 1], px[(2 * g + 2) & 7], px[(2 * g + 3) & 7]);
+        tA[2 * g] = __vimin3_u16x2(sn, pn[2 * g], __vmaxu2(R[k], R[(k + 9) & 15]));
+        tB[2 * g] = __vimax3_u16x2(sx, px[2 * g], __vminu2(R[k], R[(k + 9) & 15]));
+        tA[2 * g + 1] = __vimin3_u16x2(sn, pn[(2 * g + 4) & 7], __vmaxu2(R[k + 2], R[(k + 11) & 15]));
+        tB[2 * g + 1] = __vimax3_u16x2(sx, px[(2 * g + 4) & 7], __vminu2(R[k + 2], R[(k + 11) & 15]));
     }
+    uint32_t A = __vimax3_u16x2(__vimax3_u16x2(tA[0], tA[1], tA[2]), __vimax3_u16x2(tA[3], tA[4], tA[5]), __vmaxu2(tA[6], tA[7]));
+    uint32_t Bm = __vimin3_u16x2(__vimin3_u16x2(tB[0], tB[1], tB[2]), __vimin3_u16x2(tB[3], tB[4], tB[5]), __vminu2(tB[6], tB[7]));
     const uint32_t HI = 0xff00ff00u;
     A &= HI; Bm &= HI; c &= HI;
     const uint32_t t1 = __vmaxu2(A, c) - c;      // lanes never borrow: max(A,c) >= c
@@ -278,7 +286,8 @@ __device__ __forceinline__ uint32_t arc_score_x2(const uint32_t (&R)[16], uint32
 __device__ __forceinline__ int fdiv_small(int i, uint32_t magic) { return (int)(((uint32_t)i * magic) >> 20); }
 __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d - 1) / d; }
 
-// Layout of one CTA: CG cells of one cell row. Phases:
+// Layout of one CTA: one tile column (CG cells wide) of FAST_R consecutive cell rows of one frame, walked tile by tile (a tile = CG cells of
+// one cell row, exactly the reference's per-cell ROIs). Phases of each tile:
 //  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, (s - mt) << 8, 0 where s <= mt; mt = minTh clamped to
 //     1..255, see below).
 //     On the warp path (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant
@@ -286,8 +295,8 @@ __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d -
 //  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the same items as A -> shared list; a keypoint at
 //     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
 //  C  compaction of the selected entries into the global candidate list (one global atomic per 256 entries)
-static const int FAST_KMAX = CG * (CELL_MAX / 2) * (CELL_MAX / 2);   // NMS survivors are pairwise non-adjacent
-static const int FAST_SW = FAST_TS / 2;                              // pair-words per score row
+static const int FAST_R = 8;            // cell rows per k_fast CTA
+static const int FAST_SW = FAST_TS / 2;   // pair-words per score row
 static_assert((CG * CELL_MAX + 9) / 4 < 64 && CELL_MAX < 1024, "a live work item packs y<<6 | (wi - w0) into 16 bits");
 static_assert(CG <= 4, "FastItem packs a pixel's cell index into 2 bits");
 
@@ -323,6 +332,29 @@ struct FastCols {
     FastItem item[FAST_SW / 2];
 };
 
+// Dynamic shared memory of a k_fast CTA (byte offsets), sized from the level's cell geometry; CELL_MAX bounds it (fast_smem_max)
+struct FastSmem {
+    int items;                 // the tile column's FastCols::item table
+    int tile, tileBytes;       // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
+                               // then hCell + 6 rows of FAST_TS
+    int s2, klist;             // score map (hCell + 2 rows of FAST_SW pair-words); NMS survivors, kmax entries
+    int live, liveBytes;       // live list buffer b (u16, staged from an even index: liveCap + 1 entries) at live + b * liveBytes
+    int kmax, total;
+};
+__host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
+    FastSmem m;
+    m.tileBytes = 16 + (g.hCell + 6) * FAST_TS; m.liveBytes = (2 * g.liveCap + 2 + 15) & ~15;
+    m.kmax = CG * ((g.wCell + 1) / 2) * ((g.hCell + 1) / 2);   // NMS survivors of a cell are pairwise non-adjacent
+    m.items = 0;
+    m.tile = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);
+    m.s2 = m.tile + 2 * m.tileBytes;
+    m.live = m.s2 + (g.hCell + 2) * FAST_SW * 4;
+    m.klist = m.live + 2 * m.liveBytes;
+    m.total = m.klist + 4 * m.kmax;
+    return m;
+}
+static_assert(FAST_TS % 16 == 0 && sizeof(FastItem) % 16 == 0, "k_fast shared-memory regions stay 16-byte aligned");
+
 // Neighbourhood maximum of pair-word `cur` over its 8 same-cell neighbours: a*, b*, c* = the pair-words left of, at and right of it in the
 // row above (0), its own row (1) and the row below (2); ml / mr mask the lanes without a left / right neighbour in their cell
 __device__ __forceinline__ uint32_t nms_max(uint32_t a0, uint32_t b0, uint32_t c0, uint32_t a1, uint32_t cur, uint32_t c1, uint32_t a2, uint32_t b2,
@@ -333,193 +365,235 @@ __device__ __forceinline__ uint32_t nms_max(uint32_t a0, uint32_t b0, uint32_t c
     return __vimax3_u16x2(__vimax3_u16x2(upL, b0, upR), __vimax3_u16x2(cuL, cuR, b2), __vmaxu2(dnL, dnR));
 }
 
-__global__ void __launch_bounds__(256) k_fast(const uint8_t* __restrict__ img, LevelGeom g, int iniTh, int minTh, uint32_t* __restrict__ cand,
+__global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img, LevelGeom g, int iniTh, int minTh, uint32_t* __restrict__ cand,
                                               uint32_t* __restrict__ candCount, int countStride, int* __restrict__ errFlag,
                                               const FastCols* __restrict__ cols, const uint8_t* __restrict__ skip,
                                               const uint16_t* __restrict__ live, const uint32_t* __restrict__ liveOff) {
-    // tile rows; 16 bytes in front so that the word left of row 0's first word is addressable (phase A reads it unguarded)
-    __shared__ __align__(16) uint8_t tileBuf[16 + FAST_TH * FAST_TS];
-    uint8_t* const tile = tileBuf + 16;
+    extern __shared__ __align__(16) uint8_t fsm[];   // FastSmem
+    const FastSmem SM = fast_smem(g);
     // score map, one u16 per pixel as u16x2 pair-words: word 2*wi (+1) of row y+1 holds tile columns 4*wi..4*wi+1 (+2..+3)
-    __shared__ __align__(16) uint32_t S2[(CELL_MAX + 2) * FAST_SW];
-    __shared__ uint32_t klist[FAST_KMAX];                            // x | y<<8 | s<<16 | cell<<24
+    uint32_t* const S2 = reinterpret_cast<uint32_t*>(fsm + SM.s2);
+    uint32_t* const klist = reinterpret_cast<uint32_t*>(fsm + SM.klist);   // x | y<<8 | s<<16 | cell<<24
+    const uint4* const items = reinterpret_cast<const uint4*>(fsm + SM.items);   // FastItem wi = items[2*wi], items[2*wi+1]
+    __shared__ uint32_t rowLo[FAST_R], rowHi[FAST_R];   // live list of each strip row, [rowLo, rowHi)
+    __shared__ int rowVisit[FAST_R];                    // the strip row's tile has work (not skipped, detection rows > 0)
     __shared__ int cnt20[CG];
-    __shared__ int anyNonZero, nK, chunkBase;
+    __shared__ int nK, chunkBase;
     __shared__ int warpCnt[8];
-    const int frame = blockIdx.z, cellRow = blockIdx.y;
+    const int frame = blockIdx.z, row0 = blockIdx.y * FAST_R, nr = min(FAST_R, g.nRowsEff - row0);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tileIdx = cellRow * gridDim.x + blockIdx.x;
-    if (skip && skip[tileIdx]) return;   // tile provably corner-free (no live work item)
-    const uint8_t* I = img + (size_t)frame * g.pitch * g.h;
-    const int iniY = g.minB + cellRow * g.hCell, maxY = min(iniY + g.hCell + 6, g.maxBY);
     const FastTileX X = fast_tile_x(g, blockIdx.x);
-    const int nrows = maxY - iniY, ny = nrows - 6;   // detection rows
     const int nx = X.nx, xoff = X.xoff, w0 = X.w0, nw = X.w1 - X.w0;
-    if (nx <= 0 || ny <= 0) return;   // block-uniform: a ROI with fewer than 7 rows / columns has no detection area (cv::FAST returns nothing)
+    if (nx <= 0) return;   // block-uniform: a ROI with fewer than 7 columns has no detection area (cv::FAST returns nothing)
+    const uint8_t* I = img + (size_t)frame * g.pitch * g.h;
+    for (int i = tid; i < nr; i += 256) {
+        const int t = (row0 + i) * gridDim.x + blockIdx.x, iniY = g.minB + (row0 + i) * g.hCell;
+        // a ROI with fewer than 7 rows has no detection area; a skipped tile is provably corner-free (no live work item)
+        rowVisit[i] = min(iniY + g.hCell + 6, g.maxBY) - iniY > 6 && !(skip && skip[t]);
+        if (live) { rowLo[i] = liveOff[t]; rowHi[i] = liveOff[t + 1]; }
+    }
+    __syncthreads();
+    int cur = 0;
+    while (cur < nr && !rowVisit[cur]) cur++;
+    if (cur == nr) return;
     const FastCols* C = cols + blockIdx.x;
     const uint4 mg = __ldg(reinterpret_cast<const uint4*>(C));
     // cv::FAST clamps its threshold to 0..255 and ranks corners by s - 1, with 0 for "no corner": at threshold 0 a corner with s = 1 ties
     // with its non-corner neighbours and never survives NMS, exactly as if the threshold were 1
     const int mt = min(max(minTh, 1), 255);
     const uint32_t T = (uint32_t)mt * 0x01000100u;
-    if (tid < CG) cnt20[tid] = 0;
-    if (tid == 0) { anyNonZero = 0; nK = 0; }
-    __syncthreads();
-    uint32_t acc = 0;
-    {
-        const int nwords = X.nwords;
+    const int nwords = X.nwords;
+    // strip row i's tile rows (4-byte copies: a0 is only word-aligned) and live list (from the even index below rowLo) into buffer b
+    auto stage = [&](int i, int b) {
+        const int iniY = g.minB + (row0 + i) * g.hCell, nrows = min(iniY + g.hCell + 6, g.maxBY) - iniY;
         const uint8_t* base = I + (size_t)iniY * g.pitch + X.a0;
-        for (int i = tid; i < nwords * nrows; i += 256) {
-            const int r = fdiv_small(i, mg.x), wd = i - r * nwords;
-            const uint32_t v = __ldg(reinterpret_cast<const uint32_t*>(base + (size_t)r * g.pitch) + wd);
-            reinterpret_cast<uint32_t*>(tile + r * FAST_TS)[wd] = v;
-            acc |= v;
+        uint8_t* tile = fsm + SM.tile + b * SM.tileBytes + 16;
+        for (int k = tid; k < nwords * nrows; k += 256) {
+            const int r = fdiv_small(k, mg.x), wd = k - r * nwords;
+            cp_async4_zfill(tile + r * FAST_TS + 4 * wd, base + (size_t)r * g.pitch + 4 * wd, 4);
         }
-    }
-    if (acc) anyNonZero = 1;
-    // S2 must read 0 around the scored area (rows 0 and ny+1, the pair-words left/right of [2*w0, 2*w1)) and wherever phase A skips an item
-    {
-        const int q0 = X.q0, nq = X.q1 - X.q0;
-        for (int i = tid; i < (ny + 2) * nq; i += 256) {
-            const int r = fdiv_small(i, mg.z);
-            reinterpret_cast<uint4*>(S2 + r * FAST_SW)[q0 + i - r * nq] = make_uint4(0u, 0u, 0u, 0u);
-        }
-    }
-    __syncthreads();
-    if (!anyNonZero) return;   // an all-zero tile has no corners at any threshold
-    // ---- A
-    {
-        auto score_item = [&](int y, int wi) {
-            const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
-            const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
-            const int RS = FAST_TS / 4;
-            // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
-            // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
-            // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle
-            uint32_t V[16], U[16], Cv, Cu;
-            {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
-                const uint32_t m = r0[-1], c = r0[0], p = r0[1];
-                V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
-                U[15] = __funnelshift_r(m, c, 16); U[0] = V[15]; U[1] = c;
-            }
-            {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
-                const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
-                U[14] = __funnelshift_r(m, c, 8); U[2] = __funnelshift_r(c, p, 8);
-            }
-            {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
-                const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
-                U[13] = m; U[3] = __funnelshift_r(c, p, 16);
-            }
-            {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
-                const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
-                U[12] = m; U[4] = __funnelshift_r(c, p, 16); Cu = __funnelshift_r(m, c, 24);
-            }
-            {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
-                const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
-                U[11] = m; U[5] = __funnelshift_r(c, p, 16);
-            }
-            {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
-                const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
-                U[10] = __funnelshift_r(m, c, 8); U[6] = __funnelshift_r(c, p, 8);
-            }
-            {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
-                const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
-                U[9] = __funnelshift_r(m, c, 16); U[8] = V[9]; U[7] = c;
-            }
-            const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
-            // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
-            // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset)
-            *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
-                make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
-        };
         if (live) {
-            const uint32_t i0 = liveOff[tileIdx], i1 = liveOff[tileIdx + 1];
-            for (uint32_t it = i0 + tid; it < i1; it += 256) { const int e = live[it]; score_item(e >> 6, w0 + (e & 63)); }
-        } else {
-            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); score_item(y, w0 + (it - y * nw)); }
+            const uint32_t lo = rowLo[i] & ~1u, n = (rowHi[i] - lo + 1) >> 1;   // the list is padded to an even length
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(live + lo);
+            for (uint32_t k = tid; k < n; k += 256) cp_async4_zfill(fsm + SM.live + b * SM.liveBytes + 4 * k, src + k, 4);
         }
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
+    };
+    for (int k = tid; k < (int)(sizeof(FastItem) / 16) * (FAST_SW / 2); k += 256) {
+        const uint32_t s = (uint32_t)__cvta_generic_to_shared(fsm + SM.items + 16 * k);
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(reinterpret_cast<const uint4*>(C->item) + k) : "memory");
     }
-    __syncthreads();
-    // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
-    // non-zero only inside an item phase A scored, so B walks the same items; one thread reads the item's 3 x 4 pair-word neighbourhood once.
-    // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
-    // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
-    {
-        auto nms_item = [&](int y, int wi) {
-            const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
-            const uint4 hd = __ldg(reinterpret_cast<const uint4*>(&C->item[wi]));
-            uint2 cu = *reinterpret_cast<const uint2*>(r1);
-            cu.x &= hd.x; cu.y &= hd.y;
-            if ((cu.x | cu.y) == 0) return;
-            const uint32_t* r0 = r1 - FAST_SW; const uint32_t* r2 = r1 + FAST_SW;
-            const uint2 up = *reinterpret_cast<const uint2*>(r0), dn = *reinterpret_cast<const uint2*>(r2);
-            const uint32_t uL = wi > 0 ? r0[-1] : 0u, cL = wi > 0 ? r1[-1] : 0u, dL = wi > 0 ? r2[-1] : 0u;
-            const uint32_t uR = r0[2], cR = r1[2], dR = r2[2];
-            const uint4 lr = __ldg(reinterpret_cast<const uint4*>(&C->item[wi]) + 1);
-            const uint32_t M0 = nms_max(uL, up.x, up.y, cL, cu.x, cu.y, dL, dn.x, dn.y, lr.x, lr.z);
-            const uint32_t M1 = nms_max(up.x, up.y, uR, cu.x, cu.y, cR, dn.x, dn.y, dR, lr.y, lr.w);
-            uint32_t keep = 0;   // bit j: pixel j of the item survives
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const uint32_t c = j < 2 ? cu.x : cu.y, m = j < 2 ? M0 : M1, h = 16 * (j & 1);
-                keep |= (((c >> h) & 0xffff) > ((m >> h) & 0xffff)) ? 1u << j : 0u;
+    stage(cur, 0);   // same group as the item table
+    // Barriers of one tile (buffer b = tile parity in the strip):
+    //  top   S2 cleared, nK / cnt20 reset: the previous tile's phases B and C are done with them (its end barrier)
+    //  wait  this thread's copies of the tile landed; B1 (__syncthreads_or) makes every thread's copies visible
+    //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phases A and B, before its B3
+    //  A  -> B2 -> B (S2, item table, live list of b) -> B3 -> C (klist, nK, cnt20; its own barriers per chunk) -> end barrier
+    for (int b = 0;; b ^= 1) {
+        const int iniY = g.minB + (row0 + cur) * g.hCell, maxY = min(iniY + g.hCell + 6, g.maxBY);
+        const int nrows = maxY - iniY, ny = nrows - 6;   // detection rows
+        const uint8_t* const tile = fsm + SM.tile + b * SM.tileBytes + 16;
+        const uint16_t* const liveS = reinterpret_cast<const uint16_t*>(fsm + SM.live + b * SM.liveBytes) + (rowLo[cur] & 1u);
+        const uint32_t nLive = live ? rowHi[cur] - rowLo[cur] : 0u;
+        // S2 must read 0 around the scored area (rows 0 and ny+1, the pair-words left/right of [2*w0, 2*w1)) and wherever phase A skips an item
+        {
+            const int q0 = X.q0, nq = X.q1 - X.q0;
+            for (int i = tid; i < (ny + 2) * nq; i += 256) {
+                const int r = fdiv_small(i, mg.z);
+                reinterpret_cast<uint4*>(S2 + r * FAST_SW)[q0 + i - r * nq] = make_uint4(0u, 0u, 0u, 0u);
             }
-            while (keep) {
-                const int j = __ffs(keep) - 1;
-                keep &= keep - 1;
-                const uint32_t sv = ((j < 2 ? cu.x : cu.y) >> (16 * (j & 1))) & 0xffff;
-                const int x = 4 * wi + j - xoff, cell = (hd.z >> (2 * j)) & 3, s = (int)(sv >> 8) + mt;
-                const int pos = atomicAdd(&nK, 1);
-                if (pos >= FAST_KMAX) *errFlag = CSLAM_E_CAPACITY;
-                else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)s << 16) | ((uint32_t)cell << 24);
-                if (s > iniTh) atomicAdd(&cnt20[cell], 1);
+        }
+        if (tid < CG) cnt20[tid] = 0;
+        if (tid == 0) nK = 0;
+        asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+        // caller canvases: an all-zero tile has no corners at any threshold (OR of the words this thread staged)
+        uint32_t acc = live ? 1u : 0u;
+        if (!live)
+            for (int k = tid; k < nwords * nrows; k += 256) {
+                const int r = fdiv_small(k, mg.x);
+                acc |= reinterpret_cast<const uint32_t*>(tile + r * FAST_TS)[k - r * nwords];
             }
-        };
-        if (live) {
-            const uint32_t i0 = liveOff[tileIdx], i1 = liveOff[tileIdx + 1];
-            for (uint32_t it = i0 + tid; it < i1; it += 256) { const int e = live[it]; nms_item(e >> 6, w0 + (e & 63)); }
-        } else {
-            for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); nms_item(y, w0 + (it - y * nw)); }
+        const int any = __syncthreads_or(acc);   // B1
+        int next = cur + 1;
+        while (next < nr && !rowVisit[next]) next++;
+        if (next < nr) stage(next, b ^ 1);
+        if (!any) {   // nothing reads S2, the counters or buffer b after B1
+            if (next == nr) break;
+            cur = next;
+            continue;
         }
-    }
-    __syncthreads();
-    // ---- C
-    uint32_t* out = cand + (size_t)frame * g.candCap;
-    uint32_t* cc = candCount + (size_t)frame * countStride;
-    const int nk = min(nK, FAST_KMAX);
-    for (int base = 0; base < nk; base += 256) {
-        const int i = base + tid;
-        uint32_t e = 0; bool sel = false;
-        if (i < nk) {
-            e = klist[i];
-            const int sv = (e >> 16) & 0xff, cell = e >> 24;
-            sel = cnt20[cell] > 0 ? sv > iniTh : true;
-        }
-        const unsigned ball = __ballot_sync(0xffffffffu, sel);
-        if (lane == 0) warpCnt[warp] = __popc(ball);
-        __syncthreads();
-        if (tid == 0) {
-            int tot = 0;
-            for (int w = 0; w < 8; w++) { const int t = warpCnt[w]; warpCnt[w] = tot; tot += t; }
-            chunkBase = tot ? (int)atomicAdd(cc, (uint32_t)tot) : 0;
-        }
-        __syncthreads();
-        if (sel) {
-            const uint32_t pos = (uint32_t)chunkBase + warpCnt[warp] + __popc(ball & ((1u << lane) - 1));
-            if (pos < (uint32_t)g.candCap) {
-                const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
-                out[pos] = x | (y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
+        // ---- A
+        {
+            auto score_item = [&](int y, int wi) {
+                const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
+                const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
+                const int RS = FAST_TS / 4;
+                // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
+                // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
+                // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle
+                uint32_t V[16], U[16], Cv, Cu;
+                {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
+                    const uint32_t m = r0[-1], c = r0[0], p = r0[1];
+                    V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
+                    U[15] = __funnelshift_r(m, c, 16); U[0] = V[15]; U[1] = c;
+                }
+                {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
+                    const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
+                    U[14] = __funnelshift_r(m, c, 8); U[2] = __funnelshift_r(c, p, 8);
+                }
+                {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
+                    const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
+                    U[13] = m; U[3] = __funnelshift_r(c, p, 16);
+                }
+                {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
+                    const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
+                    U[12] = m; U[4] = __funnelshift_r(c, p, 16); Cu = __funnelshift_r(m, c, 24);
+                }
+                {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
+                    const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
+                    U[11] = m; U[5] = __funnelshift_r(c, p, 16);
+                }
+                {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
+                    const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
+                    U[10] = __funnelshift_r(m, c, 8); U[6] = __funnelshift_r(c, p, 8);
+                }
+                {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
+                    const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                    V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
+                    U[9] = __funnelshift_r(m, c, 16); U[8] = V[9]; U[7] = c;
+                }
+                const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
+                // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
+                // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset)
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
+                    make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
+            };
+            if (live) {
+                for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; score_item(e >> 6, w0 + (e & 63)); }
             } else {
-                *errFlag = CSLAM_E_CAPACITY;
+                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); score_item(y, w0 + (it - y * nw)); }
             }
         }
         __syncthreads();
+        // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
+        // non-zero only inside an item phase A scored, so B walks the same items; one thread reads the item's 3 x 4 pair-word neighbourhood once.
+        // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
+        // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
+        {
+            auto nms_item = [&](int y, int wi) {
+                const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
+                const uint4 hd = items[2 * wi];
+                uint2 cu = *reinterpret_cast<const uint2*>(r1);
+                cu.x &= hd.x; cu.y &= hd.y;
+                if ((cu.x | cu.y) == 0) return;
+                const uint32_t* r0 = r1 - FAST_SW; const uint32_t* r2 = r1 + FAST_SW;
+                const uint2 up = *reinterpret_cast<const uint2*>(r0), dn = *reinterpret_cast<const uint2*>(r2);
+                const uint32_t uL = wi > 0 ? r0[-1] : 0u, cL = wi > 0 ? r1[-1] : 0u, dL = wi > 0 ? r2[-1] : 0u;
+                const uint32_t uR = r0[2], cR = r1[2], dR = r2[2];
+                const uint4 lr = items[2 * wi + 1];
+                const uint32_t M0 = nms_max(uL, up.x, up.y, cL, cu.x, cu.y, dL, dn.x, dn.y, lr.x, lr.z);
+                const uint32_t M1 = nms_max(up.x, up.y, uR, cu.x, cu.y, cR, dn.x, dn.y, dR, lr.y, lr.w);
+                // survivors: the lanes where c > m. Every lane holds a multiple of 256 (the stored scores' low bytes are 0), so max(c, m) - m
+                // never borrows and its high byte is non-zero exactly there; byte j of `keep` is that byte of pixel j
+                uint32_t keep = __byte_perm(__vmaxu2(cu.x, M0) - M0, __vmaxu2(cu.y, M1) - M1, 0x7531);
+                while (keep) {
+                    const int j = (__ffs(keep) - 1) >> 3;
+                    keep &= ~(0xffu << (8 * j));
+                    const uint32_t sv = ((j < 2 ? cu.x : cu.y) >> (16 * (j & 1))) & 0xffff;
+                    const int x = 4 * wi + j - xoff, cell = (hd.z >> (2 * j)) & 3, s = (int)(sv >> 8) + mt;
+                    const int pos = atomicAdd(&nK, 1);
+                    if (pos >= SM.kmax) *errFlag = CSLAM_E_CAPACITY;
+                    else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)s << 16) | ((uint32_t)cell << 24);
+                    if (s > iniTh) atomicAdd(&cnt20[cell], 1);
+                }
+            };
+            if (live) {
+                for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; nms_item(e >> 6, w0 + (e & 63)); }
+            } else {
+                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); nms_item(y, w0 + (it - y * nw)); }
+            }
+        }
+        __syncthreads();
+        // ---- C
+        uint32_t* out = cand + (size_t)frame * g.candCap;
+        uint32_t* cc = candCount + (size_t)frame * countStride;
+        const int nk = min(nK, SM.kmax);
+        for (int base = 0; base < nk; base += 256) {
+            const int i = base + tid;
+            uint32_t e = 0; bool sel = false;
+            if (i < nk) {
+                e = klist[i];
+                const int sv = (e >> 16) & 0xff, cell = e >> 24;
+                sel = cnt20[cell] > 0 ? sv > iniTh : true;
+            }
+            const unsigned ball = __ballot_sync(0xffffffffu, sel);
+            if (lane == 0) warpCnt[warp] = __popc(ball);
+            __syncthreads();
+            if (tid == 0) {
+                int tot = 0;
+                for (int w = 0; w < 8; w++) { const int t = warpCnt[w]; warpCnt[w] = tot; tot += t; }
+                chunkBase = tot ? (int)atomicAdd(cc, (uint32_t)tot) : 0;
+            }
+            __syncthreads();
+            if (sel) {
+                const uint32_t pos = (uint32_t)chunkBase + warpCnt[warp] + __popc(ball & ((1u << lane) - 1));
+                if (pos < (uint32_t)g.candCap) {
+                    const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
+                    out[pos] = x | (y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
+                } else {
+                    *errFlag = CSLAM_E_CAPACITY;
+                }
+            }
+            __syncthreads();
+        }
+        if (next == nr) break;
+        __syncthreads();   // end barrier
+        cur = next;
     }
 }
 
@@ -1105,6 +1179,8 @@ static int build_static_classes(cslam_frontend* fe) {
                 sk[t] = items.size() == off[t];
             }
         off[(size_t)gx * gy] = (uint32_t)items.size();
+        for (size_t t = 0; t < (size_t)gx * gy; t++) fe->L.g[l].liveCap = std::max(fe->L.g[l].liveCap, (int)(off[t + 1] - off[t]));
+        if (items.size() & 1) items.push_back(0);   // k_fast stages the lists as whole words
         if ((rc = dev_upload(fe, &fe->L.skip[l], sk)) || (rc = dev_upload(fe, &fe->L.live[l], items)) || (rc = dev_upload(fe, &fe->L.liveOff[l], off))) return rc;
     }
     return 0;
@@ -1219,6 +1295,11 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
     fe->distributeSmem = (fe->distributeSmem + 15) & ~(size_t)15;
     if (fe->distributeSmem > 200 * 1024) { set_error("nfeatures too large for the shared-memory quadtree (%zu B)", fe->distributeSmem); return fail(CSLAM_E_BADARG); }
     if (cudaFuncSetAttribute(k_distribute, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fe->distributeSmem) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
+    {   // the largest k_fast layout any front end can launch: CELL_MAX cells, a live list covering every item of a tile
+        LevelGeom gmax = {};
+        gmax.wCell = gmax.hCell = CELL_MAX; gmax.liveCap = (FAST_SW / 2) * CELL_MAX;
+        if (cudaFuncSetAttribute(k_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, fast_smem(gmax).total) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
+    }
     // ---- System::CreateUndistortRectifyMap (src/System.cpp:301-324) on the host, then quantised like cv::remap does
     // (skipped when no fisheye geometry is given: extraction-only front end, e.g. the ORBextractor facade)
     if (cam->Iw > 0 && cam->Ih > 0) {
@@ -1389,9 +1470,9 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
     }
     for (int l = 0; l < nl; l++) {
         const LevelGeom& g = L.g[l];
-        dim3 grid(cdiv(g.nColsEff, CG), g.nRowsEff, cnt);
+        dim3 grid(cdiv(g.nColsEff, CG), cdiv(g.nRowsEff, FAST_R), cnt);
         mark(fe, st, KIND_FAST);
-        k_fast<<<grid, 256, 0, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err,
+        k_fast<<<grid, 256, fast_smem(g).total, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err,
                                      L.fcols[l], useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
     }
     CSLAM_CUDA(cudaGetLastError());
