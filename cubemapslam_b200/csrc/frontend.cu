@@ -29,7 +29,8 @@ static const int CELL_MAX = 48;     // largest supported cell edge
 static const int FAST_TS = 208;     // smem tile stride (bytes), >= CG*CELL_MAX+6+3 rounded
 static const int DESC_WARPS = 4;
 
-__constant__ int c_umax[16];
+// IC_Angle's disc by column: bit v of word 15 + u is set iff |u| <= umax[v] (ORBextractor's umax), built by cslam_frontend_create
+__device__ uint32_t g_icRows[32];
 // the BRIEF pattern as k_describe reads it: word k of lane (= output byte) `lane` at [k * 32 + lane] (coalesced; the byte-per-test table above
 // read per lane was an 8-way shared-memory bank conflict). Filled by cslam_frontend_create from the same table.
 __device__ uint32_t g_patT[8 * 32];
@@ -52,8 +53,7 @@ struct DevLevels {
     uint16_t* pnode[MAX_LEVELS];       // batch x candCap scratch for k_distribute
     const uint16_t* xofs[MAX_LEVELS];  // resize tables for building level l from l-1
     const uint32_t* xab[MAX_LEVELS];   // a0 | a1<<16
-    const uint16_t* yofs[MAX_LEVELS];
-    const uint32_t* yab[MAX_LEVELS];
+    const uint4* prows[MAX_LEVELS];    // per k_pyramid row block: source window descriptor (build_pyr_rows)
     const uint8_t* skip[MAX_LEVELS];   // per k_fast CTA: 1 = tile provably corner-free when level 0 came from k_warp (no live work item)
     const uint8_t* pskip[MAX_LEVELS];  // per k_pyramid warp (PYR_WX x PYR_RY dst px): 1 = every pixel provably 0 (black corner tiles); levels >= 1
     const uint16_t* live[MAX_LEVELS];     // k_fast phase-A work items that can score above 0 on the warp path: y<<6 | (wi - w0), per CTA tile
@@ -182,21 +182,35 @@ __global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fishey
 // cv::resize(src,dst,sz,0,0,INTER_LINEAR) 8U model: 11-bit coefficients, horizontal int pass H = S[s]*a0 + S[s+1]*a1,
 // vertical (((b0*(H0>>4))>>16)+((b1*(H1>>4))>>16)+2)>>2.  One thread = 4 consecutive dst pixels x PYR_RY dst rows:
 // the 8-byte source window of the 4 pixels is fetched with aligned 32-bit loads, the taps are gathered with PRMT and the
-// horizontal pass is two-tap IDP.2A (coefficient pair a0|a1<<16 straight from the table); a source row's H is reused by the
-// next dst row when it needs it again (1.2 source rows per dst row instead of 2).
+// horizontal pass is two-tap IDP.2A (coefficient pair a0|a1<<16 straight from the table).
+// The source rows of a CTA's PYR_RY dst rows are one contiguous window (the scale factor is > 1, so consecutive dst rows have
+// distinct top taps and every window row is the top tap of at most one dst row). Its descriptor (build_pyr_rows) is read once,
+// every window row is loaded before the first arithmetic, and each window row's H is computed once; dst row k is emitted at the
+// window row of its bottom tap. WIN bounds the window (PYR_WIN at scale factors up to about 1.4, PYR_WIN_MAX up to 2.0).
 // `skip` (warp path only): one byte per warp-sized piece (128 dst px x PYR_RY rows), 1 = every pixel of the piece is provably 0
 // (the black cubemap corners, DevLevels::pskip). The buffer already holds those zeros, so the warp exits without reading or writing.
 static const int PYR_RY = 8;
 static const int PYR_WX = 32 * 4;   // dst columns per warp
+static const int PYR_WIN = 12, PYR_WIN_MAX = 20;   // window rows (and descriptor words) of the two k_pyramid instantiations
+template <int WIN>
 __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src, int sw, int sh, int spitch, uint8_t* __restrict__ dst, int dw, int dh,
                                                  int dpitch, const uint16_t* __restrict__ xofs, const uint32_t* __restrict__ xab,
-                                                 const uint16_t* __restrict__ yofs, const uint32_t* __restrict__ yab,
-                                                 const uint8_t* __restrict__ skip) {
+                                                 const uint4* __restrict__ rows, const uint8_t* __restrict__ skip) {
+    static_assert(WIN % 4 == 0 && WIN < 32, "descriptor = WIN / 4 uint4; nwin fits the top half of word 0");
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x4 >= dw) return;
     if (skip && skip[blockIdx.y * ((dw + PYR_WX - 1) / PYR_WX) + x4 / PYR_WX]) return;   // warp-uniform
+    // row-block descriptor: word 0 = first source row | window rows << 16; word j >= 1 = b0 | b1 << 16 of the dst row whose bottom tap
+    // is window row j, 0 for none (a real pair sums to 2048)
+    uint32_t rd[WIN];
+#pragma unroll
+    for (int q = 0; q < WIN / 4; q++) {
+        const uint4 v = __ldg(rows + (size_t)blockIdx.y * (WIN / 4) + q);
+        rd[4 * q] = v.x; rd[4 * q + 1] = v.y; rd[4 * q + 2] = v.z; rd[4 * q + 3] = v.w;
+    }
+    const int src0 = rd[0] & 0xffff, nwin = rd[0] >> 16;
     const uint8_t* S = src + (size_t)blockIdx.z * spitch * sh;
-    uint8_t* D = dst + (size_t)blockIdx.z * dpitch * dh;
+    uint8_t* D = dst + ((size_t)blockIdx.z * dh + (size_t)blockIdx.y * PYR_RY) * dpitch + x4;
     int s0[4]; uint32_t ab[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) { const int x = min(x4 + k, dw - 1); s0[k] = xofs[x]; ab[k] = xab[x]; }
@@ -209,30 +223,39 @@ __global__ void __launch_bounds__(128) k_pyramid(const uint8_t* __restrict__ src
         const uint32_t pr = dl | (dr << 4);
         if (k < 2) sel01 |= pr << (8 * k); else sel23 |= pr << (8 * (k - 2));
     }
-    const bool has1 = al + 4 < spitch, has2 = al + 8 < spitch;
-    auto hrow = [&](int sy, uint32_t (&H)[4]) {
-        const uint32_t* R = reinterpret_cast<const uint32_t*>(S + (size_t)sy * spitch + al);
-        const uint32_t w0 = __ldg(R), w1 = has1 ? __ldg(R + 1) : 0u, w2 = has2 ? __ldg(R + 2) : 0u;
-        const uint32_t lo = __funnelshift_r(w0, w1, sh8), hi = __funnelshift_r(w1, w2, sh8);
+    // window row j is source row min(src0 + j, sh - 1): the clamp is cv::resize's bottom tap min(a + 1, sh - 1), and it keeps the rows past
+    // nwin (loaded unconditionally, never used) inside the level. Words past the row's pitch are never selected; the last row's run into
+    // the buffer's slack
+    const uint8_t* R0 = S + (size_t)src0 * spitch + al;
+    const uint32_t last = (uint32_t)(sh - 1 - src0);
+    uint32_t w[WIN][3];
+#pragma unroll
+    for (int j = 0; j < WIN; j++) {
+        const uint32_t* R = reinterpret_cast<const uint32_t*>(R0 + (size_t)min((uint32_t)j, last) * (uint32_t)spitch);
+        w[j][0] = __ldg(R); w[j][1] = __ldg(R + 1); w[j][2] = __ldg(R + 2);
+    }
+    uint32_t Hp[4];
+#pragma unroll
+    for (int j = 0; j < WIN; j++) {
+        if (j >= nwin) break;   // CTA-uniform
+        const uint32_t lo = __funnelshift_r(w[j][0], w[j][1], sh8), hi = __funnelshift_r(w[j][1], w[j][2], sh8);
         const uint32_t p01 = __byte_perm(lo, hi, sel01), p23 = __byte_perm(lo, hi, sel23);
+        uint32_t H[4];
         H[0] = __dp2a_lo(ab[0], p01, 0u) >> 4; H[1] = __dp2a_hi(ab[1], p01, 0u) >> 4;
         H[2] = __dp2a_lo(ab[2], p23, 0u) >> 4; H[3] = __dp2a_hi(ab[3], p23, 0u) >> 4;
-    };
-    const int y0 = blockIdx.y * PYR_RY, y1 = min(y0 + PYR_RY, dh);
-    int prevIdx = -1;
-    uint32_t prev[4] = {0, 0, 0, 0};
-    for (int y = y0; y < y1; y++) {
-        const int a = yofs[y], b = min(a + 1, sh - 1);
-        const uint32_t bb = yab[y];
-        const uint32_t b0 = bb & 0xffff, b1 = bb >> 16;
-        uint32_t r0[4], r1[4];
-        if (a == prevIdx) { r0[0] = prev[0]; r0[1] = prev[1]; r0[2] = prev[2]; r0[3] = prev[3]; } else hrow(a, r0);
-        if (b == a) { r1[0] = r0[0]; r1[1] = r0[1]; r1[2] = r0[2]; r1[3] = r0[3]; } else hrow(b, r1);
-        prevIdx = b; prev[0] = r1[0]; prev[1] = r1[1]; prev[2] = r1[2]; prev[3] = r1[3];
-        uint32_t out = 0;
+        if (j > 0 && rd[j]) {   // CTA-uniform
+            // (b * H) >> 16 == umulhi(b << 16, H). The sums are < 1024 (bytes <= 255 after >> 2, no clamp needed), so two of them
+            // share a word and one shift; PRMT picks bytes 0 and 2 of each pair
+            const uint32_t B0 = rd[j] << 16, B1 = rd[j] & 0xffff0000u;
+            uint32_t s[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) out |= ((((b0 * r0[k]) >> 16) + ((b1 * r1[k]) >> 16) + 2) >> 2) << (8 * k);   // <= 255, no clamp needed
-        *reinterpret_cast<uint32_t*>(D + (size_t)y * dpitch + x4) = out;   // pitch is a multiple of 128: padding absorbs the tail
+            for (int k = 0; k < 4; k++) s[k] = __umulhi(B0, Hp[k]) + __umulhi(B1, H[k]) + 2;
+            const uint32_t s01 = s[0] | (s[1] << 16), s23 = s[2] | (s[3] << 16);
+            *reinterpret_cast<uint32_t*>(D) = __byte_perm(s01 >> 2, s23 >> 2, 0x6420);   // pitch is a multiple of 128: padding absorbs the tail
+            D += dpitch;
+        }
+#pragma unroll
+        for (int k = 0; k < 4; k++) Hp[k] = H[k];
     }
 }
 
@@ -879,16 +902,23 @@ static const int BL_STRIDE = 44;                 // blurred patch row stride in 
 __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
     __shared__ __align__(16) uint8_t s_patch[DESC_WARPS][43 * DP_STRIDE + 16];
     __shared__ __align__(16) uint16_t s_ht[DESC_WARPS][37 * DH_STRIDE + 8];
-    const int level = blockIdx.y, frame = blockIdx.z;
+    const int frame = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t* kc = A.keptCount + (size_t)frame * A.L.nlevels;
-    const int slot = blockIdx.x * DESC_WARPS + warp;
-    int offset = 0, total = 0;
-    for (int l = 0; l < A.L.nlevels; l++) { const int c = (int)kc[l]; if (l < level) offset += c; total += c; }
-    if (blockIdx.x == 0 && level == 0 && threadIdx.x == 0) A.nOut[frame] = min(total, A.kpCap);
-    if (slot >= (int)kc[level]) return;
-    const int outIdx = offset + slot;
-    if (outIdx >= A.kpCap) { if (lane == 0) *A.errFlag = CSLAM_E_CAPACITY; return; }
+    // output slot -> (level, slot in the level's kept list): lane l < MAX_LEVELS holds the inclusive prefix sum of the kept counts up to
+    // level l (the scan spans 16 lanes: lanes >= MAX_LEVELS hold partial sums and take no part below)
+    const int outIdx = blockIdx.x * DESC_WARPS + warp;
+    const int cnt = lane < A.L.nlevels ? (int)A.keptCount[(size_t)frame * A.L.nlevels + lane] : 0;
+    int incl = cnt;
+#pragma unroll
+    for (int o = 1; o < MAX_LEVELS; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+    const int total = __shfl_sync(0xffffffffu, incl, MAX_LEVELS - 1);
+    if (outIdx == 0 && lane == 0) {
+        A.nOut[frame] = min(total, A.kpCap);
+        if (total > A.kpCap) *A.errFlag = CSLAM_E_CAPACITY;
+    }
+    if (outIdx >= min(total, A.kpCap)) return;
+    const int level = __popc(__ballot_sync(0xffffffffu, lane < A.L.nlevels && incl <= outIdx));   // levels that end at or before outIdx
+    const int slot = outIdx - __shfl_sync(0xffffffffu, incl - cnt, level);
     const LevelGeom g = A.L.g[level];
     const uint8_t* I = A.L.img[level] + (size_t)frame * g.pitch * g.h;
     const uint32_t v = A.kept[((size_t)frame * A.L.nlevels + level) * A.keptCap + slot];
@@ -913,17 +943,17 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
         }
     }
     __syncwarp();
-    // ---- IC_Angle on the unblurred patch: lane = column u in [-15,15]
+    // ---- IC_Angle on the unblurred patch: lane = column u in [-15,15], rows +-v in pairs; bit v of g_icRows[lane] = (|u| <= umax[v])
     int m10 = 0, m01 = 0;
     if (lane < 31) {
         const int u = lane - HALF_PATCH;
-        int colsum = 0;
-        for (int vv = -HALF_PATCH; vv <= HALF_PATCH; vv++) {
-            const int av = vv < 0 ? -vv : vv;
-            if ((u < 0 ? -u : u) <= c_umax[av]) {
-                const int val = P[(21 + vv) * DP_STRIDE + po + 21 + u];
-                colsum += val; m01 += vv * val;
-            }
+        const uint32_t rows = __ldg(g_icRows + lane);
+        const uint8_t* col = P + 21 * DP_STRIDE + po + 21 + u;
+        int colsum = (rows & 1u) ? col[0] : 0;
+#pragma unroll
+        for (int v = 1; v <= HALF_PATCH; v++) {
+            const int lo = col[-v * DP_STRIDE], hi = col[v * DP_STRIDE];
+            if (rows & (1u << v)) { colsum += lo + hi; m01 += v * (hi - lo); }
         }
         m10 = u * colsum;
     }
@@ -931,43 +961,49 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
     for (int o = 16; o; o >>= 1) { m10 += __shfl_xor_sync(0xffffffffu, m10, o); m01 += __shfl_xor_sync(0xffffffffu, m01, o); }
     const float angle = fast_atan2_deg((float)m01, (float)m10);
     // ---- 7x7 sigma-2 Gaussian, OpenCV 8.8 fixed point [18,34,48,56,48,34,18], only where BRIEF can sample (+-18).
-    // Horizontal: 4 outputs per item from one 12-byte window with IDP.4A; stored transposed (Ht[c][r], u16, exact: <= 65280).
+    // Horizontal: 8 outputs per item from one 20-byte window with IDP.4A; stored transposed (Ht[c][r], u16, exact: <= 65280).
+    // Columns 37..39 of the last group read past the patch's 43 columns and are not stored.
     uint16_t* Ht = s_ht[warp];
     {
         const uint32_t K0123 = 18u | (34u << 8) | (48u << 16) | (56u << 24), K456 = 48u | (34u << 8) | (18u << 16);
-        for (int it = lane; it < 43 * 10; it += 32) {   // lanes = consecutive rows of one column group: loads 13 words apart, transposed stores contiguous
+        for (int it = lane; it < 43 * 5; it += 32) {   // lanes = consecutive rows of one column group: loads 13 words apart, transposed stores contiguous
             const int cg = it / 43, r = it - cg * 43;
-            const int bidx = po + 4 * cg;
+            const int bidx = po + 8 * cg;
             const uint32_t* W = reinterpret_cast<const uint32_t*>(P + r * DP_STRIDE) + (bidx >> 2);
             const int sh = (bidx & 3) * 8;
-            const uint32_t w0 = W[0], w1 = W[1], w2 = W[2], w3 = W[3];
-            const uint32_t x0 = __funnelshift_r(w0, w1, sh), x1 = __funnelshift_r(w1, w2, sh), x2 = __funnelshift_r(w2, w3, sh);
-            uint32_t h[4];
-            h[0] = __dp4a(x0, K0123, __dp4a(x1, K456, 0u));
-            h[1] = __dp4a(__funnelshift_r(x0, x1, 8), K0123, __dp4a(__funnelshift_r(x1, x2, 8), K456, 0u));
-            h[2] = __dp4a(__funnelshift_r(x0, x1, 16), K0123, __dp4a(__funnelshift_r(x1, x2, 16), K456, 0u));
-            h[3] = __dp4a(__funnelshift_r(x0, x1, 24), K0123, __dp4a(__funnelshift_r(x1, x2, 24), K456, 0u));
+            const uint32_t w0 = W[0], w1 = W[1], w2 = W[2], w3 = W[3], w4 = W[4];
+            const uint32_t x[4] = {__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh)};
+            uint32_t h[8];
 #pragma unroll
-            for (int j = 0; j < 4; j++) if (4 * cg + j < 37) Ht[(4 * cg + j) * DH_STRIDE + r] = (uint16_t)h[j];
+            for (int j = 0; j < 8; j++) {
+                const int q = j >> 2, s = (j & 3) * 8;   // output j: bytes j..j+6 of the window
+                h[j] = __dp4a(__funnelshift_r(x[q], x[q + 1], s), K0123, __dp4a(__funnelshift_r(x[q + 1], x[q + 2], s), K456, 0u));
+            }
+#pragma unroll
+            for (int j = 0; j < 8; j++) if (8 * cg + j < 37) Ht[(8 * cg + j) * DH_STRIDE + r] = (uint16_t)h[j];
         }
     }
     __syncwarp();
-    // Vertical: 4 output rows of one column per item from five u16x2 words with IDP.2A; dst = (V + 32768) >> 16
+    // Vertical: 8 output rows of one column per item from seven u16x2 words with IDP.2A; dst = (V + 32768) >> 16. Rows 37..39 of the
+    // last group read Ht rows 43..45 (inside the column's stride, never written) and are not stored.
     uint8_t* Bl = s_patch[warp];   // the raw patch is dead after the horizontal pass
     {
         const uint32_t K01 = 18u | (34u << 8), K23 = 48u | (56u << 8), K45 = 48u | (34u << 8);
-        for (int it = lane; it < 37 * 10; it += 32) {   // lanes = consecutive columns of one row group: loads 23 words apart, byte stores contiguous
+        for (int it = lane; it < 37 * 5; it += 32) {   // lanes = consecutive columns of one row group: loads 23 words apart, byte stores contiguous
             const int rg = it / 37, c = it - rg * 37;
-            const uint32_t* Hw = reinterpret_cast<const uint32_t*>(Ht + c * DH_STRIDE) + 2 * rg;
-            const uint32_t q0 = Hw[0], q1 = Hw[1], q2 = Hw[2], q3 = Hw[3], q4 = Hw[4];
-            const uint32_t s01 = __funnelshift_r(q0, q1, 16), s12 = __funnelshift_r(q1, q2, 16), s23 = __funnelshift_r(q2, q3, 16), s34 = __funnelshift_r(q3, q4, 16);
-            uint32_t o[4];
-            o[0] = __dp2a_lo(q0, K01, __dp2a_lo(q1, K23, __dp2a_lo(q2, K45, 18u * (q3 & 0xffffu))));
-            o[1] = __dp2a_lo(s01, K01, __dp2a_lo(s12, K23, __dp2a_lo(s23, K45, 18u * (q3 >> 16))));
-            o[2] = __dp2a_lo(q1, K01, __dp2a_lo(q2, K23, __dp2a_lo(q3, K45, 18u * (q4 & 0xffffu))));
-            o[3] = __dp2a_lo(s12, K01, __dp2a_lo(s23, K23, __dp2a_lo(s34, K45, 18u * (q4 >> 16))));
+            const uint32_t* Hw = reinterpret_cast<const uint32_t*>(Ht + c * DH_STRIDE) + 4 * rg;
+            uint32_t q[7], s[6];   // q[i] = rows 2i, 2i+1 of the group; s[i] = rows 2i+1, 2i+2
 #pragma unroll
-            for (int j = 0; j < 4; j++) if (4 * rg + j < 37) Bl[(4 * rg + j) * BL_STRIDE + c] = (uint8_t)((o[j] + 32768u) >> 16);
+            for (int i = 0; i < 7; i++) q[i] = Hw[i];
+#pragma unroll
+            for (int i = 0; i < 6; i++) s[i] = __funnelshift_r(q[i], q[i + 1], 16);
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                const int i = j >> 1;
+                const uint32_t* a = (j & 1) ? s : q;
+                const uint32_t o = __dp2a_lo(a[i], K01, __dp2a_lo(a[i + 1], K23, __dp2a_lo(a[i + 2], K45, 18u * ((j & 1) ? q[i + 3] >> 16 : q[i + 3] & 0xffffu))));
+                if (8 * rg + j < 37) Bl[(8 * rg + j) * BL_STRIDE + c] = (uint8_t)((o + 32768u) >> 16);
+            }
         }
     }
     __syncwarp();
@@ -1031,6 +1067,7 @@ struct cslam_frontend {
     KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     size_t distributeSmem = 0;
+    int pyrWin[MAX_LEVELS] = {};   // k_pyramid instantiation (PYR_WIN or PYR_WIN_MAX) of each level >= 1
 };
 
 static inline void mark(cslam_frontend* fe, cudaStream_t st, int kind) {
@@ -1093,6 +1130,27 @@ static void build_resize_tables(int sn, int dn, std::vector<uint16_t>& ofs, std:
         const int a0 = cv_round_f((1.f - f) * 2048.f), a1 = cv_round_f(f * 2048.f);
         ofs[d] = (uint16_t)s; ab[d] = (uint32_t)a0 | ((uint32_t)a1 << 16);
     }
+}
+
+// k_pyramid's row-block descriptors (PYR_RY dst rows each, `win` words) from the vertical resize tables; returns the window rows the
+// widest block needs, or 0 if two dst rows of a block share a top tap (impossible for a downscale)
+static int build_pyr_rows(const std::vector<uint16_t>& yo, const std::vector<uint32_t>& ya, int win, std::vector<uint32_t>& rd) {
+    const int dh = (int)yo.size(), nb = cdiv(dh, PYR_RY);
+    rd.assign((size_t)nb * win, 0u);
+    int need = 0;
+    for (int b = 0; b < nb; b++) {
+        const int y0 = b * PYR_RY, y1 = std::min(y0 + PYR_RY, dh), src0 = yo[y0];
+        const int nwin = yo[y1 - 1] - src0 + 2;   // the last dst row's bottom tap is window row nwin - 1
+        need = std::max(need, nwin);
+        if (nwin > win) continue;
+        uint32_t* r = &rd[(size_t)b * win];
+        r[0] = (uint32_t)src0 | ((uint32_t)nwin << 16);
+        for (int y = y0; y < y1; y++) {
+            if (y > y0 && yo[y] <= yo[y - 1]) return 0;
+            r[yo[y] - src0 + 1] = ya[y];
+        }
+    }
+    return need;
 }
 
 // Static pixel classes of the warp path, fixed by the geometry alone. K_0: Z = the canvas corner tiles (never written by k_warp, zeroed at
@@ -1244,7 +1302,12 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
     for (int i = 0; i < cslam_frontend::MAX_LANES; i++)
         if (cudaStreamCreateWithFlags(&fe->lane[i], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&fe->evLane[i], cudaEventDisableTiming) != cudaSuccess) { set_error("lane stream creation failed"); return fail(CSLAM_E_CUDA); }
     if (cudaEventCreateWithFlags(&fe->evFork, cudaEventDisableTiming) != cudaSuccess) { set_error("event creation failed"); return fail(CSLAM_E_CUDA); }
-    if (cudaMemcpyToSymbol(c_umax, fe->umax, sizeof(fe->umax)) != cudaSuccess) { set_error("cudaMemcpyToSymbol failed"); return fail(CSLAM_E_CUDA); }
+    {
+        uint32_t icRows[32] = {};
+        for (int u = -HALF_PATCH; u <= HALF_PATCH; u++)
+            for (int v = 0; v <= HALF_PATCH; v++) if (std::abs(u) <= fe->umax[v]) icRows[HALF_PATCH + u] |= 1u << v;
+        if (cudaMemcpyToSymbol(g_icRows, icRows, sizeof(icRows)) != cudaSuccess) { set_error("cudaMemcpyToSymbol failed"); return fail(CSLAM_E_CUDA); }
+    }
     {
         static const signed char hostPattern[1024] = {
 #include "brief_pattern.inc"
@@ -1284,8 +1347,13 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         if (l > 0) {
             std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
             build_resize_tables(fe->L.g[l - 1].w, g.w, xo, xa); build_resize_tables(fe->L.g[l - 1].h, g.h, yo, ya);
-            if ((rc = dev_upload(fe, &fe->L.xofs[l], xo)) || (rc = dev_upload(fe, &fe->L.xab[l], xa)) || (rc = dev_upload(fe, &fe->L.yofs[l], yo)) ||
-                (rc = dev_upload(fe, &fe->L.yab[l], ya))) return fail(rc);
+            std::vector<uint32_t> rd;
+            int need = build_pyr_rows(yo, ya, PYR_WIN, rd);
+            fe->pyrWin[l] = PYR_WIN;
+            if (need > PYR_WIN) { need = build_pyr_rows(yo, ya, PYR_WIN_MAX, rd); fe->pyrWin[l] = PYR_WIN_MAX; }
+            if (need < 2 || need > PYR_WIN_MAX) { set_error("pyramid level %d: unsupported resize row window (%d rows)", l, need); return fail(CSLAM_E_BADARG); }
+            const std::vector<uint4> rd4(reinterpret_cast<const uint4*>(rd.data()), reinterpret_cast<const uint4*>(rd.data() + rd.size()));
+            if ((rc = dev_upload(fe, &fe->L.xofs[l], xo)) || (rc = dev_upload(fe, &fe->L.xab[l], xa)) || (rc = dev_upload(fe, &fe->L.prows[l], rd4))) return fail(rc);
         }
     }
     fe->M = round_up(std::max(maxQuota + 4, 16), 32);
@@ -1465,8 +1533,8 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         const LevelGeom& s = L.g[l - 1]; const LevelGeom& d = L.g[l];
         dim3 grid(cdiv(cdiv(d.w, 4), 128), cdiv(d.h, PYR_RY), cnt);
         mark(fe, st, KIND_PYRAMID);
-        k_pyramid<<<grid, 128, 0, st>>>(L.img[l - 1], s.w, s.h, s.pitch, L.img[l], d.w, d.h, d.pitch, L.xofs[l], L.xab[l], L.yofs[l], L.yab[l],
-                                        useSkip ? L.pskip[l] : nullptr);
+        (fe->pyrWin[l] == PYR_WIN ? k_pyramid<PYR_WIN> : k_pyramid<PYR_WIN_MAX>)<<<grid, 128, 0, st>>>(
+            L.img[l - 1], s.w, s.h, s.pitch, L.img[l], d.w, d.h, d.pitch, L.xofs[l], L.xab[l], L.prows[l], useSkip ? L.pskip[l] : nullptr);
     }
     for (int l = 0; l < nl; l++) {
         const LevelGeom& g = L.g[l];
@@ -1486,7 +1554,7 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
     ds.L = L; ds.kept = da.kept; ds.keptCount = da.keptCount; ds.keptCap = fe->keptCap; ds.kps = d_kps; ds.desc = d_desc; ds.nOut = d_nout; ds.kpCap = fe->kpCap;
     ds.errFlag = fe->d_err;
     mark(fe, st, KIND_DESCRIBE);
-    k_describe<<<dim3(cdiv(fe->keptCap, DESC_WARPS), nl, cnt), DESC_WARPS * 32, 0, st>>>(ds);
+    k_describe<<<dim3(cdiv(fe->kpCap, DESC_WARPS), cnt), DESC_WARPS * 32, 0, st>>>(ds);
     mark(fe, st, KIND_END);
     CSLAM_CUDA(cudaGetLastError());
     return 0;
