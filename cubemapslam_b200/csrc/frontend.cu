@@ -629,10 +629,50 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
 // One CTA per (level, frame). Nodes live in shared memory, keys stay in global/L2 with a per-key node index.
 struct QNode { uint16_t ulx, uly, brx, bry; uint32_t cnt; uint32_t seq : 31; uint32_t flagE : 1; };
 
+static const int DIST_THREADS = 256;
+static const int DIST_WARPS = DIST_THREADS / 32;
+
+// Dynamic shared memory of a k_distribute CTA (byte offsets) for a node capacity of M, a multiple of 32, so every region is 16-byte aligned
+struct DistSmem {
+    int list[2];   // node lists (QNode): a round reads one and writes the other
+    int best;      // after the rounds: the best key of each node (u64), over list 0 (no node list is read after the rounds)
+    int child;     // per node 4 x u32: key count of each child, then the child's new index (a kept node's new index in entry 0)
+    int ord;       // per node u32: a candidate's split order (normal rounds: split flags, scanned in place)
+    int kids;      // per split order u32: the candidate's non-empty children, scanned in place
+    int keep;      // per node u32, finishing rounds: unsplit flags, scanned in place
+    int split;     // per node u8: divided this round
+    int total;
+};
+__host__ __device__ inline DistSmem dist_smem(int M) {
+    DistSmem m;
+    m.list[0] = 0;
+    m.list[1] = m.list[0] + M * (int)sizeof(QNode);
+    m.best = m.list[0];
+    m.child = m.list[1] + M * (int)sizeof(QNode);
+    m.ord = m.child + 16 * M;
+    m.kids = m.ord + 4 * M;
+    m.keep = m.kids + 4 * M;
+    m.split = m.keep + 4 * M;
+    m.total = (m.split + M + 15) & ~15;
+    return m;
+}
+static_assert(sizeof(unsigned long long) <= sizeof(QNode), "best[i] fits in node i of list 0");
+
+// ExtractorNode::DivideNode: a node's split point, which gives its children's bounds and the child (n1..n4 = 0..3) each key falls in
+__device__ __forceinline__ int2 node_mid(const QNode& nd) {
+    return make_int2(nd.ulx + ((nd.brx - nd.ulx + 1) >> 1), nd.uly + ((nd.bry - nd.uly + 1) >> 1));
+}
+__device__ __forceinline__ int key_child(const QNode& nd, uint32_t v) {
+    const int2 m = node_mid(nd);
+    const int x = v & 0xfff, y = (v >> 12) & 0xfff;
+    return (x < m.x ? 0 : 1) + (y < m.y ? 0 : 2);
+}
+
+// In-place exclusive scan of data[0..n) by the whole CTA, each thread over a contiguous range; returns the total. The caller's writes
+// to data must be visible (a barrier) before the call; the scan ends with a barrier.
 __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t* data, int n, uint32_t* warpSums) {
-    // in-place exclusive scan of data[0..n) by the whole block; returns the total. n <= blockDim.x * per
-    const int T = blockDim.x, tid = threadIdx.x;
-    const int per = (n + T - 1) / T;
+    const int tid = threadIdx.x;
+    const int per = (n + DIST_THREADS - 1) / DIST_THREADS;
     const int lo = min(tid * per, n), hi = min(lo + per, n);
     uint32_t s = 0;
     for (int i = lo; i < hi; i++) s += data[i];
@@ -644,14 +684,14 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t* data, int n, 
     if (lane == 31) warpSums[wid] = v;
     __syncthreads();
     if (wid == 0) {
-        uint32_t w = lane < (T >> 5) ? warpSums[lane] : 0;
+        uint32_t w = lane < DIST_WARPS ? warpSums[lane] : 0;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
         warpSums[lane] = w;
     }
     __syncthreads();
     uint32_t excl = v - s + (wid ? warpSums[wid - 1] : 0);
-    const uint32_t total = warpSums[(T >> 5) - 1];
+    const uint32_t total = warpSums[DIST_WARPS - 1];
     for (int i = lo; i < hi; i++) { uint32_t t = data[i]; data[i] = excl; excl += t; }
     __syncthreads();
     return total;
@@ -660,62 +700,81 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t* data, int n, 
 struct DistributeArgs {
     DevLevels L;
     const uint32_t* candCount;   // batch x nlevels
-    uint32_t* kept;              // batch x nlevels x keptCap : x | y<<12 | resp<<24 in LEVEL coordinates
+    uint32_t* kept;              // batch x nlevels x M : x | y<<12 | resp<<24 in LEVEL coordinates
     uint32_t* keptCount;         // batch x nlevels
     const uint8_t* mask; int maskPitch; int imgW, imgH, faceW, faceH;
-    int keptCap, M;              // M: node capacity
+    int M;                       // node capacity, and so the capacity of a (frame, level)'s kept list (one key per node)
     int* errFlag;
 };
 
-__global__ void __launch_bounds__(256) k_distribute(DistributeArgs A) {
-    extern __shared__ __align__(16) uint8_t smem_raw[];
-    const int level = blockIdx.x, frame = blockIdx.y, tid = threadIdx.x, T = blockDim.x;
-    const LevelGeom g = A.L.g[level];
-    const int M = A.M, N = g.quota;
-    QNode* listA = reinterpret_cast<QNode*>(smem_raw);
-    QNode* listB = listA + M;
-    uint32_t* childCnt = reinterpret_cast<uint32_t*>(listB + M);   // M*4 (count, later new position)
-    uint32_t* scanA = childCnt + 4 * M;                            // M
-    uint32_t* scanB = scanA + M;                                   // M
-    uint16_t* ordOf = reinterpret_cast<uint16_t*>(scanB + M);      // M  processing order of a split node
-    uint16_t* remap = ordOf + M;                                   // M
-    uint8_t* splitF = reinterpret_cast<uint8_t*>(remap + M);       // M
+// A round divides its candidates: in a normal round every node with more than one key, in list order; in a finishing round (once the
+// list is close to N) the expandable nodes in descending (count, seq), cut after the split that makes the list reach N. Steps of a round
+// (cur / nxt: the node list read / written this round; block_exclusive_scan ends with a barrier), what each reads (r) and writes (w) in
+// shared memory, and the barrier that ends it:
+//  select     r cur; w split, ord, child = 0. Normal: ord = split flags -> barrier -> ord scan: ord = split order.
+//             Finishing: ord = rank among the expandable nodes -> barrier
+//  count      r split, cur; w child = each candidate's key count per child (shared atomics) -> barrier
+//  children   r split, ord, child; w kids[ord] = the candidate's non-empty children; sh_nExp = 0 -> barrier -> kids scan: kids[o] =
+//   scan      creation rank of candidate o's first child
+//  cut        finishing only. r kids; w sh_J = the cut J -> barrier; r sh_J, ord; w split = 0 at ord >= J, keep = unsplit flags -> barrier
+//             -> keep scan: keep = rank of a kept node among the kept nodes
+//  emit       r cur, split, ord, kids, keep, child; w nxt, child = each child's new index (a kept node's in entry 0), sh_nExp -> barrier
+//  move keys  r split, cur, child; w pnode (global) -> barrier
+//  stop test  r sh_nExp; no barrier: the select barrier of the next round orders this read before the children step resets it
+// After the rounds: best (over list 0) = max per node -> barrier; the cull compacts the nodes' best keys in list order, DIST_THREADS
+// nodes at a time (a barrier after the per-warp counts, one before the next chunk rewrites them).
+__global__ void __launch_bounds__(DIST_THREADS) k_distribute(DistributeArgs A) {
+    extern __shared__ __align__(16) uint8_t dsm[];   // DistSmem
+    const int M = A.M;
+    const DistSmem SM = dist_smem(M);
+    uint32_t* const child = reinterpret_cast<uint32_t*>(dsm + SM.child);
+    uint32_t* const ord = reinterpret_cast<uint32_t*>(dsm + SM.ord);
+    uint32_t* const kids = reinterpret_cast<uint32_t*>(dsm + SM.kids);
+    uint32_t* const keep = reinterpret_cast<uint32_t*>(dsm + SM.keep);
+    uint8_t* const split = dsm + SM.split;
     __shared__ uint32_t warpSums[32];
-    __shared__ int sh_nToExpand, sh_J;
-    __shared__ uint32_t sh_base;
+    __shared__ uint32_t warpKept[DIST_WARPS];
+    __shared__ int sh_nExp, sh_J;
+    const int level = blockIdx.x, frame = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const LevelGeom g = A.L.g[level];
+    const int N = g.quota;
 
     const uint32_t nAll = A.candCount[(size_t)frame * A.L.nlevels + level];
     const int n = (int)min(nAll, (uint32_t)g.candCap);
     const uint32_t* pts = A.L.cand[level] + (size_t)frame * g.candCap;
     uint16_t* pnode = A.L.pnode[level] + (size_t)frame * g.candCap;
-    uint32_t* keptOut = A.kept + ((size_t)frame * A.L.nlevels + level) * A.keptCap;
+    uint32_t* keptOut = A.kept + ((size_t)frame * A.L.nlevels + level) * M;
     uint32_t* keptCnt = A.keptCount + (size_t)frame * A.L.nlevels + level;
     if (n == 0) { if (tid == 0) *keptCnt = 0; return; }
 
-    QNode* cur = listA; QNode* nxt = listB;
+    QNode* cur = reinterpret_cast<QNode*>(dsm + SM.list[0]);
+    QNode* nxt = reinterpret_cast<QNode*>(dsm + SM.list[1]);
     if (tid == 0) {
         QNode r; r.ulx = 0; r.uly = 0; r.brx = (uint16_t)(g.maxBX - g.minB); r.bry = (uint16_t)(g.maxBY - g.minB);
         r.cnt = (uint32_t)n; r.flagE = 0; r.seq = 0;
         cur[0] = r;
     }
-    for (int p = tid; p < n; p += T) pnode[p] = 0;
+    for (int p = tid; p < n; p += DIST_THREADS) pnode[p] = 0;
     __syncthreads();
     int nList = 1; uint32_t seqNext = 1; bool finishMode = false;
+    int nExp = 0;   // expandable nodes (flagE) in cur: the candidates of a finishing round
 
     for (int round = 0; round < 64; round++) {
         const int prevSize = nList;
-        // ---- which nodes are candidates to split, and in which order
-        int nCandSplit = 0;
+        // ---- select: the candidates and their split order
+        int nCand;
         if (!finishMode) {
-            for (int i = tid; i < nList; i += T) scanA[i] = cur[i].cnt > 1 ? 1u : 0u;
+            for (int i = tid; i < nList; i += DIST_THREADS) {
+                const bool s = cur[i].cnt > 1;
+                split[i] = s; ord[i] = s;
+                reinterpret_cast<uint4*>(child)[i] = make_uint4(0u, 0u, 0u, 0u);
+            }
             __syncthreads();
-            for (int i = tid; i < nList; i += T) splitF[i] = (uint8_t)scanA[i];
-            __syncthreads();
-            nCandSplit = (int)block_exclusive_scan(scanA, nList, warpSums);
-            for (int i = tid; i < nList; i += T) ordOf[i] = (uint16_t)scanA[i];
+            nCand = (int)block_exclusive_scan(ord, nList, warpSums);
         } else {
+            nCand = nExp;
             // rank expandable nodes by descending (count, seq): the reference sorts ascending and walks from the back
-            for (int i = tid; i < nList; i += T) {
+            for (int i = tid; i < nList; i += DIST_THREADS) {
                 int r = 0; const bool e = cur[i].flagE != 0;
                 if (e) {
                     const uint32_t ci = cur[i].cnt, si = cur[i].seq;
@@ -725,129 +784,99 @@ __global__ void __launch_bounds__(256) k_distribute(DistributeArgs A) {
                         r += (ck > ci) || (ck == ci && sk > si);
                     }
                 }
-                splitF[i] = e; ordOf[i] = (uint16_t)r; scanA[i] = e;
+                split[i] = e; ord[i] = (uint32_t)r;
+                reinterpret_cast<uint4*>(child)[i] = make_uint4(0u, 0u, 0u, 0u);
             }
             __syncthreads();
-            nCandSplit = (int)block_exclusive_scan(scanA, nList, warpSums);
         }
-        if (nCandSplit == 0) break;   // nothing can be divided (the reference would spin forever here; see DESIGN.md)
-        // ---- children populations
-        for (int i = tid; i < 4 * nList; i += T) childCnt[i] = 0;
-        __syncthreads();
-        for (int p = tid; p < n; p += T) {
+        if (nCand == 0) break;   // nothing can be divided (the reference would spin forever here; see DESIGN.md)
+        // ---- count: children populations
+        for (int p = tid; p < n; p += DIST_THREADS) {
             const int i = pnode[p];
-            if (splitF[i]) {
-                const QNode nd = cur[i];
-                const uint32_t v = pts[p];
-                const int x = v & 0xfff, y = (v >> 12) & 0xfff;
-                const int midX = nd.ulx + ((nd.brx - nd.ulx + 1) >> 1), midY = nd.uly + ((nd.bry - nd.uly + 1) >> 1);
-                atomicAdd(&childCnt[4 * i + (x < midX ? 0 : 1) + (y < midY ? 0 : 2)], 1u);
-            }
+            if (split[i]) atomicAdd(&child[4 * i + key_child(cur[i], pts[p])], 1u);
         }
         __syncthreads();
-        // ---- finishing phase: stop after the split that makes the list reach N
-        int nSplit = nCandSplit;
+        // ---- children scan: kids[o] = the creation rank of candidate o's first child (reference creation order = split order, n1..n4)
+        for (int i = tid; i < nList; i += DIST_THREADS)
+            if (split[i]) {
+                const uint4 c = reinterpret_cast<const uint4*>(child)[i];
+                kids[ord[i]] = (c.x > 0) + (c.y > 0) + (c.z > 0) + (c.w > 0);
+            }
+        if (tid == 0) sh_nExp = 0;
+        __syncthreads();
+        const uint32_t kidsTotal = block_exclusive_scan(kids, nCand, warpSums);
+        // ---- finishing cut: stop after the split that makes the list reach N. The list holds before(o) = prevSize + kids[o] - o nodes before
+        // candidate o is divided; every candidate has a non-empty child, so before() does not decrease, and before(0) = prevSize < N. The cut
+        // J is the first o with before(o) >= N, or nCand: exactly one o in 1..nCand has before(o - 1) < N and (o == nCand or before(o) >= N)
+        int J = nCand;
         if (finishMode) {
-            for (int i = tid; i < nCandSplit; i += T) scanB[i] = 0;
+            for (int o = tid + 1; o <= nCand; o += DIST_THREADS)
+                if (prevSize + (int)kids[o - 1] - (o - 1) < N && (o == nCand || prevSize + (int)kids[o] - o >= N)) sh_J = o;
             __syncthreads();
-            for (int i = tid; i < nList; i += T) if (splitF[i]) {
-                int k = 0;
-                for (int q = 0; q < 4; q++) k += childCnt[4 * i + q] > 0;
-                scanB[ordOf[i]] = (uint32_t)(k - 1);
-            }
-            if (tid == 0) sh_J = nCandSplit;
-            __syncthreads();
-            block_exclusive_scan(scanB, nCandSplit, warpSums);
-            // scanB[o] = growth before processing o; size after o = prevSize + scanB[o] + gain(o) = prevSize + scanB[o+1]
-            for (int o = tid; o < nCandSplit; o += T) {
-                const uint32_t before = prevSize + scanB[o];
-                // size after processing o >= N  <=>  the first o whose "before" is < N but after >= N
-                // after(o) = before(o+1) for o+1 < nCandSplit; handle the last one by recomputing its gain below
-                if (before >= (uint32_t)N) atomicMin(&sh_J, o);   // o-1 was the breaking split => splits = o
+            J = sh_J;
+            for (int i = tid; i < nList; i += DIST_THREADS) {
+                if (split[i] && (int)ord[i] >= J) split[i] = 0;
+                keep[i] = !split[i];
             }
             __syncthreads();
-            nSplit = sh_J;   // number of nodes actually divided (those with ord < nSplit)
-            __syncthreads();
-            for (int i = tid; i < nList; i += T) if (splitF[i] && ordOf[i] >= nSplit) splitF[i] = 0;
-            __syncthreads();
+            block_exclusive_scan(keep, nList, warpSums);
         }
-        // ---- creation ranks of children (reference creation order = processing order, n1..n4)
-        for (int i = tid; i < nSplit; i += T) scanB[i] = 0;
-        __syncthreads();
-        for (int i = tid; i < nList; i += T) {
-            if (splitF[i]) {
-                int k = 0;
-                for (int q = 0; q < 4; q++) k += childCnt[4 * i + q] > 0;
-                scanB[ordOf[i]] = (uint32_t)k;
-            }
-            scanA[i] = splitF[i] ? 0u : 1u;
-        }
-        __syncthreads();
-        const int C = (int)block_exclusive_scan(scanB, nSplit, warpSums);
-        const int nUnsplit = (int)block_exclusive_scan(scanA, nList, warpSums);
-        const int newSize = C + nUnsplit;
+        const int C = J < nCand ? (int)kids[J] : (int)kidsTotal;   // children created
+        const int newSize = C + nList - J;
         if (newSize > M) { if (tid == 0) *A.errFlag = CSLAM_E_CAPACITY; break; }
-        if (tid == 0) sh_nToExpand = 0;
-        __syncthreads();
+        // ---- emit: children at C - 1 - rank (push_front), then the kept nodes in list order
         int myExp = 0;
-        for (int i = tid; i < nList; i += T) {
+        for (int i = tid; i < nList; i += DIST_THREADS) {
             const QNode nd = cur[i];
-            if (splitF[i]) {
-                const int midX = nd.ulx + ((nd.brx - nd.ulx + 1) >> 1), midY = nd.uly + ((nd.bry - nd.uly + 1) >> 1);
-                int r = (int)scanB[ordOf[i]];
+            if (split[i]) {
+                const int2 m = node_mid(nd);
+                int r = (int)kids[ord[i]];
                 for (int q = 0; q < 4; q++) {
-                    const uint32_t c = childCnt[4 * i + q];
+                    const uint32_t c = child[4 * i + q];
                     if (c == 0) continue;
                     QNode ch;
-                    ch.ulx = (q & 1) ? midX : nd.ulx; ch.brx = (q & 1) ? nd.brx : midX;
-                    ch.uly = (q & 2) ? midY : nd.uly; ch.bry = (q & 2) ? nd.bry : midY;
+                    ch.ulx = (q & 1) ? m.x : nd.ulx; ch.brx = (q & 1) ? nd.brx : m.x;
+                    ch.uly = (q & 2) ? m.y : nd.uly; ch.bry = (q & 2) ? nd.bry : m.y;
                     ch.cnt = c; ch.flagE = c > 1; ch.seq = seqNext + r;
                     const int pos = C - 1 - r;
                     nxt[pos] = ch;
-                    childCnt[4 * i + q] = (uint32_t)pos;
+                    child[4 * i + q] = (uint32_t)pos;
                     myExp += c > 1;
                     r++;
                 }
             } else {
-                const int pos = C + (int)scanA[i];
-                QNode keep = nd; keep.flagE = 0;
-                nxt[pos] = keep;
-                remap[i] = (uint16_t)pos;
+                // a normal round splits or keeps every node, so ord[i] nodes before i were split
+                const int pos = C + (finishMode ? (int)keep[i] : i - (int)ord[i]);
+                QNode kn = nd; kn.flagE = 0;
+                nxt[pos] = kn;
+                child[4 * i] = (uint32_t)pos;
             }
         }
-        if (myExp) atomicAdd(&sh_nToExpand, myExp);
+        if (myExp) atomicAdd(&sh_nExp, myExp);
         __syncthreads();
-        for (int p = tid; p < n; p += T) {
+        // ---- move keys
+        for (int p = tid; p < n; p += DIST_THREADS) {
             const int i = pnode[p];
-            if (splitF[i]) {
-                const QNode nd = cur[i];
-                const uint32_t v = pts[p];
-                const int x = v & 0xfff, y = (v >> 12) & 0xfff;
-                const int midX = nd.ulx + ((nd.brx - nd.ulx + 1) >> 1), midY = nd.uly + ((nd.bry - nd.uly + 1) >> 1);
-                pnode[p] = (uint16_t)childCnt[4 * i + (x < midX ? 0 : 1) + (y < midY ? 0 : 2)];
-            } else {
-                pnode[p] = remap[i];
-            }
+            pnode[p] = (uint16_t)child[4 * i + (split[i] ? key_child(cur[i], pts[p]) : 0)];
         }
         __syncthreads();
-        const int nToExpand = sh_nToExpand;
+        // ---- stop test
+        nExp = sh_nExp;
         { QNode* t = cur; cur = nxt; nxt = t; }
         nList = newSize; seqNext += C;
         if (!finishMode) {
             if (nList >= N || (nList == prevSize && nList >= N / 100)) break;
-            if (nList + 3 * nToExpand > N) finishMode = true;
+            if (nList + 3 * nExp > N) finishMode = true;
         } else {
             if (nList >= N || nList == prevSize) break;
         }
-        __syncthreads();
     }
     __syncthreads();
     // ---- best key per node: max response, ties -> earliest in (cell row, cell col, y, x) order
-    // `best` aliases the inactive list buffer (M*8 bytes <= M*16).
-    unsigned long long* best = reinterpret_cast<unsigned long long*>(nxt);
-    for (int i = tid; i < nList; i += T) best[i] = 0ull;
+    unsigned long long* best = reinterpret_cast<unsigned long long*>(dsm + SM.best);
+    for (int i = tid; i < nList; i += DIST_THREADS) best[i] = 0ull;
     __syncthreads();
-    for (int p = tid; p < n; p += T) {
+    for (int p = tid; p < n; p += DIST_THREADS) {
         const uint32_t v = pts[p];
         const uint32_t x = v & 0xfff, y = (v >> 12) & 0xfff, r = v >> 24;
         const uint32_t cy = (y - 3) / g.hCell, cx = (x - 3) / g.wCell;
@@ -856,10 +885,11 @@ __global__ void __launch_bounds__(256) k_distribute(DistributeArgs A) {
         atomicMax(&best[pnode[p]], packed);
     }
     __syncthreads();
-    // ---- cull (src/ORBExtractor.cpp:883-904) in list order, ordered compaction
-    for (int base = 0; base < nList; base += T) {
-        const int i = base + tid;
-        bool keep = false; uint32_t packedOut = 0;
+    // ---- cull (src/ORBExtractor.cpp:883-904) in list order: ordered compaction by warp ballots, DIST_THREADS nodes at a time
+    uint32_t base = 0;   // keys kept from the earlier chunks
+    for (int c0 = 0; c0 < nList; c0 += DIST_THREADS) {
+        const int i = c0 + tid;
+        bool kp = false; uint32_t packedOut = 0;
         if (i < nList) {
             const unsigned long long b = best[i];
             const uint32_t key = (uint32_t)(0xffffffffffull - (b & 0xffffffffffull));
@@ -868,30 +898,29 @@ __global__ void __launch_bounds__(256) k_distribute(DistributeArgs A) {
             const float ptx = __fmul_rn((float)lx, g.scale), pty = __fmul_rn((float)ly, g.scale);
             const bool face = face_of_pixel_f(ptx, pty, A.faceW, A.faceH) >= 0;
             const int mxI = (int)__fadd_rn(ptx, 0.5f), myI = (int)__fadd_rn(pty, 0.5f);
-            keep = face && !(ptx < 0 || mxI >= A.imgW || pty < 0 || myI >= A.imgH);
-            if (keep) keep = A.mask[(size_t)myI * A.maskPitch + mxI] != 0;
+            kp = face && !(ptx < 0 || mxI >= A.imgW || pty < 0 || myI >= A.imgH);
+            if (kp) kp = A.mask[(size_t)myI * A.maskPitch + mxI] != 0;
             packedOut = lx | (ly << 12) | (r << 24);
         }
-        scanA[tid] = keep ? 1u : 0u;
+        const unsigned ball = __ballot_sync(0xffffffffu, kp);
+        if (lane == 0) warpKept[warp] = __popc(ball);
         __syncthreads();
-        const uint32_t tot = block_exclusive_scan(scanA, T, warpSums);
-        if (tid == 0 && base == 0) sh_base = 0;
-        __syncthreads();
-        if (keep) {
-            const uint32_t pos = sh_base + scanA[tid];
-            if (pos < (uint32_t)A.keptCap) keptOut[pos] = packedOut; else *A.errFlag = CSLAM_E_CAPACITY;
+        uint32_t before = 0, tot = 0;
+        for (int w = 0; w < DIST_WARPS; w++) { const uint32_t t = warpKept[w]; before += w < warp ? t : 0u; tot += t; }
+        if (kp) {
+            const uint32_t pos = base + before + __popc(ball & ((1u << lane) - 1));
+            if (pos < (uint32_t)M) keptOut[pos] = packedOut; else *A.errFlag = CSLAM_E_CAPACITY;
         }
-        __syncthreads();
-        if (tid == 0) sh_base += tot;
-        __syncthreads();
-        if (base + T >= nList && tid == 0) *keptCnt = min(sh_base, (uint32_t)A.keptCap);
+        base += tot;
+        __syncthreads();   // warpKept is rewritten by the next chunk
     }
+    if (tid == 0) *keptCnt = min(base, (uint32_t)M);
 }
 
 // ------------------------------------------------------------------------------------------------- k_describe
 struct DescribeArgs {
     DevLevels L;
-    const uint32_t* kept; const uint32_t* keptCount; int keptCap;
+    const uint32_t* kept; const uint32_t* keptCount; int M;   // M: kept-list stride (DistributeArgs)
     cslam_keypoint* kps; uint8_t* desc; int32_t* nOut; int kpCap;
     int* errFlag;
 };
@@ -921,7 +950,7 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
     const int slot = outIdx - __shfl_sync(0xffffffffu, incl - cnt, level);
     const LevelGeom g = A.L.g[level];
     const uint8_t* I = A.L.img[level] + (size_t)frame * g.pitch * g.h;
-    const uint32_t v = A.kept[((size_t)frame * A.L.nlevels + level) * A.keptCap + slot];
+    const uint32_t v = A.kept[((size_t)frame * A.L.nlevels + level) * A.M + slot];
     const int kx = v & 0xfff, ky = (v >> 12) & 0xfff, resp = v >> 24;
 
     // ---- 43x43 neighbourhood -> P[r][po + c] (REFLECT_101 at the level edges, like the blur of the apron-less clone)
@@ -1043,7 +1072,7 @@ struct cslam_frontend {
     int device = 0;
     cslam_cam_params cam;
     cslam_orb_params orb;
-    int W = 0, H = 0, CW = 0, CH = 0, maxBatch = 0, kpCap = 0, keptCap = 0, M = 0;
+    int W = 0, H = 0, CW = 0, CH = 0, maxBatch = 0, kpCap = 0, M = 0;   // M: quadtree node capacity = kept-list capacity per (frame, level)
     cudaStream_t stream = nullptr;
     DevLevels L;                     // host copy of the device-pointer table (passed by value to kernels)
     std::vector<float> scale, invScale, sigma2, invSigma2; std::vector<int> perLevel; int umax[16];
@@ -1066,7 +1095,6 @@ struct cslam_frontend {
     int lastBatch = 0;
     KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
-    size_t distributeSmem = 0;
     int pyrWin[MAX_LEVELS] = {};   // k_pyramid instantiation (PYR_WIN or PYR_WIN_MAX) of each level >= 1
 };
 
@@ -1357,12 +1385,10 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         }
     }
     fe->M = round_up(std::max(maxQuota + 4, 16), 32);
-    fe->keptCap = fe->M;
     fe->kpCap = orb->nfeatures + 3 * nl;
-    fe->distributeSmem = (size_t)fe->M * (2 * sizeof(QNode) + 4 * 4 + 4 + 4 + 2 + 2 + 1);
-    fe->distributeSmem = (fe->distributeSmem + 15) & ~(size_t)15;
-    if (fe->distributeSmem > 200 * 1024) { set_error("nfeatures too large for the shared-memory quadtree (%zu B)", fe->distributeSmem); return fail(CSLAM_E_BADARG); }
-    if (cudaFuncSetAttribute(k_distribute, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fe->distributeSmem) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
+    const int distSmem = dist_smem(fe->M).total;
+    if (distSmem > 200 * 1024) { set_error("nfeatures too large for the shared-memory quadtree (%d B)", distSmem); return fail(CSLAM_E_BADARG); }
+    if (cudaFuncSetAttribute(k_distribute, cudaFuncAttributeMaxDynamicSharedMemorySize, distSmem) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
     {   // the largest k_fast layout any front end can launch: CELL_MAX cells, a live list covering every item of a tile
         LevelGeom gmax = {};
         gmax.wCell = gmax.hCell = CELL_MAX; gmax.liveCap = (FAST_SW / 2) * CELL_MAX;
@@ -1446,7 +1472,7 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
     // ---- batch buffers
     const size_t B = max_batch;
     if ((rc = dev_alloc(fe->owned, &fe->d_fisheye, B * cam->Iw * cam->Ih, true)) || (rc = dev_alloc(fe->owned, &fe->d_candCount, B * nl, true)) ||
-        (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->keptCap, true)) || (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) ||
+        (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->M, true)) || (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) ||
         (rc = dev_alloc(fe->owned, &fe->d_kps, B * fe->kpCap, true)) || (rc = dev_alloc(fe->owned, &fe->d_desc, B * fe->kpCap * 32, true)) ||
         (rc = dev_alloc(fe->owned, &fe->d_nout, B, true)) || (rc = dev_alloc(fe->owned, &fe->d_err, 1, true))) return fail(rc);
     const size_t inBytes = std::max((size_t)cam->Iw * cam->Ih, (size_t)fe->L.g[0].pitch * fe->CH) * B;
@@ -1545,13 +1571,13 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
     }
     CSLAM_CUDA(cudaGetLastError());
     DistributeArgs da;
-    da.L = L; da.candCount = candCount; da.kept = fe->d_kept + (size_t)f0 * nl * fe->keptCap; da.keptCount = fe->d_keptCount + (size_t)f0 * nl;
+    da.L = L; da.candCount = candCount; da.kept = fe->d_kept + (size_t)f0 * nl * fe->M; da.keptCount = fe->d_keptCount + (size_t)f0 * nl;
     da.mask = fe->d_mask; da.maskPitch = fe->maskPitch;
-    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.keptCap = fe->keptCap; da.M = fe->M; da.errFlag = fe->d_err;
+    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.M = fe->M; da.errFlag = fe->d_err;
     mark(fe, st, KIND_DISTRIBUTE);
-    k_distribute<<<dim3(nl, cnt), 256, fe->distributeSmem, st>>>(da);
+    k_distribute<<<dim3(nl, cnt), DIST_THREADS, dist_smem(fe->M).total, st>>>(da);
     DescribeArgs ds;
-    ds.L = L; ds.kept = da.kept; ds.keptCount = da.keptCount; ds.keptCap = fe->keptCap; ds.kps = d_kps; ds.desc = d_desc; ds.nOut = d_nout; ds.kpCap = fe->kpCap;
+    ds.L = L; ds.kept = da.kept; ds.keptCount = da.keptCount; ds.M = fe->M; ds.kps = d_kps; ds.desc = d_desc; ds.nOut = d_nout; ds.kpCap = fe->kpCap;
     ds.errFlag = fe->d_err;
     mark(fe, st, KIND_DESCRIBE);
     k_describe<<<dim3(cdiv(fe->kpCap, DESC_WARPS), cnt), DESC_WARPS * 32, 0, st>>>(ds);

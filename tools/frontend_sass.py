@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""Static instruction budget of k_pyramid and k_describe (frontend.cu) from their sm_90a SASS; needs nvcc/cuobjdump, no GPU.
+"""Static instruction budget of k_pyramid, k_distribute and k_describe (frontend.cu) from their sm_90a SASS; needs nvcc/cuobjdump, no GPU.
 
 Compiles cubemapslam_b200/csrc/frontend.cu (or --src) for sm_90a with the library's flags, or reads --cubin, disassembles every
-instantiation of the two kernels and prints one JSON object per kernel name (template instantiations are listed separately):
+instantiation of the three kernels and prints one JSON object per kernel name (template instantiations are listed separately):
 
   registers, spill_bytes, smem_bytes   ptxas's resource report (only when this tool compiled the source)
   instructions                         static instructions of the whole kernel
+  barriers                             static BAR instructions
   straight                             static instructions outside every loop
   loops                                each loop: [start, end] byte offsets, the body's instruction count and its opcode histogram
 
@@ -25,7 +26,7 @@ from collections import Counter
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-KERNELS = ("k_pyramid", "k_describe")
+KERNELS = ("k_pyramid", "k_distribute", "k_describe")
 INSN = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P\w+\s+)?([A-Z][A-Z0-9_.x]*)([^;]*);")
 RES = re.compile(r"Used (\d+) registers")
 SMEM = re.compile(r"(\d+) bytes smem")
@@ -99,6 +100,7 @@ def main():
         inside = lambda a: any(lo <= a <= hi for lo, hi in lp)
         entry = dict(res.get(name, {}))
         entry["instructions"] = len(live)
+        entry["barriers"] = sum(1 for _, op in live if op.split(".")[0] == "BAR")
         entry["straight"] = sum(1 for a, _ in live if not inside(a))
         entry["loops"] = []
         for lo, hi in lp:
