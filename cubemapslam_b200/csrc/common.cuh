@@ -43,12 +43,13 @@ static int dev_alloc(std::vector<void*>& owned, T** p, size_t count, bool zero) 
 // cudaFree per call would cost more than many of the calls themselves. Pieces are 256-byte aligned and go to the first chunk with room; a new
 // chunk is max(request, minimum) bytes, so a call sequence of fixed shape lands on the same pieces every time and stops allocating after its
 // first call. Rules:
-// - Only public entry points call reset(), and only on entry, before anything is taken. All of a handle's work runs on its one stream, so a
-//   piece is reused only by work enqueued after the work that last used it.
+// - Only public entry points call reset(), and only on entry, before anything is taken. All of a handle's work is ordered by its one
+//   stream, so a piece is reused only by work enqueued after the work that last used it.
 // - A function that another entry point calls never resets: a host form that called a resetting _dev form would give its staged inputs
 //   away to the _dev form's scratch.
-// - Every fill or copy into arena memory is cudaMemsetAsync / cudaMemcpyAsync on the handle's stream. A legacy-stream cudaMemset /
-//   cudaMemcpy does not order against a non-blocking stream.
+// - Work on arena memory runs on the handle's stream, or on streams forked from it (the front end's lanes) if they are joined back into
+//   it and the entry point synchronises the handle's stream before it returns. Every fill or copy into arena memory is cudaMemsetAsync /
+//   cudaMemcpyAsync on one of those streams: a legacy-stream cudaMemset / cudaMemcpy does not order against a non-blocking stream.
 // - Chunks are freed only by the destructor: cudaFree synchronises the device, and a _dev call may still be in flight.
 class DevArena {
   public:

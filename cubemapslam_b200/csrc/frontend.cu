@@ -1080,19 +1080,17 @@ struct cslam_frontend {
     const WarpTile* d_wtiles = nullptr; const uint32_t* d_went = nullptr;   // k_warp tiles and their WT_W x WT_H entry tables
     int nWarpTiles = 0, warpSlot = 0;   // warpSlot: staged source box bytes per frame (largest staged box, rounded to 16)
     uint8_t* d_mask = nullptr; int maskPitch = 0;
-    uint8_t* d_fisheye = nullptr;    // staging for host entry points: maxBatch x Ih x Iw
     uint32_t* d_candCount = nullptr; // maxBatch x nlevels
     uint32_t* d_kept = nullptr; uint32_t* d_keptCount = nullptr;
-    cslam_keypoint* d_kps = nullptr; uint8_t* d_desc = nullptr; int32_t* d_nout = nullptr;
     int* d_err = nullptr;
     uint8_t* h_pin_in = nullptr; cslam_keypoint* h_pin_kps = nullptr; uint8_t* h_pin_desc = nullptr; int32_t* h_pin_n = nullptr; int* h_pin_err = nullptr;
     std::vector<void*> owned;
+    DevArena arena;                  // device staging of the host entry points: fisheye frames, key points, descriptors, counts
     static const int MAX_LANES = 4;
     cudaStream_t lane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evLane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evFork = nullptr;
     static constexpr int DEV_LANES = 2;     // lanes used by cslam_frontend_run_dev
     static constexpr int HOST_CHUNKS = 8;   // most chunks a host-buffer batch is cut into
     int64_t launches = 0;
-    int lastBatch = 0;
     KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     int pyrWin[MAX_LEVELS] = {};   // k_pyramid instantiation (PYR_WIN or PYR_WIN_MAX) of each level >= 1
@@ -1159,6 +1157,7 @@ static void build_resize_tables(int sn, int dn, std::vector<uint16_t>& ofs, std:
         ofs[d] = (uint16_t)s; ab[d] = (uint32_t)a0 | ((uint32_t)a1 << 16);
     }
 }
+struct ResizeTables { std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya; };   // level l-1 -> l, both axes
 
 // k_pyramid's row-block descriptors (PYR_RY dst rows each, `win` words) from the vertical resize tables; returns the window rows the
 // widest block needs, or 0 if two dst rows of a block share a top tap (impossible for a downscale)
@@ -1188,7 +1187,7 @@ static int build_pyr_rows(const std::vector<uint16_t>& yo, const std::vector<uin
 // From them: k_pyramid pieces inside Z_l (pskip); and, per k_fast CTA tile, the phase-A work items holding a pixel whose 7x7 window is not
 // all Z or all C (live / liveOff). Every other pixel's ring and centre are equal, so its arc score is 0 at any threshold and for any frame.
 // A tile without live items has no corner: its skip byte is set and its CTA exits before loading the tile.
-static int build_static_classes(cslam_frontend* fe) {
+static int build_static_classes(cslam_frontend* fe, const std::vector<ResizeTables>& rt) {
     enum : uint8_t { K_LIVE = 0, K_Z = 1, K_C = 2 };
     int rc;
     std::vector<uint8_t> K((size_t)fe->CW * fe->CH), Kn;
@@ -1203,17 +1202,16 @@ static int build_static_classes(cslam_frontend* fe) {
         const int w = g.w, h = g.h;
         if (l > 0) {
             const LevelGeom& sg = fe->L.g[l - 1];
-            std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
-            build_resize_tables(sg.w, w, xo, xa); build_resize_tables(sg.h, h, yo, ya);
+            const ResizeTables& r = rt[l];
             Kn.assign((size_t)w * h, K_LIVE);
             for (int y = 0; y < h; y++) {
-                const int y0 = yo[y], y1 = std::min(y0 + 1, sg.h - 1);
-                const bool unitY = (ya[y] & 0xffff) + (ya[y] >> 16) == 2048;
+                const int y0 = r.yo[y], y1 = std::min(y0 + 1, sg.h - 1);
+                const bool unitY = (r.ya[y] & 0xffff) + (r.ya[y] >> 16) == 2048;
                 for (int x = 0; x < w; x++) {
-                    const int x0 = xo[x], x1 = std::min(x0 + 1, sg.w - 1);
+                    const int x0 = r.xo[x], x1 = std::min(x0 + 1, sg.w - 1);
                     const uint8_t k = K[(size_t)y0 * sg.w + x0];
                     if (k == K_LIVE || K[(size_t)y0 * sg.w + x1] != k || K[(size_t)y1 * sg.w + x0] != k || K[(size_t)y1 * sg.w + x1] != k) continue;
-                    if (k == K_Z || (unitY && (xa[x] & 0xffff) + (xa[x] >> 16) == 2048)) Kn[(size_t)y * w + x] = k;
+                    if (k == K_Z || (unitY && (r.xa[x] & 0xffff) + (r.xa[x] >> 16) == 2048)) Kn[(size_t)y * w + x] = k;
                 }
             }
             K.swap(Kn);
@@ -1352,6 +1350,7 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
     std::memset(&fe->L, 0, sizeof(fe->L));
     fe->L.nlevels = nl;
     int maxQuota = 0;
+    std::vector<ResizeTables> rt(nl);   // entry 0 unused
     for (int l = 0; l < nl; l++) {
         LevelGeom& g = fe->L.g[l];
         g.w = cv_round_f((float)fe->CW * fe->invScale[l]); g.h = cv_round_f((float)fe->CH * fe->invScale[l]);
@@ -1373,15 +1372,15 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         if ((rc = dev_alloc(fe->owned, &fe->L.pnode[l], (size_t)max_batch * g.candCap, false))) return fail(rc);
         if ((rc = dev_upload(fe, &fe->L.fcols[l], build_fast_cols(g)))) return fail(rc);
         if (l > 0) {
-            std::vector<uint16_t> xo, yo; std::vector<uint32_t> xa, ya;
-            build_resize_tables(fe->L.g[l - 1].w, g.w, xo, xa); build_resize_tables(fe->L.g[l - 1].h, g.h, yo, ya);
+            ResizeTables& r = rt[l];
+            build_resize_tables(fe->L.g[l - 1].w, g.w, r.xo, r.xa); build_resize_tables(fe->L.g[l - 1].h, g.h, r.yo, r.ya);
             std::vector<uint32_t> rd;
-            int need = build_pyr_rows(yo, ya, PYR_WIN, rd);
+            int need = build_pyr_rows(r.yo, r.ya, PYR_WIN, rd);
             fe->pyrWin[l] = PYR_WIN;
-            if (need > PYR_WIN) { need = build_pyr_rows(yo, ya, PYR_WIN_MAX, rd); fe->pyrWin[l] = PYR_WIN_MAX; }
+            if (need > PYR_WIN) { need = build_pyr_rows(r.yo, r.ya, PYR_WIN_MAX, rd); fe->pyrWin[l] = PYR_WIN_MAX; }
             if (need < 2 || need > PYR_WIN_MAX) { set_error("pyramid level %d: unsupported resize row window (%d rows)", l, need); return fail(CSLAM_E_BADARG); }
             const std::vector<uint4> rd4(reinterpret_cast<const uint4*>(rd.data()), reinterpret_cast<const uint4*>(rd.data() + rd.size()));
-            if ((rc = dev_upload(fe, &fe->L.xofs[l], xo)) || (rc = dev_upload(fe, &fe->L.xab[l], xa)) || (rc = dev_upload(fe, &fe->L.prows[l], rd4))) return fail(rc);
+            if ((rc = dev_upload(fe, &fe->L.xofs[l], r.xo)) || (rc = dev_upload(fe, &fe->L.xab[l], r.xa)) || (rc = dev_upload(fe, &fe->L.prows[l], rd4))) return fail(rc);
         }
     }
     fe->M = round_up(std::max(maxQuota + 4, 16), 32);
@@ -1463,20 +1462,19 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         if ((rc = dev_upload(fe, &dt, tb)) || (rc = dev_upload(fe, &fe->d_went, ent))) return fail(rc);
         fe->d_wtiles = reinterpret_cast<const WarpTile*>(dt);
         if (cudaFuncSetAttribute(k_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, WARP_FPT * fe->warpSlot + 16) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
-        if ((rc = build_static_classes(fe))) return fail(rc);
+        if ((rc = build_static_classes(fe, rt))) return fail(rc);
     }
     // ---- mask
     fe->maskPitch = round_up(fe->CW, 128);
     if ((rc = dev_alloc(fe->owned, &fe->d_mask, (size_t)fe->maskPitch * fe->CH, true))) return fail(rc);
     if (cudaMemcpy2D(fe->d_mask, fe->maskPitch, mask, mask_pitch, fe->CW, fe->CH, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("mask upload failed"); return fail(CSLAM_E_CUDA); }
-    // ---- batch buffers
-    const size_t B = max_batch;
-    if ((rc = dev_alloc(fe->owned, &fe->d_fisheye, B * cam->Iw * cam->Ih, true)) || (rc = dev_alloc(fe->owned, &fe->d_candCount, B * nl, true)) ||
-        (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->M, true)) || (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) ||
-        (rc = dev_alloc(fe->owned, &fe->d_kps, B * fe->kpCap, true)) || (rc = dev_alloc(fe->owned, &fe->d_desc, B * fe->kpCap * 32, true)) ||
-        (rc = dev_alloc(fe->owned, &fe->d_nout, B, true)) || (rc = dev_alloc(fe->owned, &fe->d_err, 1, true))) return fail(rc);
-    const size_t inBytes = std::max((size_t)cam->Iw * cam->Ih, (size_t)fe->L.g[0].pitch * fe->CH) * B;
-    if (cudaMallocHost(&fe->h_pin_in, inBytes) != cudaSuccess || cudaMallocHost(&fe->h_pin_kps, B * fe->kpCap * sizeof(cslam_keypoint)) != cudaSuccess ||
+    // ---- batch buffers. The host entry points' device staging comes from the arena; its first chunk holds a max_batch call.
+    const size_t B = max_batch, fb = (size_t)cam->Iw * cam->Ih;
+    if ((rc = dev_alloc(fe->owned, &fe->d_candCount, B * nl, true)) || (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->M, true)) ||
+        (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) || (rc = dev_alloc(fe->owned, &fe->d_err, 1, true))) return fail(rc);
+    auto piece = [](size_t bytes) { return (bytes + 255) & ~(size_t)255; };   // DevArena::take's rounding
+    fe->arena.bind(fe->stream, piece(B * fb) + piece(B * fe->kpCap * sizeof(cslam_keypoint)) + piece(B * fe->kpCap * 32) + piece(B * sizeof(int32_t)));
+    if (cudaMallocHost(&fe->h_pin_in, std::max<size_t>(B * fb, 1)) != cudaSuccess || cudaMallocHost(&fe->h_pin_kps, B * fe->kpCap * sizeof(cslam_keypoint)) != cudaSuccess ||
         cudaMallocHost(&fe->h_pin_desc, B * fe->kpCap * 32) != cudaSuccess || cudaMallocHost(&fe->h_pin_n, B * sizeof(int32_t)) != cudaSuccess ||
         cudaMallocHost(&fe->h_pin_err, sizeof(int)) != cudaSuccess) { set_error("pinned host allocation failed"); return fail(CSLAM_E_CUDA); }
     *out = fe;
@@ -1586,8 +1584,12 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
     return 0;
 }
 
-static int check_batch(cslam_frontend* fe, int batch, const void* a, const void* b) {
-    if (!fe || !a || !b || batch <= 0 || batch > fe->maxBatch) { set_error("bad argument (batch must be in 1..%d)", fe ? fe->maxBatch : 0); return CSLAM_E_BADARG; }
+// the arguments every batch entry point checks (`call` names it in the message); then selects the front end's device
+static int check_batch(cslam_frontend* fe, const char* call, int batch, std::initializer_list<const void*> bufs) {
+    if (!fe || batch <= 0 || batch > fe->maxBatch || std::count(bufs.begin(), bufs.end(), nullptr)) {
+        set_error("%s: null buffer, or batch outside 1..%d", call, fe ? fe->maxBatch : 0);
+        return CSLAM_E_BADARG;
+    }
     CSLAM_CUDA(cudaSetDevice(fe->device));
     return 0;
 }
@@ -1598,17 +1600,24 @@ static bool is_pinned(const void* p) {
     return at.type == cudaMemoryTypeHost;
 }
 
-// Lanes: the batch is cut into contiguous frame ranges, each enqueued on its own stream (forked from / joined into the
-// front end's main stream). Different lanes touch disjoint slices of every buffer, so the copy engines and the
-// latency-bound k_distribute of one lane overlap with the ALU-bound kernels of the others.
-static int fork_lanes(cslam_frontend* fe, int nl) {
-    CSLAM_CUDA(cudaEventRecord(fe->evFork, fe->stream));
-    for (int i = 0; i < nl; i++) CSLAM_CUDA(cudaStreamWaitEvent(fe->lane[i], fe->evFork, 0));
-    return 0;
-}
 static int join_lanes(cslam_frontend* fe, int nl) {
     for (int i = 0; i < nl; i++) { CSLAM_CUDA(cudaEventRecord(fe->evLane[i], fe->lane[i])); CSLAM_CUDA(cudaStreamWaitEvent(fe->stream, fe->evLane[i], 0)); }
     return 0;
+}
+// Lanes: chunk ck of `nchunks` contiguous frame ranges is enqueued by fn(stream, f0, cnt) on lane ck % nlanes. The lanes are forked from the
+// main stream and joined back into it, also when fn fails; returns the first error. Chunks touch disjoint slices of every buffer, so the copy
+// engines and the latency-bound k_distribute of one lane overlap with the ALU-bound kernels of the others.
+template <class Fn>
+static int enqueue(cslam_frontend* fe, int batch, int nlanes, int nchunks, Fn&& fn) {
+    CSLAM_CUDA(cudaEventRecord(fe->evFork, fe->stream));
+    for (int i = 0; i < nlanes; i++) CSLAM_CUDA(cudaStreamWaitEvent(fe->lane[i], fe->evFork, 0));
+    int rc = 0;
+    for (int ck = 0; ck < nchunks && !rc; ck++) {
+        const int f0 = (int)((long long)batch * ck / nchunks), f1 = (int)((long long)batch * (ck + 1) / nchunks);
+        if (f1 > f0) rc = fn(fe->lane[ck % nlanes], f0, f1 - f0);
+    }
+    const int jrc = join_lanes(fe, nlanes);
+    return rc ? rc : jrc;
 }
 static int prepare_level0(cslam_frontend* fe, bool fromWarp) {
     // the warp never writes the 4 corner tiles; they must read as the reference's zeroed canvas. The warp path's k_pyramid does not
@@ -1626,66 +1635,62 @@ static int lanes_for(const cslam_frontend* fe, int batch, int want) {
     return std::max(1, std::min(std::min(want, cslam_frontend::MAX_LANES), batch));
 }
 
+// frames [f0, f0+cnt) of a host fisheye batch, through h_pin_in unless the caller's buffer is page-locked, to `dfe` and warped into level 0
+static int warp_host(cslam_frontend* fe, cudaStream_t st, const uint8_t* in, bool pinIn, uint8_t* dfe, int f0, int cnt) {
+    const size_t fb = (size_t)fe->cam.Iw * fe->cam.Ih, off = (size_t)f0 * fb;
+    const uint8_t* src = in + off;
+    if (!pinIn) { std::memcpy(fe->h_pin_in + off, src, (size_t)cnt * fb); src = fe->h_pin_in + off; }
+    CSLAM_CUDA(cudaMemcpyAsync(dfe + off, src, (size_t)cnt * fb, cudaMemcpyHostToDevice, st));
+    return launch_warp(fe, st, dfe + off, f0, cnt);
+}
+
 extern "C" int cslam_warp(cslam_frontend* fe, const uint8_t* fisheye, int batch, uint8_t* canvas, int canvas_pitch) {
-    int rc = check_batch(fe, batch, fisheye, canvas);
+    int rc = check_batch(fe, "cslam_warp", batch, {fisheye, canvas});
     if (rc) return rc;
-    if ((rc = prepare_level0(fe, true))) return rc;
-    const size_t fb = (size_t)fe->cam.Iw * fe->cam.Ih * batch;
-    const uint8_t* src = fisheye;
-    if (!is_pinned(fisheye)) { std::memcpy(fe->h_pin_in, fisheye, fb); src = fe->h_pin_in; }
-    CSLAM_CUDA(cudaMemcpyAsync(fe->d_fisheye, src, fb, cudaMemcpyHostToDevice, fe->stream));
-    if ((rc = launch_warp(fe, fe->stream, fe->d_fisheye, 0, batch))) return rc;
-    // the reference writes only the five face ROIs; corner tiles of the caller's canvas are left untouched
-    const int W = fe->W, pitch = fe->L.g[0].pitch;
-    for (int f = 0; f < batch; f++)
-        for (int t = 0; t < 5; t++) {
-            const size_t row = (size_t)FACE_TILE_ROW[t] * W, col = (size_t)FACE_TILE_COL[t] * W;
-            CSLAM_CUDA(cudaMemcpy2DAsync(canvas + (size_t)f * canvas_pitch * fe->CH + row * canvas_pitch + col, canvas_pitch,
-                                         fe->L.img[0] + (size_t)f * pitch * fe->CH + row * pitch + col, pitch, W, W, cudaMemcpyDeviceToHost, fe->stream));
-        }
+    fe->arena.reset();
+    uint8_t* dfe = nullptr;
+    if ((rc = prepare_level0(fe, true)) || (rc = fe->arena.take(&dfe, (size_t)batch * fe->cam.Iw * fe->cam.Ih))) return rc;
+    rc = enqueue(fe, batch, 1, 1, [&](cudaStream_t st, int f0, int cnt) -> int {
+        if (int rc = warp_host(fe, st, fisheye, is_pinned(fisheye), dfe, f0, cnt)) return rc;
+        // the reference writes only the five face ROIs; corner tiles of the caller's canvas are left untouched
+        const int W = fe->W, pitch = fe->L.g[0].pitch;
+        for (int f = f0; f < f0 + cnt; f++)
+            for (int t = 0; t < 5; t++) {
+                const size_t row = (size_t)FACE_TILE_ROW[t] * W, col = (size_t)FACE_TILE_COL[t] * W;
+                CSLAM_CUDA(cudaMemcpy2DAsync(canvas + (size_t)f * canvas_pitch * fe->CH + row * canvas_pitch + col, canvas_pitch,
+                                             fe->L.img[0] + (size_t)f * pitch * fe->CH + row * pitch + col, pitch, W, W, cudaMemcpyDeviceToHost, st));
+            }
+        return 0;
+    });
+    if (rc) { cudaStreamSynchronize(fe->stream); return rc; }
     return cslam_frontend_sync(fe);
 }
 
-// host entry points: H2D -> kernels -> D2H per lane; caller buffers are used directly when they are page-locked
-static int run_host(cslam_frontend* fe, const uint8_t* in, size_t inFrameBytes, int inPitch, bool fromWarp, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
+// host entry points: H2D -> kernels -> D2H per chunk; caller buffers are used directly when they are page-locked. The caller has reset the arena.
+static int run_host(cslam_frontend* fe, const uint8_t* in, int inPitch, bool fromWarp, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
+    const size_t nk = (size_t)fe->kpCap;
+    uint8_t* dfe = nullptr; cslam_keypoint* dk = nullptr; uint8_t* dd = nullptr; int32_t* dn = nullptr;
     int rc;
-    if ((rc = prepare_level0(fe, fromWarp))) return rc;
+    if ((rc = prepare_level0(fe, fromWarp)) || (fromWarp && (rc = fe->arena.take(&dfe, (size_t)batch * fe->cam.Iw * fe->cam.Ih))) ||
+        (rc = fe->arena.take(&dk, batch * nk)) || (rc = fe->arena.take(&dd, batch * nk * 32)) || (rc = fe->arena.take(&dn, (size_t)batch))) return rc;
     const int nlanes = lanes_for(fe, batch, 4);
     // the batch is cut into more chunks than there are streams (chunk c runs on stream c % nlanes): the first upload - the only one nothing overlaps -
     // is then 1/8 of the batch instead of 1/4, and the copy engines stay busy behind the kernels of earlier chunks
     const int nchunks = fe->timer.on() ? 1 : std::max(nlanes, std::min(cslam_frontend::HOST_CHUNKS, std::max(1, batch / 8)));
     const bool pinIn = is_pinned(in), pinK = is_pinned(kps), pinD = is_pinned(desc), pinN = is_pinned(n_out);
-    const size_t nk = (size_t)fe->kpCap;
-    if ((rc = fork_lanes(fe, nlanes))) return rc;
-    // errors inside the loop leave through join_lanes: a lane that was forked is always joined before this function returns
-    auto chunk = [&](int ck) -> int {
+    rc = enqueue(fe, batch, nlanes, nchunks, [&](cudaStream_t st, int f0, int cnt) -> int {
+        const int pitch = fe->L.g[0].pitch;
         int rc = 0;
-        const int f0 = (int)((long long)batch * ck / nchunks), f1 = (int)((long long)batch * (ck + 1) / nchunks), cnt = f1 - f0;
-        if (cnt <= 0) return 0;
-        cudaStream_t st = fe->lane[ck % nlanes];
-        if (fromWarp) {
-            const uint8_t* src = in + (size_t)f0 * inFrameBytes;
-            if (!pinIn) { std::memcpy(fe->h_pin_in + (size_t)f0 * inFrameBytes, src, (size_t)cnt * inFrameBytes); src = fe->h_pin_in + (size_t)f0 * inFrameBytes; }
-            uint8_t* dfe = fe->d_fisheye + (size_t)f0 * inFrameBytes;
-            CSLAM_CUDA(cudaMemcpyAsync(dfe, src, (size_t)cnt * inFrameBytes, cudaMemcpyHostToDevice, st));
-            if ((rc = launch_warp(fe, st, dfe, f0, cnt))) return rc;
-        } else {
-            const int pitch = fe->L.g[0].pitch;
-            CSLAM_CUDA(cudaMemcpy2DAsync(fe->L.img[0] + (size_t)f0 * pitch * fe->CH, pitch, in + (size_t)f0 * inPitch * fe->CH, inPitch, fe->CW, (size_t)fe->CH * cnt,
-                                         cudaMemcpyHostToDevice, st));
-        }
-        if ((rc = launch_extract(fe, st, f0, cnt, fe->d_kps + (size_t)f0 * nk, fe->d_desc + (size_t)f0 * nk * 32, fe->d_nout + f0, fromWarp))) return rc;
-        CSLAM_CUDA(cudaMemcpyAsync((pinK ? kps : fe->h_pin_kps) + (size_t)f0 * nk, fe->d_kps + (size_t)f0 * nk, (size_t)cnt * nk * sizeof(cslam_keypoint), cudaMemcpyDeviceToHost, st));
-        CSLAM_CUDA(cudaMemcpyAsync((pinD ? desc : fe->h_pin_desc) + (size_t)f0 * nk * 32, fe->d_desc + (size_t)f0 * nk * 32, (size_t)cnt * nk * 32, cudaMemcpyDeviceToHost, st));
-        CSLAM_CUDA(cudaMemcpyAsync((pinN ? n_out : fe->h_pin_n) + f0, fe->d_nout + f0, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (fromWarp) rc = warp_host(fe, st, in, pinIn, dfe, f0, cnt);
+        else CSLAM_CUDA(cudaMemcpy2DAsync(fe->L.img[0] + (size_t)f0 * pitch * fe->CH, pitch, in + (size_t)f0 * inPitch * fe->CH, inPitch, fe->CW, (size_t)fe->CH * cnt,
+                                          cudaMemcpyHostToDevice, st));
+        if (rc || (rc = launch_extract(fe, st, f0, cnt, dk + (size_t)f0 * nk, dd + (size_t)f0 * nk * 32, dn + f0, fromWarp))) return rc;
+        CSLAM_CUDA(cudaMemcpyAsync((pinK ? kps : fe->h_pin_kps) + (size_t)f0 * nk, dk + (size_t)f0 * nk, (size_t)cnt * nk * sizeof(cslam_keypoint), cudaMemcpyDeviceToHost, st));
+        CSLAM_CUDA(cudaMemcpyAsync((pinD ? desc : fe->h_pin_desc) + (size_t)f0 * nk * 32, dd + (size_t)f0 * nk * 32, (size_t)cnt * nk * 32, cudaMemcpyDeviceToHost, st));
+        CSLAM_CUDA(cudaMemcpyAsync((pinN ? n_out : fe->h_pin_n) + f0, dn + f0, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         return 0;
-    };
-    int erc = 0;
-    for (int ck = 0; ck < nchunks && !erc; ck++) erc = chunk(ck);
-    rc = join_lanes(fe, nlanes);
-    if (erc) { cudaStreamSynchronize(fe->stream); return erc; }
-    if (rc) return rc;
-    fe->lastBatch = batch;
+    });
+    if (rc) { cudaStreamSynchronize(fe->stream); return rc; }
     if ((rc = cslam_frontend_sync(fe))) return rc;
     const size_t tot = (size_t)batch * nk;
     if (!pinK) std::memcpy(kps, fe->h_pin_kps, tot * sizeof(cslam_keypoint));
@@ -1695,37 +1700,30 @@ static int run_host(cslam_frontend* fe, const uint8_t* in, size_t inFrameBytes, 
 }
 
 extern "C" int cslam_orb_extract(cslam_frontend* fe, const uint8_t* canvas, int canvas_pitch, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
-    int rc = check_batch(fe, batch, canvas, kps);
+    int rc = check_batch(fe, "cslam_orb_extract", batch, {canvas, kps, desc, n_out});
     if (rc) return rc;
-    if (!desc || !n_out || canvas_pitch < fe->CW) { set_error("cslam_orb_extract: bad argument"); return CSLAM_E_BADARG; }
-    return run_host(fe, canvas, 0, canvas_pitch, false, batch, kps, desc, n_out);
+    if (canvas_pitch < fe->CW) { set_error("cslam_orb_extract: canvas pitch %d is below the canvas width %d", canvas_pitch, fe->CW); return CSLAM_E_BADARG; }
+    fe->arena.reset();
+    return run_host(fe, canvas, canvas_pitch, false, batch, kps, desc, n_out);
 }
 
 extern "C" int cslam_frontend_run(cslam_frontend* fe, const uint8_t* fisheye, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
-    int rc = check_batch(fe, batch, fisheye, kps);
+    int rc = check_batch(fe, "cslam_frontend_run", batch, {fisheye, kps, desc, n_out});
     if (rc) return rc;
-    if (!desc || !n_out) { set_error("cslam_frontend_run: null output"); return CSLAM_E_BADARG; }
-    return run_host(fe, fisheye, (size_t)fe->cam.Iw * fe->cam.Ih, 0, true, batch, kps, desc, n_out);
+    fe->arena.reset();
+    return run_host(fe, fisheye, 0, true, batch, kps, desc, n_out);
 }
 
+// returns without synchronising, so it takes nothing from the arena
 extern "C" int cslam_frontend_run_dev(cslam_frontend* fe, const uint8_t* fisheye_dev, int batch, cslam_keypoint* kps_dev, uint8_t* desc_dev, int32_t* n_out_dev) {
-    int rc = check_batch(fe, batch, fisheye_dev, kps_dev);
-    if (rc) return rc;
-    if (!desc_dev || !n_out_dev) { set_error("cslam_frontend_run_dev: null output"); return CSLAM_E_BADARG; }
-    if ((rc = prepare_level0(fe, true))) return rc;
+    int rc = check_batch(fe, "cslam_frontend_run_dev", batch, {fisheye_dev, kps_dev, desc_dev, n_out_dev});
+    if (rc || (rc = prepare_level0(fe, true))) return rc;
     const int nlanes = lanes_for(fe, batch, cslam_frontend::DEV_LANES);
     const size_t nk = (size_t)fe->kpCap, fsz = (size_t)fe->cam.Iw * fe->cam.Ih;
-    if ((rc = fork_lanes(fe, nlanes))) return rc;
-    int erc = 0;
-    for (int ln = 0; ln < nlanes && !erc; ln++) {
-        const int f0 = (int)((long long)batch * ln / nlanes), f1 = (int)((long long)batch * (ln + 1) / nlanes), cnt = f1 - f0;
-        if (cnt <= 0) continue;
-        if ((erc = launch_warp(fe, fe->lane[ln], fisheye_dev + (size_t)f0 * fsz, f0, cnt))) break;
-        erc = launch_extract(fe, fe->lane[ln], f0, cnt, kps_dev + (size_t)f0 * nk, desc_dev + (size_t)f0 * nk * 32, n_out_dev + f0, true);
-    }
-    fe->lastBatch = batch;
-    rc = join_lanes(fe, nlanes);   // forked lanes are joined on the error path too
-    return erc ? erc : rc;
+    return enqueue(fe, batch, nlanes, nlanes, [&](cudaStream_t st, int f0, int cnt) -> int {
+        const int rc = launch_warp(fe, st, fisheye_dev + (size_t)f0 * fsz, f0, cnt);
+        return rc ? rc : launch_extract(fe, st, f0, cnt, kps_dev + (size_t)f0 * nk, desc_dev + (size_t)f0 * nk * 32, n_out_dev + f0, true);
+    });
 }
 
 extern "C" int cslam_frontend_level_size(const cslam_frontend* fe, int level, int* w, int* h) {
