@@ -26,7 +26,7 @@ static const int PATCH_SIZE = 31, HALF_PATCH = 15, EDGE_THRESHOLD = 19;
 static const int MAX_LEVELS = 16;
 static const int CG = 4;            // cells per CTA (x) in k_fast
 static const int CELL_MAX = 48;     // largest supported cell edge
-static const int FAST_TS = 208;     // smem tile stride (bytes), >= CG*CELL_MAX+6+3 rounded
+static const int FAST_TS = 224;     // smem tile stride (bytes): whole 16-byte columns of CG*CELL_MAX+6 columns from a 16-byte column
 static const int DESC_WARPS = 4;
 
 // IC_Angle's disc by column: bit v of word 15 + u is set iff |u| <= umax[v] (ORBextractor's umax), built by cslam_frontend_create
@@ -105,6 +105,10 @@ struct WarpTile {
 __device__ __forceinline__ void cp_async4_zfill(void* smem, const void* gmem, int srcBytes) {
     const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(s), "l"(gmem), "r"(srcBytes) : "memory");
+}
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {   // both 16-byte aligned
+    const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem) : "memory");
 }
 
 __global__ void __launch_bounds__(256) k_warp(const uint8_t* __restrict__ fisheye, int Iw, int Ih, const WarpTile* __restrict__ tiles,
@@ -317,16 +321,21 @@ __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d -
 //     (DevLevels::live), so its scores are 0, which the zeroed S already holds
 //  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the same items as A -> shared list; a keypoint at
 //     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
-//  C  compaction of the selected entries into the global candidate list (one global atomic per 256 entries)
+//  C  the selected entries (the per-cell fallback filter) appended to the strip's output buffer, one shared atomic per warp; the buffer is
+//     copied to the global candidate list (one global atomic) at the end of the strip, or at the end of a tile after which it could not
+//     hold another tile's survivors
 static const int FAST_R = 8;            // cell rows per k_fast CTA
 static const int FAST_SW = FAST_TS / 2;   // pair-words per score row
-static_assert((CG * CELL_MAX + 9) / 4 < 64 && CELL_MAX < 1024, "a live work item packs y<<6 | (wi - w0) into 16 bits");
+static const int FAST_OUT = CG * ((CELL_MAX + 1) / 2) * ((CELL_MAX + 1) / 2);   // candidates the strip's output buffer holds: >= any kmax
+static_assert(16 * ((15 + CG * CELL_MAX + 6 + 15) / 16) <= FAST_TS && FAST_TS / 16 <= 16,
+              "a tile row is at most FAST_TS / 16 <= 16 columns of 16 bytes (k_fast stages a row with 16 lanes)");
+static_assert((15 + CG * CELL_MAX + 6) / 4 < 64 && CELL_MAX < 1024, "a live work item packs y<<6 | (wi - w0) into 16 bits");
 static_assert(CG <= 4, "FastItem packs a pixel's cell index into 2 bits");
 
-// Column geometry of the k_fast CTA tile in tile column cx (blockIdx.x) of a level. The tile's rows start at a0 = tx0 & ~3 (word-aligned
+// Column geometry of the k_fast CTA tile in tile column cx (blockIdx.x) of a level. The tile's rows start at a0 = tx0 & ~15 (16-byte
 // loads); work item wi covers tile columns 4*wi..4*wi+3, and detection x = tile column - xoff.
 struct FastTileX {
-    int tx0, a0, nwords;   // first ROI column, first loaded column, loaded words per row
+    int tx0, a0, nvec;     // first ROI column, first loaded column, loaded 16-byte columns per row
     int nx, xoff;          // detection width, tile column of detection x = 0
     int w0, w1;            // work items [w0, w1) cover the detection columns
     int q0, q1;            // uint4 columns [q0, q1) of an S2 row cover the pair-words phase B reads, [2*w0 - 1, 2*w1 + 1)
@@ -336,7 +345,7 @@ __host__ __device__ inline FastTileX fast_tile_x(const LevelGeom& g, int cx) {
     const int j0 = cx * CG, ncell = min(CG, g.nColsEff - j0);
     t.tx0 = g.minB + j0 * g.wCell;
     const int tx1 = min(t.tx0 + ncell * g.wCell + 6, g.maxBX);
-    t.a0 = t.tx0 & ~3; t.nwords = (tx1 - t.a0 + 3) >> 2;
+    t.a0 = t.tx0 & ~15; t.nvec = (tx1 - t.a0 + 15) >> 4;   // tx1 + 15 <= maxBX + 15 < w: the last column stays inside the row
     t.nx = tx1 - t.tx0 - 6; t.xoff = t.tx0 - t.a0 + 3;
     t.w0 = t.xoff >> 2; t.w1 = (t.xoff + t.nx + 3) >> 2;
     t.q0 = max(2 * t.w0 - 1, 0) >> 2; t.q1 = (t.w1 + 2) >> 1;
@@ -351,7 +360,7 @@ struct FastItem {
 };
 // Everything k_fast needs that depends on the tile column alone; built once per level at create time (build_fast_cols)
 struct FastCols {
-    uint32_t mgWords, mgItems, mgZero, pad;   // fdiv_magic of nwords, w1 - w0 and q1 - q0
+    uint32_t mgItems, mgZero, pad[2];   // fdiv_magic of w1 - w0 and q1 - q0
     FastItem item[FAST_SW / 2];
 };
 
@@ -361,12 +370,12 @@ struct FastSmem {
     int tile, tileBytes;       // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
                                // then hCell + 6 rows of FAST_TS
     int s2, klist;             // score map (hCell + 2 rows of FAST_SW pair-words); NMS survivors, kmax entries
-    int live, liveBytes;       // live list buffer b (u16, staged from an even index: liveCap + 1 entries) at live + b * liveBytes
+    int live, liveBytes;       // live list buffer b (u16, staged in 16-byte pieces from an index that is a multiple of 8) at live + b * liveBytes
     int kmax, total;
 };
 __host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
     FastSmem m;
-    m.tileBytes = 16 + (g.hCell + 6) * FAST_TS; m.liveBytes = (2 * g.liveCap + 2 + 15) & ~15;
+    m.tileBytes = 16 + (g.hCell + 6) * FAST_TS; m.liveBytes = 16 * ((g.liveCap + 14) / 8);
     m.kmax = CG * ((g.wCell + 1) / 2) * ((g.hCell + 1) / 2);   // NMS survivors of a cell are pairwise non-adjacent
     m.items = 0;
     m.tile = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);
@@ -400,14 +409,21 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
     const uint4* const items = reinterpret_cast<const uint4*>(fsm + SM.items);   // FastItem wi = items[2*wi], items[2*wi+1]
     __shared__ uint32_t rowLo[FAST_R], rowHi[FAST_R];   // live list of each strip row, [rowLo, rowHi)
     __shared__ int rowVisit[FAST_R];                    // the strip row's tile has work (not skipped, detection rows > 0)
+    __shared__ uint32_t sout[FAST_OUT];   // the strip's selected candidates, packed as in cand
     __shared__ int cnt20[CG];
-    __shared__ int nK, chunkBase;
-    __shared__ int warpCnt[8];
+    __shared__ int nK, nOut, flushN;
+    __shared__ uint32_t flushBase;
     const int frame = blockIdx.z, row0 = blockIdx.y * FAST_R, nr = min(FAST_R, g.nRowsEff - row0);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const FastTileX X = fast_tile_x(g, blockIdx.x);
-    const int nx = X.nx, xoff = X.xoff, w0 = X.w0, nw = X.w1 - X.w0;
-    if (nx <= 0) return;   // block-uniform: a ROI with fewer than 7 columns has no detection area (cv::FAST returns nothing)
+    const int tid = threadIdx.x, lane = tid & 31;
+    // the tile column's geometry and division magics, read from shared memory after each barrier rather than held in registers across phase A
+    __shared__ FastTileX X;
+    __shared__ uint2 mg;   // FastCols::mgItems, mgZero
+    const FastCols* C = cols + blockIdx.x;
+    {
+        const FastTileX t = fast_tile_x(g, blockIdx.x);
+        if (t.nx <= 0) return;   // block-uniform: a ROI with fewer than 7 columns has no detection area (cv::FAST returns nothing)
+        if (tid == 0) { X = t; mg = __ldg(reinterpret_cast<const uint2*>(C)); }
+    }
     const uint8_t* I = img + (size_t)frame * g.pitch * g.h;
     for (int i = tid; i < nr; i += 256) {
         const int t = (row0 + i) * gridDim.x + blockIdx.x, iniY = g.minB + (row0 + i) * g.hCell;
@@ -415,78 +431,90 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         rowVisit[i] = min(iniY + g.hCell + 6, g.maxBY) - iniY > 6 && !(skip && skip[t]);
         if (live) { rowLo[i] = liveOff[t]; rowHi[i] = liveOff[t + 1]; }
     }
+    if (tid == 0) nOut = 0;
     __syncthreads();
     int cur = 0;
     while (cur < nr && !rowVisit[cur]) cur++;
     if (cur == nr) return;
-    const FastCols* C = cols + blockIdx.x;
-    const uint4 mg = __ldg(reinterpret_cast<const uint4*>(C));
     // cv::FAST clamps its threshold to 0..255 and ranks corners by s - 1, with 0 for "no corner": at threshold 0 a corner with s = 1 ties
     // with its non-corner neighbours and never survives NMS, exactly as if the threshold were 1
     const int mt = min(max(minTh, 1), 255);
     const uint32_t T = (uint32_t)mt * 0x01000100u;
-    const int nwords = X.nwords;
-    // strip row i's tile rows (4-byte copies: a0 is only word-aligned) and live list (from the even index below rowLo) into buffer b
+    // strip row i's tile rows and live list (from the multiple of 8 at or below rowLo) into buffer b, by 16-byte copies: a0 and the level
+    // pitch are multiples of 16. Thread tid copies 16-byte column tid % 16 of tile rows tid / 16, tid / 16 + 16, ... (a row has at most 16)
     auto stage = [&](int i, int b) {
-        const int iniY = g.minB + (row0 + i) * g.hCell, nrows = min(iniY + g.hCell + 6, g.maxBY) - iniY;
-        const uint8_t* base = I + (size_t)iniY * g.pitch + X.a0;
-        uint8_t* tile = fsm + SM.tile + b * SM.tileBytes + 16;
-        for (int k = tid; k < nwords * nrows; k += 256) {
-            const int r = fdiv_small(k, mg.x), wd = k - r * nwords;
-            cp_async4_zfill(tile + r * FAST_TS + 4 * wd, base + (size_t)r * g.pitch + 4 * wd, 4);
-        }
+        const int iniY = g.minB + (row0 + i) * g.hCell, nrows = min(iniY + g.hCell + 6, g.maxBY) - iniY, vc = tid & 15;
+        const uint8_t* base = I + (size_t)iniY * g.pitch + X.a0 + 16 * vc;
+        uint8_t* tile = fsm + SM.tile + b * SM.tileBytes + 16 + 16 * vc;
+        if (vc < X.nvec)
+#pragma unroll 1
+            for (int r = tid >> 4; r < nrows; r += 16) cp_async16(tile + r * FAST_TS, base + (size_t)r * g.pitch);
         if (live) {
-            const uint32_t lo = rowLo[i] & ~1u, n = (rowHi[i] - lo + 1) >> 1;   // the list is padded to an even length
-            const uint32_t* src = reinterpret_cast<const uint32_t*>(live + lo);
-            for (uint32_t k = tid; k < n; k += 256) cp_async4_zfill(fsm + SM.live + b * SM.liveBytes + 4 * k, src + k, 4);
+            const uint32_t lo = rowLo[i] & ~7u, n = (rowHi[i] - lo + 7) >> 3;   // the list is padded to a multiple of 8 entries
+            const uint4* src = reinterpret_cast<const uint4*>(live + lo);
+            for (uint32_t k = tid; k < n; k += 256) cp_async16(fsm + SM.live + b * SM.liveBytes + 16 * k, src + k);
         }
         asm volatile("cp.async.commit_group;\n" ::: "memory");
     };
-    for (int k = tid; k < (int)(sizeof(FastItem) / 16) * (FAST_SW / 2); k += 256) {
-        const uint32_t s = (uint32_t)__cvta_generic_to_shared(fsm + SM.items + 16 * k);
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(reinterpret_cast<const uint4*>(C->item) + k) : "memory");
-    }
+    for (int k = tid; k < (int)(sizeof(FastItem) / 16) * (FAST_SW / 2); k += 256) cp_async16(fsm + SM.items + 16 * k, reinterpret_cast<const uint4*>(C->item) + k);
     stage(cur, 0);   // same group as the item table
+    // the strip's output buffer to the frame's candidate list. Called after a barrier that follows every append to it (block-uniform); the
+    // next appends come after at least one more barrier, which also publishes nOut = 0. The count grows past candCap like the list would.
+    auto flush = [&]() {
+        if (tid == 0) { const int n = nOut; flushN = n; flushBase = atomicAdd(candCount + (size_t)frame * countStride, (uint32_t)n); }
+        __syncthreads();
+        if (tid == 0) nOut = 0;
+        const int n = flushN;
+        uint32_t* out = cand + (size_t)frame * g.candCap;
+        for (int i = tid; i < n; i += 256) {
+            const uint32_t pos = flushBase + i;
+            if (pos < (uint32_t)g.candCap) out[pos] = sout[i];
+            else *errFlag = CSLAM_E_CAPACITY;
+        }
+    };
     // Barriers of one tile (buffer b = tile parity in the strip):
     //  top   S2 cleared, nK / cnt20 reset: the previous tile's phases B and C are done with them (its end barrier)
     //  wait  this thread's copies of the tile landed; B1 (__syncthreads_or) makes every thread's copies visible
     //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phases A and B, before its B3
-    //  A  -> B2 -> B (S2, item table, live list of b) -> B3 -> C (klist, nK, cnt20; its own barriers per chunk) -> end barrier
+    //  A  -> B2 -> B (S2, item table, live list of b) -> B3 -> C (klist, nK, cnt20; appends to the output buffer) -> end barrier
+    //  after the end barrier: flush when the buffer could not hold another tile's kmax entries, and at the end of the strip (one barrier
+    //  more; the next appends follow the next tile's B1)
     for (int b = 0;; b ^= 1) {
         const int iniY = g.minB + (row0 + cur) * g.hCell, maxY = min(iniY + g.hCell + 6, g.maxBY);
         const int nrows = maxY - iniY, ny = nrows - 6;   // detection rows
         const uint8_t* const tile = fsm + SM.tile + b * SM.tileBytes + 16;
-        const uint16_t* const liveS = reinterpret_cast<const uint16_t*>(fsm + SM.live + b * SM.liveBytes) + (rowLo[cur] & 1u);
+        const uint16_t* const liveS = reinterpret_cast<const uint16_t*>(fsm + SM.live + b * SM.liveBytes) + (rowLo[cur] & 7u);
         const uint32_t nLive = live ? rowHi[cur] - rowLo[cur] : 0u;
         // S2 must read 0 around the scored area (rows 0 and ny+1, the pair-words left/right of [2*w0, 2*w1)) and wherever phase A skips an item
         {
-            const int q0 = X.q0, nq = X.q1 - X.q0;
+            const int q0 = X.q0, nq = X.q1 - X.q0; const uint32_t mgZero = mg.y;
             for (int i = tid; i < (ny + 2) * nq; i += 256) {
-                const int r = fdiv_small(i, mg.z);
+                const int r = fdiv_small(i, mgZero);
                 reinterpret_cast<uint4*>(S2 + r * FAST_SW)[q0 + i - r * nq] = make_uint4(0u, 0u, 0u, 0u);
             }
         }
         if (tid < CG) cnt20[tid] = 0;
         if (tid == 0) nK = 0;
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-        // caller canvases: an all-zero tile has no corners at any threshold (OR of the words this thread staged)
+        // caller canvases: an all-zero tile has no corners at any threshold (OR of the columns this thread staged)
         uint32_t acc = live ? 1u : 0u;
-        if (!live)
-            for (int k = tid; k < nwords * nrows; k += 256) {
-                const int r = fdiv_small(k, mg.x);
-                acc |= reinterpret_cast<const uint32_t*>(tile + r * FAST_TS)[k - r * nwords];
+        if (!live && (tid & 15) < X.nvec)
+            for (int r = tid >> 4; r < nrows; r += 16) {
+                const uint4 v = *reinterpret_cast<const uint4*>(tile + r * FAST_TS + 16 * (tid & 15));
+                acc |= v.x | v.y | v.z | v.w;
             }
         const int any = __syncthreads_or(acc);   // B1
         int next = cur + 1;
         while (next < nr && !rowVisit[next]) next++;
         if (next < nr) stage(next, b ^ 1);
-        if (!any) {   // nothing reads S2, the counters or buffer b after B1
+        if (!any) {   // nothing reads S2, the counters or buffer b after B1 (the output buffer is as the last end barrier left it)
             if (next == nr) break;
             cur = next;
             continue;
         }
         // ---- A
         {
+            const int w0 = X.w0;
             auto score_item = [&](int y, int wi) {
                 const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
                 const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
@@ -539,7 +567,8 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
             if (live) {
                 for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; score_item(e >> 6, w0 + (e & 63)); }
             } else {
-                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); score_item(y, w0 + (it - y * nw)); }
+                const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
+                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgItems); score_item(y, w0 + (it - y * nw)); }
             }
         }
         __syncthreads();
@@ -548,6 +577,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
         // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
         {
+            const int w0 = X.w0, xoff = X.xoff;
             auto nms_item = [&](int y, int wi) {
                 const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
                 const uint4 hd = items[2 * wi];
@@ -578,46 +608,36 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
             if (live) {
                 for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; nms_item(e >> 6, w0 + (e & 63)); }
             } else {
-                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mg.y); nms_item(y, w0 + (it - y * nw)); }
+                const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
+                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgItems); nms_item(y, w0 + (it - y * nw)); }
             }
         }
         __syncthreads();
-        // ---- C
-        uint32_t* out = cand + (size_t)frame * g.candCap;
-        uint32_t* cc = candCount + (size_t)frame * countStride;
+        // ---- C: each warp filters its stride of klist and appends with one shared atomic; the buffer has room for nk <= kmax entries
         const int nk = min(nK, SM.kmax);
-        for (int base = 0; base < nk; base += 256) {
-            const int i = base + tid;
-            uint32_t e = 0; bool sel = false;
-            if (i < nk) {
-                e = klist[i];
+#pragma unroll 1
+        for (int i = tid - lane; i < nk; i += 256) {   // warp-uniform bounds
+            uint32_t v = 0; bool sel = false;
+            if (i + lane < nk) {
+                const uint32_t e = klist[i + lane];
                 const int sv = (e >> 16) & 0xff, cell = e >> 24;
                 sel = cnt20[cell] > 0 ? sv > iniTh : true;
+                const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
+                v = x | (y << 12) | ((uint32_t)(sv - 1) << 24);
             }
             const unsigned ball = __ballot_sync(0xffffffffu, sel);
-            if (lane == 0) warpCnt[warp] = __popc(ball);
-            __syncthreads();
-            if (tid == 0) {
-                int tot = 0;
-                for (int w = 0; w < 8; w++) { const int t = warpCnt[w]; warpCnt[w] = tot; tot += t; }
-                chunkBase = tot ? (int)atomicAdd(cc, (uint32_t)tot) : 0;
-            }
-            __syncthreads();
-            if (sel) {
-                const uint32_t pos = (uint32_t)chunkBase + warpCnt[warp] + __popc(ball & ((1u << lane) - 1));
-                if (pos < (uint32_t)g.candCap) {
-                    const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
-                    out[pos] = x | (y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
-                } else {
-                    *errFlag = CSLAM_E_CAPACITY;
-                }
-            }
-            __syncthreads();
+            if (ball == 0) continue;
+            int pos = 0;
+            if (lane == 0) pos = atomicAdd(&nOut, __popc(ball));
+            pos = __shfl_sync(0xffffffffu, pos, 0);
+            if (sel) sout[pos + __popc(ball & ((1u << lane) - 1))] = v;
         }
-        if (next == nr) break;
         __syncthreads();   // end barrier
+        if (next == nr) break;
+        if (nOut > FAST_OUT - SM.kmax) flush();
         cur = next;
     }
+    if (nOut > 0) flush();   // after the last tile's end barrier or B1
 }
 
 // ------------------------------------------------------------------------------------------------- k_distribute
@@ -1238,7 +1258,7 @@ static int build_static_classes(cslam_frontend* fe, const std::vector<ResizeTabl
                 for (int d = -3; d <= 3 && same; d++) same = Hr[(size_t)(y + d) * w + x] == k;
                 if (same) U[(size_t)y * w + x] = k;
             }
-        // work items in k_fast's order and geometry (tile rows iniY.., tile columns from a0 = tx0 & ~3, item = tile word wi of detection row y)
+        // work items in k_fast's order and geometry (tile rows iniY.., tile columns from a0 = tx0 & ~15, item = tile word wi of detection row y)
         const int gx = cdiv(g.nColsEff, CG), gy = g.nRowsEff;
         std::vector<FastTileX> tx(gx);
         for (int cxg = 0; cxg < gx; cxg++) tx[cxg] = fast_tile_x(g, cxg);
@@ -1264,7 +1284,7 @@ static int build_static_classes(cslam_frontend* fe, const std::vector<ResizeTabl
             }
         off[(size_t)gx * gy] = (uint32_t)items.size();
         for (size_t t = 0; t < (size_t)gx * gy; t++) fe->L.g[l].liveCap = std::max(fe->L.g[l].liveCap, (int)(off[t + 1] - off[t]));
-        if (items.size() & 1) items.push_back(0);   // k_fast stages the lists as whole words
+        while (items.size() & 7) items.push_back(0);   // k_fast stages the lists in 16-byte pieces
         if ((rc = dev_upload(fe, &fe->L.skip[l], sk)) || (rc = dev_upload(fe, &fe->L.live[l], items)) || (rc = dev_upload(fe, &fe->L.liveOff[l], off))) return rc;
     }
     return 0;
@@ -1278,7 +1298,7 @@ static std::vector<FastCols> build_fast_cols(const LevelGeom& g) {
         const FastTileX t = fast_tile_x(g, (int)cx);
         FastCols& c = cols[cx];
         if (t.nx <= 0) continue;   // k_fast exits before reading the table
-        c.mgWords = fdiv_magic(t.nwords); c.mgItems = fdiv_magic(t.w1 - t.w0); c.mgZero = fdiv_magic(t.q1 - t.q0);
+        c.mgItems = fdiv_magic(t.w1 - t.w0); c.mgZero = fdiv_magic(t.q1 - t.q0);
         for (int wi = 0; wi < FAST_SW / 2; wi++)
             for (int j = 0; j < 4; j++) {
                 const int x = 4 * wi + j - t.xoff;   // detection x of tile column 4*wi + j

@@ -6,7 +6,9 @@ object:
 
   registers, spill_bytes, smem_bytes   ptxas's resource report for k_fast (only when this tool compiled it)
   prologue                             instructions before the strip loop: total and the integer-division opcodes (I2F, MUFU, F2I)
-  strip                                the loop over a CTA's cell rows (a loop with a barrier around >= 64 VIMNMX3 / VIMNMX: it holds phases A to C)
+  strip                                the loop over a CTA's cell rows (a loop with a barrier around >= 64 VIMNMX3 / VIMNMX: it holds phases A to C),
+                                       with its BAR and ATOMG counts (`bar`, `atomg`: every path of one pass, flush of the output buffer included)
+  staging                              each tile-staging loop (a loop whose body issues cp.async, LDGSTS, and no score arithmetic)
   phase_a                              each scoring loop (a loop without a barrier whose body issues >= 64 VIMNMX3 / VIMNMX), `live` when its body loads
                                        the u16 live list (staged in shared memory)
   phase_b                              each NMS loop (a loop with a shared-memory atomic and no barrier)
@@ -95,19 +97,22 @@ def main():
             cubin = os.path.join(tmp, "frontend.cubin")
             res = compile_cubin(cubin)
         insns = k_fast_sass(cubin)
-    strip, phase_a, phase_b = [], [], []
+    strip, phase_a, phase_b, staging = [], [], [], []
     for lo, hi in loops(insns):
         b = body(insns, lo, hi)
         h = hist(b)
         entry = {"range": [hex(lo), hex(hi)], "instructions": len(b), "histogram": h}
         minmax = h.get("VIMNMX3", 0) + h.get("VIMNMX", 0)
         if minmax >= 64 and h.get("BAR", 0):
+            entry["bar"], entry["atomg"] = h.get("BAR", 0), h.get("ATOMG", 0)
             strip.append(entry)
         elif minmax >= 64:
             entry["live"] = any(op.startswith("LDS") and ".U16" in op for op, _ in b)
             phase_a.append(entry)
         elif h.get("ATOMS", 0) and not h.get("BAR", 0):
             phase_b.append(entry)
+        elif h.get("LDGSTS", 0):
+            staging.append(entry)
     first_a = min((int(e["range"][0], 16) for e in strip + phase_a), default=insns[-1][0] + 1)
     pro = [op for a, op, _ in insns if a < first_a and op != "NOP"]
     pro_h = Counter(op.split(".")[0] for op in pro)
@@ -116,6 +121,7 @@ def main():
     out["strip"] = strip
     out["phase_a"] = phase_a
     out["phase_b"] = phase_b
+    out["staging"] = staging
     print(json.dumps(out, indent=1))
 
 
