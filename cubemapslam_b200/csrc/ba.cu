@@ -16,10 +16,10 @@
 //                    with the right-hand side carried as an extra row; panel factorisation and trailing update spread over
 //                    the cluster's SMs, panels exchanged through L2, cluster barriers between phases; no size cap
 //   k_ba_backsub / k_ba_update / k_ba_scale / k_ba_restore   landmark back-substitution, oplus (with backup), gain-ratio scale
-// Multi-GPU: landmarks (with their edges) are sharded l % nranks; every rank forms its partial [S | g | bpr | chi2 | scale]
-// and the partials are summed either by one ncclAllReduce or by the one-shot NVLink kernel k_ba_xchg_reduce (peer pointers),
-// in fixed rank order so that every rank solves bit-identical systems. Payloads are double-buffered by epoch parity: a rank may run one
-// exchange ahead of a peer that is still reading the previous one.
+// Multi-GPU: landmarks (with their edges) are sharded l % nranks; every rank forms its partial reduced system [S | g | bpr] and the
+// partials are summed either by one ncclAllReduce or by the one-shot NVLink kernel k_ba_xchg_reduce (peer pointers), in fixed rank order
+// so that every rank solves bit-identical systems. The trial's scalars (chi2, scale) travel through k_ba_small_xchg. Payloads are
+// double-buffered by epoch parity: a rank may run one exchange ahead of a peer that is still reading the previous one.
 // LM control flow (accept/reject, lambda schedule, ORB-SLAM2's stop rule, pbStopFlag) stays on the host like in the reference.
 #include <cooperative_groups.h>
 #include <dlfcn.h>
@@ -33,6 +33,9 @@ namespace cg = cooperative_groups;
 
 namespace cslam {
 
+// Ownership: landmark l belongs to rank l % nranks, and a rank's edge arrays hold only the edges of its own landmarks. Everything below is
+// built from those edges, so another rank's landmark has an empty lmStart range and is inactive (ptAct == 0): kernels over edges, tuples
+// or active landmarks need no owner test. Only k_ba_mask_points makes one, when the points of all ranks are summed.
 struct BADev {
     int nKF, nMP, nE, nQ, nP, n;     // nQ non-fixed key frames (static per call), nP active free poses, n = 6 nP
     double f;                        // fx=fy=cx=cy
@@ -49,17 +52,15 @@ struct BADev {
     const long long* pairStart;      // nQ*nQ+1: co-observation list of (q1,q2), q1<=q2, row-major
     const int4* tuples;              // (a1, a2, landmark, -): the landmark rides along so that k_ba_schur has no tuple -> edge -> landmark load chain
     double *Hpp, *bp, *Hll, *bl, *Hpl, *Dinv, *db, *xp, *xl;
-    double *S, *g, *bpr, *tail;      // one contiguous exchange buffer: [S n*n | g n | bpr n | tail 4]; tail = chi2, scale, -, -
+    double *S, *bpr;                 // the reduced camera system [S n*n | g n | bpr n] in BAHost::red; k_ba_solve reads g as row n of S
     double* scal;                    // [0] chi2, [1] scale, [2] max diag (as bits), [3] solve flag, [4] lambda of the current trial
     double* part; unsigned* ticket;  // block partials + arrival counter of the deterministic grid reductions
     double* posePart; unsigned* poseTicket;   // k_ba_lin_poses: slice sums [nQ][POSE_SPLIT][27] + arrival counter per pose
     int robust; double delta, dsqr;
-    int rank, nranks;                // landmark l is owned by rank l % nranks
+    int rank, nranks;                // k_ba_mask_points' owner test; k_ba_scale adds the replicated pose term on rank 0 only
 };
 
 static const int DINV_LD = 10;   // doubles per landmark in Dinv: 9 + 1 pad, so that every block is 16-byte aligned for the 128-bit loads of k_ba_schur
-
-__device__ __forceinline__ bool owned(const BADev& D, int l) { return D.nranks == 1 || (l % D.nranks) == D.rank; }
 
 // Deterministic grid-wide sum: fixed-shape block sums, block partials in part[], the last block to arrive adds them in a fixed shape.
 // Returns true in thread 0 of the last block, with the total in *total.
@@ -86,7 +87,7 @@ __global__ void __launch_bounds__(256) k_ba_errors(BADev D, double* out) {
     __shared__ double sh[32];
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     double c = 0;
-    if (e < D.nE && D.level[e] == 0 && owned(D, D.eMP[e])) {
+    if (e < D.nE && D.level[e] == 0) {
         double Xc[3], er[2];
         pose_map(D.pose[D.eKF[e]], D.X + 3 * D.eMP[e], Xc);
         edge_error(D.face[e], D.f, D.obs[3 * e], D.obs[3 * e + 1], Xc, er);
@@ -122,9 +123,9 @@ __device__ __forceinline__ void linearize_edge(const BADev& D, int e, bool needP
 static const int LM_LANES = 4;   // lanes that share one landmark in k_ba_lin_points / k_ba_backsub (edge a of the landmark goes to lane a % 4)
 __global__ void __launch_bounds__(128) k_ba_lin_points(BADev D) {
     const int l = (blockIdx.x * blockDim.x + threadIdx.x) / LM_LANES, sub = threadIdx.x % LM_LANES;
-    const bool mine = l < D.nMP && owned(D, l);
+    const bool in = l < D.nMP;
     double H[6] = {0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
-    const int eBeg = mine ? D.lmStart[l] : 0, eEnd = mine ? D.lmStart[l + 1] : 0;
+    const int eBeg = in ? D.lmStart[l] : 0, eEnd = in ? D.lmStart[l + 1] : 0;
     for (int e = eBeg + sub; e < eEnd; e += LM_LANES) {
         double* B = D.Hpl + 18 * (size_t)e;
         const int pi = D.poseIdx[D.eKF[e]];
@@ -157,7 +158,7 @@ __global__ void __launch_bounds__(128) k_ba_lin_points(BADev D) {
     for (int i = 0; i < 6; i++) { H[i] += __shfl_xor_sync(0xffffffffu, H[i], 1); H[i] += __shfl_xor_sync(0xffffffffu, H[i], 2); }
 #pragma unroll
     for (int i = 0; i < 3; i++) { b[i] += __shfl_xor_sync(0xffffffffu, b[i], 1); b[i] += __shfl_xor_sync(0xffffffffu, b[i], 2); }
-    if (!mine || sub) return;
+    if (!in || sub) return;
     double* Hl = D.Hll + 9 * (size_t)l;
     Hl[0] = H[0]; Hl[1] = H[1]; Hl[2] = H[2]; Hl[3] = H[1]; Hl[4] = H[3]; Hl[5] = H[4]; Hl[6] = H[2]; Hl[7] = H[4]; Hl[8] = H[5];
     D.bl[3 * l] = b[0]; D.bl[3 * l + 1] = b[1]; D.bl[3 * l + 2] = b[2];
@@ -177,7 +178,7 @@ __global__ void __launch_bounds__(256) k_ba_lin_poses(BADev D) {
     for (int i = 0; i < 27; i++) acc[i] = 0.0;
     for (int q = D.peStart[k] + sl * 256 + threadIdx.x; q < D.peStart[k + 1]; q += POSE_SPLIT * 256) {
         const int e = D.peList[q];
-        if (D.level[e] != 0 || !owned(D, D.eMP[e])) continue;
+        if (D.level[e] != 0) continue;
         EdgeLin L;
         linearize_edge(D, e, true, L);
         int t = 0;
@@ -229,7 +230,7 @@ __global__ void __launch_bounds__(256) k_ba_maxdiag(BADev D) {
     double m = 0;
     if (i < D.nP * 6) m = fabs(D.Hpp[36 * (i / 6) + 7 * (i % 6)]);
     const int j = i - D.nP * 6;
-    if (j >= 0 && j < D.nMP * 3) { const int l = j / 3; if (D.ptAct[l] && owned(D, l)) m = fabs(D.Hll[9 * l + 4 * (j % 3)]); }
+    if (j >= 0 && j < D.nMP * 3) { const int l = j / 3; if (D.ptAct[l]) m = fabs(D.Hll[9 * l + 4 * (j % 3)]); }
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(reinterpret_cast<unsigned long long*>(&D.scal[2]), (unsigned long long)__double_as_longlong(m));
@@ -239,7 +240,7 @@ __global__ void __launch_bounds__(256) k_ba_maxdiag(BADev D) {
 __global__ void __launch_bounds__(256) k_ba_dinv(BADev D) {
     const double lambda = D.scal[4];
     const int l = blockIdx.x * blockDim.x + threadIdx.x;
-    if (l >= D.nMP || !owned(D, l)) return;
+    if (l >= D.nMP) return;
     double* Dv = D.Dinv + DINV_LD * (size_t)l;
     if (!D.ptAct[l]) {
 #pragma unroll
@@ -345,8 +346,9 @@ __global__ void __launch_bounds__(128) k_ba_pairs_fill(BADev D, const long long*
 // pair's co-observation list, then a fixed-shape reduction. The diagonal pair also forms g = bp - sum B (Dinv bl) and bpr = bp.
 // Two threads share a tuple (rows 0-2 / rows 3-5 of the 6x6 block): 18 + 3 accumulators per thread keep the kernel at a register count
 // that lets the list loads of many tuples be in flight per SM (the kernel is L2-latency bound, the Hpl / Dinv blocks are L2 resident).
+// The rank's partial system [S n*n | g n | bpr n] goes to `out`: the reduced system itself on one GPU, the rank's exchange payload otherwise.
 static const int SCHUR_T = 256;
-__global__ void __launch_bounds__(SCHUR_T) k_ba_schur(BADev D, int addLambda) {
+__global__ void __launch_bounds__(SCHUR_T) k_ba_schur(BADev D, double* out, int addLambda) {
     const double lambdaDiag = addLambda ? D.scal[4] : 0.0;
     __shared__ double red[SCHUR_T / 32][44];
     const int q1 = blockIdx.y, q2 = blockIdx.x;
@@ -365,7 +367,6 @@ __global__ void __launch_bounds__(SCHUR_T) k_ba_schur(BADev D, int addLambda) {
         const int4 tp = nxt;
         if (t + SCHUR_T / 2 < end) nxt = D.tuples[t + SCHUR_T / 2];   // the next tuple's index load flies under this tuple's block loads
         const int l = tp.z;
-        if (!owned(D, l)) continue;
         // 19 128-bit loads per thread: every lane reads a different block, so the L1 wavefront count per byte is what bounds this kernel
         const double2* B1v = reinterpret_cast<const double2*>(D.Hpl + 18 * (size_t)tp.x) + 4 * h;   // doubles 8h .. 8h+9: rows 3h..3h+2 are w[h .. h+8]
         const double2* B2v = reinterpret_cast<const double2*>(D.Hpl + 18 * (size_t)tp.y);
@@ -410,16 +411,17 @@ __global__ void __launch_bounds__(SCHUR_T) k_ba_schur(BADev D, int addLambda) {
         for (int ww = 0; ww < SCHUR_T / 32; ww++) s += red[ww][threadIdx.x];
         double v = -s;
         if (diag) { v += D.Hpp[36 * p1 + threadIdx.x]; if (i == j) v += lambdaDiag; }
-        D.S[(size_t)(6 * p1 + i) * n + 6 * p2 + j] = v;
-        if (!diag) D.S[(size_t)(6 * p2 + j) * n + 6 * p1 + i] = v;
+        out[(size_t)(6 * p1 + i) * n + 6 * p2 + j] = v;
+        if (!diag) out[(size_t)(6 * p2 + j) * n + 6 * p1 + i] = v;
     } else if (diag && threadIdx.x < 42) {
         const int i = threadIdx.x - 36;
         double s = 0;
 #pragma unroll
         for (int ww = 0; ww < SCHUR_T / 32; ww++) s += red[ww][threadIdx.x];
         const double b = D.bp[6 * p1 + i];
-        D.g[6 * p1 + i] = b - s;
-        D.bpr[6 * p1 + i] = b;
+        double* g = out + (size_t)n * n;
+        g[6 * p1 + i] = b - s;
+        g[n + 6 * p1 + i] = b;   // bpr
     }
 }
 
@@ -687,7 +689,7 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
 // xl = Dinv (bl - Hpl^T xp)   (block_solver.hpp:461-481)
 __global__ void __launch_bounds__(128) k_ba_backsub(BADev D) {
     const int l = (blockIdx.x * blockDim.x + threadIdx.x) / LM_LANES, sub = threadIdx.x % LM_LANES;
-    const bool in = l < D.nMP, act = in && D.ptAct[l] && owned(D, l);
+    const bool in = l < D.nMP, act = in && D.ptAct[l];
     double cl[3] = {0, 0, 0};
     const int eBeg = act ? D.lmStart[l] : 0, eEnd = act ? D.lmStart[l + 1] : 0;
     for (int a = eBeg + sub; a < eEnd; a += LM_LANES) {
@@ -721,7 +723,7 @@ __global__ void __launch_bounds__(256) k_ba_update(BADev D) {
     if (i < D.nMP) {
         const double x = D.X[3 * i], y = D.X[3 * i + 1], z = D.X[3 * i + 2];
         D.Xbak[3 * i] = x; D.Xbak[3 * i + 1] = y; D.Xbak[3 * i + 2] = z;
-        if (D.ptAct[i] && owned(D, i)) { D.X[3 * i] = x + D.xl[3 * i]; D.X[3 * i + 1] = y + D.xl[3 * i + 1]; D.X[3 * i + 2] = z + D.xl[3 * i + 2]; }
+        if (D.ptAct[i]) { D.X[3 * i] = x + D.xl[3 * i]; D.X[3 * i + 1] = y + D.xl[3 * i + 1]; D.X[3 * i + 2] = z + D.xl[3 * i + 2]; }
     }
 }
 // pop()
@@ -739,7 +741,7 @@ __global__ void __launch_bounds__(256) k_ba_scale(BADev D, double* out) {
     double v = 0;
     if (i < D.n && D.rank == 0) v = D.xp[i] * (lambda * D.xp[i] + D.bpr[i]);
     const int j = i - D.n;
-    if (j >= 0 && j < 3 * D.nMP) { const int l = j / 3; if (D.ptAct[l] && owned(D, l)) v = D.xl[j] * (lambda * D.xl[j] + D.bl[j]); }
+    if (j >= 0 && j < 3 * D.nMP) { const int l = j / 3; if (D.ptAct[l]) v = D.xl[j] * (lambda * D.xl[j] + D.bl[j]); }
     double tot;
     if (grid_sum(v, D.part, D.ticket, sh, &tot)) *out = tot;
 }
@@ -756,11 +758,12 @@ __global__ void __launch_bounds__(256) k_ba_classify(BADev D, uint8_t* flag) {
 }
 
 // ---------------------------------------------------------------------------------------------- one-shot NVLink all-reduce
-// Multi-GPU LocalBA: every rank owns an exchange buffer [payload doubles | flags] that all peers map (CUDA IPC). After the Schur
-// kernel has written the rank's partial [S | g | bpr | tail] into its own buffer, k_ba_xchg_signal publishes `epoch` in every peer's
-// flag slot for this rank (system-scope release); k_ba_xchg_reduce waits until all peers have published `epoch`, then every rank sums
-// the payloads of all ranks in rank order (identical result everywhere) into its private S / g / bpr / tail and adds lambda to the
-// diagonal. One 0.7 MB exchange per LM trial instead of five NCCL calls; a bounded spin turns a lost peer into an error, not a hang.
+// Multi-GPU LocalBA: every rank owns an exchange region that all peers map (CUDA IPC): two payloads [S n*n | g n | bpr n] (epoch
+// parity), then 256 bytes of flags and the small-exchange slots. After k_ba_schur has written the rank's partial system into its payload
+// of this epoch, k_ba_xchg_signal publishes `epoch` in every peer's flag slot for this rank (system-scope release); k_ba_xchg_reduce waits
+// until all peers have published `epoch`, then every rank sums the payloads of all ranks in rank order (identical result everywhere) into
+// its private reduced system BAHost::red and adds lambda to the diagonal. One 0.7 MB exchange per LM trial instead of five NCCL calls; a
+// bounded spin turns a lost peer into an error, not a hang.
 struct XchgPeers { const double* payload[8]; volatile unsigned* flags[8]; int n, rank; };
 __global__ void k_ba_xchg_signal(XchgPeers P, unsigned epoch) {
     if (threadIdx.x < P.n) {
@@ -823,6 +826,16 @@ __global__ void __launch_bounds__(256) k_ba_scatter_flags(int nLocal, const int*
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < nLocal) out[perm[s]] = flag[s];
 }
+// NCCL path: lambda goes onto the diagonal of the summed system (the one-shot path adds it in k_ba_xchg_reduce)
+__global__ void __launch_bounds__(256) k_ba_add_lambda(double* S, int n, double lambda) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) S[(size_t)i * n + i] += lambda;
+}
+// a rank's copy of another rank's point is stale: every point is taken from its owner (sum over ranks of owner ? X : 0)
+__global__ void __launch_bounds__(256) k_ba_mask_points(BADev D) {
+    const int l = blockIdx.x * blockDim.x + threadIdx.x;
+    if (l < D.nMP && l % D.nranks != D.rank) { D.X[3 * l] = 0; D.X[3 * l + 1] = 0; D.X[3 * l + 2] = 0; }
+}
 
 }  // namespace cslam
 
@@ -859,7 +872,6 @@ static NcclApi* nccl_api() {
 enum { NCCL_U8 = 1, NCCL_I32 = 2, NCCL_F64 = 8, NCCL_SUM = 0, NCCL_MAX = 2 };
 enum { BK_ERRORS = 0, BK_LIN_POINTS, BK_LIN_POSES, BK_DINV, BK_SCHUR, BK_XCHG, BK_SOLVE, BK_BACKSUB, BK_UPDATE, BK_SCALE, BK_COUNT, BK_END = KernelTimer::END };
 static const char* kBaKindNames[BK_COUNT] = {"k_ba_errors", "k_ba_lin_points", "k_ba_lin_poses", "k_ba_dinv", "k_ba_schur", "exchange", "k_ba_solve", "k_ba_backsub", "k_ba_update", "k_ba_scale"};
-
 
 extern "C" int cslam_optimizer_create(cslam_optimizer** out, int device) {
     if (!out) return CSLAM_E_BADARG;
@@ -980,36 +992,156 @@ __global__ void __launch_bounds__(256) k_ba_prep_points(int n3, const float* __r
     if (i < n3) out[i] = (double)in[i];
 }
 
+static int grid(int n, int t = 256) { return std::max(1, cdiv(n, t)); }   // blocks of t threads for n items, at least one
+
 namespace {
 struct BAHost {
-    cslam_optimizer* o; BADev D; cslam_ba_result* res;
+    cslam_optimizer* o; BADev D; cslam_ba_problem* p; cslam_ba_result* res;
+    int nEg = 0;                      // the caller's edges (D.nE: the edges this rank works on)
     const int* perm = nullptr;        // sorted edge position -> caller's edge index; nullptr = identity (input already grouped by landmark)
-    std::vector<uint8_t> level; std::vector<int> poseIdx; std::vector<uint8_t> ptAct, fixed;
+    const int* h_eMP = nullptr; const int* h_eKF = nullptr; int nActive = 0;   // landmark-sorted edge endpoints on the host
+    std::vector<Pose> poses; std::vector<uint8_t> level; std::vector<int> poseIdx; std::vector<uint8_t> ptAct;
+    const int* d_perm = nullptr; int* d_bad = nullptr; long long* pairCnt = nullptr;
     int* d_poseIdx = nullptr; uint8_t* d_ptAct = nullptr; uint8_t* d_flag = nullptr; int* d_pact = nullptr;
     double* Lt = nullptr; double* LDt = nullptr; double* Minv = nullptr; int ldp = 0;   // panel buffers, inverses of the diagonal blocks' unit factors
-    double* red = nullptr;            // private reduce buffer [S | g | bpr | tail]
+    double* red = nullptr;            // the reduced camera system [S | g | bpr], private to the rank
     double* HppFull = nullptr;        // multi-GPU: all-reduced copy of the pose blocks for computeLambdaInit
     size_t xstride = 0;               // one-shot path: doubles between the two payload buffers of an exchange region
     int* d_xerr = nullptr;
     double lambda = -1, ni = 2; int nBad = 0; int iterations = 0, trials = 0;
     bool errorsCurrent = false; double lastChi = 0;   // D.err / chi2 belong to the current state (set by an accepted trial)
     const volatile uint8_t* stop = nullptr;
-    const int* h_eMP = nullptr; const int* h_eKF = nullptr; int nActive = 0;   // landmark-sorted edge endpoints on the host
     bool useOneShot = false;
+    cudaGraphExec_t trialGraph = nullptr; int64_t launchesPerTrial = 0;
+    ~BAHost() { drop_graph(); }
     bool terminate() const { return stop ? (*stop != 0) : false; }
-    int grid(int n, int t = 256) const { return std::max(1, cdiv(n, t)); }
-    size_t payload() const { return (size_t)D.n * D.n + 2 * (size_t)D.n + 4; }
+    size_t payload() const { return (size_t)D.n * D.n + 2 * (size_t)D.n; }
+    void tick(int kind) { o->timer.record(o->stream, kind); }
+    void drop_graph() { if (trialGraph) { cudaGraphExecDestroy(trialGraph); trialGraph = nullptr; } }
 
-    int allreduce(double* buf, size_t count, int op) {
+    // ---- set-up of one call, in call order
+    // Edges sorted by landmark (stable), CSR by landmark and by key frame. On several GPUs a rank keeps only the edges of its own landmarks
+    // (see BADev), so every per-edge kernel, the co-observation lists and the Schur work shrink by 1 / nranks. Host work is two passes over
+    // the endpoint arrays, in scratch vectors that live in the optimizer object (no page faults per call).
+    int sort_edges() {
+        cslam_optimizer::HostScratch& hs = o->hs;
+        const bool multi = o->nranks > 1;
+        auto mine = [&](int l) { return !multi || l % o->nranks == o->rank; };
+        hs.lmStart.assign(D.nMP + 1, 0);
+        bool grouped = !multi;
+        int nE = 0;
+        for (int e = 0; e < nEg; e++) {
+            const int l = p->edge_mp[e], k = p->edge_kf[e];
+            if (l < 0 || l >= D.nMP || k < 0 || k >= D.nKF) { set_error("edge %d references a vertex out of range", e); return CSLAM_E_BADARG; }
+            if (!mine(l)) continue;
+            hs.lmStart[l + 1]++; nE++;
+            if (e && l < p->edge_mp[e - 1]) grouped = false;
+        }
+        D.nE = nE;
+        for (int l = 0; l < D.nMP; l++) hs.lmStart[l + 1] += hs.lmStart[l];
+        if (grouped) { perm = nullptr; h_eMP = p->edge_mp; h_eKF = p->edge_kf; }
+        else {
+            hs.perm.resize(nE); hs.eMP.resize(nE); hs.eKF.resize(nE); hs.fill.assign(hs.lmStart.begin(), hs.lmStart.end() - 1);
+            for (int e = 0; e < nEg; e++) { const int l = p->edge_mp[e]; if (mine(l)) hs.perm[hs.fill[l]++] = e; }
+            for (int s = 0; s < nE; s++) { const int e = hs.perm[s]; hs.eMP[s] = p->edge_mp[e]; hs.eKF[s] = p->edge_kf[e]; }
+            perm = hs.perm.data(); h_eMP = hs.eMP.data(); h_eKF = hs.eKF.data();
+        }
+        hs.peStart.assign(D.nKF + 1, 0); hs.peList.resize(nE);
+        for (int s = 0; s < nE; s++) hs.peStart[h_eKF[s] + 1]++;
+        for (int k = 0; k < D.nKF; k++) hs.peStart[k + 1] += hs.peStart[k];
+        hs.fill.assign(hs.peStart.begin(), hs.peStart.end() - 1);
+        for (int s = 0; s < nE; s++) hs.peList[hs.fill[h_eKF[s]]++] = s;
+        return 0;
+    }
+    // Poses, CSRs and sorted endpoints to the device. k_ba_prep_edges forms each edge's face, position in the face and weight, and leaves
+    // the smallest caller index of an off-face key point in d_bad (checked by build_pairs); k_ba_prep_points converts the points to fp64.
+    // Every host source of an upload outlives the call (BAHost members, the optimizer's scratch, the caller's arrays), so the copies stay
+    // valid whether or not the runtime has staged them when cudaMemcpyAsync returns.
+    int stage_inputs() {
+        const int nKF = D.nKF, nMP = D.nMP, nE = D.nE;
+        cslam_optimizer::HostScratch& hs = o->hs;
+        poses.resize(nKF);
+        for (int k = 0; k < nKF; k++) poses[k] = pose_from_Tcw32(p->Tcw + 16 * k);
+        level.assign(nE, 0); poseIdx.assign(nKF, -1); ptAct.assign(nMP, 0);
+        hs.kfOfQ.clear();
+        for (int k = 0; k < nKF; k++) if (!p->kf_fixed[k]) hs.kfOfQ.push_back(k);
+        D.nQ = (int)hs.kfOfQ.size();
+        const Pose* cpose = nullptr; const float2* d_kp = nullptr; const float* d_isig = nullptr; const float* d_pts32 = nullptr;
+        double* d_obs = nullptr; int8_t* d_face = nullptr;
+        DevArena& A = o->arena;
+        int rc;
+        if ((rc = A.upload(&cpose, poses.data(), poses.size())) || (rc = A.upload(&D.lmStart, hs.lmStart.data(), hs.lmStart.size())) ||
+            (rc = A.upload(&D.peStart, hs.peStart.data(), hs.peStart.size())) || (rc = A.upload(&D.peList, hs.peList.data(), hs.peList.size())) ||
+            (rc = A.upload(&D.kfOfQ, hs.kfOfQ.data(), hs.kfOfQ.size())) || (rc = A.upload(&D.eMP, h_eMP, nE)) || (rc = A.upload(&D.eKF, h_eKF, nE)) ||
+            (rc = A.upload(&d_kp, reinterpret_cast<const float2*>(p->kp_xy), nEg)) || (rc = A.upload(&d_isig, p->inv_sigma2, nEg)) ||
+            (rc = A.upload(&d_pts32, p->points, (size_t)nMP * 3)) || (rc = A.take(&D.X, (size_t)nMP * 3)) || (rc = A.take(&d_obs, (size_t)nE * 3)) ||
+            (rc = A.take(&d_face, nE)) || (rc = A.take(&d_bad, 1)) || (perm && (rc = A.upload(&d_perm, perm, nE)))) return rc;
+        CSLAM_CUDA(cudaMemsetAsync(d_bad, 0x7f, sizeof(int), o->stream));
+        if (nE > 0) { k_ba_prep_edges<<<grid(nE), 256, 0, o->stream>>>(nE, d_perm, d_kp, d_isig, p->face_w, p->face_h, d_obs, d_face, d_bad); o->launches++; }
+        if (nMP > 0) { k_ba_prep_points<<<grid(nMP * 3), 256, 0, o->stream>>>(nMP * 3, d_pts32, D.X); o->launches++; }
+        D.obs = d_obs; D.face = d_face; D.pose = const_cast<Pose*>(cpose);
+        // device state of the LM loop, sized for every candidate pose; on several GPUs, the exchange path of the reduced system
+        const int nQ = D.nQ, nmax = 6 * nQ;
+        const size_t payloadMax = (size_t)nmax * nmax + 2 * (size_t)nmax;
+        const int maxBlocks = std::max(grid(nE), grid(nmax + 3 * nMP));
+        ldp = ((nmax + 1 + 8) + 3) & ~3;
+        if ((rc = A.take(&D.poseBak, nKF)) || (rc = A.take(&D.Xbak, (size_t)nMP * 3)) || (rc = A.take(&D.err, (size_t)nE * 2, true)) || (rc = A.take(&D.level, nE, true)) ||
+            (rc = A.take(&d_poseIdx, nKF)) || (rc = A.take(&d_pact, nKF + 1)) || (rc = A.take(&d_ptAct, nMP)) || (rc = A.take(&d_flag, nE)) ||
+            (rc = A.take(&D.Hpp, (size_t)std::max(nQ, 1) * 36)) || (rc = A.take(&D.bp, (size_t)std::max(nQ, 1) * 6)) || (rc = A.take(&D.Hll, (size_t)nMP * 9)) ||
+            (rc = A.take(&D.bl, (size_t)nMP * 3)) || (rc = A.take(&D.Hpl, (size_t)nE * 18)) || (rc = A.take(&D.Dinv, (size_t)nMP * DINV_LD)) ||
+            (rc = A.take(&D.db, (size_t)nMP * 3)) || (rc = A.take(&red, payloadMax)) || (rc = A.take(&D.xp, std::max(nmax, 1), true)) ||
+            (rc = A.take(&D.xl, (size_t)nMP * 3, true)) || (rc = A.take(&D.scal, 8, true)) || (rc = A.take(&D.part, maxBlocks)) || (rc = A.take(&D.ticket, 4, true)) ||
+            (rc = A.take(&D.posePart, (size_t)std::max(nQ, 1) * POSE_SPLIT * 27)) || (rc = A.take(&D.poseTicket, std::max(nQ, 1), true)) ||
+            (rc = A.take(&Lt, (size_t)LD_NB * ldp)) || (rc = A.take(&LDt, (size_t)LD_NB * ldp)) || (rc = A.take(&Minv, (size_t)(nmax / LD_NB + 1) * LD_NB * LD_NB)) ||
+            (rc = A.take(&pairCnt, (size_t)nQ * nQ + 1)) || (rc = A.take(&d_xerr, 1, true))) return rc;
+        D.poseIdx = d_poseIdx; D.ptAct = d_ptAct;
+        if (o->nranks > 1) {
+            // The one-shot path falls back to ncclAllReduce by itself where CUDA IPC is unavailable; CSLAM_BA_NCCL_ONLY forces that
+            // fallback, the only way to exercise it on a machine where IPC works.
+            const bool ncclOnly = getenv("CSLAM_BA_NCCL_ONLY") != nullptr;
+            if (!ncclOnly && (!o->oneShot || o->xchgBytes < payloadMax * 8)) {
+                const int xr = setup_xchg(o, payloadMax * 8);
+                if (xr < 0) return xr;
+            }
+            useOneShot = o->oneShot && o->xchgBytes >= payloadMax * 8 && !ncclOnly;
+            xstride = ((o->xchgBytes + 255) & ~(size_t)255) / 8;
+            if ((rc = A.take(&HppFull, (size_t)std::max(nQ, 1) * 36))) return rc;
+        }
+        return 0;
+    }
+    // Co-observation lists (once per call, over all of the rank's edges), and the off-face check of k_ba_prep_edges at the same synchronise.
+    int build_pairs() {
+        const int nQ = D.nQ;
+        long long total = 0; int badEdge = 0;
+        if (nQ > 0) {
+            k_ba_pairs_count<<<dim3(nQ, nQ), 128, 0, o->stream>>>(D, pairCnt); o->launches++;
+            k_ba_pairs_scan<<<1, 1024, 0, o->stream>>>(pairCnt, nQ * nQ); o->launches++;
+            CSLAM_CUDA(cudaMemcpyAsync(&total, pairCnt + (size_t)nQ * nQ, sizeof(long long), cudaMemcpyDeviceToHost, o->stream));
+        }
+        CSLAM_CUDA(cudaMemcpyAsync(&badEdge, d_bad, sizeof(int), cudaMemcpyDeviceToHost, o->stream));
+        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
+        if (badEdge < nEg) { set_error("edge %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", badEdge, p->kp_xy[2 * badEdge], p->kp_xy[2 * badEdge + 1]); return CSLAM_E_BADARG; }
+        if (nQ == 0) return 0;
+        int4* tuples = nullptr;
+        int rc;
+        if ((rc = o->arena.take(&tuples, (size_t)std::max<long long>(total, 1)))) return rc;
+        k_ba_pairs_fill<<<dim3(nQ, nQ), 128, 0, o->stream>>>(D, pairCnt, tuples); o->launches++;
+        CSLAM_CUDA(cudaGetLastError());
+        D.pairStart = pairCnt; D.tuples = tuples;
+        return 0;
+    }
+
+    // ---- the LM loop
+    int allreduce(const char* what, void* buf, size_t count, int op, int type = NCCL_F64) {   // in place; `what` names the data in the error
         if (o->nranks <= 1) return 0;
-        int rc = nccl_api()->AllReduce(buf, buf, count, NCCL_F64, op, o->comm, o->stream);
-        if (rc) { set_error("ncclAllReduce failed (%d)", rc); return CSLAM_E_NCCL; }
+        int rc = nccl_api()->AllReduce(buf, buf, count, type, op, o->comm, o->stream);
+        if (rc) { set_error("ncclAllReduce (%s) failed (%d)", what, rc); return CSLAM_E_NCCL; }
         return 0;
     }
     // <= 4 doubles, in place: the one-shot path when the peer views exist, NCCL otherwise
     int allreduce_small(double* buf, int count, bool isMax) {
         if (o->nranks <= 1) return 0;
-        if (!useOneShot) return allreduce(buf, count, isMax ? NCCL_MAX : NCCL_SUM);
+        if (!useOneShot) return allreduce("trial scalars", buf, count, isMax ? NCCL_MAX : NCCL_SUM);
         SmallPeers P; P.n = o->nranks; P.rank = o->rank;
         const size_t off = 2 * xstride * 8;
         for (int r = 0; r < o->nranks; r++) { P.flags[r] = (volatile unsigned*)((char*)o->peers[r].base + off + 64); P.slot[r] = (const double*)((char*)o->peers[r].base + off + 128); }
@@ -1022,36 +1154,29 @@ struct BAHost {
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
         return 0;
     }
-    void bind(unsigned epoch = 0) {   // partial system of this rank goes to `w` (exchange payload of this epoch on the one-shot path), the reduced one lives in `red`
-        double* w = (o->nranks > 1 && useOneShot) ? (double*)o->peers[o->rank].base + (epoch & 1) * xstride : red;
-        D.S = w; D.g = w + (size_t)D.n * D.n; D.bpr = D.g + D.n; D.tail = D.bpr + D.n;
-    }
-    BADev reducedView() const { BADev R = D; R.S = red; R.g = red + (size_t)D.n * D.n; R.bpr = R.g + D.n; R.tail = R.bpr + D.n; return R; }
 
     // initializeOptimization(level 0): active edges, active vertices, compact pose indices (sparse_optimizer.cpp:206-267,166-190)
     int initialize() {
         std::vector<int> pAct(D.nKF + 1, 0);   // [nKF] = this rank has an active edge
         std::fill(ptAct.begin(), ptAct.end(), 0);
-        const int* eMP = h_eMP; const int* eKF = h_eKF;
         nActive = 0;
-        for (int e = 0; e < D.nE; e++) if (level[e] == 0) { pAct[eKF[e]] = 1; ptAct[eMP[e]] = 1; nActive++; }
+        for (int e = 0; e < D.nE; e++) if (level[e] == 0) { pAct[h_eKF[e]] = 1; ptAct[h_eMP[e]] = 1; nActive++; }
         pAct[D.nKF] = nActive > 0;
         if (o->nranks > 1) {   // a rank sees the edges of its own landmarks only: pose activity and "anything to optimize" are global facts
             CSLAM_CUDA(cudaMemcpyAsync(d_pact, pAct.data(), (D.nKF + 1) * sizeof(int), cudaMemcpyHostToDevice, o->stream));
-            int rc = nccl_api()->AllReduce(d_pact, d_pact, D.nKF + 1, NCCL_I32, NCCL_MAX, o->comm, o->stream);
-            if (rc) { set_error("ncclAllReduce (pose activity) failed (%d)", rc); return CSLAM_E_NCCL; }
+            if (int rc = allreduce("pose activity", d_pact, D.nKF + 1, NCCL_MAX, NCCL_I32)) return rc;
             CSLAM_CUDA(cudaMemcpyAsync(pAct.data(), d_pact, (D.nKF + 1) * sizeof(int), cudaMemcpyDeviceToHost, o->stream));
             CSLAM_CUDA(cudaStreamSynchronize(o->stream));
             nActive = pAct[D.nKF];   // only tested against zero
         }
         int nP = 0;
-        for (int k = 0; k < D.nKF; k++) poseIdx[k] = (pAct[k] && !fixed[k]) ? nP++ : -1;
+        for (int k = 0; k < D.nKF; k++) poseIdx[k] = (pAct[k] && !p->kf_fixed[k]) ? nP++ : -1;
         D.nP = nP; D.n = 6 * nP;
+        D.S = red; D.bpr = red + (size_t)D.n * D.n + D.n;
         CSLAM_CUDA(cudaMemcpyAsync(d_poseIdx, poseIdx.data(), D.nKF * sizeof(int), cudaMemcpyHostToDevice, o->stream));
         CSLAM_CUDA(cudaMemcpyAsync(d_ptAct, ptAct.data(), D.nMP, cudaMemcpyHostToDevice, o->stream));
         CSLAM_CUDA(cudaMemcpyAsync(D.level, level.data(), D.nE, cudaMemcpyHostToDevice, o->stream));
         errorsCurrent = false;   // level / robust kernel changed
-        bind();
         drop_graph();   // the captured trial bakes in nP / n / the level array's meaning
         return 0;
     }
@@ -1076,7 +1201,7 @@ struct BAHost {
         BADev M = D;
         if (o->nranks > 1 && D.nP > 0) {   // computeLambdaInit needs the full pose blocks: sum a COPY of the partial blocks once per optimize()
             CSLAM_CUDA(cudaMemcpyAsync(HppFull, D.Hpp, (size_t)D.nP * 36 * 8, cudaMemcpyDeviceToDevice, o->stream));
-            if ((rc = allreduce(HppFull, (size_t)D.nP * 36, NCCL_SUM))) return rc;
+            if ((rc = allreduce("pose blocks", HppFull, (size_t)D.nP * 36, NCCL_SUM))) return rc;
             M.Hpp = HppFull;
         }
         k_ba_maxdiag<<<grid(D.nP * 6 + D.nMP * 3), 256, 0, o->stream>>>(M); o->launches++;
@@ -1085,7 +1210,6 @@ struct BAHost {
         *lam = 1e-5 * o->h_scal[2];
         return 0;
     }
-    void tick(int kind) { o->timer.record(o->stream, kind); }
     // One LM trial on the stream: lambda -> device, BlockSolver::solve (Dinv, Schur, [exchange], reduced solve, back substitution), push + oplus,
     // computeActiveErrors + activeRobustChi2, computeScale, the four scalars -> pinned host memory. Single-GPU trials are replayed as ONE CUDA graph.
     int enqueue_trial() {
@@ -1093,29 +1217,24 @@ struct BAHost {
         CSLAM_CUDA(cudaMemcpyAsync(D.scal + 4, o->h_scal + 8, sizeof(double), cudaMemcpyHostToDevice, o->stream));   // h_scal[8] = lambda
         tick(BK_DINV);
         k_ba_dinv<<<grid(D.nMP), 256, 0, o->stream>>>(D); o->launches++;
-        BADev SV = D;
         if (D.n > 0) {
-            const bool multi = o->nranks > 1;
-            const unsigned ep = (multi && useOneShot) ? ++o->epoch : 0;
-            bind(ep);
+            const bool multi = o->nranks > 1, oneShot = multi && useOneShot;
+            const unsigned ep = oneShot ? ++o->epoch : 0;
+            double* part = oneShot ? (double*)o->peers[o->rank].base + (ep & 1) * xstride : red;   // where this rank's partial system goes
             tick(BK_SCHUR);
-            k_ba_schur<<<dim3(D.nQ, D.nQ), SCHUR_T, 0, o->stream>>>(D, multi ? 0 : 1); o->launches++;
-            BADev R = D;
+            k_ba_schur<<<dim3(D.nQ, D.nQ), SCHUR_T, 0, o->stream>>>(D, part, multi ? 0 : 1); o->launches++;
             if (multi) {
-                R = reducedView();
                 tick(BK_XCHG);
-                if (useOneShot) {
+                if (oneShot) {
                     XchgPeers P; P.n = o->nranks; P.rank = o->rank;
                     const size_t off = 2 * xstride * 8;
                     for (int r = 0; r < o->nranks; r++) { P.payload[r] = (const double*)o->peers[r].base + (ep & 1) * xstride; P.flags[r] = (volatile unsigned*)((char*)o->peers[r].base + off); }
                     k_ba_xchg_signal<<<1, 32, 0, o->stream>>>(P, ep); o->launches++;
                     k_ba_xchg_reduce<<<std::min(132, grid((int)std::min<size_t>(payload(), 1u << 30))), 256, 0, o->stream>>>(P, ep, red, payload(), D.n, D.scal + 4, d_xerr); o->launches++;
                 } else {
-                    CSLAM_CUDA(cudaMemcpyAsync(red, D.S, payload() * 8, cudaMemcpyDeviceToDevice, o->stream));
-                    if ((rc = allreduce(red, payload(), NCCL_SUM))) return rc;
-                    k_ba_add_lambda_launch(R);
+                    if ((rc = allreduce("reduced system", red, payload(), NCCL_SUM))) return rc;
+                    k_ba_add_lambda<<<grid(D.n), 256, 0, o->stream>>>(red, D.n, lambda); o->launches++;
                 }
-                SV.bpr = R.bpr;
             }
             CSLAM_CUDA(cudaMemsetAsync(D.scal + 3, 0, sizeof(double), o->stream));
             tick(BK_SOLVE);
@@ -1126,7 +1245,7 @@ struct BAHost {
             cudaLaunchAttribute at[1];
             at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = SOLVE_CLUSTER; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
             cfg.attrs = at; cfg.numAttrs = 1;
-            CSLAM_CUDA(cudaLaunchKernelEx(&cfg, k_ba_solve, R, Lt, LDt, Minv, ldp, stage)); o->launches++;
+            CSLAM_CUDA(cudaLaunchKernelEx(&cfg, k_ba_solve, D, Lt, LDt, Minv, ldp, stage)); o->launches++;
         }
         tick(BK_BACKSUB);
         k_ba_backsub<<<grid(D.nMP * LM_LANES, 128), 128, 0, o->stream>>>(D); o->launches++;
@@ -1135,15 +1254,13 @@ struct BAHost {
         tick(BK_ERRORS);
         k_ba_errors<<<grid(D.nE), 256, 0, o->stream>>>(D, D.scal); o->launches++;
         tick(BK_SCALE);
-        k_ba_scale<<<grid(D.n + 3 * D.nMP), 256, 0, o->stream>>>(SV, D.scal + 1); o->launches++;
+        k_ba_scale<<<grid(D.n + 3 * D.nMP), 256, 0, o->stream>>>(D, D.scal + 1); o->launches++;
         tick(BK_END);
         if ((rc = allreduce_small(D.scal, 2, false))) return rc;
         CSLAM_CUDA(cudaMemcpyAsync(o->h_scal, D.scal, 4 * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
         CSLAM_CUDA(cudaGetLastError());
         return 0;
     }
-    cudaGraphExec_t trialGraph = nullptr;
-    void drop_graph() { if (trialGraph) { cudaGraphExecDestroy(trialGraph); trialGraph = nullptr; } }
     int run_trial() {
         int rc;
         o->h_scal[8] = lambda;
@@ -1168,8 +1285,6 @@ struct BAHost {
         o->timer.collect();
         return 0;
     }
-    int64_t launchesPerTrial = 0;
-    void k_ba_add_lambda_launch(const BADev& R);
     // OptimizationAlgorithmLevenberg::solve ; result 0 OK, 1 Terminate
     int lm_iteration(int iteration, int* result) {
         int rc; double currentChi = 0;
@@ -1235,18 +1350,40 @@ struct BAHost {
         CSLAM_CUDA(cudaStreamSynchronize(o->stream));
         return 0;
     }
+    // src/Optimizer.cpp:397-450: outlier flags in the caller's edge order, float32 poses and points (fp64 copies on request). On several GPUs
+    // every rank returns the flags of all edges (max over the owners' flags) and every point from its owner.
+    int write_back(const std::vector<uint8_t>& flags) {
+        int rc;
+        const int nKF = D.nKF, nMP = D.nMP;
+        const bool multi = o->nranks > 1;
+        std::vector<uint8_t> gflags;
+        if (multi) {
+            uint8_t* d_gflag = nullptr;
+            if ((rc = o->arena.take(&d_gflag, std::max(nEg, 1), true))) return rc;
+            if (D.nE > 0) { k_ba_scatter_flags<<<grid(D.nE), 256, 0, o->stream>>>(D.nE, d_perm, d_flag, d_gflag); o->launches++; }
+            if ((rc = allreduce("flags", d_gflag, nEg, NCCL_MAX, NCCL_U8))) return rc;
+            gflags.resize(nEg);
+            CSLAM_CUDA(cudaMemcpyAsync(gflags.data(), d_gflag, nEg, cudaMemcpyDeviceToHost, o->stream));
+            k_ba_mask_points<<<grid(nMP), 256, 0, o->stream>>>(D); o->launches++;
+            if ((rc = allreduce("points", D.X, (size_t)nMP * 3, NCCL_SUM))) return rc;
+        }
+        CSLAM_CUDA(cudaMemcpyAsync(poses.data(), D.pose, nKF * sizeof(Pose), cudaMemcpyDeviceToHost, o->stream));
+        std::vector<double>& X = o->hs.X;
+        X.resize((size_t)nMP * 3);
+        CSLAM_CUDA(cudaMemcpyAsync(X.data(), D.X, X.size() * 8, cudaMemcpyDeviceToHost, o->stream));
+        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
+        for (int k = 0; k < nKF; k++) {
+            pose_to_Tcw32(poses[k], p->Tcw + 16 * k);
+            if (res && res->pose_fp64) pose_to_fp64(poses[k], res->pose_fp64 + 7 * k);
+        }
+        for (size_t i = 0; i < X.size(); i++) { p->points[i] = (float)X[i]; if (res && res->points_fp64) res->points_fp64[i] = X[i]; }
+        if (res) {
+            if (res->outlier) { if (multi) std::memcpy(res->outlier, gflags.data(), nEg); else for (int s = 0; s < D.nE; s++) res->outlier[perm ? perm[s] : s] = flags[s]; }
+            res->iterations = iterations; res->trials = trials;
+        }
+        return CSLAM_OK;
+    }
 };
-__global__ void __launch_bounds__(256) k_ba_add_lambda(double* S, int n, double lambda) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) S[(size_t)i * n + i] += lambda;
-}
-void BAHost::k_ba_add_lambda_launch(const BADev& R) { k_ba_add_lambda<<<grid(R.n), 256, 0, o->stream>>>(R.S, R.n, lambda); o->launches++; }
-
-// non-owner points are stale on a rank: every point is taken from its owner (sum of owner ? X : 0)
-__global__ void __launch_bounds__(256) k_ba_mask_points(BADev D) {
-    const int l = blockIdx.x * blockDim.x + threadIdx.x;
-    if (l < D.nMP && !owned(D, l)) { D.X[3 * l] = 0; D.X[3 * l + 1] = 0; D.X[3 * l + 2] = 0; }
-}
 }  // namespace
 
 extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const volatile uint8_t* stop_flag, int its1, int its2, cslam_ba_result* r) {
@@ -1254,162 +1391,23 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     if (p->face_w != p->face_h || p->face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(o->device));
     o->arena.reset();
-    const int nKF = p->n_kf, nMP = p->n_mp, nEg = p->n_edges;   // nEg: the caller's edges; nE below: the edges this rank works on
-    if (r) { r->iterations = 0; r->trials = 0; if (r->outlier) std::memset(r->outlier, 0, nEg); }
+    if (r) { r->iterations = 0; r->trials = 0; if (r->outlier) std::memset(r->outlier, 0, p->n_edges); }
     if (stop_flag && *stop_flag) return CSLAM_OK;   // src/Optimizer.cpp:359-361
-    BAHost H; H.o = o; H.res = r; H.stop = stop_flag;
+    BAHost H; H.o = o; H.p = p; H.res = r; H.stop = stop_flag; H.nEg = p->n_edges;
     BADev& D = H.D; std::memset(&D, 0, sizeof(D));
-    D.nKF = nKF; D.nMP = nMP; D.f = p->face_w / 2.0; D.rank = o->rank; D.nranks = o->nranks;
-    const float dlt = (float)std::sqrt(5.991); D.delta = (double)dlt; D.dsqr = D.delta * D.delta; D.robust = 1;
-    // ---- edges sorted by landmark (stable), CSR by landmark and by keyframe. Host work is two passes over the endpoint arrays (in scratch
-    // vectors that live in the optimizer object: no page faults per call); the per-edge float work happens on the device (k_ba_prep_edges).
-    cslam_optimizer::HostScratch& hs = o->hs;
-    hs.lmStart.assign(nMP + 1, 0);
-    // Multi-GPU: landmark l (with all its edges) belongs to rank l % nranks; a rank works on the edges of its own landmarks ONLY, so every
-    // per-edge kernel, the co-observation lists and the Schur work shrink by 1 / nranks; the reduced camera system is what gets exchanged.
-    const bool multi = o->nranks > 1;
-    bool grouped = !multi;
-    int nLocal = 0;
-    for (int e = 0; e < nEg; e++) {
-        const int l = p->edge_mp[e], k = p->edge_kf[e];
-        if (l < 0 || l >= nMP || k < 0 || k >= nKF) { set_error("edge %d references a vertex out of range", e); return CSLAM_E_BADARG; }
-        if (multi && (l % o->nranks) != o->rank) continue;
-        hs.lmStart[l + 1]++; nLocal++;
-        if (e && l < p->edge_mp[e - 1]) grouped = false;
-    }
-    const int nE = nLocal;
-    D.nE = nE;
-    for (int l = 0; l < nMP; l++) hs.lmStart[l + 1] += hs.lmStart[l];
-    if (grouped) { H.perm = nullptr; H.h_eMP = p->edge_mp; H.h_eKF = p->edge_kf; }
-    else {
-        hs.perm.resize(nE); hs.eMP.resize(nE); hs.eKF.resize(nE); hs.fill.assign(hs.lmStart.begin(), hs.lmStart.end() - 1);
-        for (int e = 0; e < nEg; e++) { const int l = p->edge_mp[e]; if (!multi || (l % o->nranks) == o->rank) hs.perm[hs.fill[l]++] = e; }
-        for (int s = 0; s < nE; s++) { const int e = hs.perm[s]; hs.eMP[s] = p->edge_mp[e]; hs.eKF[s] = p->edge_kf[e]; }
-        H.perm = hs.perm.data(); H.h_eMP = hs.eMP.data(); H.h_eKF = hs.eKF.data();
-    }
-    hs.peStart.assign(nKF + 1, 0); hs.peList.resize(nE);
-    for (int s = 0; s < nE; s++) hs.peStart[H.h_eKF[s] + 1]++;
-    for (int k = 0; k < nKF; k++) hs.peStart[k + 1] += hs.peStart[k];
-    hs.fill.assign(hs.peStart.begin(), hs.peStart.end() - 1);
-    for (int s = 0; s < nE; s++) hs.peList[hs.fill[H.h_eKF[s]]++] = s;
-    std::vector<Pose> poses(nKF);
-    for (int k = 0; k < nKF; k++) poses[k] = pose_from_Tcw32(p->Tcw + 16 * k);
-    H.fixed.assign(p->kf_fixed, p->kf_fixed + nKF); H.level.assign(nE, 0); H.poseIdx.assign(nKF, -1); H.ptAct.assign(nMP, 0);
-    std::vector<int> kfOfQ;
-    for (int k = 0; k < nKF; k++) if (!H.fixed[k]) kfOfQ.push_back(k);
-    const int nQ = (int)kfOfQ.size();
-    D.nQ = nQ;
+    D.nKF = p->n_kf; D.nMP = p->n_mp; D.f = p->face_w / 2.0; D.rank = o->rank; D.nranks = o->nranks;
+    D.robust = 1; D.delta = huber_delta(); D.dsqr = D.delta * D.delta;
     int rc;
-    const int nmax = 6 * nQ;
-    const Pose* cpose = nullptr; double* cX = nullptr;
-    int* d_eMP = nullptr; int* d_eKF = nullptr; int* d_perm = nullptr; float2* d_kp = nullptr; float* d_isig = nullptr; float* d_pts32 = nullptr; int* d_bad = nullptr;
-    double* d_obs = nullptr; int8_t* d_face = nullptr;
-    if ((rc = o->arena.upload(&cpose, poses.data(), poses.size())) || (rc = o->arena.upload(&D.lmStart, hs.lmStart.data(), hs.lmStart.size())) || (rc = o->arena.upload(&D.peStart, hs.peStart.data(), hs.peStart.size())) || (rc = o->arena.upload(&D.peList, hs.peList.data(), hs.peList.size())) ||
-        (rc = o->arena.upload(&D.kfOfQ, kfOfQ.data(), kfOfQ.size())) || (rc = o->arena.take(&d_eMP, nE)) || (rc = o->arena.take(&d_eKF, nE)) || (rc = o->arena.take(&d_kp, nEg)) || (rc = o->arena.take(&d_isig, nEg)) ||
-        (rc = o->arena.take(&d_pts32, (size_t)nMP * 3)) || (rc = o->arena.take(&cX, (size_t)nMP * 3)) || (rc = o->arena.take(&d_obs, (size_t)nE * 3)) || (rc = o->arena.take(&d_face, nE)) ||
-        (rc = o->arena.take(&d_bad, 1)) || (!grouped && (rc = o->arena.take(&d_perm, nE)))) return rc;
-    if (nE > 0) {
-        CSLAM_CUDA(cudaMemcpyAsync(d_eMP, H.h_eMP, (size_t)nE * 4, cudaMemcpyHostToDevice, o->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(d_eKF, H.h_eKF, (size_t)nE * 4, cudaMemcpyHostToDevice, o->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(d_kp, p->kp_xy, (size_t)nEg * 8, cudaMemcpyHostToDevice, o->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(d_isig, p->inv_sigma2, (size_t)nEg * 4, cudaMemcpyHostToDevice, o->stream));
-        if (!grouped) CSLAM_CUDA(cudaMemcpyAsync(d_perm, H.perm, (size_t)nE * 4, cudaMemcpyHostToDevice, o->stream));
-    }
-    if (nMP > 0) CSLAM_CUDA(cudaMemcpyAsync(d_pts32, p->points, (size_t)nMP * 12, cudaMemcpyHostToDevice, o->stream));
-    CSLAM_CUDA(cudaMemsetAsync(d_bad, 0x7f, sizeof(int), o->stream));
-    if (nE > 0) { k_ba_prep_edges<<<cdiv(nE, 256), 256, 0, o->stream>>>(nE, d_perm, d_kp, d_isig, p->face_w, p->face_h, d_obs, d_face, d_bad); o->launches++; }
-    if (nMP > 0) { k_ba_prep_points<<<cdiv(nMP * 3, 256), 256, 0, o->stream>>>(nMP * 3, d_pts32, cX); o->launches++; }
-    D.eMP = d_eMP; D.eKF = d_eKF; D.obs = d_obs; D.face = d_face;
-    D.pose = const_cast<Pose*>(cpose); D.X = cX;
-    H.ldp = ((nmax + 1 + 8) + 3) & ~3;
-    const size_t payloadMax = (size_t)nmax * nmax + 2 * (size_t)nmax + 4;
-    const int maxBlocks = std::max({cdiv(nE, 256), cdiv(nmax + 3 * nMP, 256), 1});
-    long long* pairCnt = nullptr;
-    if ((rc = o->arena.take(&D.poseBak, nKF)) || (rc = o->arena.take(&D.Xbak, (size_t)nMP * 3)) || (rc = o->arena.take(&D.err, (size_t)nE * 2, true)) || (rc = o->arena.take(&D.level, nE, true)) ||
-        (rc = o->arena.take(&H.d_poseIdx, nKF)) || (rc = o->arena.take(&H.d_pact, nKF + 1)) || (rc = o->arena.take(&H.d_ptAct, nMP)) || (rc = o->arena.take(&H.d_flag, nE)) || (rc = o->arena.take(&D.Hpp, (size_t)std::max(nQ, 1) * 36)) ||
-        (rc = o->arena.take(&D.bp, (size_t)std::max(nQ, 1) * 6)) || (rc = o->arena.take(&D.Hll, (size_t)nMP * 9)) || (rc = o->arena.take(&D.bl, (size_t)nMP * 3)) ||
-        (rc = o->arena.take(&D.Hpl, (size_t)nE * 18)) || (rc = o->arena.take(&D.Dinv, (size_t)nMP * DINV_LD)) || (rc = o->arena.take(&D.db, (size_t)nMP * 3)) ||
-        (rc = o->arena.take(&H.red, payloadMax)) || (rc = o->arena.take(&D.xp, std::max(nmax, 1), true)) || (rc = o->arena.take(&D.xl, (size_t)nMP * 3, true)) ||
-        (rc = o->arena.take(&D.scal, 8, true)) || (rc = o->arena.take(&D.part, maxBlocks)) || (rc = o->arena.take(&D.ticket, 4, true)) || (rc = o->arena.take(&D.posePart, (size_t)std::max(nQ, 1) * POSE_SPLIT * 27)) || (rc = o->arena.take(&D.poseTicket, std::max(nQ, 1), true)) ||
-        (rc = o->arena.take(&H.Lt, (size_t)LD_NB * H.ldp)) || (rc = o->arena.take(&H.LDt, (size_t)LD_NB * H.ldp)) || (rc = o->arena.take(&H.Minv, (size_t)(nmax / LD_NB + 1) * LD_NB * LD_NB)) || (rc = o->arena.take(&pairCnt, (size_t)nQ * nQ + 1)) ||
-        (rc = o->arena.take(&H.d_xerr, 1, true))) return rc;
-    D.poseIdx = H.d_poseIdx; D.ptAct = H.d_ptAct;
-    // ---- multi-GPU exchange path
-    if (o->nranks > 1) {
-        // The one-shot path falls back to ncclAllReduce by itself where CUDA IPC is unavailable; CSLAM_BA_NCCL_ONLY forces that
-        // fallback, the only way to exercise it on a machine where IPC works.
-        const bool ncclOnly = getenv("CSLAM_BA_NCCL_ONLY") != nullptr;
-        if (!ncclOnly && (!o->oneShot || o->xchgBytes < payloadMax * 8)) {
-            const int xr = setup_xchg(o, payloadMax * 8);
-            if (xr < 0) return xr;
-        }
-        H.useOneShot = o->oneShot && o->xchgBytes >= payloadMax * 8 && !ncclOnly;
-        H.xstride = ((o->xchgBytes + 255) & ~(size_t)255) / 8;
-        if ((rc = o->arena.take(&H.HppFull, (size_t)std::max(nQ, 1) * 36))) return rc;
-    }
-    // ---- co-observation lists (once per call, all edges)
-    int badEdge = 0x7f7f7f7f;
-    if (nQ > 0) {
-        k_ba_pairs_count<<<dim3(nQ, nQ), 128, 0, o->stream>>>(D, pairCnt); o->launches++;
-        k_ba_pairs_scan<<<1, 1024, 0, o->stream>>>(pairCnt, nQ * nQ); o->launches++;
-        long long total = 0;
-        CSLAM_CUDA(cudaMemcpyAsync(&total, pairCnt + (size_t)nQ * nQ, sizeof(long long), cudaMemcpyDeviceToHost, o->stream));
-        CSLAM_CUDA(cudaMemcpyAsync(&badEdge, d_bad, sizeof(int), cudaMemcpyDeviceToHost, o->stream));
-        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-        if (badEdge < nEg) { set_error("edge %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", badEdge, p->kp_xy[2 * badEdge], p->kp_xy[2 * badEdge + 1]); return CSLAM_E_BADARG; }
-        int4* tuples = nullptr;
-        if ((rc = o->arena.take(&tuples, (size_t)std::max<long long>(total, 1)))) return rc;
-        k_ba_pairs_fill<<<dim3(nQ, nQ), 128, 0, o->stream>>>(D, pairCnt, tuples); o->launches++;
-        CSLAM_CUDA(cudaGetLastError());
-        D.pairStart = pairCnt; D.tuples = tuples;
-    }
-    if (nQ == 0) {
-        CSLAM_CUDA(cudaMemcpyAsync(&badEdge, d_bad, sizeof(int), cudaMemcpyDeviceToHost, o->stream));
-        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-        if (badEdge < nEg) { set_error("edge %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", badEdge, p->kp_xy[2 * badEdge], p->kp_xy[2 * badEdge + 1]); return CSLAM_E_BADARG; }
-    }
-    // ---- src/Optimizer.cpp:363-395
-    if ((rc = H.initialize())) return rc;
-    if ((rc = H.optimize(its1))) return rc;
+    if ((rc = H.sort_edges()) || (rc = H.stage_inputs()) || (rc = H.build_pairs())) return rc;
+    // src/Optimizer.cpp:363-395: optimize(5); unless stopped, drop the outliers and the robust kernel and optimize(10); classify again
     std::vector<uint8_t> flags;
+    if ((rc = H.initialize()) || (rc = H.optimize(its1))) return rc;
     if (!H.terminate()) {
         if ((rc = H.classify(flags))) return rc;
-        for (int s = 0; s < nE; s++) if (flags[s]) H.level[s] = 1;
+        for (int s = 0; s < D.nE; s++) if (flags[s]) H.level[s] = 1;
         D.robust = 0;
-        if ((rc = H.initialize())) return rc;
-        if ((rc = H.optimize(its2))) return rc;
+        if ((rc = H.initialize()) || (rc = H.optimize(its2))) return rc;
     }
     if ((rc = H.classify(flags))) return rc;
-    std::vector<uint8_t> gflags;   // multi-GPU: every rank returns the flags of ALL edges (max over the owners' flags, in the caller's order)
-    if (multi) {
-        uint8_t* d_gflag = nullptr;
-        if ((rc = o->arena.take(&d_gflag, std::max(nEg, 1), true))) return rc;
-        if (nE > 0) { k_ba_scatter_flags<<<cdiv(nE, 256), 256, 0, o->stream>>>(nE, d_perm, H.d_flag, d_gflag); o->launches++; }
-        rc = nccl_api()->AllReduce(d_gflag, d_gflag, nEg, NCCL_U8, NCCL_MAX, o->comm, o->stream);
-        if (rc) { set_error("ncclAllReduce (flags) failed (%d)", rc); return CSLAM_E_NCCL; }
-        gflags.resize(nEg);
-        CSLAM_CUDA(cudaMemcpyAsync(gflags.data(), d_gflag, nEg, cudaMemcpyDeviceToHost, o->stream));
-        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-    }
-    H.drop_graph();
-    // ---- write back (src/Optimizer.cpp:432-450): float32 poses / points; with landmark sharding every rank holds its own points
-    if (o->nranks > 1) {
-        k_ba_mask_points<<<H.grid(nMP), 256, 0, o->stream>>>(D); o->launches++;
-        if ((rc = H.allreduce(D.X, (size_t)nMP * 3, NCCL_SUM))) return rc;
-    }
-    CSLAM_CUDA(cudaMemcpyAsync(poses.data(), D.pose, nKF * sizeof(Pose), cudaMemcpyDeviceToHost, o->stream));
-    hs.X.resize((size_t)nMP * 3);
-    std::vector<double>& X = hs.X;
-    CSLAM_CUDA(cudaMemcpyAsync(X.data(), D.X, X.size() * 8, cudaMemcpyDeviceToHost, o->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-    for (int k = 0; k < nKF; k++) {
-        pose_to_Tcw32(poses[k], p->Tcw + 16 * k);
-        if (r && r->pose_fp64) { double* q = r->pose_fp64 + 7 * k; q[0] = poses[k].t[0]; q[1] = poses[k].t[1]; q[2] = poses[k].t[2]; q[3] = poses[k].q[0]; q[4] = poses[k].q[1]; q[5] = poses[k].q[2]; q[6] = poses[k].q[3]; }
-    }
-    for (size_t i = 0; i < X.size(); i++) { p->points[i] = (float)X[i]; if (r && r->points_fp64) r->points_fp64[i] = X[i]; }
-    if (r) {
-        if (r->outlier) { if (multi) std::memcpy(r->outlier, gflags.data(), nEg); else for (int s = 0; s < nE; s++) r->outlier[H.perm ? H.perm[s] : s] = flags[s]; }
-        r->iterations = H.iterations; r->trials = H.trials;
-    }
-    return CSLAM_OK;
+    return H.write_back(flags);
 }

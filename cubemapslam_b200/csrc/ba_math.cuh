@@ -68,6 +68,10 @@ BA_HD void pose_to_Tcw32(const Pose& p, float* T) {
     for (int i = 0; i < 3; i++) { for (int j = 0; j < 3; j++) T[i * 4 + j] = (float)R[i][j]; T[i * 4 + 3] = (float)p.t[i]; }
     T[12] = 0; T[13] = 0; T[14] = 0; T[15] = 1;
 }
+// the 7-double pose record of the fp64 outputs (pose_fp64): t, then q = (x, y, z, w)
+BA_HD void pose_to_fp64(const Pose& p, double* r) {
+    r[0] = p.t[0]; r[1] = p.t[1]; r[2] = p.t[2]; r[3] = p.q[0]; r[4] = p.q[1]; r[5] = p.q[2]; r[6] = p.q[3];
+}
 // estimate <- SE3Quat::exp(update) * estimate   (VertexSE3Expmap::oplusImpl), update = [omega, upsilon]
 BA_HD Pose pose_oplus(const Pose& est, const double* u) {
     const double w[3] = {u[0], u[1], u[2]}, up[3] = {u[3], u[4], u[5]};
@@ -138,7 +142,9 @@ BA_HD void edge_Jpose(const double G[2][3], const double* Xc, double Jp[2][6]) {
         Jp[i][j + 3] = G[i][j];
     }
 }
-// Huber (RobustKernelHuber::robustify, delta = (double)(float)sqrt(5.991))
+// Huber delta of both optimizers: the reference's float thHuberMono = sqrt(5.991), widened to double
+BA_HD double huber_delta() { return (double)(float)sqrt(5.991); }
+// Huber (RobustKernelHuber::robustify)
 BA_HD void huber(double delta, double dsqr, double e, double& rho0, double& rho1) {
     if (e <= dsqr) { rho0 = e; rho1 = 1.0; }
     else { const double s = sqrt(e); rho0 = 2 * s * delta - dsqr; rho1 = delta / s; }

@@ -16,7 +16,7 @@ struct cslam_optimizer {
     cslam::DevArena arena;      // 64 MB chunks
     double* h_scal = nullptr;   // pinned, 16 doubles
     // host scratch of cslam_local_ba, kept across calls (fresh multi-megabyte vectors cost page faults on every call)
-    struct HostScratch { std::vector<int> lmStart, perm, eMP, eKF, fill, peStart, peList; std::vector<double> X; } hs;
+    struct HostScratch { std::vector<int> lmStart, perm, eMP, eKF, fill, peStart, peList, kfOfQ; std::vector<double> X; } hs;
     cslam::KernelTimer timer;   // optional per-kernel timing (cslam_optimizer_set_timing); LM trials then run eagerly instead of as a graph
     // one-shot NVLink all-reduce of the reduced camera system (multi-GPU LocalBA): peer views of every rank's exchange buffer
     struct Peer { void* base = nullptr; bool mine = false; };

@@ -138,12 +138,12 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
     PoFrame F;
     F.Xw = A.Xw; F.kpxy = A.kpxy; F.invSigma2 = A.invSigma2; F.err = A.err; F.level = A.level; F.outlier = A.outlier;
     if (A.offset) { F.beg = A.offset[f]; F.n = A.offset[f + 1] - F.beg; } else { F.beg = f * A.stride; F.n = min(A.count[f], A.stride); } F.faceW = A.faceW; F.faceH = A.faceH; F.fc = A.faceW / 2.0;
-    const float dlt = (float)sqrt(5.991); F.delta = (double)dlt; F.dsqr = F.delta * F.delta;
+    F.delta = huber_delta(); F.dsqr = F.delta * F.delta;
     const int beg = F.beg, n = F.n;
     if (tid == 0) { S.pose0 = pose_from_Tcw32(A.Tcw + 16 * f); S.pose = S.pose0; }
     for (int i = tid; i < n; i += T) { A.outlier[beg + i] = 0; A.level[beg + i] = 0; A.err[2 * (beg + i)] = 0; A.err[2 * (beg + i) + 1] = 0; }
     __syncthreads();
-    if (n < 3) { if (tid == 0) { A.inliers[f] = 0; if (A.pose64) { for (int i = 0; i < 3; i++) A.pose64[7 * f + i] = S.pose0.t[i]; for (int i = 0; i < 4; i++) A.pose64[7 * f + 3 + i] = S.pose0.q[i]; } } return; }
+    if (n < 3) { if (tid == 0) { A.inliers[f] = 0; if (A.pose64) pose_to_fp64(S.pose0, A.pose64 + 7 * f); } return; }
     int nBadEdges = 0;
     bool robust = true;
     for (int it = 0; it < 4; it++) {
@@ -198,13 +198,22 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
     if (tid == 0) {
         A.inliers[f] = n - nBadEdges;
         pose_to_Tcw32(S.pose, A.Tcw + 16 * f);
-        if (A.pose64) { for (int i = 0; i < 3; i++) A.pose64[7 * f + i] = S.pose.t[i]; for (int i = 0; i < 4; i++) A.pose64[7 * f + 3 + i] = S.pose.q[i]; }
+        if (A.pose64) pose_to_fp64(S.pose, A.pose64 + 7 * f);
     }
 }
 
 }  // namespace cslam
 
 using namespace cslam;
+
+// Both entry points: one CTA per frame on the optimizer's stream; the per-correspondence errors and levels are arena scratch of the call.
+static int launch_pose_opt(cslam_optimizer* o, int nframes, size_t nCorr, PoseOptArgs A) {
+    int rc;
+    if ((rc = o->arena.take(&A.err, nCorr * 2)) || (rc = o->arena.take(&A.level, nCorr))) return rc;
+    k_pose_opt<<<nframes, 256, 0, o->stream>>>(A); o->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    return CSLAM_OK;
+}
 
 extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw, const float* kp_xy, const float* inv_sigma2,
                                        int face_w, int face_h, uint8_t* outlier, int32_t* inliers, double* pose_fp64) {
@@ -214,11 +223,10 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
     o->arena.reset();
     const int n = offset[nframes];
     PoseOptArgs A; std::memset(&A, 0, sizeof(A));
-    int* d_off; float *d_T, *d_X, *d_kp, *d_w; uint8_t *d_out, *d_lvl; int32_t* d_inl; double *d_p64, *d_err;
+    int* d_off; float *d_T, *d_X, *d_kp, *d_w; uint8_t* d_out; int32_t* d_inl; double* d_p64;
     int rc;
     if ((rc = o->arena.take(&d_off, nframes + 1)) || (rc = o->arena.take(&d_T, (size_t)nframes * 16)) || (rc = o->arena.take(&d_X, (size_t)n * 3)) || (rc = o->arena.take(&d_kp, (size_t)n * 2)) ||
-        (rc = o->arena.take(&d_w, n)) || (rc = o->arena.take(&d_out, n)) || (rc = o->arena.take(&d_lvl, n)) || (rc = o->arena.take(&d_inl, nframes)) || (rc = o->arena.take(&d_p64, (size_t)nframes * 7)) ||
-        (rc = o->arena.take(&d_err, (size_t)n * 2))) return rc;
+        (rc = o->arena.take(&d_w, n)) || (rc = o->arena.take(&d_out, n)) || (rc = o->arena.take(&d_inl, nframes)) || (rc = o->arena.take(&d_p64, (size_t)nframes * 7))) return rc;
     CSLAM_CUDA(cudaMemcpyAsync(d_off, offset, (nframes + 1) * 4, cudaMemcpyHostToDevice, o->stream));
     CSLAM_CUDA(cudaMemcpyAsync(d_T, Tcw, (size_t)nframes * 64, cudaMemcpyHostToDevice, o->stream));
     if (n) {
@@ -227,9 +235,8 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
         CSLAM_CUDA(cudaMemcpyAsync(d_w, inv_sigma2, (size_t)n * 4, cudaMemcpyHostToDevice, o->stream));
     }
     A.offset = d_off; A.Tcw = d_T; A.Xw = d_X; A.kpxy = d_kp; A.invSigma2 = d_w; A.faceW = face_w; A.faceH = face_h; A.outlier = d_out; A.inliers = d_inl;
-    A.pose64 = d_p64; A.err = d_err; A.level = d_lvl;
-    k_pose_opt<<<nframes, 256, 0, o->stream>>>(A); o->launches++;
-    CSLAM_CUDA(cudaGetLastError());
+    A.pose64 = d_p64;
+    if ((rc = launch_pose_opt(o, nframes, n, A))) return rc;
     // frames with < 3 correspondences are returned untouched (src/Optimizer.cpp:133-134): copy back only the others
     std::vector<float> Tout((size_t)nframes * 16);
     CSLAM_CUDA(cudaMemcpyAsync(Tout.data(), d_T, Tout.size() * 4, cudaMemcpyDeviceToHost, o->stream));
@@ -249,14 +256,9 @@ extern "C" int cslam_pose_optimization_dev(cslam_optimizer* o, int nframes, int 
     CSLAM_CUDA(cudaSetDevice(o->device));
     o->arena.reset();
     PoseOptArgs A; std::memset(&A, 0, sizeof(A));
-    double* d_err; uint8_t* d_lvl; int rc;
-    const size_t n = (size_t)nframes * stride;
-    if ((rc = o->arena.take(&d_err, n * 2)) || (rc = o->arena.take(&d_lvl, n))) return rc;
-    A.offset = nullptr; A.count = count; A.stride = stride; A.Tcw = Tcw; A.Xw = Xw; A.kpxy = kp_xy; A.invSigma2 = inv_sigma2; A.faceW = face_w; A.faceH = face_h;
-    A.outlier = outlier; A.inliers = inliers; A.pose64 = nullptr; A.err = d_err; A.level = d_lvl;
-    k_pose_opt<<<nframes, 256, 0, o->stream>>>(A); o->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    return CSLAM_OK;
+    A.count = count; A.stride = stride; A.Tcw = Tcw; A.Xw = Xw; A.kpxy = kp_xy; A.invSigma2 = inv_sigma2; A.faceW = face_w; A.faceH = face_h;
+    A.outlier = outlier; A.inliers = inliers;
+    return launch_pose_opt(o, nframes, (size_t)nframes * stride, A);
 }
 extern "C" void* cslam_optimizer_stream(const cslam_optimizer* o) { return o ? (void*)o->stream : nullptr; }
 extern "C" int cslam_optimizer_sync(cslam_optimizer* o) {

@@ -66,6 +66,36 @@ def test_local_ba_edge_cases(oracle, opt):
     assert g["iters"] == 0 and np.array_equal(g["pts"], p["pts"]) and not g["outlier"].any()
 
 
+def _all_fixed_problem():
+    p = synth.ba_problem(nKF=6, nMP=200, kmin=2, kmax=5, faceW=450, seed=21, radius=1.5)
+    p["kf_fixed"][:] = 1
+    return p
+
+
+def test_local_ba_all_keyframes_fixed(oracle, opt):
+    """Every key frame fixed: only the points are free, so an LM trial has no Schur complement and no reduced solve."""
+    p = _all_fixed_problem()
+    r, g = _compare_ba(oracle, opt, p)
+    assert r["iters"] > 0 and not np.array_equal(g["pts"], p["pts"])
+
+
+def test_local_ba_all_keyframes_fixed_off_face(oracle, opt):
+    """An off-face key point in a problem without free poses is reported with the caller's edge index, like one with free poses."""
+    p = _all_fixed_problem()
+    perm = np.random.default_rng(3).permutation(len(p["eMP"]))
+    q = {k: (np.ascontiguousarray(p[k][perm]) if k in ("eMP", "eKF", "kpxy", "inv_sigma2") else p[k]) for k in p}
+    bad = q["kpxy"].copy(); bad[23] = (10.0, 10.0)    # top-left corner of the canvas: no face
+    with pytest.raises(Exception, match="edge 23"):
+        opt.LocalBundleAdjustment(q["Tcw"], q["kf_fixed"], q["pts"], q["eMP"], q["eKF"], bad, q["inv_sigma2"], 450, 450)
+
+
+def test_local_ba_no_edges(oracle, opt):
+    p = synth.ba_problem(nKF=4, nMP=50, kmin=2, kmax=4, faceW=450, seed=6, radius=1.5)
+    p["eMP"] = p["eMP"][:0]; p["eKF"] = p["eKF"][:0]; p["kpxy"] = p["kpxy"][:0]; p["inv_sigma2"] = p["inv_sigma2"][:0]
+    r, g = _compare_ba(oracle, opt, p)
+    assert g["iters"] == 0 and g["outlier"].size == 0 and np.array_equal(g["pts"], p["pts"])
+
+
 def test_pose_optimization_batch(oracle, opt):
     probs = [synth.pose_problem(n=n, faceW=450, seed=s, outlier_frac=0.15) for n, s in ((300, 5), (200, 6), (40, 7), (2, 8), (9, 9))]
     off = np.cumsum([0] + [len(q["Xw"]) for q in probs]).astype(np.int32)
