@@ -318,8 +318,9 @@ __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d -
 //  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, (s - mt) << 8, 0 where s <= mt; mt = minTh clamped to
 //     1..255, see below).
 //     On the warp path (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant
-//     (DevLevels::live), so its scores are 0, which the zeroed S already holds
-//  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the same items as A -> shared list; a keypoint at
+//     (DevLevels::live), so its scores are 0, which the zeroed S already holds. Each warp appends the items it scored non-zero to the
+//     tile's nz list (one shared atomic per warp)
+//  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the nz list -> shared list; a keypoint at
 //     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
 //  C  the selected entries (the per-cell fallback filter) appended to the strip's output buffer, one shared atomic per warp; the buffer is
 //     copied to the global candidate list (one global atomic) at the end of the strip, or at the end of a tile after which it could not
@@ -367,7 +368,9 @@ struct FastCols {
 // Dynamic shared memory of a k_fast CTA (byte offsets), sized from the level's cell geometry; CELL_MAX bounds it (fast_smem_max)
 struct FastSmem {
     int items;                 // the tile column's FastCols::item table
-    int tile, tileBytes;       // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
+    int nz;                    // the current tile's items phase A scored non-zero (u16, encoded as the live list): phase B's work list.
+                               // Its own region: warps append ahead of other warps' live-list reads, and the other buffers hold the next tile
+    int tile, tileBytes;     // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
                                // then hCell + 6 rows of FAST_TS
     int s2, klist;             // score map (hCell + 2 rows of FAST_SW pair-words); NMS survivors, kmax entries
     int live, liveBytes;       // live list buffer b (u16, staged in 16-byte pieces from an index that is a multiple of 8) at live + b * liveBytes
@@ -377,8 +380,11 @@ __host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
     FastSmem m;
     m.tileBytes = 16 + (g.hCell + 6) * FAST_TS; m.liveBytes = 16 * ((g.liveCap + 14) / 8);
     m.kmax = CG * ((g.wCell + 1) / 2) * ((g.hCell + 1) / 2);   // NMS survivors of a cell are pairwise non-adjacent
+    // items of a tile: nw <= (nx + 6) / 4 (fast_tile_x, nx <= CG * wCell) per detection row, hCell rows at most
+    const int nzCap = max(g.liveCap, ((CG * g.wCell + 6) >> 2) * g.hCell);
     m.items = 0;
-    m.tile = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);
+    m.nz = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);   // a constant offset: no register holds its address
+    m.tile = m.nz + 16 * ((nzCap + 7) / 8);
     m.s2 = m.tile + 2 * m.tileBytes;
     m.live = m.s2 + (g.hCell + 2) * FAST_SW * 4;
     m.klist = m.live + 2 * m.liveBytes;
@@ -411,7 +417,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
     __shared__ int rowVisit[FAST_R];                    // the strip row's tile has work (not skipped, detection rows > 0)
     __shared__ uint32_t sout[FAST_OUT];   // the strip's selected candidates, packed as in cand
     __shared__ int cnt20[CG];
-    __shared__ int nK, nOut, flushN;
+    __shared__ int nK, nNZ, nOut, flushN;
     __shared__ uint32_t flushBase;
     const int frame = blockIdx.z, row0 = blockIdx.y * FAST_R, nr = min(FAST_R, g.nRowsEff - row0);
     const int tid = threadIdx.x, lane = tid & 31;
@@ -473,10 +479,11 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         }
     };
     // Barriers of one tile (buffer b = tile parity in the strip):
-    //  top   S2 cleared, nK / cnt20 reset: the previous tile's phases B and C are done with them (its end barrier)
+    //  top   S2 cleared, nK / nNZ / cnt20 reset: the previous tile's phases B and C are done with them (its end barrier)
     //  wait  this thread's copies of the tile landed; B1 (__syncthreads_or) makes every thread's copies visible
-    //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phases A and B, before its B3
-    //  A  -> B2 -> B (S2, item table, live list of b) -> B3 -> C (klist, nK, cnt20; appends to the output buffer) -> end barrier
+    //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phase A, before its B2
+    //  A (reads the live list of b; appends to the nz list, nNZ) -> B2 -> B (S2, item table, nz list, nNZ) -> B3 -> C (klist, nK, cnt20;
+    //  appends to the output buffer) -> end barrier
     //  after the end barrier: flush when the buffer could not hold another tile's kmax entries, and at the end of the strip (one barrier
     //  more; the next appends follow the next tile's B1)
     for (int b = 0;; b ^= 1) {
@@ -494,7 +501,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
             }
         }
         if (tid < CG) cnt20[tid] = 0;
-        if (tid == 0) nK = 0;
+        if (tid == 0) { nK = 0; nNZ = 0; }
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         // caller canvases: an all-zero tile has no corners at any threshold (OR of the columns this thread staged)
         uint32_t acc = live ? 1u : 0u;
@@ -560,20 +567,37 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
                 }
                 const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
                 // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
-                // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset)
-                *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
-                    make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
+                // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset). An all-zero item is not stored:
+                // S2 already reads 0 there
+                const bool nz = (s02 | s13) != 0u;
+                if (nz)
+                    *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
+                        make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
+                return nz;
             };
+            // items scored non-zero go to the tile's nz list, encoded as the live list (y<<6 | (wi - w0)). ptxas aggregates the atomic: one
+            // ATOMS per warp (tools/kfast_sass.py). The entry is formed again after the score rather than held across it (register pressure)
+            uint16_t* const nzS = reinterpret_cast<uint16_t*>(fsm + SM.nz);
             if (live) {
-                for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; score_item(e >> 6, w0 + (e & 63)); }
+                for (uint32_t it = tid; it < nLive; it += 256) {
+                    const int e = liveS[it];
+                    if (score_item(e >> 6, w0 + (e & 63))) nzS[atomicAdd(&nNZ, 1)] = liveS[it];
+                }
             } else {
                 const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
-                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgItems); score_item(y, w0 + (it - y * nw)); }
+                for (int it = tid; it < nw * ny; it += 256) {
+                    const int y = fdiv_small(it, mgItems);
+                    if (score_item(y, w0 + (it - y * nw))) {
+                        const int y2 = fdiv_small(it, mgItems);
+                        nzS[atomicAdd(&nNZ, 1)] = (uint16_t)(y2 << 6 | (it - y2 * nw));
+                    }
+                }
             }
         }
         __syncthreads();
         // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
-        // non-zero only inside an item phase A scored, so B walks the same items; one thread reads the item's 3 x 4 pair-word neighbourhood once.
+        // non-zero only inside an item phase A scored non-zero, so B walks the tile's nz list; one thread reads the item's 3 x 4 pair-word
+        // neighbourhood once.
         // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
         // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
         {
@@ -605,12 +629,9 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
                     if (s > iniTh) atomicAdd(&cnt20[cell], 1);
                 }
             };
-            if (live) {
-                for (uint32_t it = tid; it < nLive; it += 256) { const int e = liveS[it]; nms_item(e >> 6, w0 + (e & 63)); }
-            } else {
-                const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
-                for (int it = tid; it < nw * ny; it += 256) { const int y = fdiv_small(it, mgItems); nms_item(y, w0 + (it - y * nw)); }
-            }
+            const uint16_t* const nzS = reinterpret_cast<const uint16_t*>(fsm + SM.nz);
+            const int nnz = nNZ;
+            for (int it = tid; it < nnz; it += 256) { const int e = nzS[it]; nms_item(e >> 6, w0 + (e & 63)); }
         }
         __syncthreads();
         // ---- C: each warp filters its stride of klist and appends with one shared atomic; the buffer has room for nk <= kmax entries

@@ -1,0 +1,119 @@
+#!/usr/bin/env python
+"""How much of k_fast's phase-B work (3x3 NMS) the nz list removes, at bench.py's headline shape; CPU only (the oracle, numpy, no GPU).
+
+The bench's fisheye frames go through the oracle's warp and pyramid (oracle.ORBextractor.level_image). Per level, FAST-9 arc scores are
+computed in numpy from the definition, without NMS, and the detection area is cut into k_fast's tiles and 4-pixel work items (the geometry
+of fast_tile_x in frontend.cu). Per level, summed over --frames frames, one JSON line on stdout:
+
+  live_items       items with a pixel of the detection area whose 7x7 window is not all one value: what phase A scores, and phase B scored
+                   before the nz list (within 1 % of the real live lists, DESIGN.md section 4)
+  nz_items         live items with a pixel of the detection area whose score is above minThFAST: what phase B scores now
+  nz_fraction      nz_items / live_items
+  zero_warp_groups share of 32-item groups of a tile's live items (one warp's items in one pass) that hold no nz item: what phase B's
+                   early return for an all-zero item already skipped as a whole warp
+
+  python tools/fast_nz_items.py [--frames 2]
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+CG = 4                      # k_fast cells per tile, as in frontend.cu
+RING = [(0, -3), (1, -3), (2, -2), (3, -1), (3, 0), (3, 1), (2, 2), (1, 3), (0, 3), (-1, 3), (-2, 2), (-3, 1), (-3, 0), (-3, -1), (-2, -2), (-1, -3)]
+
+
+def fast_scores(img):
+    """Arc score s of every pixel at least 3 from the border (0 elsewhere): the largest t such that 9 contiguous ring pixels are all
+    brighter than centre + t or all darker than centre - t, at least 0. corner(thr) <=> s > thr."""
+    h, w = img.shape
+    c = img[3:h - 3, 3:w - 3].astype(np.int16)
+    d = np.stack([c - img[3 + dy:h - 3 + dy, 3 + dx:w - 3 + dx].astype(np.int16) for dx, dy in RING])   # centre minus ring
+    d = np.concatenate([d, d[:8]])
+    s = np.zeros(c.shape, np.int16)
+    for k in range(16):
+        lo, hi = d[k:k + 9].min(0), d[k:k + 9].max(0)
+        s = np.maximum(s, np.maximum(lo, -hi))
+    out = np.zeros((h, w), np.int16)
+    out[3:h - 3, 3:w - 3] = s
+    return out
+
+
+def single_valued(img):
+    """True where the 7x7 window centred on the pixel holds one value."""
+    from scipy.ndimage import maximum_filter, minimum_filter
+    return maximum_filter(img, size=7, mode="nearest") == minimum_filter(img, size=7, mode="nearest")
+
+
+def tile_items(score, flat, minth, minB, maxBX, maxBY, wCell, hCell, nColsEff, nRowsEff):
+    """Per k_fast tile, its items in list order (detection row, then item): (live, nz) boolean vectors."""
+    for cy in range(nRowsEff):
+        iniY = minB + cy * hCell
+        ny = min(iniY + hCell + 6, maxBY) - iniY - 6
+        for cx in range(-(-nColsEff // CG)):
+            ncell = min(CG, nColsEff - cx * CG)
+            tx0 = minB + cx * CG * wCell
+            tx1 = min(tx0 + ncell * wCell + 6, maxBX)
+            nx = tx1 - tx0 - 6
+            if nx <= 0 or ny <= 0:
+                continue
+            a0 = tx0 & ~15
+            xoff = tx0 - a0 + 3
+            w0, w1 = xoff >> 2, (xoff + nx + 3) >> 2
+            cols = np.arange(4 * w0, 4 * w1) + a0                    # level x of the items' pixels
+            valid = (cols >= tx0 + 3) & (cols < tx0 + 3 + nx)
+            ys = iniY + 3 + np.arange(ny)
+            cc = np.clip(cols, 0, score.shape[1] - 1)
+            lv = ~flat[ys][:, cc] & valid
+            nz = (score[ys][:, cc] > minth) & valid
+            yield lv.reshape(ny, -1, 4).any(2).ravel(), nz.reshape(ny, -1, 4).any(2).ravel()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=2)
+    args = ap.parse_args()
+    import oracle as orc
+    from cubemapslam_b200 import _capi, config, synth
+    import bench
+    from fast_live_roofline import _grid
+    cfg = config.front_1024()
+    o = _capi.orb_params(cfg)
+    cp = orc.cam_params(cfg)
+    m1, m2 = orc.build_maps(cp)
+    mask = bench.load_mask()
+    levels = [dict(live_items=0, nz_items=0, groups=0, zero_groups=0) for _ in range(o.nlevels)]
+    for f in range(args.frames):
+        ex = orc.ORBextractor(o.nfeatures, o.scale_factor, o.nlevels, o.ini_th_fast, o.min_th_fast, cp.faceW, cp.faceH)
+        ex(orc.warp(cp, synth.fisheye_frame(cfg, f), m1, m2), mask)
+        for l in range(o.nlevels):
+            img = ex.level_image(l)
+            h, w = img.shape
+            score, flat = fast_scores(img), single_valued(img)
+            L = levels[l]
+            L["side"] = w
+            for live, nz in tile_items(score, flat, o.min_th_fast, *_grid(w, h)):
+                nzl = nz[live]                                       # the live list, in k_fast's order
+                L["live_items"] += int(live.sum())
+                L["nz_items"] += int(nzl.sum())
+                for g in range(0, len(nzl), 32):
+                    L["groups"] += 1
+                    L["zero_groups"] += int(not nzl[g:g + 32].any())
+    out = []
+    for L in levels:
+        out.append({"side": L["side"], "live_items": L["live_items"] // args.frames, "nz_items": L["nz_items"] // args.frames,
+                    "nz_fraction": round(L["nz_items"] / max(L["live_items"], 1), 4),
+                    "zero_warp_groups": round(L["zero_groups"] / max(L["groups"], 1), 4)})
+    tl = sum(L["live_items"] for L in levels); tn = sum(L["nz_items"] for L in levels)
+    print(json.dumps({"frames": args.frames, "min_th_fast": o.min_th_fast, "per_frame": out,
+                      "total": {"live_items": tl // args.frames, "nz_items": tn // args.frames, "nz_fraction": round(tn / max(tl, 1), 4)}}))
+
+
+if __name__ == "__main__":
+    main()

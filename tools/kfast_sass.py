@@ -10,8 +10,11 @@ object:
                                        with its BAR and ATOMG counts (`bar`, `atomg`: every path of one pass, flush of the output buffer included)
   staging                              each tile-staging loop (a loop whose body issues cp.async, LDGSTS, and no score arithmetic)
   phase_a                              each scoring loop (a loop without a barrier whose body issues >= 64 VIMNMX3 / VIMNMX), `live` when its body loads
-                                       the u16 live list (staged in shared memory)
-  phase_b                              each NMS loop (a loop with a shared-memory atomic and no barrier)
+                                       the u16 live list (staged in shared memory); `append`: the instructions of its body that append a non-zero
+                                       item to the nz list (the atomic ptxas aggregates per warp and the u16 store: VOTEU, FLO, POPC, S2R, SHFL,
+                                       ATOMS, STS.U16 and the uniform address arithmetic)
+  phase_b                              each NMS loop (a loop with a shared-memory atomic, VIMNMX3 and no barrier)
+  compaction                           the other loops with a shared-memory atomic and no barrier (NMS survivors, phase C)
   each loop                            [start, end] byte offsets, the body's instruction count and its opcode histogram
 
 A loop is the address range from a backward branch's target to the branch. Counts are static: one pass through the body, every path
@@ -32,6 +35,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 INSN = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P\w+\s+)?([A-Z][A-Z0-9_.x]*)([^;]*);")
 RES = re.compile(r"Used (\d+) registers.*?(\d+) bytes smem")
+APPEND = {"VOTEU", "FLO", "POPC", "S2R", "S2UR", "SHFL", "ATOMS", "UMOV", "UIADD3", "ULEA"}
 SPILL = re.compile(r"(\d+) bytes spill stores, (\d+) bytes spill loads")
 
 
@@ -97,7 +101,7 @@ def main():
             cubin = os.path.join(tmp, "frontend.cubin")
             res = compile_cubin(cubin)
         insns = k_fast_sass(cubin)
-    strip, phase_a, phase_b, staging = [], [], [], []
+    strip, phase_a, phase_b, compaction, staging = [], [], [], [], []
     for lo, hi in loops(insns):
         b = body(insns, lo, hi)
         h = hist(b)
@@ -108,9 +112,10 @@ def main():
             strip.append(entry)
         elif minmax >= 64:
             entry["live"] = any(op.startswith("LDS") and ".U16" in op for op, _ in b)
+            entry["append"] = sum(1 for op, _ in b if op.split(".")[0] in APPEND or op.startswith("STS.U16"))
             phase_a.append(entry)
         elif h.get("ATOMS", 0) and not h.get("BAR", 0):
-            phase_b.append(entry)
+            (phase_b if h.get("VIMNMX3", 0) else compaction).append(entry)
         elif h.get("LDGSTS", 0):
             staging.append(entry)
     first_a = min((int(e["range"][0], 16) for e in strip + phase_a), default=insns[-1][0] + 1)
@@ -121,6 +126,7 @@ def main():
     out["strip"] = strip
     out["phase_a"] = phase_a
     out["phase_b"] = phase_b
+    out["compaction"] = compaction
     out["staging"] = staging
     print(json.dumps(out, indent=1))
 
