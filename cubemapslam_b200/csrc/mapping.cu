@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
     const float ex = epi[0], ey = epi[1];
     for (int i1 = tid; i1 < n1; i1 += TRI_THREADS) {
         int bestIdx2 = -1;
-        if (!M1[i1]) {
+        if (!M1[i1] && N1[i1] >= 0) {   // node -1: in no FeatureVector node of KF1, never a query
             const int lo = node_lower_bound(key2, n2, (uint32_t)N1[i1]);
             const uint4 a0 = __ldg(D1 + 2 * i1), a1 = __ldg(D1 + 2 * i1 + 1);
             const float r0 = R1[3 * i1], r1 = R1[3 * i1 + 1], r2 = R1[3 * i1 + 2];
@@ -344,8 +344,11 @@ extern "C" int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const
     }
     if (npairs == 0) return CSLAM_OK;
     const size_t t1 = (size_t)npairs * stride1, t2 = (size_t)npairs * stride2;
-    for (size_t i = 0; i < t1; i++) if (node1[i] < 0 || node1[i] >= (1 << 20) - 1) { set_error("cslam_search_for_triangulation: node ids must be in [0, 2^20 - 1)"); return CSLAM_E_BADARG; }
-    for (size_t i = 0; i < t2; i++) if (node2[i] < 0 || node2[i] >= (1 << 20) - 1) { set_error("cslam_search_for_triangulation: node ids must be in [0, 2^20 - 1)"); return CSLAM_E_BADARG; }
+    for (int p = 0; p < npairs; p++)   // only the rows the kernel reads: [p*stride, p*stride + min(n[p], stride))
+        if (!node_ids_ok(node1 + (size_t)p * stride1, (size_t)std::max(0, std::min(n1[p], stride1))) ||
+            !node_ids_ok(node2 + (size_t)p * stride2, (size_t)std::max(0, std::min(n2[p], stride2)))) {
+            set_error("cslam_search_for_triangulation: node ids must be in [-1, 2^20 - 1) (pair %d)", p); return CSLAM_E_BADARG;
+        }
     CSLAM_CUDA(cudaSetDevice(m->device));
     m->arena.reset();
     DevArena& a = m->arena;

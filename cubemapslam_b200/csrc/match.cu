@@ -214,7 +214,8 @@ __global__ void __launch_bounds__(BF_THREADS) k_match_bruteforce(const uint8_t* 
 // ------------------------------------------------------------------------------------------------- SearchByBoW
 static const int BOW_THREADS = 256;
 
-// keys: node << 12 | index (index < 4096, node < 2^20). Shared memory: keyKF[n2K], keyF[n2F], takenF[nF] bytes.
+// keys: node << 12 | index (index < 4096, node in [-1, 2^20 - 1): node -1 = in no FeatureVector node, key group 0xfffff, never matched).
+// Shared memory: keyKF[n2K], keyF[n2F], takenF[nF] bytes.
 __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __restrict__ descKF, const float* __restrict__ angKF,
                                                                const uint8_t* __restrict__ kfValid, const int32_t* __restrict__ nodeKF, int nKF,
                                                                const uint8_t* __restrict__ descF, const float* __restrict__ angF,
@@ -250,7 +251,7 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
         // warps take candidate group starts round-robin: position s is a start iff s==0 or node differs from s-1
         // (cheap: every warp scans its own positions; groups are independent of each other)
         const uint32_t node = keyKF[s] >> 12;
-        if (s > 0 && (keyKF[s - 1] >> 12) == node) continue;
+        if (node == 0xfffffu || (s > 0 && (keyKF[s - 1] >> 12) == node)) continue;   // 0xfffff: node -1, in no FeatureVector node
         // KF group [s, e)
         int e = s + 1;
         while (e < nKF && (keyKF[e] >> 12) == node) e++;
@@ -606,8 +607,9 @@ extern "C" int cslam_search_by_bow(cslam_matcher* m, const uint8_t* descKF, cons
                                    int32_t* nmatches) {
     int rc = check_sizes(m, nKF, nF, npairs);
     if (rc) return rc;
-    m->arena.reset();
     const size_t nk = (size_t)npairs * nKF, nf = (size_t)npairs * nF;
+    if (!node_ids_ok(node_kf, nk) || !node_ids_ok(node_f, nf)) { set_error("cslam_search_by_bow: node ids must be in [-1, 2^20 - 1)"); return CSLAM_E_BADARG; }
+    m->arena.reset();
     const uint8_t *dK, *dValid, *dF; const float *aK, *aF; const int32_t *nodeK, *nodeF; int32_t *dMatch, *dN;
     if ((rc = m->arena.upload(&dK, descKF, nk * 32)) || (rc = m->arena.upload(&aK, angKF, nk)) || (rc = m->arena.upload(&dValid, kf_valid, nk)) ||
         (rc = m->arena.upload(&nodeK, node_kf, nk)) || (rc = m->arena.upload(&dF, descF, nf * 32)) || (rc = m->arena.upload(&aF, angF, nf)) ||
@@ -639,6 +641,9 @@ extern "C" int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, co
                                       int check_ori, int32_t* match12, int32_t* nmatches) {
     int rc = check_sizes(m, n1, n2, npairs);
     if (rc) return rc;
+    if (!node_ids_ok(node1, (size_t)npairs * n1) || !node_ids_ok(node2, (size_t)npairs * n2)) {
+        set_error("cslam_search_by_bow_kf: node ids must be in [-1, 2^20 - 1)"); return CSLAM_E_BADARG;
+    }
     if (n1 == 0 || n2 == 0) { for (size_t i = 0; i < (size_t)npairs * n1; i++) match12[i] = -1; for (int p = 0; p < npairs; p++) nmatches[p] = 0; return CSLAM_OK; }
     m->arena.reset();
     const size_t k1 = (size_t)npairs * n1, k2 = (size_t)npairs * n2;

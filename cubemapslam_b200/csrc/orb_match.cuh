@@ -65,4 +65,12 @@ __device__ __forceinline__ int node_lower_bound(const uint32_t* key, int n, uint
     return lo;
 }
 
+// Node ids the keys hold apart: [-1, 2^20 - 1). -1 (a stopped word's feature, in no FeatureVector node) packs to group 0xfffff, which the
+// searches skip; 2^20 - 1 would share that group, and anything else outside the range would alias another node through the 32-bit key.
+static const int NODE_ID_END = (1 << 20) - 1;
+static inline bool node_ids_ok(const int32_t* node, size_t n) {
+    for (size_t i = 0; i < n; i++) if (node[i] < -1 || node[i] >= NODE_ID_END) return false;
+    return true;
+}
+
 }  // namespace cslam

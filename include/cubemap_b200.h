@@ -127,7 +127,9 @@ int cslam_ubench_bmma(cslam_matcher* m, double* bmma_products_per_s, double* imm
 /* Same for 3-input u16x2 min/max (VIMNMX3.U16x2), the instruction k_fast is bound by; out: thread-level operations per second. */
 int cslam_ubench_minmax3(cslam_matcher* m, double* ops_per_s);
 /* ORBMatcher::SearchByBoW(KeyFrame*, Frame&, vector<MapPoint*>&) (src/ORBMatcher.cpp:409-539) for npairs (KF,F) pairs.
- * kf_valid: 1 where the KF feature has a good MapPoint; node_kf/node_f: DBoW2 FeatureVector node id per feature.
+ * kf_valid: 1 where the KF feature has a good MapPoint; node_kf/node_f: DBoW2 FeatureVector node id per feature, in [-1, 2^20 - 1);
+ * -1 = in no FeatureVector node (a stopped word, as cslam_bow_transform writes it): such a feature is never matched. The host form
+ * rejects any other id with CSLAM_E_BADARG; the _dev form cannot check device arrays and requires the same range.
  * match_f: npairs x nF (index of the KF feature whose MapPoint is assigned, or -1); nmatches: npairs. */
 int cslam_search_by_bow(cslam_matcher* m, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid,
                         const int32_t* node_kf, int nKF, const uint8_t* descF, const float* angF, const int32_t* node_f,
@@ -138,6 +140,7 @@ int cslam_search_by_bow_dev(cslam_matcher* m, const uint8_t* descKF, const float
 
 /* ORBMatcher::SearchByBoW(KeyFrame*, KeyFrame*, vector<MapPoint*>&) (src/ORBMatcher.cpp:541-674, loop closing): both sides need a good
  * MapPoint (valid1/valid2), features of the second key frame are consumed, acceptance is the strict best < TH_LOW.
+ * node1/node2: FeatureVector node ids in [-1, 2^20 - 1), -1 = in no node (never matched); any other id is CSLAM_E_BADARG.
  * match12: npairs x n1 (index of the matched feature of key frame 2, or -1). */
 int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, const float* ang1, const uint8_t* valid1, const int32_t* node1, int n1,
                            const uint8_t* desc2, const float* ang2, const uint8_t* valid2, const int32_t* node2, int n2, int npairs,
@@ -296,7 +299,8 @@ int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, const uint8_t
 /* ORBMatcher::SearchForTriangulation(pKF1, pKF2, E12, vMatchedPairs) (reference src/ORBMatcher.cpp:971-1124) for `npairs` key-frame pairs in one
  * launch (LocalMapping::CreateNewMapPoints matches the new key frame against ~20 neighbours). Pair p reads rows [p*stride, p*stride + n[p]) of
  * the per-feature arrays: key points, descriptors, bearing vectors (mvKeyRays), has_mp (GetMapPoint(idx) != NULL), node = the vocabulary node of
- * the feature in mFeatVec (levelsup 4; in [0, 2^20 - 1)). Ow1 = pKF1->GetCameraCenter() (3), Tcw2 = pKF2's pose (16), E12 (9, row-major).
+ * the feature in mFeatVec (levelsup 4; in [-1, 2^20 - 1), -1 = in no node, as cslam_bow_transform writes a stopped word's feature: never
+ * matched; any other id in the rows read is CSLAM_E_BADARG, rows past n[p] are not read or checked). Ow1 = pKF1->GetCameraCenter() (3), Tcw2 = pKF2's pose (16), E12 (9, row-major).
  * scale_factors / level_sigma2 = pKF2->mvScaleFactors / mvLevelSigma2. match12[p*stride1 + i1] = matched feature of KF2 or -1; nmatches[p].
  * (As in the reference, vbMatched2 is never set: two features of KF1 may choose the same feature of KF2.) */
 int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const cslam_keypoint* k1, const uint8_t* d1, const float* rays1, const uint8_t* has_mp1, const int32_t* node1,

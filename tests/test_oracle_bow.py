@@ -33,3 +33,23 @@ def test_transform_matches_reference_dbow2(oracle, tmp_path, k, L, levelsup):
     assert same(np.asarray(node, np.int32), rnode)                                            # FeatureVector membership of every feature
     assert abs(bv.sum() - 1.0) < 1e-12 and len(bw) > 300
     assert (node[word >= 0] >= 0).mean() > 0.95                           # a few stopped words (weight 0) are excluded like in the reference
+
+
+def test_transform_unbalanced_tree_with_ties_matches_reference_dbow2(oracle, tmp_path):
+    """ORBvoc's shape with 1..10 children per node and leaves at depths 2..6, at levelsup 4 (Frame::ComputeBoW), and features tied between
+    two siblings at every level (the first in file order must win): the oracle's descent against the reference's."""
+    from tests.test_gpu_bow_limits import unbalanced_features, unbalanced_tree
+    voc = unbalanced_tree(0)
+    feats, lev, _ = unbalanced_features(voc)
+    ov = oracle.Vocabulary(voc["k"], voc["L"], voc["parent"], voc["is_leaf"], voc["desc"], voc["weight"])
+    bw, bv, node, word = ov.transform(feats, 4)
+
+    def run():
+        path = tmp_path / "voc.txt"
+        synth.write_vocabulary_text(voc, str(path))
+        rv = ref.RefVocabulary(str(path))
+        return (rv.size(),) + rv.transform(feats, 4)
+    size, rbw, rbv, rnode = REC("transform_unbalanced_ties", run, digest=(1, 2, 3))
+    assert size == int(voc["is_leaf"].sum()) and sorted(set(lev.tolist())) == [1, 2, 3, 4, 5, 6]
+    assert same(np.asarray(bw, np.int32), rbw) and same(np.asarray(bv, np.float64), rbv)
+    assert same(np.asarray(node, np.int32), rnode)
