@@ -51,20 +51,49 @@ def lib():
                              "the package has no CPU fallback")
         _lib = C.CDLL(LIB_PATH)
         _lib.cslam_last_error.restype = C.c_char_p
-        _lib.cslam_frontend_stream.restype = C.c_void_p
-        _lib.cslam_frontend_launches.restype = C.c_int64
-        for name in ("cslam_matcher_stream",):
-            if hasattr(_lib, name):
-                getattr(_lib, name).restype = C.c_void_p
-        for name in ("cslam_matcher_launches", "cslam_optimizer_launches"):
-            if hasattr(_lib, name):
-                getattr(_lib, name).restype = C.c_int64
+        for kind in ("frontend", "matcher", "vocabulary", "tracker", "optimizer"):
+            getattr(_lib, "cslam_%s_stream" % kind).restype = C.c_void_p
+        for kind in ("frontend", "matcher", "tracker", "optimizer", "mapper"):
+            getattr(_lib, "cslam_%s_launches" % kind).restype = C.c_int64
     return _lib
 
 
 def check(rc):
     if rc != 0:
         raise CslamError("libcubemap_b200: error %d: %s" % (rc, lib().cslam_last_error().decode()))
+
+
+class Handle:
+    """One handle of the C ABI: cslam_<KIND>_create(&h, *args) on construction, cslam_<KIND>_destroy on close() (safe to call twice) or
+    garbage collection. stream, launches and sync forward to cslam_<KIND>_stream / _launches / _sync; a handle whose C ABI lacks one of
+    them raises AttributeError there."""
+    KIND = None
+
+    def __init__(self, *args):
+        self._h = C.c_void_p()
+        check(getattr(lib(), "cslam_%s_create" % self.KIND)(C.byref(self._h), *args))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            getattr(lib(), "cslam_%s_destroy" % self.KIND)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def stream(self):
+        return getattr(lib(), "cslam_%s_stream" % self.KIND)(self._h)
+
+    @property
+    def launches(self):
+        return getattr(lib(), "cslam_%s_launches" % self.KIND)(self._h)
+
+    def sync(self):
+        check(getattr(lib(), "cslam_%s_sync" % self.KIND)(self._h))
 
 
 def ptr(a):

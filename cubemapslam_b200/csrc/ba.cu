@@ -875,27 +875,21 @@ static const char* kBaKindNames[BK_COUNT] = {"k_ba_errors", "k_ba_lin_points", "
 
 extern "C" int cslam_optimizer_create(cslam_optimizer** out, int device) {
     if (!out) return CSLAM_E_BADARG;
-    const int rc = check_device(device);
-    if (rc) return rc;
-    cslam_optimizer* o = new cslam_optimizer; o->device = device;
-    if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMallocHost(&o->h_scal, 16 * sizeof(double)) != cudaSuccess) {
-        set_error("optimizer: stream / pinned allocation failed"); delete o; return CSLAM_E_CUDA;
-    }
-    o->arena.bind(o->stream, (size_t)64 << 20);
+    cslam_optimizer* o = new cslam_optimizer;
+    int rc;
+    if ((rc = o->open(device, (size_t)64 << 20, false)) || (rc = pinned_alloc(o->pinned, &o->h_scal, 16))) { destroy_handle(o); return rc; }
     cudaFuncSetAttribute(k_ba_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, 204 * 1024);
     *out = o;
     return CSLAM_OK;
 }
-extern "C" void cslam_optimizer_destroy(cslam_optimizer* o) {
-    if (!o) return;
-    cudaSetDevice(o->device);
-    if (o->stream) cudaStreamSynchronize(o->stream);
+static void close_peers(cslam_optimizer* o) {
     for (auto& p : o->peers) { if (p.base && !p.mine) cudaIpcCloseMemHandle(p.base); else if (p.base) cudaFree(p.base); }
-    if (o->comm && nccl_api()) nccl_api()->CommDestroy(o->comm);
-    if (o->stream) cudaStreamDestroy(o->stream);
-    if (o->h_scal) cudaFreeHost(o->h_scal);
-    delete o;
 }
+cslam_optimizer::~cslam_optimizer() {
+    close_peers(this);
+    if (comm && nccl_api()) nccl_api()->CommDestroy(comm);
+}
+extern "C" void cslam_optimizer_destroy(cslam_optimizer* o) { destroy_handle(o); }
 extern "C" int64_t cslam_optimizer_launches(const cslam_optimizer* o) { return o ? o->launches : 0; }
 extern "C" int cslam_optimizer_set_timing(cslam_optimizer* o, int enable) {
     if (!o) return CSLAM_E_BADARG;
@@ -920,7 +914,7 @@ static const size_t XCHG_FLAG_BYTES = 256;
 static int setup_xchg(cslam_optimizer* o, size_t payloadBytes) {
     NcclApi* a = nccl_api();
     if (o->nranks > 8 || !a->AllGather) return 1;   // fall back to NCCL
-    for (auto& p : o->peers) { if (p.base && !p.mine) cudaIpcCloseMemHandle(p.base); else if (p.base) cudaFree(p.base); }
+    close_peers(o);
     o->peers.assign(o->nranks, cslam_optimizer::Peer());
     void* mine = nullptr;
     const size_t bytes = 2 * ((payloadBytes + 255) & ~(size_t)255) + XCHG_FLAG_BYTES;   // two payload buffers (epoch parity) + the flag slots
@@ -1371,7 +1365,7 @@ struct BAHost {
         std::vector<double>& X = o->hs.X;
         X.resize((size_t)nMP * 3);
         CSLAM_CUDA(cudaMemcpyAsync(X.data(), D.X, X.size() * 8, cudaMemcpyDeviceToHost, o->stream));
-        CSLAM_CUDA(cudaStreamSynchronize(o->stream));
+        if ((rc = o->sync())) return rc;
         for (int k = 0; k < nKF; k++) {
             pose_to_Tcw32(poses[k], p->Tcw + 16 * k);
             if (res && res->pose_fp64) pose_to_fp64(poses[k], res->pose_fp64 + 7 * k);

@@ -95,47 +95,38 @@ __global__ void __launch_bounds__(256) k_bow_vector(VocDev V, const int32_t* __r
 
 using namespace cslam;
 
-struct cslam_vocabulary {
-    int device = 0; VocDev V; cudaStream_t stream = nullptr; std::vector<void*> owned; int64_t launches = 0;
-    int maxFrames = 0, maxFeat = 0;
-    DevArena arena;   // staging of cslam_bow_transform
+// arena: staging of cslam_bow_transform
+struct cslam_vocabulary : cslam::Handle {
+    VocDev V; int maxFrames = 0, maxFeat = 0;
 };
 
-extern "C" void cslam_vocabulary_destroy(cslam_vocabulary* v) {
-    if (!v) return;
-    cudaSetDevice(v->device);
-    if (v->stream) { cudaStreamSynchronize(v->stream); cudaStreamDestroy(v->stream); }
-    for (void* p : v->owned) cudaFree(p);
-    delete v;
-}
+extern "C" void cslam_vocabulary_destroy(cslam_vocabulary* v) { destroy_handle(v); }
 
 // nodes 1..n_nodes in ORBvoc.txt's order (TemplatedVocabulary::loadFromTextFile :1337-1415): parent id, leaf flag, 32 descriptor bytes, weight
 extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k, int L, int n_nodes, const int32_t* parent, const uint8_t* is_leaf, const uint8_t* desc,
                                        const double* weight, int max_frames, int max_features) {
     if (!out || k < 2 || L < 1 || n_nodes <= 0 || !parent || !is_leaf || !desc || !weight || max_frames <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_vocabulary_create: bad argument"); return CSLAM_E_BADARG; }
-    int rc = check_device(device);
-    if (rc) return rc;
+    cslam_vocabulary* v = new cslam_vocabulary; v->maxFrames = max_frames; v->maxFeat = max_features;
+    auto fail = [&](int code) { destroy_handle(v); return code; };
+    // chunks: room for the descriptors, four int32 arrays and the double weights of a call at the handle's limits, at most 64 MB
+    int rc = v->open(device, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * (32 + 4 * 4 + 8) + (size_t)max_frames * 8), false);
+    if (rc) return fail(rc);
     const int N = n_nodes + 1;
     std::vector<int> cnt(N + 1, 0), wordId(N, -1);
     int words = 0;
     for (int i = 0; i < n_nodes; i++) {
-        if (parent[i] < 0 || parent[i] > i) { set_error("vocabulary node %d: parent %d must precede it", i + 1, parent[i]); return CSLAM_E_BADARG; }
+        if (parent[i] < 0 || parent[i] > i) { set_error("vocabulary node %d: parent %d must precede it", i + 1, parent[i]); return fail(CSLAM_E_BADARG); }
         cnt[parent[i] + 1]++;
         if (is_leaf[i]) wordId[i + 1] = words++;
     }
-    if (words >= (1 << 20)) { set_error("vocabulary has %d words; the packed sort keys hold word ids < 2^20", words); return CSLAM_E_BADARG; }
+    if (words >= (1 << 20)) { set_error("vocabulary has %d words; the packed sort keys hold word ids < 2^20", words); return fail(CSLAM_E_BADARG); }
     for (int i = 0; i < N; i++) cnt[i + 1] += cnt[i];
     std::vector<int> start(cnt), fill(cnt.begin(), cnt.end() - 1), list(n_nodes);
     for (int i = 0; i < n_nodes; i++) list[fill[parent[i]]++] = i + 1;       // children in file order (push_back order)
     std::vector<uint8_t> d((size_t)N * 32, 0); std::vector<double> w(N, 0.0);
     std::memcpy(d.data() + 32, desc, (size_t)n_nodes * 32);
     std::memcpy(w.data() + 1, weight, (size_t)n_nodes * 8);
-    cslam_vocabulary* v = new cslam_vocabulary; v->device = device; v->maxFrames = max_frames; v->maxFeat = max_features;
     int *dStart, *dList, *dWid; uint4* dDesc; double* dW;
-    auto fail = [&](int code) { cslam_vocabulary_destroy(v); return code; };
-    if (cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); return fail(CSLAM_E_CUDA); }
-    // chunks: room for the descriptors, four int32 arrays and the double weights of a call at the handle's limits, at most 64 MB
-    v->arena.bind(v->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * (32 + 4 * 4 + 8) + (size_t)max_frames * 8));
     auto valloc = [&](auto** p, size_t n) { return dev_alloc(v->owned, p, n, false); };
     if ((rc = valloc(&dStart, N + 1)) || (rc = valloc(&dList, n_nodes)) || (rc = valloc(&dWid, N)) || (rc = valloc(&dDesc, (size_t)N * 2)) || (rc = valloc(&dW, N))) return fail(rc);
     if (cudaMemcpy(dStart, start.data(), (N + 1) * 4, cudaMemcpyHostToDevice) != cudaSuccess || cudaMemcpy(dList, list.data(), (size_t)n_nodes * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -147,7 +138,7 @@ extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k
     return CSLAM_OK;
 }
 extern "C" void* cslam_vocabulary_stream(const cslam_vocabulary* v) { return v ? (void*)v->stream : nullptr; }
-extern "C" int cslam_vocabulary_sync(cslam_vocabulary* v) { if (!v) return CSLAM_E_BADARG; CSLAM_CUDA(cudaSetDevice(v->device)); CSLAM_CUDA(cudaStreamSynchronize(v->stream)); return CSLAM_OK; }
+extern "C" int cslam_vocabulary_sync(cslam_vocabulary* v) { return v ? v->sync() : CSLAM_E_BADARG; }
 
 extern "C" int cslam_bow_transform_dev(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* word, int32_t* leaf, int32_t* node,
                                        int32_t* bow_word, double* bow_val, int32_t* bow_count) {
@@ -176,6 +167,5 @@ extern "C" int cslam_bow_transform(cslam_vocabulary* v, const uint8_t* desc, con
     CSLAM_CUDA(cudaMemcpyAsync(bow_word, dBowWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
     CSLAM_CUDA(cudaMemcpyAsync(bow_val, dBowVal, nf * 8, cudaMemcpyDeviceToHost, v->stream));
     CSLAM_CUDA(cudaMemcpyAsync(bow_count, dBowCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(v->stream));
-    return CSLAM_OK;
+    return v->sync();
 }

@@ -11,8 +11,6 @@
 namespace cslam {
 
 void set_error(const char* fmt, ...);   // thread-local message behind cslam_last_error()
-// every handle constructor: CSLAM_E_NODEVICE without a CUDA device (no CPU fallback), CSLAM_E_BADARG for a device out of range, else cudaSetDevice
-int check_device(int device);
 
 #define CSLAM_CUDA(expr)                                                                        \
     do {                                                                                        \
@@ -38,6 +36,15 @@ static int dev_alloc(std::vector<void*>& owned, T** p, size_t count, bool zero) 
     *p = (T*)q;
     return 0;
 }
+// Page-locked host buffer of `count` elements (at least one) owned by a handle: it goes onto `pinned`, which the handle's destroy frees.
+template <class T>
+static int pinned_alloc(std::vector<void*>& pinned, T** p, size_t count) {
+    void* q = nullptr;
+    CSLAM_CUDA(cudaMallocHost(&q, std::max<size_t>(count, 1) * sizeof(T)));
+    pinned.push_back(q);
+    *p = (T*)q;
+    return 0;
+}
 
 // Device memory of a handle's single calls (staged inputs, outputs, scratch), carved from chunks the handle keeps across calls: cudaMalloc /
 // cudaFree per call would cost more than many of the calls themselves. Pieces are 256-byte aligned and go to the first chunk with room; a new
@@ -57,7 +64,6 @@ class DevArena {
     DevArena(const DevArena&) = delete;
     DevArena& operator=(const DevArena&) = delete;
     ~DevArena() { for (auto& c : chunks) cudaFree(c.p); }
-    void bind(cudaStream_t s, size_t minChunk) { stream = s; minBytes = minChunk; }   // once, when the handle's stream exists
     void reset() { for (auto& c : chunks) c.used = 0; }
     // `count` elements (at least one); zero: cleared on the stream
     template <class T>
@@ -86,11 +92,48 @@ class DevArena {
     }
 
   private:
+    friend struct Handle;   // Handle::open gives the arena its stream and minimum chunk
     struct Chunk { char* p; size_t size, used; };
     std::vector<Chunk> chunks;
     cudaStream_t stream = nullptr;
     size_t minBytes = 0;
 };
+
+// What every handle of the C ABI owns, with one definition of its lifecycle (capi_common.cu). The handle structs derive from it.
+// - open(): check the device, create the handle's non-blocking stream (all of its work is ordered by it), give the arena that stream and
+//   its minimum chunk, and, for handles whose kernels report overflow, allocate the zeroed device error flag and its pinned host copy.
+// - sync(): wait for the stream; a set error flag is cleared and reported once, with the handle's message, as the code the kernel wrote.
+//   Every synchronous host entry point ends with it.
+// - destroy_handle(): the one way a handle ends, also on the failure paths of its create.
+struct Handle {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    DevArena arena;                 // staging of the host entry points
+    std::vector<void*> owned;       // dev_alloc
+    std::vector<void*> pinned;      // pinned_alloc
+    int64_t launches = 0;
+    int* errFlag = nullptr;         // device; CSLAM_E_* of the first overflow since the last sync(); nullptr: the handle has none
+    int* errHost = nullptr;         // pinned copy of *errFlag
+
+    Handle() = default;
+    Handle(const Handle&) = delete;
+    Handle& operator=(const Handle&) = delete;
+    ~Handle();   // frees owned, pinned, the arena's chunks and the stream: only through destroy_handle, which has waited for the stream
+    int open(int device, size_t arenaMinChunk, bool wantErrFlag);
+    int sync(const char* overflowMessage = nullptr);
+};
+
+// Waits for the handle's stream, then deletes it. The wait cannot live in ~Handle: a derived handle's members are destroyed before the
+// base destructor runs, and a derived destructor may free what the stream's work still uses.
+template <class H>
+static void destroy_handle(H* h) {
+    if (!h) return;
+    if (h->stream) {   // nothing is allocated before open() has created the stream
+        cudaSetDevice(h->device);
+        cudaStreamSynchronize(h->stream);
+    }
+    delete h;
+}
 
 // Optional per-kernel timing of a handle (cslam_*_set_timing / cslam_*_get_timing): record() puts an event on the stream before each
 // launch, and collect() adds the time from every event to the next one to the kind of the earlier event. A handle records END after its

@@ -1109,12 +1109,12 @@ using namespace cslam;
 enum { KIND_WARP = 0, KIND_PYRAMID, KIND_FAST, KIND_DISTRIBUTE, KIND_DESCRIBE, KIND_COUNT, KIND_END = KernelTimer::END };
 static const char* kKindNames[KIND_COUNT] = {"k_warp", "k_pyramid", "k_fast", "k_distribute", "k_describe"};
 
-struct cslam_frontend {
-    int device = 0;
+// error flag: set by k_fast, k_distribute and k_describe when a fixed-capacity buffer overflows. arena: device staging of the host entry
+// points (fisheye frames, key points, descriptors, counts).
+struct cslam_frontend : cslam::Handle {
     cslam_cam_params cam;
     cslam_orb_params orb;
     int W = 0, H = 0, CW = 0, CH = 0, maxBatch = 0, kpCap = 0, M = 0;   // M: quadtree node capacity = kept-list capacity per (frame, level)
-    cudaStream_t stream = nullptr;
     DevLevels L;                     // host copy of the device-pointer table (passed by value to kernels)
     std::vector<float> scale, invScale, sigma2, invSigma2; std::vector<int> perLevel; int umax[16];
     std::vector<float> map1, map2;   // host float maps (3H x 3W), kept for cslam_frontend_get_maps
@@ -1123,18 +1123,21 @@ struct cslam_frontend {
     uint8_t* d_mask = nullptr; int maskPitch = 0;
     uint32_t* d_candCount = nullptr; // maxBatch x nlevels
     uint32_t* d_kept = nullptr; uint32_t* d_keptCount = nullptr;
-    int* d_err = nullptr;
-    uint8_t* h_pin_in = nullptr; cslam_keypoint* h_pin_kps = nullptr; uint8_t* h_pin_desc = nullptr; int32_t* h_pin_n = nullptr; int* h_pin_err = nullptr;
-    std::vector<void*> owned;
-    DevArena arena;                  // device staging of the host entry points: fisheye frames, key points, descriptors, counts
+    uint8_t* h_pin_in = nullptr; cslam_keypoint* h_pin_kps = nullptr; uint8_t* h_pin_desc = nullptr; int32_t* h_pin_n = nullptr;
     static const int MAX_LANES = 4;
     cudaStream_t lane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evLane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evFork = nullptr;
     static constexpr int DEV_LANES = 2;     // lanes used by cslam_frontend_run_dev
     static constexpr int HOST_CHUNKS = 8;   // most chunks a host-buffer batch is cut into
-    int64_t launches = 0;
     KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     int pyrWin[MAX_LEVELS] = {};   // k_pyramid instantiation (PYR_WIN or PYR_WIN_MAX) of each level >= 1
+    ~cslam_frontend() {   // the lanes' work is joined into the handle's stream, which destroy_handle has waited for; the lanes are waited for too
+        for (int i = 0; i < MAX_LANES; i++) {
+            if (lane[i]) { cudaStreamSynchronize(lane[i]); cudaStreamDestroy(lane[i]); }
+            if (evLane[i]) cudaEventDestroy(evLane[i]);
+        }
+        if (evFork) cudaEventDestroy(evFork);
+    }
 };
 
 static inline void mark(cslam_frontend* fe, cudaStream_t st, int kind) {
@@ -1339,15 +1342,20 @@ static std::vector<FastCols> build_fast_cols(const LevelGeom& g) {
 extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const cslam_cam_params* cam, const cslam_orb_params* orb,
                                      const uint8_t* mask, int mask_pitch, int max_batch) {
     if (!out || !cam || !orb || !mask || max_batch <= 0) { set_error("cslam_frontend_create: null/invalid argument"); return CSLAM_E_BADARG; }
-    int rc = check_device(device);
-    if (rc) return rc;
     if (cam->face_w != cam->face_h || cam->face_w <= 0) { set_error("cube faces must be square (got %dx%d)", cam->face_w, cam->face_h); return CSLAM_E_BADARG; }
     if (3 * cam->face_w > 4095 || cam->Iw * 32 > 65535 || cam->Ih * 32 > 65535) { set_error("image too large for the packed coordinate formats"); return CSLAM_E_BADARG; }
     if (orb->nlevels < 1 || orb->nlevels > MAX_LEVELS || orb->nfeatures < 1 || orb->scale_factor <= 1.f || orb->scale_factor > 2.f) { set_error("bad ORB parameters (need 1 < scaleFactor <= 2)"); return CSLAM_E_BADARG; }
     cslam_frontend* fe = new cslam_frontend;
-    fe->device = device; fe->cam = *cam; fe->orb = *orb; fe->maxBatch = max_batch;
+    fe->cam = *cam; fe->orb = *orb; fe->maxBatch = max_batch;
     fe->W = cam->face_w; fe->H = cam->face_h; fe->CW = 3 * fe->W; fe->CH = 3 * fe->H;
     const int nl = orb->nlevels;
+    fe->kpCap = orb->nfeatures + 3 * nl;
+    auto fail = [&](int code) { destroy_handle(fe); return code; };
+    // the host entry points' device staging: the arena's first chunk holds a max_batch call
+    const size_t B = max_batch, fb = (size_t)cam->Iw * cam->Ih;
+    auto piece = [](size_t bytes) { return (bytes + 255) & ~(size_t)255; };   // DevArena::take's rounding
+    int rc = fe->open(device, piece(B * fb) + piece(B * fe->kpCap * sizeof(cslam_keypoint)) + piece(B * fe->kpCap * 32) + piece(B * sizeof(int32_t)), true);
+    if (rc) return fail(rc);
     // ---- ORBextractor::ORBextractor (src/ORBExtractor.cpp:381-442): scale tables, per-level quotas, umax
     fe->scale.resize(nl); fe->invScale.resize(nl); fe->sigma2.resize(nl); fe->invSigma2.resize(nl); fe->perLevel.resize(nl);
     fe->scale[0] = 1.f; fe->sigma2[0] = 1.f;
@@ -1364,8 +1372,6 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         for (v = 0; v <= vmax; ++v) fe->umax[v] = cv_round_d(std::sqrt(hp2 - v * v));
         for (v = HALF_PATCH, v0 = 0; v >= vmin; --v) { while (fe->umax[v0] == fe->umax[v0 + 1]) ++v0; fe->umax[v] = v0; ++v0; }
     }
-    auto fail = [&](int code) { cslam_frontend_destroy(fe); return code; };
-    if (cudaStreamCreateWithFlags(&fe->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("cudaStreamCreate failed"); return fail(CSLAM_E_CUDA); }
     for (int i = 0; i < cslam_frontend::MAX_LANES; i++)
         if (cudaStreamCreateWithFlags(&fe->lane[i], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&fe->evLane[i], cudaEventDisableTiming) != cudaSuccess) { set_error("lane stream creation failed"); return fail(CSLAM_E_CUDA); }
     if (cudaEventCreateWithFlags(&fe->evFork, cudaEventDisableTiming) != cudaSuccess) { set_error("event creation failed"); return fail(CSLAM_E_CUDA); }
@@ -1425,7 +1431,6 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         }
     }
     fe->M = round_up(std::max(maxQuota + 4, 16), 32);
-    fe->kpCap = orb->nfeatures + 3 * nl;
     const int distSmem = dist_smem(fe->M).total;
     if (distSmem > 200 * 1024) { set_error("nfeatures too large for the shared-memory quadtree (%d B)", distSmem); return fail(CSLAM_E_BADARG); }
     if (cudaFuncSetAttribute(k_distribute, cudaFuncAttributeMaxDynamicSharedMemorySize, distSmem) != cudaSuccess) { set_error("cudaFuncSetAttribute failed"); return fail(CSLAM_E_CUDA); }
@@ -1509,34 +1514,16 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
     fe->maskPitch = round_up(fe->CW, 128);
     if ((rc = dev_alloc(fe->owned, &fe->d_mask, (size_t)fe->maskPitch * fe->CH, true))) return fail(rc);
     if (cudaMemcpy2D(fe->d_mask, fe->maskPitch, mask, mask_pitch, fe->CW, fe->CH, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("mask upload failed"); return fail(CSLAM_E_CUDA); }
-    // ---- batch buffers. The host entry points' device staging comes from the arena; its first chunk holds a max_batch call.
-    const size_t B = max_batch, fb = (size_t)cam->Iw * cam->Ih;
+    // ---- batch buffers
     if ((rc = dev_alloc(fe->owned, &fe->d_candCount, B * nl, true)) || (rc = dev_alloc(fe->owned, &fe->d_kept, B * nl * fe->M, true)) ||
-        (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) || (rc = dev_alloc(fe->owned, &fe->d_err, 1, true))) return fail(rc);
-    auto piece = [](size_t bytes) { return (bytes + 255) & ~(size_t)255; };   // DevArena::take's rounding
-    fe->arena.bind(fe->stream, piece(B * fb) + piece(B * fe->kpCap * sizeof(cslam_keypoint)) + piece(B * fe->kpCap * 32) + piece(B * sizeof(int32_t)));
-    if (cudaMallocHost(&fe->h_pin_in, std::max<size_t>(B * fb, 1)) != cudaSuccess || cudaMallocHost(&fe->h_pin_kps, B * fe->kpCap * sizeof(cslam_keypoint)) != cudaSuccess ||
-        cudaMallocHost(&fe->h_pin_desc, B * fe->kpCap * 32) != cudaSuccess || cudaMallocHost(&fe->h_pin_n, B * sizeof(int32_t)) != cudaSuccess ||
-        cudaMallocHost(&fe->h_pin_err, sizeof(int)) != cudaSuccess) { set_error("pinned host allocation failed"); return fail(CSLAM_E_CUDA); }
+        (rc = dev_alloc(fe->owned, &fe->d_keptCount, B * nl, true)) || (rc = pinned_alloc(fe->pinned, &fe->h_pin_in, B * fb)) ||
+        (rc = pinned_alloc(fe->pinned, &fe->h_pin_kps, B * fe->kpCap)) || (rc = pinned_alloc(fe->pinned, &fe->h_pin_desc, B * fe->kpCap * 32)) ||
+        (rc = pinned_alloc(fe->pinned, &fe->h_pin_n, B))) return fail(rc);
     *out = fe;
     return CSLAM_OK;
 }
 
-extern "C" void cslam_frontend_destroy(cslam_frontend* fe) {
-    if (!fe) return;
-    cudaSetDevice(fe->device);
-    cudaDeviceSynchronize();
-    for (int i = 0; i < cslam_frontend::MAX_LANES; i++) { if (fe->lane[i]) cudaStreamDestroy(fe->lane[i]); if (fe->evLane[i]) cudaEventDestroy(fe->evLane[i]); }
-    if (fe->evFork) cudaEventDestroy(fe->evFork);
-    if (fe->stream) cudaStreamDestroy(fe->stream);
-    for (void* p : fe->owned) cudaFree(p);
-    if (fe->h_pin_in) cudaFreeHost(fe->h_pin_in);
-    if (fe->h_pin_kps) cudaFreeHost(fe->h_pin_kps);
-    if (fe->h_pin_desc) cudaFreeHost(fe->h_pin_desc);
-    if (fe->h_pin_n) cudaFreeHost(fe->h_pin_n);
-    if (fe->h_pin_err) cudaFreeHost(fe->h_pin_err);
-    delete fe;
-}
+extern "C" void cslam_frontend_destroy(cslam_frontend* fe) { destroy_handle(fe); }
 
 extern "C" int cslam_frontend_set_timing(cslam_frontend* fe, int enable) {
     if (!fe) return CSLAM_E_BADARG;
@@ -1552,17 +1539,9 @@ extern "C" int64_t cslam_frontend_launches(const cslam_frontend* fe) { return fe
 
 extern "C" int cslam_frontend_sync(cslam_frontend* fe) {
     if (!fe) return CSLAM_E_BADARG;
-    CSLAM_CUDA(cudaSetDevice(fe->device));
-    CSLAM_CUDA(cudaMemcpyAsync(fe->h_pin_err, fe->d_err, sizeof(int), cudaMemcpyDeviceToHost, fe->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(fe->stream));
+    const int rc = fe->sync("front end: a fixed-capacity buffer overflowed on the device (candidates / nodes / keypoints)");
     fe->timer.collect();
-    if (*fe->h_pin_err != 0) {
-        const int code = *fe->h_pin_err;
-        cudaMemsetAsync(fe->d_err, 0, sizeof(int), fe->stream);
-        set_error("front end: a fixed-capacity buffer overflowed on the device (candidates / nodes / keypoints)");
-        return code;
-    }
-    return CSLAM_OK;
+    return rc;
 }
 
 // Frame range [f0, f0+cnt) of the per-batch buffers, for one lane
@@ -1605,19 +1584,19 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         const LevelGeom& g = L.g[l];
         dim3 grid(cdiv(g.nColsEff, CG), cdiv(g.nRowsEff, FAST_R), cnt);
         mark(fe, st, KIND_FAST);
-        k_fast<<<grid, 256, fast_smem(g).total, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->d_err,
+        k_fast<<<grid, 256, fast_smem(g).total, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->errFlag,
                                      L.fcols[l], useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
     }
     CSLAM_CUDA(cudaGetLastError());
     DistributeArgs da;
     da.L = L; da.candCount = candCount; da.kept = fe->d_kept + (size_t)f0 * nl * fe->M; da.keptCount = fe->d_keptCount + (size_t)f0 * nl;
     da.mask = fe->d_mask; da.maskPitch = fe->maskPitch;
-    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.M = fe->M; da.errFlag = fe->d_err;
+    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.M = fe->M; da.errFlag = fe->errFlag;
     mark(fe, st, KIND_DISTRIBUTE);
     k_distribute<<<dim3(nl, cnt), DIST_THREADS, dist_smem(fe->M).total, st>>>(da);
     DescribeArgs ds;
     ds.L = L; ds.kept = da.kept; ds.keptCount = da.keptCount; ds.M = fe->M; ds.kps = d_kps; ds.desc = d_desc; ds.nOut = d_nout; ds.kpCap = fe->kpCap;
-    ds.errFlag = fe->d_err;
+    ds.errFlag = fe->errFlag;
     mark(fe, st, KIND_DESCRIBE);
     k_describe<<<dim3(cdiv(fe->kpCap, DESC_WARPS), cnt), DESC_WARPS * 32, 0, st>>>(ds);
     mark(fe, st, KIND_END);

@@ -256,35 +256,19 @@ __global__ void __launch_bounds__(TRI_THREADS) k_triangulation(TriArgs A) {
 
 using namespace cslam;
 
-struct cslam_mapper {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    cslam_tracker* trk = nullptr;   // for the frame index of the key frame (k_frame_index)
-    DevArena arena;                 // staging of the host entry points
-    int64_t launches = 0;
-};
+struct cslam_mapper : cslam::Handle {};
 
 extern "C" int cslam_mapper_create(cslam_mapper** out, int device) {
     if (!out) return CSLAM_E_BADARG;
-    int rc = check_device(device);
-    if (rc) return rc;
-    cslam_mapper* m = new cslam_mapper; m->device = device;
-    rc = cslam_tracker_create(&m->trk, device, 1, 4096);
-    if (rc) { delete m; return rc; }
-    m->stream = (cudaStream_t)cslam_tracker_stream(m->trk);   // one stream: the frame index and the searches are ordered
-    m->arena.bind(m->stream, (size_t)1 << 20);
+    cslam_mapper* m = new cslam_mapper;
+    int rc;
+    if ((rc = m->open(device, (size_t)1 << 20, false)) || (rc = prepare_frame_index())) { destroy_handle(m); return rc; }
     cudaFuncSetAttribute(k_triangulation, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 4);
     *out = m;
     return CSLAM_OK;
 }
-extern "C" void cslam_mapper_destroy(cslam_mapper* m) {
-    if (!m) return;
-    cudaSetDevice(m->device);
-    if (m->stream) cudaStreamSynchronize(m->stream);
-    cslam_tracker_destroy(m->trk);
-    delete m;
-}
-extern "C" int64_t cslam_mapper_launches(const cslam_mapper* m) { return m ? m->launches + cslam_tracker_launches(m->trk) : 0; }
+extern "C" void cslam_mapper_destroy(cslam_mapper* m) { destroy_handle(m); }
+extern "C" int64_t cslam_mapper_launches(const cslam_mapper* m) { return m ? m->launches : 0; }
 
 extern "C" int cslam_distinctive_descriptors(cslam_mapper* m, const uint8_t* desc, const int32_t* offset, int n_points, int32_t* best) {
     if (!m || !offset || !best || n_points < 0 || (n_points && offset[n_points] > 0 && !desc)) { set_error("cslam_distinctive_descriptors: bad argument"); return CSLAM_E_BADARG; }
@@ -299,8 +283,7 @@ extern "C" int cslam_distinctive_descriptors(cslam_mapper* m, const uint8_t* des
     k_distinctive<<<n_points, DD_THREADS, 0, m->stream>>>(dD, dO, dB); m->launches++;
     CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(best, dB, (size_t)n_points * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 extern "C" int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, const uint8_t* d_kf, int n_kf, const float* Tcw, int n_mp, const uint8_t* mp_valid, const float* mp_xw,
@@ -318,7 +301,7 @@ extern "C" int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, co
     if ((rc = a.upload(&dK, k_kf, n_kf)) || (rc = a.upload(&dD, d_kf, (size_t)n_kf * 32)) || (rc = a.upload(&dN, &n_kf, 1)) || (rc = a.take(&dCS, MAP_NCELLS + 1)) ||
         (rc = a.take(&dCI, cap)) || (rc = a.upload(&dV, mp_valid, n_mp)) || (rc = a.upload(&dX, mp_xw, (size_t)n_mp * 3)) || (rc = a.upload(&dL, mp_level, n_mp)) ||
         (rc = a.upload(&dM, mp_desc, (size_t)n_mp * 32)) || (rc = a.take(&dBI, n_mp)) || (rc = a.take(&dBD, n_mp)) ||
-        (rc = cslam_frame_index_dev(m->trk, dK, dN, 1, cap, face_w, face_h, nullptr, dCS, dCI))) return rc;
+        (rc = frame_index(m->stream, m->launches, dK, dN, 1, cap, face_w, face_h, nullptr, dCS, dCI))) return rc;
     FuseArgs A;
     A.kKF = dK; A.dKF = dD; A.cellStart = dCS; A.cellIdx = dCI; A.nKF = n_kf;
     for (int i = 0; i < 12; i++) A.Tcw[i] = Tcw[i];
@@ -329,8 +312,7 @@ extern "C" int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, co
     CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(best_idx, dBI, (size_t)n_mp * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(best_dist, dBD, (size_t)n_mp * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 extern "C" int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const cslam_keypoint* k1, const uint8_t* d1, const float* rays1, const uint8_t* has_mp1,
@@ -369,6 +351,5 @@ extern "C" int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const
     CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(match12, dOut, t1 * 4, cudaMemcpyDeviceToHost, st));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)npairs * 4, cudaMemcpyDeviceToHost, st));
-    CSLAM_CUDA(cudaStreamSynchronize(st));
-    return CSLAM_OK;
+    return m->sync();
 }

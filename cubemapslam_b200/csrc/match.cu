@@ -328,41 +328,27 @@ __global__ void k_hamming(const uint8_t* __restrict__ a, const uint8_t* __restri
 
 using namespace cslam;
 
-struct cslam_matcher {
-    int device = 0, maxPairs = 0, maxFeat = 0;
-    cudaStream_t stream = nullptr;
-    DevArena arena;   // staging of the host entry points, the row-split histogram and the micro-benchmarks' output sink
-    int64_t launches = 0;
+// arena: staging of the host entry points, the row-split histogram and the micro-benchmarks' output sink
+struct cslam_matcher : cslam::Handle {
+    int maxPairs = 0, maxFeat = 0;
 };
 
 extern "C" int cslam_matcher_create(cslam_matcher** out, int device, int max_pairs, int max_features) {
     if (!out || max_pairs <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_matcher_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
-    const int rc = check_device(device);
-    if (rc) return rc;
     cslam_matcher* m = new cslam_matcher;
-    m->device = device; m->maxPairs = max_pairs; m->maxFeat = max_features;
-    if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); cslam_matcher_destroy(m); return CSLAM_E_CUDA; }
+    m->maxPairs = max_pairs; m->maxFeat = max_features;
     // chunks: room for both descriptor sets, a flag and seven 4-byte arrays per feature at the handle's limits, at most 64 MB
-    m->arena.bind(m->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_pairs * max_features * (2 * 32 + 1 + 7 * 4) + (size_t)max_pairs * 4));
+    const int rc = m->open(device, std::min<size_t>((size_t)64 << 20, (size_t)max_pairs * max_features * (2 * 32 + 1 + 7 * 4) + (size_t)max_pairs * 4), false);
+    if (rc) { destroy_handle(m); return rc; }
     cudaFuncSetAttribute(k_search_by_bow, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
     *out = m;
     return CSLAM_OK;
 }
 
-extern "C" void cslam_matcher_destroy(cslam_matcher* m) {
-    if (!m) return;
-    cudaSetDevice(m->device);
-    if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-    delete m;
-}
+extern "C" void cslam_matcher_destroy(cslam_matcher* m) { destroy_handle(m); }
 extern "C" void* cslam_matcher_stream(const cslam_matcher* m) { return m ? (void*)m->stream : nullptr; }
 extern "C" int64_t cslam_matcher_launches(const cslam_matcher* m) { return m ? m->launches : 0; }
-extern "C" int cslam_matcher_sync(cslam_matcher* m) {
-    if (!m) return CSLAM_E_BADARG;
-    CSLAM_CUDA(cudaSetDevice(m->device));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
-}
+extern "C" int cslam_matcher_sync(cslam_matcher* m) { return m ? m->sync() : CSLAM_E_BADARG; }
 
 // The brute-force launch of every entry point: one CTA per BF_ROWS rows of the largest A a pair can have (L.strideA); with more than one, the
 // per-pair rotation histogram is a zeroed arena piece.
@@ -421,8 +407,7 @@ extern "C" int cslam_match_bruteforce(cslam_matcher* m, const uint8_t* descA, co
         if (second12) CSLAM_CUDA(cudaMemcpyAsync(second12, dSecond, na * 4, cudaMemcpyDeviceToHost, m->stream));
     }
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 // All-pairs matcher between consecutive frames of a front-end batch, straight from cslam_frontend_run_dev's output layout: frame f (rows
@@ -450,8 +435,7 @@ extern "C" int cslam_match_frames(cslam_matcher* m, const cslam_keypoint* kps, c
         (rc = m->arena.take(&dNm, nframes - 1)) || (rc = frames_launch(m, dK, dD, dN, kp_stride, nframes, nnratio, th_low, check_ori, dMatch, dNm))) return rc;
     CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, nm * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)(nframes - 1) * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 // Harness of the register-only issue-rate micro-benchmarks below: 8 CTAs per SM, a warm-up launch of 100 iterations, then the timed
@@ -617,8 +601,7 @@ extern "C" int cslam_search_by_bow(cslam_matcher* m, const uint8_t* descKF, cons
         (rc = cslam_search_by_bow_dev(m, dK, aK, dValid, nodeK, nKF, dF, aF, nodeF, nF, npairs, nnratio, check_ori, dMatch, dN))) return rc;
     if (nf) CSLAM_CUDA(cudaMemcpyAsync(match_f, dMatch, nf * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 extern "C" int cslam_hamming(cslam_matcher* m, const uint8_t* a, const uint8_t* b, int n, int32_t* dist) {
@@ -631,8 +614,7 @@ extern "C" int cslam_hamming(cslam_matcher* m, const uint8_t* a, const uint8_t* 
     k_hamming<<<cdiv(n, 256), 256, 0, m->stream>>>(dA, dB, n, dDist);
     m->launches++;
     CSLAM_CUDA(cudaMemcpyAsync(dist, dDist, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }
 
 // ORBMatcher::SearchByBoW(KeyFrame*, KeyFrame*, vector<MapPoint*>&)  (reference src/ORBMatcher.cpp:541-674), host buffers.
@@ -654,6 +636,5 @@ extern "C" int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, co
         (rc = bow_launch(m, dD1, dA1, dV1, dN1, n1, dD2, dA2, dN2, n2, dV2, npairs, nnratio, check_ori, dMatch, dNm))) return rc;
     CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, k1 * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(m->stream));
-    return CSLAM_OK;
+    return m->sync();
 }

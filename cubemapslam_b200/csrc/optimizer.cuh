@@ -8,12 +8,8 @@
 
 typedef void* nccl_comm_t;
 
-struct cslam_optimizer {
-    int device = 0;
-    cudaStream_t stream = nullptr;
+struct cslam_optimizer : cslam::Handle {
     nccl_comm_t comm = nullptr; int rank = 0, nranks = 1;
-    int64_t launches = 0;
-    cslam::DevArena arena;      // 64 MB chunks
     double* h_scal = nullptr;   // pinned, 16 doubles
     // host scratch of cslam_local_ba, kept across calls (fresh multi-megabyte vectors cost page faults on every call)
     struct HostScratch { std::vector<int> lmStart, perm, eMP, eKF, fill, peStart, peList, kfOfQ; std::vector<double> X; } hs;
@@ -21,6 +17,7 @@ struct cslam_optimizer {
     // one-shot NVLink all-reduce of the reduced camera system (multi-GPU LocalBA): peer views of every rank's exchange buffer
     struct Peer { void* base = nullptr; bool mine = false; };
     std::vector<Peer> peers; size_t xchgBytes = 0; uint32_t epoch = 0, epoch2 = 0; bool oneShot = false;
+    ~cslam_optimizer();   // ba.cu: the peers' exchange buffers and the NCCL communicator
 };
 
 namespace cslam {

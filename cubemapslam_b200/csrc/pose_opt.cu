@@ -243,7 +243,7 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
     if (n && outlier) CSLAM_CUDA(cudaMemcpyAsync(outlier, d_out, n, cudaMemcpyDeviceToHost, o->stream));
     CSLAM_CUDA(cudaMemcpyAsync(inliers, d_inl, nframes * 4, cudaMemcpyDeviceToHost, o->stream));
     if (pose_fp64) CSLAM_CUDA(cudaMemcpyAsync(pose_fp64, d_p64, (size_t)nframes * 56, cudaMemcpyDeviceToHost, o->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(o->stream));
+    if ((rc = o->sync())) return rc;
     for (int f = 0; f < nframes; f++) if (offset[f + 1] - offset[f] >= 3) std::memcpy(Tcw + 16 * f, Tout.data() + 16 * f, 64);
     return CSLAM_OK;
 }
@@ -261,9 +261,4 @@ extern "C" int cslam_pose_optimization_dev(cslam_optimizer* o, int nframes, int 
     return launch_pose_opt(o, nframes, (size_t)nframes * stride, A);
 }
 extern "C" void* cslam_optimizer_stream(const cslam_optimizer* o) { return o ? (void*)o->stream : nullptr; }
-extern "C" int cslam_optimizer_sync(cslam_optimizer* o) {
-    if (!o) return CSLAM_E_BADARG;
-    CSLAM_CUDA(cudaSetDevice(o->device));
-    CSLAM_CUDA(cudaStreamSynchronize(o->stream));
-    return CSLAM_OK;
-}
+extern "C" int cslam_optimizer_sync(cslam_optimizer* o) { return o ? o->sync() : CSLAM_E_BADARG; }

@@ -305,47 +305,26 @@ extern "C" int cslam_area_rects(float x, float y, float r, int face_w, int face_
     return n;
 }
 
-struct cslam_tracker {
-    int device = 0, maxFrames = 0, maxFeat = 0;
-    cudaStream_t stream = nullptr;
-    int* err = nullptr;   // CSLAM_E_CAPACITY once a search window overflowed; read and cleared by cslam_tracker_sync
-    std::vector<void*> owned;
-    DevArena arena;       // staging of the host entry points
-    int64_t launches = 0;
+// error flag: CSLAM_E_CAPACITY once a search window overflowed
+struct cslam_tracker : cslam::Handle {
+    int maxFrames = 0, maxFeat = 0;
 };
 
 extern "C" int cslam_tracker_create(cslam_tracker** out, int device, int max_frames, int max_features) {
     if (!out || max_frames <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_tracker_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
-    int rc = check_device(device);
-    if (rc) return rc;
-    cslam_tracker* t = new cslam_tracker; t->device = device; t->maxFrames = max_frames; t->maxFeat = max_features;
-    if (cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("stream creation failed"); delete t; return CSLAM_E_CUDA; }
-    if ((rc = dev_alloc(t->owned, &t->err, 1, true))) { cslam_tracker_destroy(t); return rc; }
+    cslam_tracker* t = new cslam_tracker; t->maxFrames = max_frames; t->maxFeat = max_features;
     // chunks: room for every array the host calls stage at the handle's limits, at most 64 MB
     const size_t perFeature = 2 * sizeof(cslam_keypoint) + 2 * 32 + 3 + 2 * 4 + 3 * 4 + 2 * 4 + 4 + 3 * 4 + 2, perFrame = 3 * 4 + 16 * 4 + (NCELLS + 1) * 2;
-    t->arena.bind(t->stream, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * perFeature + (size_t)max_frames * perFrame));
-    cudaFuncSetAttribute(k_frame_index, cudaFuncAttributeMaxDynamicSharedMemorySize, NCELLS * 4);
+    int rc;
+    if ((rc = t->open(device, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * perFeature + (size_t)max_frames * perFrame), true)) ||
+        (rc = prepare_frame_index())) { destroy_handle(t); return rc; }
     *out = t;
     return CSLAM_OK;
 }
-extern "C" void cslam_tracker_destroy(cslam_tracker* t) {
-    if (!t) return;
-    cudaSetDevice(t->device);
-    if (t->stream) { cudaStreamSynchronize(t->stream); cudaStreamDestroy(t->stream); }
-    for (void* p : t->owned) cudaFree(p);
-    delete t;
-}
+extern "C" void cslam_tracker_destroy(cslam_tracker* t) { destroy_handle(t); }
 extern "C" void* cslam_tracker_stream(const cslam_tracker* t) { return t ? (void*)t->stream : nullptr; }
 extern "C" int64_t cslam_tracker_launches(const cslam_tracker* t) { return t ? t->launches : 0; }
-extern "C" int cslam_tracker_sync(cslam_tracker* t) {
-    if (!t) return CSLAM_E_BADARG;
-    CSLAM_CUDA(cudaSetDevice(t->device));
-    int e = 0;
-    CSLAM_CUDA(cudaMemcpyAsync(&e, t->err, sizeof(int), cudaMemcpyDeviceToHost, t->stream));
-    CSLAM_CUDA(cudaStreamSynchronize(t->stream));
-    if (e) { cudaMemsetAsync(t->err, 0, sizeof(int), t->stream); set_error("tracker: a search window held more candidates than the fixed capacity"); return e; }
-    return CSLAM_OK;
-}
+extern "C" int cslam_tracker_sync(cslam_tracker* t) { return t ? t->sync("tracker: a search window held more candidates than the fixed capacity") : CSLAM_E_BADARG; }
 
 extern "C" int cslam_tracker_gather_pose_inputs_dev(cslam_tracker* t, int npairs, const int32_t* match_cur, const cslam_keypoint* k_cur, const int32_t* n_cur, int cur_stride,
                                                     const float* rays_cur, float cos_fov_th, const float* Xw_last, int last_stride, const float* inv_sigma2_levels_dev,
@@ -359,13 +338,23 @@ extern "C" int cslam_tracker_gather_pose_inputs_dev(cslam_tracker* t, int npairs
     return CSLAM_OK;
 }
 
-extern "C" int cslam_frame_index_dev(cslam_tracker* t, const cslam_keypoint* kps, const int32_t* n, int nframes, int kp_stride, int face_w, int face_h, float* rays,
-                                     uint16_t* cell_start, uint16_t* cell_idx) {
-    if (!t || !kps || !n || !cell_start || !cell_idx || nframes <= 0 || kp_stride <= 0 || kp_stride > 4096 || face_w <= 0 || face_w != face_h) { set_error("cslam_frame_index: bad argument"); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(t->device));
-    k_frame_index<<<nframes, 256, NCELLS * 4, t->stream>>>(kps, n, kp_stride, face_w, face_h, rays, cell_start, cell_idx); t->launches++;
+int cslam::prepare_frame_index() {
+    CSLAM_CUDA(cudaFuncSetAttribute(k_frame_index, cudaFuncAttributeMaxDynamicSharedMemorySize, NCELLS * 4));
+    return CSLAM_OK;
+}
+int cslam::frame_index(cudaStream_t stream, int64_t& launches, const cslam_keypoint* kps, const int32_t* n, int nframes, int kpStride, int faceW, int faceH, float* rays,
+                       uint16_t* cellStart, uint16_t* cellIdx) {
+    if (!kps || !n || !cellStart || !cellIdx || nframes <= 0 || kpStride <= 0 || kpStride > 4096 || faceW <= 0 || faceW != faceH) { set_error("cslam_frame_index: bad argument"); return CSLAM_E_BADARG; }
+    k_frame_index<<<nframes, 256, NCELLS * 4, stream>>>(kps, n, kpStride, faceW, faceH, rays, cellStart, cellIdx); launches++;
     CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;
+}
+
+extern "C" int cslam_frame_index_dev(cslam_tracker* t, const cslam_keypoint* kps, const int32_t* n, int nframes, int kp_stride, int face_w, int face_h, float* rays,
+                                     uint16_t* cell_start, uint16_t* cell_idx) {
+    if (!t) { set_error("cslam_frame_index: bad argument"); return CSLAM_E_BADARG; }
+    CSLAM_CUDA(cudaSetDevice(t->device));
+    return frame_index(t->stream, t->launches, kps, n, nframes, kp_stride, face_w, face_h, rays, cell_start, cell_idx);
 }
 extern "C" int cslam_frame_index(cslam_tracker* t, const cslam_keypoint* kps, const int32_t* n, int nframes, int kp_stride, int face_w, int face_h, float* rays, uint16_t* cell_start,
                                  uint16_t* cell_idx) {
@@ -399,7 +388,7 @@ extern "C" int cslam_search_by_projection_last_dev(cslam_tracker* t, int npairs,
     A.kCur = k_cur; A.dCur = d_cur; A.nCur = n_cur; A.cellStart = cell_start; A.cellIdx = cell_idx; A.curTaken = cur_taken; A.curStride = cur_stride;
     A.nQ = n_last; A.qStride = last_stride; A.qValid = has_mp; A.qDesc = d_mp; A.qObs = mp_obs; A.qXw = Xw; A.kLast = k_last; A.TcwCur = Tcw_cur;
     A.mode = 0; A.W = face_w; A.H = face_h; A.checkOri = check_ori; A.th = th; A.nnratio = 0; A.cosFovTh = cos_fov_th; fill_scales(A, scale_factor, nlevels);
-    A.match = match_cur; A.nmatches = nmatches; A.errFlag = t->err;
+    A.match = match_cur; A.nmatches = nmatches; A.errFlag = t->errFlag;
     k_search_by_projection<<<npairs, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
     CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;
@@ -416,7 +405,7 @@ extern "C" int cslam_search_by_projection_local_dev(cslam_tracker* t, int nframe
     A.kCur = k_f; A.dCur = d_f; A.nCur = n_f; A.cellStart = cell_start; A.cellIdx = cell_idx; A.curTaken = f_taken; A.curStride = f_stride;
     A.nQ = n_mp; A.qStride = mp_stride; A.qValid = in_view; A.qDesc = d_mp; A.qObs = mp_obs; A.qProj = proj_xy; A.qLevel = level; A.qViewCos = view_cos;
     A.mode = 1; A.W = face_w; A.H = face_h; A.checkOri = 0; A.th = th; A.nnratio = nnratio; fill_scales(A, scale_factor, nlevels);
-    A.match = match_f; A.nmatches = nmatches; A.errFlag = t->err;
+    A.match = match_f; A.nmatches = nmatches; A.errFlag = t->errFlag;
     k_search_by_projection<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
     CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;

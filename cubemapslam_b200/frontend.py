@@ -11,7 +11,9 @@ from . import _capi
 from ._capi import KP_DTYPE, check, lib, ptr
 
 
-class FrontEnd:
+class FrontEnd(_capi.Handle):
+    KIND = "frontend"
+
     def __init__(self, cfg, mask, max_batch=8, device=0, orb=None):
         self.cfg = cfg
         self.cam = _capi.cam_params(cfg)
@@ -20,22 +22,10 @@ class FrontEnd:
         self.CW, self.CH = 3 * self.cam.face_w, 3 * self.cam.face_h
         if mask.shape != (self.CH, self.CW):
             raise ValueError("mask must be %dx%d (same size as the cubemap canvas, reference src/ORBExtractor.cpp:848)" % (self.CH, self.CW))
-        self._h = C.c_void_p()
-        check(lib().cslam_frontend_create(C.byref(self._h), int(device), C.byref(self.cam), C.byref(self.orb), ptr(mask), mask.shape[1], int(max_batch)))
+        super().__init__(int(device), C.byref(self.cam), C.byref(self.orb), ptr(mask), mask.shape[1], int(max_batch))
         self.max_batch = max_batch
         self.kp_cap = lib().cslam_frontend_kp_capacity(self._h)
         self.nlevels = self.orb.nlevels
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_frontend_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- reference-facing calls (host buffers)
     def warp(self, fisheye, canvas=None):
@@ -79,17 +69,6 @@ class FrontEnd:
     # ---- device-resident path (addresses as ints, e.g. torch.Tensor.data_ptr())
     def run_dev(self, fisheye_dev, batch, kps_dev, desc_dev, n_dev):
         check(lib().cslam_frontend_run_dev(self._h, ptr(fisheye_dev), int(batch), ptr(kps_dev), ptr(desc_dev), ptr(n_dev)))
-
-    def sync(self):
-        check(lib().cslam_frontend_sync(self._h))
-
-    @property
-    def stream(self):
-        return lib().cslam_frontend_stream(self._h)
-
-    @property
-    def launches(self):
-        return lib().cslam_frontend_launches(self._h)
 
     def set_timing(self, enable):
         check(lib().cslam_frontend_set_timing(self._h, int(enable)))

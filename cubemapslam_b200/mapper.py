@@ -7,29 +7,14 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import KP_DTYPE, check, lib, ptr
+from ._capi import KP_DTYPE, Handle, check, lib, ptr
 
 
-class Mapper:
+class Mapper(Handle):
+    KIND = "mapper"
+
     def __init__(self, device=0):
-        self._h = C.c_void_p()
-        lib().cslam_mapper_launches.restype = C.c_int64
-        check(lib().cslam_mapper_create(C.byref(self._h), int(device)))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_mapper_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def launches(self):
-        return int(lib().cslam_mapper_launches(self._h))
+        super().__init__(int(device))
 
     def ComputeDistinctiveDescriptors(self, desc, offset):
         desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32); offset = np.ascontiguousarray(offset, np.int32)

@@ -9,41 +9,20 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import check, lib, ptr
+from ._capi import Handle, check, lib, ptr
 
 TH_HIGH = 100
 TH_LOW = 50
 HISTO_LENGTH = 12
 
 
-class ORBMatcher:
+class ORBMatcher(Handle):
+    KIND = "matcher"
+
     def __init__(self, nnratio=0.6, checkOri=True, max_pairs=64, max_features=2048, device=0):
         self.nnratio = float(nnratio); self.check_ori = bool(checkOri)
-        self._h = C.c_void_p()
-        check(lib().cslam_matcher_create(C.byref(self._h), int(device), int(max_pairs), int(max_features)))
+        super().__init__(int(device), int(max_pairs), int(max_features))
         self.max_pairs, self.max_features = max_pairs, max_features
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_matcher_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def stream(self):
-        return lib().cslam_matcher_stream(self._h)
-
-    @property
-    def launches(self):
-        return lib().cslam_matcher_launches(self._h)
-
-    def sync(self):
-        check(lib().cslam_matcher_sync(self._h))
 
     def DescriptorDistance(self, a, b):
         a = np.ascontiguousarray(a, np.uint8).reshape(-1, 32); b = np.ascontiguousarray(b, np.uint8).reshape(-1, 32)

@@ -7,28 +7,14 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import BAProblem, BAResult, check, lib, ptr
+from ._capi import BAProblem, BAResult, Handle, check, lib, ptr
 
 
-class Optimizer:
+class Optimizer(Handle):
+    KIND = "optimizer"
+
     def __init__(self, device=0):
-        self._h = C.c_void_p()
-        check(lib().cslam_optimizer_create(C.byref(self._h), int(device)))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_optimizer_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def launches(self):
-        return lib().cslam_optimizer_launches(self._h)
+        super().__init__(int(device))
 
     def set_timing(self, on):
         check(lib().cslam_optimizer_set_timing(self._h, int(bool(on))))
@@ -65,14 +51,6 @@ class Optimizer:
         check(lib().cslam_local_ba(self._h, C.byref(p), sf, int(its1), int(its2), C.byref(r)))
         return dict(Tcw=Tcw.reshape(nKF, 4, 4), pts=pts, outlier=outlier[:nE], pose64=pose64, pts64=pts64[:nMP], log=log[:r.iterations], iters=r.iterations,
                     trials=r.trials)
-
-    @property
-    def stream(self):
-        lib().cslam_optimizer_stream.restype = C.c_void_p
-        return lib().cslam_optimizer_stream(self._h)
-
-    def sync(self):
-        check(lib().cslam_optimizer_sync(self._h))
 
     def pose_optimization_dev(self, nframes, stride, count, Tcw, Xw, kpxy, inv_sigma2, faceW, faceH, outlier, inliers):
         check(lib().cslam_pose_optimization_dev(self._h, int(nframes), int(stride), ptr(count), ptr(Tcw), ptr(Xw), ptr(kpxy), ptr(inv_sigma2), int(faceW), int(faceH), ptr(outlier),

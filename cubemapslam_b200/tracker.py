@@ -9,7 +9,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import KP_DTYPE, check, lib, ptr
+from ._capi import KP_DTYPE, Handle, check, lib, ptr
 
 NCELLS = 5 * 50 * 50
 
@@ -25,35 +25,12 @@ def _b(a, dtype, single):
     return a[None] if single else a
 
 
-class Tracker:
+class Tracker(Handle):
+    KIND = "tracker"
+
     def __init__(self, max_frames=8, max_features=4096, device=0):
-        self._h = C.c_void_p()
-        lib().cslam_tracker_stream.restype = C.c_void_p
-        lib().cslam_tracker_launches.restype = C.c_int64
-        check(lib().cslam_tracker_create(C.byref(self._h), int(device), int(max_frames), int(max_features)))
+        super().__init__(int(device), int(max_frames), int(max_features))
         self.max_frames, self.max_features = max_frames, max_features
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_tracker_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def stream(self):
-        return lib().cslam_tracker_stream(self._h)
-
-    @property
-    def launches(self):
-        return lib().cslam_tracker_launches(self._h)
-
-    def sync(self):
-        check(lib().cslam_tracker_sync(self._h))
 
     def frame_index(self, kps, face_w, face_h, n=None):
         """kps: (stride,) or (F, stride) cv::KeyPoint records. Returns rays (F, stride, 3), cell_start (F, 12501) u16, cell_idx (F, stride) u16."""

@@ -1,28 +1,17 @@
 """Host-side mirror of ORBVocabulary::transform (reference include/ORBVocabulary.h:35-36, ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1262) on the C ABI."""
-import ctypes as C
 
 import numpy as np
 
-from ._capi import check, lib, ptr
+from ._capi import Handle, check, lib, ptr
 
 
-class Vocabulary:
+class Vocabulary(Handle):
+    KIND = "vocabulary"
+
     def __init__(self, k, L, parent, is_leaf, desc, weight, max_frames=8, max_features=4096, device=0):
         parent = np.ascontiguousarray(parent, np.int32); is_leaf = np.ascontiguousarray(is_leaf, np.uint8); desc = np.ascontiguousarray(desc, np.uint8)
         weight = np.ascontiguousarray(weight, np.float64)
-        self._h = C.c_void_p()
-        check(lib().cslam_vocabulary_create(C.byref(self._h), int(device), int(k), int(L), len(parent), ptr(parent), ptr(is_leaf), ptr(desc), ptr(weight), int(max_frames), int(max_features)))
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib().cslam_vocabulary_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(int(device), int(k), int(L), len(parent), ptr(parent), ptr(is_leaf), ptr(desc), ptr(weight), int(max_frames), int(max_features))
 
     def transform(self, desc, n=None, levelsup=4):
         """desc: (stride, 32) or (F, stride, 32). Returns per frame: word (stride,), node (stride,), bow_word (m,), bow_val (m,)."""
