@@ -6,12 +6,12 @@
 //     ComputePyramid :928-953, ComputeKeyPointsOctTree :739-827 (cv::FAST per 30-px cell, DistributeOctTree
 //     :511-737, IC_Angle :48-75), cull :883-904, GaussianBlur :907-908, computeOrbDescriptor :79-118
 //
-// Kernels (all HBM/L2-bound byte work; no tensor cores on this path):
+// Kernels (byte work; k_describe's blur runs on the integer tensor cores):
 //   k_warp        canvas face tiles <- bilinear gather of the fisheye frame through a pre-quantised map
 //   k_pyramid     level l <- cv::resize(INTER_LINEAR) fixed-point model of level l-1
 //   k_fast        per 30-px cell FAST-9/16 arc score, in-cell NMS, 20->7 threshold fallback, candidate append
 //   k_distribute  the reference's quadtree, restated as data-parallel rounds over nodes (see DESIGN.md)
-//   k_describe    IC angle + 7x7 Gaussian of the 43x43 neighbourhood + steered BRIEF, one warp per keypoint
+//   k_describe    IC angle + 7x7 Gaussian of the 43x43 neighbourhood (IMMA) + steered BRIEF, one warp per keypoint
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -31,9 +31,9 @@ static const int DESC_WARPS = 4;
 
 // IC_Angle's disc by column: bit v of word 15 + u is set iff |u| <= umax[v] (ORBextractor's umax), built by cslam_frontend_create
 __device__ uint32_t g_icRows[32];
-// the BRIEF pattern as k_describe reads it: word k of lane (= output byte) `lane` at [k * 32 + lane] (coalesced; the byte-per-test table above
-// read per lane was an 8-way shared-memory bank conflict). Filled by cslam_frontend_create from the same table.
-__device__ uint32_t g_patT[8 * 32];
+// the BRIEF pattern as k_describe reads it: test k of lane (= output byte) `lane` as floats (x0, y0, x1, y1) at [k * 32 + lane] (coalesced;
+// a byte-per-test table read per lane was an 8-way shared-memory bank conflict). Filled by cslam_frontend_create from the same table.
+__device__ float4 g_pat[8 * 32];
 
 struct LevelGeom {
     int w, h, pitch;          // image size, row pitch in bytes
@@ -966,12 +966,55 @@ struct DescribeArgs {
     int* errFlag;
 };
 
-static const int DP_STRIDE = 52;                 // patch row stride (bytes): 43 px + up to 3 bytes of word misalignment; 13 words: consecutive rows fall in distinct banks
-static const int DH_STRIDE = 46;                 // transposed H: u16 per row index, per column (23 words: the 4-column stride of the transposed stores, 92 words, spreads over 8 banks)
-static const int BL_STRIDE = 44;                 // blurred patch row stride in bytes (11 words: 4-row stride 44 words -> 8 banks; 40 gave 4)
+// The 7x7 blur runs on the integer tensor cores: OpenCV's 8U fixed point is exact in integers (H = sum g P <= 65280, dst = (sum g H + 32768)
+// >> 16 with g = [18,34,48,56,48,34,18]), and mma.sync m16n8k32 u8 x u8 -> s32 gives the same bits.
+//   pass 1  Ht[c][n] = sum_j G[c][j] P[pi(n)][j]: A = band G[c][j] = g[j - po - c] (M = output column c, 37 -> 48; K = patch column j, 64),
+//           B = the row-major patch, loaded as-is with ldmatrix, its rows permuted by pi so that the accumulators come out as pass 2's operands;
+//   pass 2  V[r][c] = sum_k Gv[r][k] H[k][c] on the two byte planes of H: A = band Gv[r][k] = g[k - r] (M = output row, 37 -> 48; K = H row),
+//           B = Hh, then Hl accumulated onto 256 Vh + 32768, so dst is byte 2 of the sum.
+// pi: in the n-tile pair (2p, 2p+1), column 2t + e holds patch row 16p + 4t + e of tile 2p and 16p + 4t + 2 + e of tile 2p+1. Lane (g, t)'s
+// accumulators then hold H rows 16p + 4t .. 16p + 4t + 3 of Ht row c = 16mt + g (+8), which is exactly its pass-2 B fragment (K rows 4t..4t+3
+// of column g): four byte permutes per fragment and plane, no shared-memory round trip.
+// Band-limited tiles are skipped: pass 1 runs (mt, kt) = (0,0) (0,1) (1,0) (1,1) (2,1), pass 2 runs (mt, kt) = (0,0) (1,0) (1,1) (2,1) and no
+// n-tile 5 (columns 40..47): 30 + 40 IMMA per key point.
+static const int DP_STRIDE = 64;    // patch row stride: four 16-byte chunks; chunk q of row r is stored at chunk q ^ ((r >> 2) & 3) (dp_at)
+static const int DP_ROWS = 48;      // rows the pass-1 n-tiles read; rows 43..47 (never written) only reach blurred rows 37..47, which are discarded
+static const int BL_STRIDE = 48;    // blurred patch row stride (12 words: the 8 rows of a fragment's u16 stores fall in distinct banks)
+static const int BL_ROWS = 40;      // blurred rows stored: 0..36 are read, 37..39 are the m-tile's padding
+// Band operands: the A register of lane (g, t) for tile (mt, kt), half h of K and rows +8v is bytes g[d .. d+3] with d = 4t - g - po + 8s,
+// s = 4kt + 2h - 2mt - v (po = 0 in pass 2). A word table indexed by d gives each of them as one shared load at a constant offset from a
+// per-lane base, so the per-key-point band for any po costs 10 loads (pass 2: 8) and no byte shuffling.
+static const int BAND_LO = -46, BAND_N = 107;   // band word table: bytes g[d .. d+3] for d in [-46, 60]
+// A lane's ldmatrix rows of one 8x16-byte matrix are 16p + {0,1,4,5,8,9,12,13} (+2): with a 64-byte stride even and odd rows fall in
+// different halves of the 128 bytes, and the swizzle spreads rows 4 apart over the four chunks of a half, so no two rows share banks.
+__device__ __forceinline__ int dp_at(int r, int x) { return r * DP_STRIDE + (x ^ (((r >> 2) & 3) << 4)); }
+
+__device__ __forceinline__ void ldsm_x4(uint32_t (&b)[4], uint32_t addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void ldsm_x2(uint32_t (&b)[2], uint32_t addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];\n" : "=r"(b[0]), "=r"(b[1]) : "r"(addr) : "memory");
+}
+// d = A (16x32 u8, row) * B (32x8 u8, col) + c
+__device__ __forceinline__ void mma_u8(uint32_t (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1, const uint32_t (&c)[4]) {
+    asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%11,%12,%13};\n"
+        : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "r"(c[0]), "r"(c[1]), "r"(c[2]), "r"(c[3]));
+}
+
 __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
-    __shared__ __align__(16) uint8_t s_patch[DESC_WARPS][43 * DP_STRIDE + 16];
-    __shared__ __align__(16) uint16_t s_ht[DESC_WARPS][37 * DH_STRIDE + 8];
+    __shared__ __align__(16) uint8_t s_patch[DESC_WARPS][DP_ROWS * DP_STRIDE];
+    __shared__ __align__(16) uint8_t s_bl[DESC_WARPS][BL_ROWS * BL_STRIDE];
+    __shared__ uint32_t s_band[BAND_N];
+    if (threadIdx.x < BAND_N) {   // word d - BAND_LO: bytes g[d], g[d+1], g[d+2], g[d+3] (0 outside the kernel's 7 taps)
+        const unsigned long long G = 0x12ull | 0x22ull << 8 | 0x30ull << 16 | 0x38ull << 24 | 0x30ull << 32 | 0x22ull << 40 | 0x12ull << 48;
+        const int d = (int)threadIdx.x + BAND_LO;
+        uint32_t w = 0;
+        for (int i = 0; i < 4; i++)
+            if (d + i >= 0 && d + i < 7) w |= (uint32_t)((G >> (8 * (d + i))) & 0xff) << (8 * i);
+        s_band[threadIdx.x] = w;
+    }
+    __syncthreads();
     const int frame = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // output slot -> (level, slot in the level's kept list): lane l < MAX_LEVELS holds the inclusive prefix sum of the kept counts up to
@@ -993,23 +1036,40 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
     const uint8_t* I = A.L.img[level] + (size_t)frame * g.pitch * g.h;
     const uint32_t v = A.kept[((size_t)frame * A.L.nlevels + level) * A.M + slot];
     const int kx = v & 0xfff, ky = (v >> 12) & 0xfff, resp = v >> 24;
+    // the key-point record, written before the blur so that none of its fields stays live across it; the angle follows at the end
+    cslam_keypoint* kpo = A.kps + (size_t)frame * A.kpCap + outIdx;
+    if (lane == 0) {
+        kpo->x = __fmul_rn((float)kx, g.scale); kpo->y = __fmul_rn((float)ky, g.scale);
+        kpo->size = g.sizeF; kpo->response = (float)resp; kpo->octave = level; kpo->class_id = -1;
+    }
 
-    // ---- 43x43 neighbourhood -> P[r][po + c] (REFLECT_101 at the level edges, like the blur of the apron-less clone)
+    // ---- 43x43 neighbourhood -> patch row r, byte po + c (REFLECT_101 at the level edges, like the blur of the apron-less clone)
     uint8_t* P = s_patch[warp];
     int po;
     if (kx >= 21 && ky >= 21 && kx + 21 < g.w && ky + 21 < g.h) {
-        // interior: aligned 32-bit loads, two rows (16 lanes each, 12 words used) per step
-        const int x0 = kx - 21; po = x0 & 3;
-        const int wd = lane & 15, rs = lane >> 4;
-        const uint8_t* base = I + (size_t)(ky - 21) * g.pitch + (x0 & ~3);
-        for (int r = rs; r < 43; r += 2)
-            if (wd < 12) reinterpret_cast<uint32_t*>(P + r * DP_STRIDE)[wd] = __ldg(reinterpret_cast<const uint32_t*>(base + (size_t)r * g.pitch) + wd);
+        // interior: 16-byte loads (rows are 16-byte aligned: the pitch is a multiple of 128), all issued before the first store. A row needs
+        // chunks 0..2, and chunk 3 when po > 5; that chunk starts at or before column kx + 21 < w, so it ends inside the row's pitch.
+        const int x0 = kx - 21, xa = x0 & ~15;
+        po = x0 - xa;
+        const int nch = (po + 43 + 15) >> 4;
+        const uint8_t* base = I + (size_t)(ky - 21) * g.pitch + xa;
+        uint4 q[6];
+#pragma unroll
+        for (int k = 0; k < 6; k++) {
+            const int i = lane + 32 * k, r = i >> 2, ch = i & 3;
+            if (i < 43 * 4 && ch < nch) q[k] = __ldg(reinterpret_cast<const uint4*>(base + (size_t)r * g.pitch) + ch);
+        }
+#pragma unroll
+        for (int k = 0; k < 6; k++) {
+            const int i = lane + 32 * k, r = i >> 2, ch = i & 3;
+            if (i < 43 * 4 && ch < nch) *reinterpret_cast<uint4*>(P + dp_at(r, 16 * ch)) = q[k];
+        }
     } else {
         po = 0;
         for (int i = lane; i < 43 * 43; i += 32) {
             const int r = i / 43, c = i - r * 43;
             const int yy = reflect101(ky - 21 + r, g.h), xx = reflect101(kx - 21 + c, g.w);
-            P[r * DP_STRIDE + c] = __ldg(I + (size_t)yy * g.pitch + xx);
+            P[dp_at(r, c)] = __ldg(I + (size_t)yy * g.pitch + xx);
         }
     }
     __syncwarp();
@@ -1018,11 +1078,11 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
     if (lane < 31) {
         const int u = lane - HALF_PATCH;
         const uint32_t rows = __ldg(g_icRows + lane);
-        const uint8_t* col = P + 21 * DP_STRIDE + po + 21 + u;
-        int colsum = (rows & 1u) ? col[0] : 0;
+        const int x = po + 21 + u;
+        int colsum = (rows & 1u) ? P[dp_at(21, x)] : 0;
 #pragma unroll
         for (int v = 1; v <= HALF_PATCH; v++) {
-            const int lo = col[-v * DP_STRIDE], hi = col[v * DP_STRIDE];
+            const int lo = P[dp_at(21 - v, x)], hi = P[dp_at(21 + v, x)];
             if (rows & (1u << v)) { colsum += lo + hi; m01 += v * (hi - lo); }
         }
         m10 = u * colsum;
@@ -1030,75 +1090,100 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_describe(DescribeArgs A) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) { m10 += __shfl_xor_sync(0xffffffffu, m10, o); m01 += __shfl_xor_sync(0xffffffffu, m01, o); }
     const float angle = fast_atan2_deg((float)m01, (float)m10);
-    // ---- 7x7 sigma-2 Gaussian, OpenCV 8.8 fixed point [18,34,48,56,48,34,18], only where BRIEF can sample (+-18).
-    // Horizontal: 8 outputs per item from one 20-byte window with IDP.4A; stored transposed (Ht[c][r], u16, exact: <= 65280).
-    // Columns 37..39 of the last group read past the patch's 43 columns and are not stored.
-    uint16_t* Ht = s_ht[warp];
+    // ---- 7x7 sigma-2 Gaussian on IMMA (see above), only where BRIEF can sample (+-18): 37 x 37 outputs into Bl
+    uint8_t* Bl = s_bl[warp];
     {
-        const uint32_t K0123 = 18u | (34u << 8) | (48u << 16) | (56u << 24), K456 = 48u | (34u << 8) | (18u << 16);
-        for (int it = lane; it < 43 * 5; it += 32) {   // lanes = consecutive rows of one column group: loads 13 words apart, transposed stores contiguous
-            const int cg = it / 43, r = it - cg * 43;
-            const int bidx = po + 8 * cg;
-            const uint32_t* W = reinterpret_cast<const uint32_t*>(P + r * DP_STRIDE) + (bidx >> 2);
-            const int sh = (bidx & 3) * 8;
-            const uint32_t w0 = W[0], w1 = W[1], w2 = W[2], w3 = W[3], w4 = W[4];
-            const uint32_t x[4] = {__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh)};
-            uint32_t h[8];
+        const int gq = lane >> 2, tq = lane & 3;
+        // band words: pass 1 A register (mt, kt, h, v) is word d = 4t - g - po + 8s with s = 4kt + 2h - 2mt - v, s in [-3, 6];
+        // pass 2 the same with po = 0, s in [-3, 4]
+        uint32_t a1[10], a2[8];
 #pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int q = j >> 2, s = (j & 3) * 8;   // output j: bytes j..j+6 of the window
-                h[j] = __dp4a(__funnelshift_r(x[q], x[q + 1], s), K0123, __dp4a(__funnelshift_r(x[q + 1], x[q + 2], s), K456, 0u));
+        for (int s = -3; s <= 6; s++) a1[s + 3] = s_band[4 * tq - gq - po + 8 * s - BAND_LO];
+#pragma unroll
+        for (int s = -3; s <= 4; s++) a2[s + 3] = s_band[4 * tq - gq + 8 * s - BAND_LO];
+        // ldmatrix row addresses: lane L gives row 4((L & 7) >> 1) + (L & 1) (+ the n-tile's 16p + 2e) of matrix L >> 3; x4 = chunks 0..3, x2 = 2..3
+        const int rb = 4 * ((lane & 7) >> 1) + (lane & 1), sw = (rb >> 2) & 3;
+        const uint32_t pb = (uint32_t)__cvta_generic_to_shared(P) + rb * DP_STRIDE;
+        const uint32_t ad4 = pb + 16 * ((lane >> 3) ^ sw), ad2 = pb + 16 * ((2 + ((lane >> 3) & 1)) ^ sw);
+        const uint32_t zero[4] = {0u, 0u, 0u, 0u};
+#define A1(mt, kt) a1[4 * (kt) - 2 * (mt) + 3], a1[4 * (kt) - 2 * (mt) + 2], a1[4 * (kt) - 2 * (mt) + 5], a1[4 * (kt) - 2 * (mt) + 4]
+#define A2(mt, kt) a2[4 * (kt) - 2 * (mt) + 3], a2[4 * (kt) - 2 * (mt) + 2], a2[4 * (kt) - 2 * (mt) + 5], a2[4 * (kt) - 2 * (mt) + 4]
+#pragma unroll
+        for (int mt = 0; mt < 3; mt++) {
+            // pass 1, m-tile mt: Ht rows 16mt + g (+8) against all 48 patch rows
+            uint32_t h[6][4];
+#pragma unroll
+            for (int nt = 0; nt < 6; nt++) {
+                const uint32_t roff = (16 * (nt >> 1) + 2 * (nt & 1)) * DP_STRIDE;
+                if (mt < 2) {
+                    uint32_t b[4];
+                    ldsm_x4(b, ad4 + roff);
+                    mma_u8(h[nt], A1(mt, 0), b[0], b[1], zero);
+                    mma_u8(h[nt], A1(mt, 1), b[2], b[3], h[nt]);
+                } else {   // columns 32..47 meet only patch columns 32..63
+                    uint32_t b[2];
+                    ldsm_x2(b, ad2 + roff);
+                    mma_u8(h[nt], A1(mt, 1), b[0], b[1], zero);
+                }
             }
+            // pass 2 on n-tiles 2mt + v (columns 16mt + 8v + g): B fragment p (K rows 16p + 4t .. +3) of each byte plane
 #pragma unroll
-            for (int j = 0; j < 8; j++) if (8 * cg + j < 37) Ht[(8 * cg + j) * DH_STRIDE + r] = (uint16_t)h[j];
+            for (int v = 0; v < 2; v++) {
+                if (mt == 2 && v == 1) continue;   // columns 40..47
+                uint32_t lo[3], hi[3];
+#pragma unroll
+                for (int p = 0; p < 3; p++) {
+                    const uint32_t y01 = __byte_perm(h[2 * p][2 * v], h[2 * p][2 * v + 1], 0x5410), y23 = __byte_perm(h[2 * p + 1][2 * v], h[2 * p + 1][2 * v + 1], 0x5410);
+                    lo[p] = __byte_perm(y01, y23, 0x6420);
+                    hi[p] = __byte_perm(y01, y23, 0x7531);
+                }
+                // high plane first; its products, times 256 plus the rounding 32768, are the low plane's accumulator inputs
+                uint32_t vs[3][4];
+                mma_u8(vs[0], A2(0, 0), hi[0], hi[1], zero);
+                mma_u8(vs[1], A2(1, 0), hi[0], hi[1], zero);
+                mma_u8(vs[1], A2(1, 1), hi[2], 0u, vs[1]);
+                mma_u8(vs[2], A2(2, 1), hi[2], 0u, zero);
+#pragma unroll
+                for (int m2 = 0; m2 < 3; m2++)
+#pragma unroll
+                    for (int i = 0; i < (m2 == 2 ? 2 : 4); i++) vs[m2][i] = vs[m2][i] * 256u + 32768u;   // rows 40..47 are discarded
+                mma_u8(vs[0], A2(0, 0), lo[0], lo[1], vs[0]);
+                mma_u8(vs[1], A2(1, 0), lo[0], lo[1], vs[1]);
+                mma_u8(vs[1], A2(1, 1), lo[2], 0u, vs[1]);
+                mma_u8(vs[2], A2(2, 1), lo[2], 0u, vs[2]);
+                const int col = 16 * mt + 8 * v + 2 * tq;
+#pragma unroll
+                for (int m2 = 0; m2 < 3; m2++)
+#pragma unroll
+                    for (int hv = 0; hv < (m2 == 2 ? 1 : 2); hv++)   // dst = byte 2 of 256 Vh + Vl + 32768
+                        *reinterpret_cast<uint16_t*>(Bl + (16 * m2 + 8 * hv + gq) * BL_STRIDE + col) = (uint16_t)__byte_perm(vs[m2][2 * hv], vs[m2][2 * hv + 1], 0x0062);
+            }
         }
+#undef A1
+#undef A2
     }
     __syncwarp();
-    // Vertical: 8 output rows of one column per item from seven u16x2 words with IDP.2A; dst = (V + 32768) >> 16. Rows 37..39 of the
-    // last group read Ht rows 43..45 (inside the column's stride, never written) and are not stored.
-    uint8_t* Bl = s_patch[warp];   // the raw patch is dead after the horizontal pass
-    {
-        const uint32_t K01 = 18u | (34u << 8), K23 = 48u | (56u << 8), K45 = 48u | (34u << 8);
-        for (int it = lane; it < 37 * 5; it += 32) {   // lanes = consecutive columns of one row group: loads 23 words apart, byte stores contiguous
-            const int rg = it / 37, c = it - rg * 37;
-            const uint32_t* Hw = reinterpret_cast<const uint32_t*>(Ht + c * DH_STRIDE) + 4 * rg;
-            uint32_t q[7], s[6];   // q[i] = rows 2i, 2i+1 of the group; s[i] = rows 2i+1, 2i+2
-#pragma unroll
-            for (int i = 0; i < 7; i++) q[i] = Hw[i];
-#pragma unroll
-            for (int i = 0; i < 6; i++) s[i] = __funnelshift_r(q[i], q[i + 1], 16);
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int i = j >> 1;
-                const uint32_t* a = (j & 1) ? s : q;
-                const uint32_t o = __dp2a_lo(a[i], K01, __dp2a_lo(a[i + 1], K23, __dp2a_lo(a[i + 2], K45, 18u * ((j & 1) ? q[i + 3] >> 16 : q[i + 3] & 0xffffu))));
-                if (8 * rg + j < 37) Bl[(8 * rg + j) * BL_STRIDE + c] = (uint8_t)((o + 32768u) >> 16);
-            }
-        }
-    }
-    __syncwarp();
-    // ---- steered BRIEF: lane = output byte
+    // ---- steered BRIEF: lane = output byte. A rotated coordinate x (|x| < 19) rounds to nearest even as the low bits of x + 1.5 * 2^23,
+    // like __float2int_rn, without a conversion.
     const float factorPI = (float)(3.14159265358979323846 / 180.0);
     float a, b;
     det_sincosf(__fmul_rn(angle, factorPI), &b, &a);
+    const float RND = 12582912.0f;   // 0x1.8p23
+    // sample (r, c) at Bl[(r + 18) * BL_STRIDE + c + 18]; with R, C the bit patterns of r + RND, c + RND the offset is R * BL_STRIDE + C + k0 (mod 2^32)
+    const uint32_t k0 = (uint32_t)(18 * BL_STRIDE + 18) - (uint32_t)(BL_STRIDE + 1) * (uint32_t)__float_as_int(RND);
     uint32_t val = 0;
 #pragma unroll
     for (int k = 0; k < 8; k++) {
-        const uint32_t pw = __ldg(g_patT + k * 32 + lane);
-        const float x0 = (float)(int)(signed char)(pw & 0xff), y0 = (float)(int)(signed char)((pw >> 8) & 0xff), x1 = (float)(int)(signed char)((pw >> 16) & 0xff),
-                    y1 = (float)(int)(signed char)(pw >> 24);
-        const int r0 = __float2int_rn(__fadd_rn(__fmul_rn(x0, b), __fmul_rn(y0, a))), c0 = __float2int_rn(__fsub_rn(__fmul_rn(x0, a), __fmul_rn(y0, b)));
-        const int r1 = __float2int_rn(__fadd_rn(__fmul_rn(x1, b), __fmul_rn(y1, a))), c1 = __float2int_rn(__fsub_rn(__fmul_rn(x1, a), __fmul_rn(y1, b)));
-        const int t0 = Bl[(r0 + 18) * BL_STRIDE + c0 + 18], t1 = Bl[(r1 + 18) * BL_STRIDE + c1 + 18];
+        const float4 pt = __ldg(g_pat + k * 32 + lane);   // x0, y0, x1, y1
+        const uint32_t r0 = __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(pt.x, b), __fmul_rn(pt.y, a)), RND)),
+                       c0 = __float_as_uint(__fadd_rn(__fsub_rn(__fmul_rn(pt.x, a), __fmul_rn(pt.y, b)), RND));
+        const uint32_t r1 = __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(pt.z, b), __fmul_rn(pt.w, a)), RND)),
+                       c1 = __float_as_uint(__fadd_rn(__fsub_rn(__fmul_rn(pt.z, a), __fmul_rn(pt.w, b)), RND));
+        const int t0 = Bl[(int)(r0 * BL_STRIDE + c0 + k0)], t1 = Bl[(int)(r1 * BL_STRIDE + c1 + k0)];
         val |= (uint32_t)(t0 < t1) << k;
     }
     A.desc[((size_t)frame * A.kpCap + outIdx) * 32 + lane] = (uint8_t)val;
-    if (lane == 0) {
-        cslam_keypoint kp;
-        kp.x = __fmul_rn((float)kx, g.scale); kp.y = __fmul_rn((float)ky, g.scale);
-        kp.size = g.sizeF; kp.angle = angle; kp.response = (float)resp; kp.octave = level; kp.class_id = -1;
-        A.kps[(size_t)frame * A.kpCap + outIdx] = kp;
-    }
+    if (lane == 0) kpo->angle = angle;
 }
 
 }  // namespace cslam
@@ -1385,13 +1470,13 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         static const signed char hostPattern[1024] = {
 #include "brief_pattern.inc"
         };
-        uint32_t patT[8 * 32];
+        float4 pat[8 * 32];
         for (int ln = 0; ln < 32; ln++)
             for (int k = 0; k < 8; k++) {
-                const unsigned char* q = reinterpret_cast<const unsigned char*>(hostPattern) + ln * 32 + 4 * k;
-                patT[k * 32 + ln] = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
+                const signed char* q = hostPattern + ln * 32 + 4 * k;
+                pat[k * 32 + ln] = make_float4(q[0], q[1], q[2], q[3]);
             }
-        if (cudaMemcpyToSymbol(g_patT, patT, sizeof(patT)) != cudaSuccess) { set_error("cudaMemcpyToSymbol failed"); return fail(CSLAM_E_CUDA); }
+        if (cudaMemcpyToSymbol(g_pat, pat, sizeof(pat)) != cudaSuccess) { set_error("cudaMemcpyToSymbol failed"); return fail(CSLAM_E_CUDA); }
     }
     // ---- level geometry (ComputePyramid :930-936, ComputeKeyPointsOctTree :747-761)
     std::memset(&fe->L, 0, sizeof(fe->L));
