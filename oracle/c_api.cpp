@@ -69,28 +69,6 @@ void orc_orb_stage_get(void* hv, int level, int stage, KeyPoint* out) {
     ORBextractor& e = *((OrbHandle*)hv)->ex; const std::vector<KeyPoint>& v = stage == 0 ? e.mvCandidates[level] : e.mvDistributed[level];
     if (!v.empty()) std::memcpy(out, v.data(), v.size() * sizeof(KeyPoint));
 }
-// timed CPU baseline: warp + extract over `nframes` fisheye frames with `nthreads` independent workers
-// (each worker owns its extractor, like one reference process per core). Returns total keypoints.
-long orc_warp_extract_batch(const CamParams* cp, const uint8_t* fisheyes, int nframes, const float* map1, const float* map2, const uint8_t* mask,
-                            int nfeatures, float scaleFactor, int nlevels, int iniTh, int minTh, int nthreads) {
-    std::vector<long> totals(nthreads, 0);
-    auto work = [&](int t) {
-        ORBextractor ex(nfeatures, scaleFactor, nlevels, iniTh, minTh, cp->faceW, cp->faceH);
-        const int W3 = 3 * cp->faceW, H3 = 3 * cp->faceH;
-        std::vector<uint8_t> canvas((size_t)W3 * H3, 0), desc; std::vector<KeyPoint> kps;
-        for (int f = t; f < nframes; f += nthreads) {
-            warp_fisheye_to_cubemap(*cp, fisheyes + (size_t)f * cp->Iw * cp->Ih, cp->Iw, map1, map2, canvas.data(), W3);
-            ex(canvas.data(), W3, H3, W3, mask, W3, kps, desc);
-            totals[t] += (long)kps.size();
-        }
-    };
-    std::vector<std::thread> th;
-    for (int t = 1; t < nthreads; t++) th.emplace_back(work, t);
-    work(0);
-    for (auto& x : th) x.join();
-    long s = 0; for (long v : totals) s += v; return s;
-}
-
 // ---- matcher
 int orc_descriptor_distance(const uint8_t* a, const uint8_t* b) { return descriptor_distance(a, b); }
 int orc_search_by_bow(const uint8_t* descKF, const float* angKF, const uint8_t* kfValid, const int* nodeKF, int nKF, const uint8_t* descF,
@@ -140,7 +118,8 @@ long orc_match_frames_batch(const KeyPoint* kps, const uint8_t* desc, const int*
     for (auto& x : th) x.join();
     long s = 0; for (long v : totals) s += v; return s;
 }
-// warp + extract with per-frame outputs (for the extract+match CPU baseline): kps / desc: nframes x cap
+// timed CPU baseline: warp + extract over `nframes` fisheye frames with `nthreads` independent workers (each worker owns its extractor, like one
+// reference process per core), with per-frame outputs for the extract+match baseline: kps / desc: nframes x cap. Returns total keypoints.
 long orc_warp_extract_batch_out(const CamParams* cp, const uint8_t* fisheyes, int nframes, const float* map1, const float* map2, const uint8_t* mask, int nfeatures, float scaleFactor,
                                 int nlevels, int iniTh, int minTh, int nthreads, int cap, KeyPoint* kpsOut, uint8_t* descOut, int* nOut) {
     std::vector<long> totals(nthreads, 0);

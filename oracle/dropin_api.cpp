@@ -8,28 +8,20 @@
 //     Optimizer::LocalBundleAdjustment(mpCurrentKeyFrame, &mbAbortBA, mpMap)               src/LocalMapping.cpp:86
 // run unchanged against libcubemap_b200.so. The reference's own src/ORBMatcher.cpp is linked too, with the replaced method renamed
 // (-DSearchByBoW=SearchByBoW_cpu -DSearchByProjection=SearchByProjection_cpu, see oracle/Makefile) so the same objects can be matched by the reference's CPU code for comparison.
+// The objects come from oracle/ref_scene.cpp, which libref.so shares: the drop-in is checked on the scenes the CPU reference tests check.
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <vector>
 
-#include "CamModelGeneral.h"
-#include "Converter.h"
-#include "Frame.h"
-#include "KeyFrame.h"
 #include "KeyFrameDatabase.h"
-#include "Map.h"
-#include "MapPoint.h"
 #include "ORBExtractor.h"
 #include "ORBMatcher.h"
 #include "Optimizer.h"
+#include "ref_scene.h"
 
-// src/Converter.cpp:29-39 (Converter.cpp itself needs Eigen / g2o)
-std::vector<cv::Mat> Converter::toDescriptorVector(const cv::Mat& Descriptors) {
-    std::vector<cv::Mat> vDesc;
-    vDesc.reserve(Descriptors.rows);
-    for (int j = 0; j < Descriptors.rows; j++) vDesc.push_back(Descriptors.row(j));
-    return vDesc;
-}
+using namespace scene;
+
 // the out-of-scope optimisations declared by include/Optimizer.h are never called by the harness
 // (src/Optimizer.cpp needs g2o / Eigen and is not part of this library)
 
@@ -41,59 +33,46 @@ int cslam_cpu_Fuse(ORBMatcher* m, KeyFrame* pKF, const std::vector<MapPoint*>& v
 int cslam_cpu_SearchForTriangulation(ORBMatcher* m, KeyFrame* pKF1, KeyFrame* pKF2, cv::Mat E12, std::vector<std::pair<size_t, size_t> >& vMatchedPairs);
 namespace cubemap_b200 { void DistinctiveDescriptors(const std::vector<MapPoint*>& vpMPs, std::vector<cv::Mat>& out); }
 
-struct RefCam { double c, d, e, u0, v0, p[5], invp[12]; int Iw, Ih, faceW, faceH; double fov; };
-
 namespace {
-struct KpPOD { float x, y, size, angle, response; int octave, class_id; };
-cv::Mat mat_from(const float* T, int r, int c) { cv::Mat m(r, c, CV_32F); for (int i = 0; i < r * c; i++) m.at<float>(i / c, i % c) = T[i]; return m; }
-
-// a Frame carrying given keypoints / descriptors instead of extracted ones (what Tracking holds after Frame::Frame)
-Frame* make_frame(int n, const KpPOD* kps, const uint8_t* desc, const float* Tcw, int nlevels, float scaleFactor) {
-    Frame* F = new Frame();
-    F->mnId = Frame::nNextId++;
-    F->N = n;
-    F->mvKeys.resize(n);
-    if (n) std::memcpy((void*)F->mvKeys.data(), kps, (size_t)n * sizeof(KpPOD));
-    F->mDescriptors = cv::Mat(n, 32, CV_8UC1);
-    if (desc) for (int i = 0; i < n; i++) std::memcpy(F->mDescriptors.ptr<uchar>(i), desc + 32 * (size_t)i, 32); else F->mDescriptors.setTo(0);
-    F->mvKeyRays.resize(n);
-    for (int i = 0; i < n; i++) CamModelGeneral::GetCamera()->TransformCubemapToRays(F->mvKeyRays[i], F->mvKeys[i].pt);   // Frame::ComputeKeyPointRays
-    F->mvpMapPoints.assign(n, static_cast<MapPoint*>(NULL));
-    F->mvbOutlier.assign(n, false);
-    F->mnScaleLevels = nlevels; F->mfScaleFactor = scaleFactor; F->mfLogScaleFactor = log(scaleFactor);
-    F->mvScaleFactors.resize(nlevels); F->mvLevelSigma2.resize(nlevels); F->mvInvScaleFactors.resize(nlevels); F->mvInvLevelSigma2.resize(nlevels);
-    F->mvScaleFactors[0] = 1.0f; F->mvLevelSigma2[0] = 1.0f;
-    for (int i = 1; i < nlevels; i++) { F->mvScaleFactors[i] = F->mvScaleFactors[i - 1] * scaleFactor; F->mvLevelSigma2[i] = F->mvScaleFactors[i] * F->mvScaleFactors[i]; }
-    for (int i = 0; i < nlevels; i++) { F->mvInvScaleFactors[i] = 1.0f / F->mvScaleFactors[i]; F->mvInvLevelSigma2[i] = 1.0f / F->mvLevelSigma2[i]; }
-    if (Tcw) F->SetPose(mat_from(Tcw, 4, 4));
-    return F;
-}
-// Frame::AssignFeaturesToGrid is private: replay it (src/Frame.cpp:158-176) with the public PosInGrid
-void build_grid(Frame* F) {
-    const int W3 = 3 * CamModelGeneral::GetCamera()->GetCubeFaceWidth();
-    Frame::mnMinX = 0.0f; Frame::mnMaxX = (float)W3; Frame::mnMinY = 0.0f; Frame::mnMaxY = (float)(3 * CamModelGeneral::GetCamera()->GetCubeFaceHeight());
-    Frame::mfGridElementLengthInv = static_cast<float>(3 * CUBEFACE_GRID_COLS) / static_cast<float>(Frame::mnMaxX - Frame::mnMinX);
-    Frame::mfGridElementLength = static_cast<float>(Frame::mnMaxX - Frame::mnMinX) / static_cast<float>(3 * CUBEFACE_GRID_COLS);
-    for (int i = 0; i < F->N; i++) {
-        CamModelGeneral::eFace face; int gx, gy;
-        if (F->PosInGrid(F->mvKeys[i], face, gx, gy)) F->mGrid[face][gx][gy].push_back(i);
-    }
-}
 void fill_featvec(DBoW2::FeatureVector& fv, const int32_t* node, int n) { for (int i = 0; i < n; i++) if (node[i] >= 0) fv.addFeature((DBoW2::NodeId)node[i], (unsigned)i); }
+
+// A Map built through the reference's own API (KeyFrame / MapPoint / Map, AddObservation, AddMapPoint) from nE edges (MapPoint eMP[e] seen by key
+// frame eKF[e] at kpxy[e] with octave[e]); key frame k has pose Tcw[16k], MapPoint l position pts[3l], and both are numbered from 0 (mnId).
+struct BAMap {
+    Map map; KFArray kfs; std::vector<MapPoint*> mps;
+    BAMap(int nKF, int nMP, int nE, const float* Tcw, const float* pts, const int32_t* eMP, const int32_t* eKF, const float* kpxy, const int32_t* octave)
+        : kfs(nKF), mps(nMP, static_cast<MapPoint*>(NULL)) {
+        KeyFrame::nNextId = 0; MapPoint::nNextId = 0;
+        std::vector<std::vector<int> > edgesOfKF(nKF);
+        for (int e = 0; e < nE; e++) edgesOfKF[eKF[e]].push_back(e);
+        std::vector<int> slot(nE);
+        for (int k = 0; k < nKF; k++) {
+            const int n = (int)edgesOfKF[k].size();
+            std::vector<KpPOD> kps(n);
+            for (int i = 0; i < n; i++) { const int e = edgesOfKF[k][i]; slot[e] = i; kps[i] = KpPOD{kpxy[2 * e], kpxy[2 * e + 1], 31, 0, 0, octave[e], -1}; }
+            Frame* F = make_frame(n, kps.data(), NULL, Tcw + 16 * k);
+            map.AddKeyFrame(kfs.make(k, *F, &map));
+            delete F;
+        }
+        for (int e = 0; e < nE; e++) {
+            const int l = eMP[e];
+            if (!mps[l]) { mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs.kf[eKF[e]], &map); map.AddMapPoint(mps[l]); }
+        }
+        for (int l = 0; l < nMP; l++) if (!mps[l]) mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs.kf[0], &map);   // unobserved point (keeps mnId == l)
+        for (int e = 0; e < nE; e++) { mps[eMP[e]]->AddObservation(kfs.kf[eKF[e]], slot[e]); kfs.kf[eKF[e]]->AddMapPoint(mps[eMP[e]], slot[e]); }
+    }
+    ~BAMap() { for (MapPoint* mp : mps) delete mp; }
+    // KeyFrame::GetPose / MapPoint::GetWorldPos of every key frame and point
+    void read(float* Tcw, float* pts) const {
+        for (size_t k = 0; k < kfs.kf.size(); k++) { const cv::Mat T = kfs.kf[k]->GetPose(); for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) Tcw[16 * k + 4 * r + c] = T.at<float>(r, c); }
+        for (size_t l = 0; l < mps.size(); l++) { const cv::Mat P = mps[l]->GetWorldPos(); for (int c = 0; c < 3; c++) pts[3 * l + c] = P.at<float>(c); }
+    }
+};
 }  // namespace
 
 extern "C" {
 
-void dropin_set_camera(const RefCam* cp) {   // System::System, src/System.cpp:63-89
-    cv::Mat_<double> poly = cv::Mat::zeros(5, 1, CV_64F), invpoly = cv::Mat::zeros(12, 1, CV_64F);
-    for (int i = 0; i < 5; ++i) poly.at<double>(i, 0) = cp->p[i];
-    for (int i = 0; i < 12; ++i) invpoly.at<double>(i, 0) = cp->invp[i];
-    double cdeu0v0[5] = {cp->c, cp->d, cp->e, cp->u0, cp->v0};
-    const double fx = static_cast<double>(cp->faceW) / 2, fy = static_cast<double>(cp->faceH) / 2;
-    std::streambuf* old = std::cout.rdbuf(nullptr);
-    CamModelGeneral::GetCamera()->SetCamParams(cdeu0v0, poly, invpoly, cp->Iw, cp->Ih, fx, fy, fx, fy, cp->faceW, cp->faceH, cp->fov);
-    std::cout.rdbuf(old);
-}
+void dropin_set_camera(const RefCam* cp) { set_camera(cp); }
 
 // Frame::Frame(imGray, mask, timeStamp, extractor, voc) with the GPU drop-in ORBextractor: extraction, rays, grid. Returns N.
 // kps: cap x 28 B, desc: cap x 32, rays: cap x 3, gridCount: 5*50*50 (mGrid[face][col][row].size())
@@ -106,12 +85,7 @@ int dropin_frame_from_image(const uint8_t* img, const uint8_t* mask, int rows, i
     cv::Mat im(rows, cols, CV_8UC1, (void*)img), mk(rows, cols, CV_8UC1, (void*)mask);
     Frame::mbInitialComputations = true;
     Frame F(im, mk, 0.0, ex, static_cast<ORBVocabulary*>(NULL));
-    const int n = std::min(F.N, cap);
-    if (n) std::memcpy((void*)kps, F.mvKeys.data(), (size_t)n * sizeof(KpPOD));
-    for (int i = 0; i < n; i++) { std::memcpy(desc + 32 * (size_t)i, F.mDescriptors.ptr<uchar>(i), 32); for (int c = 0; c < 3; c++) rays[3 * i + c] = F.mvKeyRays[i](c); }
-    if (gridCount)
-        for (int f = 0; f < CUBEMAP_FACES; f++) for (int x = 0; x < CUBEFACE_GRID_COLS; x++) for (int y = 0; y < CUBEFACE_GRID_ROWS; y++)
-            gridCount[(f * CUBEFACE_GRID_COLS + x) * CUBEFACE_GRID_ROWS + y] = (int)F.mGrid[f][x][y].size();
+    read_frame(F, std::min(F.N, cap), kps, desc, rays, gridCount);
     return F.N;
 }
 
@@ -120,14 +94,12 @@ int dropin_frame_from_image(const uint8_t* img, const uint8_t* mask, int rows, i
 void dropin_search_by_bow(int nKF, const KpPOD* kpK, const uint8_t* descK, const uint8_t* valid, const int32_t* nodeK, int nF, const KpPOD* kpF, const uint8_t* descF,
                           const int32_t* nodeF, float nnratio, int checkOri, int32_t* matchGpu, int32_t* nGpu, int32_t* matchCpu, int32_t* nCpu) {
     Map map; KeyFrameDatabase* db = NULL;
-    const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    Frame* FK = make_frame(nKF, kpK, descK, I4, 8, 1.2f);
+    Frame* FK = make_frame(nKF, kpK, descK, I4);
     fill_featvec(FK->mFeatVec, nodeK, nKF);
     KeyFrame* pKF = new KeyFrame(*FK, &map, db);
     std::map<MapPoint*, int> idxOf;
-    const float P0[3] = {0, 0, 1};
     for (int i = 0; i < nKF; i++) if (valid[i]) { MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), pKF, &map); pKF->AddMapPoint(mp, i); idxOf[mp] = i; }
-    Frame* F = make_frame(nF, kpF, descF, I4, 8, 1.2f);
+    Frame* F = make_frame(nF, kpF, descF, I4);
     fill_featvec(F->mFeatVec, nodeF, nF);
     std::vector<MapPoint*> out;
     ORBMatcher matcher(nnratio, checkOri != 0);
@@ -139,47 +111,27 @@ void dropin_search_by_bow(int nKF, const KpPOD* kpK, const uint8_t* descK, const
     delete pKF; delete FK; delete F;
 }
 
-// ORBMatcher(0.9, checkOri).SearchByProjection(CurrentFrame, LastFrame, th, true) (src/Tracking.cpp:634) on reference Frame / MapPoint objects:
-// GPU drop-in and the reference's CPU body from identical starting states. match*[i2]: LastFrame feature index now in the slot, -1 empty, -2 a
-// pre-existing MapPoint that was left alone.
+// ORBMatcher(0.9, checkOri).SearchByProjection(CurrentFrame, LastFrame, th, true) (src/Tracking.cpp:634) on ProjectionLastScene: GPU drop-in and
+// the reference's CPU body from identical starting states (the search only writes CurrentFrame.mvpMapPoints, which is restored in between).
 void dropin_search_by_projection_last(int nCur, const KpPOD* kCur, const uint8_t* dCur, const float* TcwCur, int nLast, const KpPOD* kLast, const float* TcwLast,
                                       const uint8_t* hasMP, const float* Xw, const uint8_t* dMP, const int32_t* mpObs, const uint8_t* curTaken, float th, int checkOri,
                                       int32_t* matchGpu, int32_t* nGpu, int32_t* matchCpu, int32_t* nCpu) {
-    Map map;
-    Frame* last = make_frame(nLast, kLast, dMP, TcwLast, 8, 1.2f);
-    KeyFrame* kfObs = new KeyFrame(*last, &map, NULL);
-    std::map<MapPoint*, int> idxOf; std::vector<MapPoint*> owned;
-    for (int i = 0; i < nLast; i++) {
-        if (!hasMP[i]) continue;
-        MapPoint* mp = new MapPoint(mat_from(Xw + 3 * i, 3, 1), &map, last, i);
-        if (mpObs[i] > 0) mp->AddObservation(kfObs, i);
-        last->mvpMapPoints[i] = mp; idxOf[mp] = i; owned.push_back(mp);
-    }
-    const float P0[3] = {0, 0, 1};
-    std::vector<MapPoint*> pre(nCur, static_cast<MapPoint*>(NULL));
-    for (int i2 = 0; i2 < nCur; i2++) if (curTaken[i2]) { pre[i2] = new MapPoint(mat_from(P0, 3, 1), kfObs, &map); pre[i2]->AddObservation(kfObs, 0); idxOf[pre[i2]] = -2; owned.push_back(pre[i2]); }
-    for (int pass = 0; pass < 2; pass++) {
-        Frame* cur = make_frame(nCur, kCur, dCur, TcwCur, 8, 1.2f);
-        build_grid(cur);
-        for (int i2 = 0; i2 < nCur; i2++) cur->mvpMapPoints[i2] = pre[i2];
-        ORBMatcher matcher(0.9f, checkOri != 0);
-        int32_t* out = pass == 0 ? matchGpu : matchCpu;
-        const int n = pass == 0 ? matcher.SearchByProjection(*cur, *last, th, true)              // dropin/ORBMatcher_b200.cpp -> libcubemap_b200.so
-                                : cslam_cpu_SearchByProjection(&matcher, *cur, *last, th, true);   // src/ORBMatcher.cpp:130-251
-        (pass == 0 ? *nGpu : *nCpu) = n;
-        for (int i2 = 0; i2 < nCur; i2++) out[i2] = cur->mvpMapPoints[i2] ? idxOf[cur->mvpMapPoints[i2]] : -1;
-        delete cur;
-    }
-    for (MapPoint* mp : owned) delete mp;
-    delete kfObs; delete last;
+    ProjectionLastScene s(nCur, kCur, dCur, TcwCur, nLast, kLast, TcwLast, hasMP, Xw, dMP, mpObs, curTaken);
+    const std::vector<MapPoint*> pre = s.cur->mvpMapPoints;
+    ORBMatcher matcher(0.9f, checkOri != 0);
+    *nGpu = matcher.SearchByProjection(*s.cur, *s.last, th, true);                         // dropin/ORBMatcher_b200.cpp -> libcubemap_b200.so
+    s.read(matchGpu);
+    s.cur->mvpMapPoints = pre;
+    *nCpu = cslam_cpu_SearchByProjection(&matcher, *s.cur, *s.last, th, true);             // src/ORBMatcher.cpp:130-251
+    s.read(matchCpu);
 }
 
 // Optimizer::PoseOptimization(&frame): n correspondences (keypoint, octave, world point). Returns inliers; Tcw in/out; outlier[n] = mvbOutlier.
 int dropin_pose_optimization(int n, const float* kpxy, const int32_t* octave, const float* Xw, float* Tcw, uint8_t* outlier) {
     Map map;
     std::vector<KpPOD> kps(n);
-    for (int i = 0; i < n; i++) { kps[i].x = kpxy[2 * i]; kps[i].y = kpxy[2 * i + 1]; kps[i].size = 31; kps[i].angle = 0; kps[i].response = 0; kps[i].octave = octave[i]; kps[i].class_id = -1; }
-    Frame* F = make_frame(n, kps.data(), NULL, Tcw, 8, 1.2f);
+    for (int i = 0; i < n; i++) kps[i] = KpPOD{kpxy[2 * i], kpxy[2 * i + 1], 31, 0, 0, octave[i], -1};
+    Frame* F = make_frame(n, kps.data(), NULL, Tcw);
     std::vector<MapPoint*> mps(n);
     for (int i = 0; i < n; i++) { mps[i] = new MapPoint(mat_from(Xw + 3 * i, 3, 1), &map, F, i); F->mvpMapPoints[i] = mps[i]; }
     const int inl = Optimizer::PoseOptimization(F);                          // dropin/Optimizer_b200.cpp
@@ -190,158 +142,69 @@ int dropin_pose_optimization(int n, const float* kpxy, const int32_t* octave, co
     return inl;
 }
 
-// Optimizer::LocalBundleAdjustment(pKF, &stop, &map) on a map built through the reference's own API (KeyFrame / MapPoint / Map, AddObservation,
-// AddMapPoint, UpdateConnections). Edges: (mp, kf, kpxy, octave). On return Tcw / pts hold KeyFrame::GetPose / MapPoint::GetWorldPos and
-// erased[e] = 1 where the observation was erased. Returns the number of key frames in the local window (covisible with curKF, incl. itself).
+// Optimizer::LocalBundleAdjustment(pKF, &stop, &map) on a BAMap whose key frames ran UpdateConnections. On return Tcw / pts hold KeyFrame::GetPose /
+// MapPoint::GetWorldPos and erased[e] = 1 where the observation was erased. Returns the number of key frames in the local window (covisible with
+// curKF, incl. itself).
 int dropin_local_ba(int nKF, int nMP, int nE, float* Tcw, float* pts, const int32_t* eMP, const int32_t* eKF, const float* kpxy, const int32_t* octave, int curKF,
                     uint8_t* erased) {
-    KeyFrame::nNextId = 0; MapPoint::nNextId = 0;
-    Map* map = new Map();
-    std::vector<std::vector<int> > edgesOfKF(nKF);
-    for (int e = 0; e < nE; e++) edgesOfKF[eKF[e]].push_back(e);
-    std::vector<KeyFrame*> kfs(nKF); std::vector<int> slot(nE);
-    for (int k = 0; k < nKF; k++) {
-        const int n = (int)edgesOfKF[k].size();
-        std::vector<KpPOD> kps(n);
-        for (int i = 0; i < n; i++) { const int e = edgesOfKF[k][i]; slot[e] = i; kps[i].x = kpxy[2 * e]; kps[i].y = kpxy[2 * e + 1]; kps[i].size = 31; kps[i].angle = 0; kps[i].response = 0; kps[i].octave = octave[e]; kps[i].class_id = -1; }
-        Frame* F = make_frame(n, kps.data(), NULL, Tcw + 16 * k, 8, 1.2f);
-        kfs[k] = new KeyFrame(*F, map, NULL);
-        map->AddKeyFrame(kfs[k]);
-        delete F;
-    }
-    std::vector<MapPoint*> mps(nMP, static_cast<MapPoint*>(NULL));
-    for (int e = 0; e < nE; e++) {
-        const int l = eMP[e];
-        if (!mps[l]) { mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs[eKF[e]], map); map->AddMapPoint(mps[l]); }
-    }
-    for (int l = 0; l < nMP; l++) if (!mps[l]) { mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs[0], map); }   // unobserved point (keeps mnId == l)
-    for (int e = 0; e < nE; e++) { mps[eMP[e]]->AddObservation(kfs[eKF[e]], slot[e]); kfs[eKF[e]]->AddMapPoint(mps[eMP[e]], slot[e]); }
-    for (int k = 0; k < nKF; k++) kfs[k]->UpdateConnections();
+    BAMap m(nKF, nMP, nE, Tcw, pts, eMP, eKF, kpxy, octave);
+    for (int k = 0; k < nKF; k++) m.kfs.kf[k]->UpdateConnections();
     bool stop = false;
-    const int window = (int)kfs[curKF]->GetVectorCovisibleKeyFrames().size() + 1;
-    Optimizer::LocalBundleAdjustment(kfs[curKF], &stop, map);                // dropin/Optimizer_b200.cpp
-    for (int k = 0; k < nKF; k++) { const cv::Mat T = kfs[k]->GetPose(); for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) Tcw[16 * k + 4 * r + c] = T.at<float>(r, c); }
-    for (int l = 0; l < nMP; l++) { const cv::Mat P = mps[l]->GetWorldPos(); for (int c = 0; c < 3; c++) pts[3 * l + c] = P.at<float>(c); }
-    for (int e = 0; e < nE; e++) erased[e] = mps[eMP[e]]->IsInKeyFrame(kfs[eKF[e]]) ? 0 : 1;
-    return window;   // (objects are intentionally leaked: the reference's Map owns raw pointers and has no teardown, include/System.h:93-95)
+    const int window = (int)m.kfs.kf[curKF]->GetVectorCovisibleKeyFrames().size() + 1;
+    Optimizer::LocalBundleAdjustment(m.kfs.kf[curKF], &stop, &m.map);       // dropin/Optimizer_b200.cpp
+    m.read(Tcw, pts);
+    for (int e = 0; e < nE; e++) erased[e] = m.mps[eMP[e]]->IsInKeyFrame(m.kfs.kf[eKF[e]]) ? 0 : 1;
+    return window;
 }
 
-
-// Optimizer::GlobalBundleAdjustemnt(pMap, nIterations, NULL, 0, true) (src/Tracking.cpp:514 after map initialisation, src/LoopClosing.cpp:649) on a Map built
-// with the reference's API: all key frames / MapPoints, one optimize(nIterations), poses / points written back through SetPose / SetWorldPos.
+// Optimizer::GlobalBundleAdjustemnt(pMap, nIterations, NULL, 0, true) (src/Tracking.cpp:514 after map initialisation, src/LoopClosing.cpp:649) on a
+// BAMap: all key frames / MapPoints, one optimize(nIterations), poses / points written back through SetPose / SetWorldPos.
 void dropin_global_ba(int nKF, int nMP, int nE, float* Tcw, float* pts, const int32_t* eMP, const int32_t* eKF, const float* kpxy, const int32_t* octave, int nIterations) {
-    KeyFrame::nNextId = 0; MapPoint::nNextId = 0;
-    Map* map = new Map();
-    std::vector<std::vector<int> > edgesOfKF(nKF);
-    for (int e = 0; e < nE; e++) edgesOfKF[eKF[e]].push_back(e);
-    std::vector<KeyFrame*> kfs(nKF); std::vector<int> slot(nE);
-    for (int k = 0; k < nKF; k++) {
-        const int n = (int)edgesOfKF[k].size();
-        std::vector<KpPOD> kps(n);
-        for (int i = 0; i < n; i++) { const int e = edgesOfKF[k][i]; slot[e] = i; kps[i].x = kpxy[2 * e]; kps[i].y = kpxy[2 * e + 1]; kps[i].size = 31; kps[i].angle = 0; kps[i].response = 0; kps[i].octave = octave[e]; kps[i].class_id = -1; }
-        Frame* F = make_frame(n, kps.data(), NULL, Tcw + 16 * k, 8, 1.2f);
-        kfs[k] = new KeyFrame(*F, map, NULL);
-        map->AddKeyFrame(kfs[k]);
-        delete F;
-    }
-    std::vector<MapPoint*> mps(nMP, static_cast<MapPoint*>(NULL));
-    for (int e = 0; e < nE; e++) {
-        const int l = eMP[e];
-        if (!mps[l]) { mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs[eKF[e]], map); map->AddMapPoint(mps[l]); }
-    }
-    for (int l = 0; l < nMP; l++) if (!mps[l]) { mps[l] = new MapPoint(mat_from(pts + 3 * l, 3, 1), kfs[0], map); }
-    for (int e = 0; e < nE; e++) { mps[eMP[e]]->AddObservation(kfs[eKF[e]], slot[e]); kfs[eKF[e]]->AddMapPoint(mps[eMP[e]], slot[e]); }
-    Optimizer::GlobalBundleAdjustemnt(map, nIterations, NULL, 0, true);      // dropin/Optimizer_b200.cpp
-    for (int k = 0; k < nKF; k++) { const cv::Mat T = kfs[k]->GetPose(); for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) Tcw[16 * k + 4 * r + c] = T.at<float>(r, c); }
-    for (int l = 0; l < nMP; l++) { const cv::Mat P = mps[l]->GetWorldPos(); for (int c = 0; c < 3; c++) pts[3 * l + c] = P.at<float>(c); }
+    BAMap m(nKF, nMP, nE, Tcw, pts, eMP, eKF, kpxy, octave);
+    Optimizer::GlobalBundleAdjustemnt(&m.map, nIterations, NULL, 0, true);  // dropin/Optimizer_b200.cpp
+    m.read(Tcw, pts);
 }
 
-// ORBMatcher(0.6).Fuse(pKF, vpMapPoints, th) (LocalMapping::SearchInNeighbors): the GPU drop-in and the reference's own CPU body on identical object
-// graphs (a key frame without MapPoints; MapPoint m observed once, by key point m of a second key frame). idx*[m] = key point of pKF on which the
-// MapPoint (or what replaced it) sits afterwards, -1 none; bad*[m] = isBad(). nFused by return values.
+// ORBMatcher(0.6).Fuse(pKF, vpMapPoints, th) (LocalMapping::SearchInNeighbors): the GPU drop-in and the reference's own CPU body, each on a fresh
+// FuseScene. idx*[m] = FuseScene::index_in_kf afterwards; bad*[m] = isBad(). nFused by return values.
 void dropin_fuse(int nKF, const KpPOD* kKF, const uint8_t* dKF, const float* Tcw, int nMP, const float* Xw, const KpPOD* kObs, const uint8_t* dMP, const float* TcwObs, float th,
                  int32_t* idxGpu, uint8_t* badGpu, int32_t* nGpu, int32_t* idxCpu, uint8_t* badCpu, int32_t* nCpu) {
     for (int pass = 0; pass < 2; pass++) {
-        Map* map = new Map();
-        Frame* F = make_frame(nKF, kKF, dKF, Tcw, 8, 1.2f); build_grid(F);
-        Frame* Fo = make_frame(nMP, kObs, dMP, TcwObs, 8, 1.2f); build_grid(Fo);
-        KeyFrame* pKF = new KeyFrame(*F, map, NULL); KeyFrame* pObs = new KeyFrame(*Fo, map, NULL);
-        delete F; delete Fo;
-        std::vector<MapPoint*> mps(nMP);
-        for (int m = 0; m < nMP; m++) {
-            MapPoint* mp = new MapPoint(mat_from(Xw + 3 * m, 3, 1), pObs, map);
-            mp->AddObservation(pObs, m); pObs->AddMapPoint(mp, m);
-            mp->ComputeDistinctiveDescriptors(); mp->UpdateNormalAndDepth();
-            mps[m] = mp;
-        }
+        FuseScene s(nKF, kKF, dKF, Tcw, nMP, Xw, kObs, dMP, TcwObs);
         ORBMatcher matcher(0.6f, true);
-        const int n = pass == 0 ? matcher.Fuse(pKF, mps, th)                 // dropin/ORBMatcher_mapping_b200.cpp -> libcubemap_b200.so
-                                : cslam_cpu_Fuse(&matcher, pKF, mps, th);    // src/ORBMatcher.cpp:1126-1240
+        const int n = pass == 0 ? matcher.Fuse(s.pKF, s.mps, th)                 // dropin/ORBMatcher_mapping_b200.cpp -> libcubemap_b200.so
+                                : cslam_cpu_Fuse(&matcher, s.pKF, s.mps, th);    // src/ORBMatcher.cpp:1126-1240
         (pass == 0 ? *nGpu : *nCpu) = n;
         int32_t* idx = pass == 0 ? idxGpu : idxCpu; uint8_t* bad = pass == 0 ? badGpu : badCpu;
-        for (int m = 0; m < nMP; m++) {
-            MapPoint* q = mps[m];
-            bad[m] = q->isBad();
-            while (q->GetReplaced()) q = q->GetReplaced();
-            idx[m] = q->GetIndexInKeyFrame(pKF);
-        }
-        // (objects are intentionally leaked: the reference's Map owns raw pointers and has no teardown)
+        for (int m = 0; m < nMP; m++) { bad[m] = s.mps[m]->isBad(); idx[m] = s.index_in_kf(m); }
     }
 }
 
-// ORBMatcher(0.6, checkOri).SearchForTriangulation(pKF1, pKF2, E12, pairs) (LocalMapping::CreateNewMapPoints): GPU drop-in vs the reference's CPU body
+// ORBMatcher(0.6, checkOri).SearchForTriangulation(pKF1, pKF2, E12, pairs) (LocalMapping::CreateNewMapPoints) on TriangulationScene: GPU drop-in vs
+// the reference's CPU body
 void dropin_search_for_triangulation(int n1, const KpPOD* k1, const uint8_t* d1, const float* Tcw1, const uint8_t* hasMP1, const int32_t* node1, int n2, const KpPOD* k2,
                                      const uint8_t* d2, const float* Tcw2, const uint8_t* hasMP2, const int32_t* node2, const float* E12, int checkOri, int32_t* matchGpu,
                                      int32_t* nGpu, int32_t* matchCpu, int32_t* nCpu) {
-    Map* map = new Map();
-    Frame* F1 = make_frame(n1, k1, d1, Tcw1, 8, 1.2f); build_grid(F1);
-    Frame* F2 = make_frame(n2, k2, d2, Tcw2, 8, 1.2f); build_grid(F2);
-    KeyFrame* kf1 = new KeyFrame(*F1, map, NULL); KeyFrame* kf2 = new KeyFrame(*F2, map, NULL);
-    delete F1; delete F2;
-    for (int i = 0; i < n1; i++) kf1->mFeatVec.addFeature(node1[i], i);
-    for (int i = 0; i < n2; i++) kf2->mFeatVec.addFeature(node2[i], i);
-    const float P0[3] = {0, 0, 1};
-    for (int i = 0; i < n1; i++) if (hasMP1[i]) kf1->AddMapPoint(new MapPoint(mat_from(P0, 3, 1), kf1, map), i);
-    for (int i = 0; i < n2; i++) if (hasMP2[i]) kf2->AddMapPoint(new MapPoint(mat_from(P0, 3, 1), kf2, map), i);
+    TriangulationScene s(n1, k1, d1, Tcw1, hasMP1, node1, n2, k2, d2, Tcw2, hasMP2, node2);
     for (int pass = 0; pass < 2; pass++) {
         ORBMatcher matcher(0.6f, checkOri != 0);
         std::vector<std::pair<size_t, size_t> > pairs;
-        const int n = pass == 0 ? matcher.SearchForTriangulation(kf1, kf2, mat_from(E12, 3, 3), pairs)                  // dropin/ORBMatcher_mapping_b200.cpp
-                                : cslam_cpu_SearchForTriangulation(&matcher, kf1, kf2, mat_from(E12, 3, 3), pairs);    // src/ORBMatcher.cpp:971-1124
+        const int n = pass == 0 ? matcher.SearchForTriangulation(s.kf1, s.kf2, mat_from(E12, 3, 3), pairs)                  // dropin/ORBMatcher_mapping_b200.cpp
+                                : cslam_cpu_SearchForTriangulation(&matcher, s.kf1, s.kf2, mat_from(E12, 3, 3), pairs);    // src/ORBMatcher.cpp:971-1124
         (pass == 0 ? *nGpu : *nCpu) = n;
-        int32_t* out = pass == 0 ? matchGpu : matchCpu;
-        for (int i = 0; i < n1; i++) out[i] = -1;
-        for (size_t i = 0; i < pairs.size(); i++) out[pairs[i].first] = (int32_t)pairs[i].second;
+        s.read(pairs, pass == 0 ? matchGpu : matchCpu);
     }
 }
 
-// cubemap_b200::DistinctiveDescriptors (the batched form of MapPoint::ComputeDistinctiveDescriptors) vs the member itself, on MapPoints observed
-// in `nobs[p]` key frames each (descriptor rows back to back). equal[p] = the batched descriptor is byte-identical to mDescriptor after the member ran.
+// cubemap_b200::DistinctiveDescriptors (the batched form of MapPoint::ComputeDistinctiveDescriptors) vs the member itself, on DistinctiveScene.
+// equal[p] = the batched descriptor is byte-identical to mDescriptor after the member ran.
 void dropin_distinctive_batch(int nPoints, const int32_t* offset, const uint8_t* desc, uint8_t* equal) {
-    Map* map = new Map();
-    const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    const float P0[3] = {0, 0, 1};
-    int maxObs = 0;
-    for (int p = 0; p < nPoints; p++) maxObs = std::max(maxObs, offset[p + 1] - offset[p]);
-    // key frame j lends row p of its descriptors to MapPoint p (rows of points with fewer observations stay unused)
-    std::vector<KeyFrame*> kfs(maxObs);
-    for (int j = 0; j < maxObs; j++) {
-        std::vector<KpPOD> kps(nPoints, KpPOD{700, 700, 31, 0, 0, 0, -1}); std::vector<uint8_t> d((size_t)nPoints * 32, 0);
-        for (int p = 0; p < nPoints; p++) if (offset[p] + j < offset[p + 1]) std::memcpy(&d[(size_t)p * 32], desc + 32 * (size_t)(offset[p] + j), 32);
-        Frame* F = make_frame(nPoints, kps.data(), d.data(), I4, 8, 1.2f);
-        kfs[j] = new KeyFrame(*F, map, NULL);
-        delete F;
-    }
-    std::vector<MapPoint*> mps(nPoints);
-    for (int p = 0; p < nPoints; p++) {
-        mps[p] = new MapPoint(mat_from(P0, 3, 1), kfs.empty() ? static_cast<KeyFrame*>(NULL) : kfs[0], map);
-        for (int j = 0; offset[p] + j < offset[p + 1]; j++) mps[p]->AddObservation(kfs[j], p);
-    }
+    DistinctiveScene s(nPoints, offset, desc);
     std::vector<cv::Mat> batched;
-    cubemap_b200::DistinctiveDescriptors(mps, batched);                        // dropin/MapPoint_batch_b200.cpp -> libcubemap_b200.so
+    cubemap_b200::DistinctiveDescriptors(s.mps, batched);                      // dropin/MapPoint_batch_b200.cpp -> libcubemap_b200.so
     for (int p = 0; p < nPoints; p++) {
-        mps[p]->ComputeDistinctiveDescriptors();                               // src/MapPoint.cpp:243-303
-        const cv::Mat d = mps[p]->GetDescriptor();
+        s.mps[p]->ComputeDistinctiveDescriptors();                             // src/MapPoint.cpp:243-303
+        const cv::Mat d = s.mps[p]->GetDescriptor();
         if (offset[p + 1] == offset[p]) equal[p] = batched[p].empty();
         else equal[p] = !batched[p].empty() && std::memcmp(batched[p].ptr<uchar>(0), d.ptr<uchar>(0), 32) == 0;
     }

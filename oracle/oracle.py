@@ -47,7 +47,6 @@ def lib():
             build()
         _LIB = C.CDLL(path)
         _LIB.orc_orb_create.restype = C.c_void_p
-        _LIB.orc_warp_extract_batch.restype = C.c_long
     return _LIB
 
 
@@ -169,12 +168,6 @@ class ORBextractor:
         out = np.empty(n, KP_DTYPE)
         lib().orc_orb_stage_get(self._h, level, stage, _p(out))
         return out
-
-
-def warp_extract_batch(cp, fisheyes, m1, m2, mask, nfeatures, scaleFactor, nlevels, iniTh, minTh, nthreads):
-    fisheyes = _u8(fisheyes); mask = _u8(mask)
-    return lib().orc_warp_extract_batch(C.byref(cp), _p(fisheyes), fisheyes.shape[0], _p(m1), _p(m2), _p(mask), int(nfeatures),
-                                        C.c_float(scaleFactor), int(nlevels), int(iniTh), int(minTh), int(nthreads))
 
 
 def warp_extract_batch_out(cp, fisheyes, m1, m2, mask, nfeatures, scaleFactor, nlevels, iniTh, minTh, nthreads, cap):

@@ -1,5 +1,5 @@
 """ctypes wrapper around oracle/_ref/libref.so = the reference's own sources compiled unmodified against the cv:: shim
-(ORACLE: test infrastructure, not product code; recipe in oracle/Makefile, entry points in oracle/ref_api.cpp).
+(ORACLE: test infrastructure, not product code; recipe in oracle/Makefile, entry points in oracle/ref_api.cpp, scenes in oracle/ref_scene.cpp).
 
 The library is built in the build container (where /root/reference exists) and travels to the GPU box as a prebuilt file;
 nothing here reads /root/reference at run time."""
@@ -32,11 +32,9 @@ def lib(variant="libref.so"):
         if not os.path.exists(path):
             build()
         L = C.CDLL(path)
-        L.ref_orb_create.restype = C.c_void_p
-        L.ref_frame_from_image.restype = C.c_void_p
-        L.ref_warp_extract_batch.restype = C.c_long
-        L.ref_cos_fov_th.restype = C.c_float
-        L.ref_arena_used.restype = C.c_size_t
+        for name, t in (("ref_orb_create", C.c_void_p), ("ref_frame_from_image", C.c_void_p), ("ref_voc_load", C.c_void_p), ("ref_cos_fov_th", C.c_float),
+                        ("ref_vector_sigma", C.c_float), ("ref_arena_used", C.c_size_t), ("ref_warp_extract_batch_out", C.c_long)):
+            getattr(L, name).restype = t
         _LIBS[variant] = L
     return _LIBS[variant]
 
@@ -48,12 +46,16 @@ class Ref:
         self.L = lib(variant)
         self.cp = cam_params
         self.L.ref_set_pins(0)
-        self.L.ref_set_camera(C.byref(cam_params))
+        self._cam()
         self.pins = pins
 
+    def _cam(self):
+        """The library, with the singleton camera set to this configuration."""
+        self.L.ref_set_camera(C.byref(self.cp))
+        return self.L
+
     def _pinned(self):
-        self.L.ref_set_camera(C.byref(self.cp))       # singleton: make sure it is this configuration
-        self.L.ref_set_pins(int(self.pins))
+        self._cam().ref_set_pins(int(self.pins))
 
     def cos_fov_th(self):
         return float(self.L.ref_cos_fov_th())
@@ -61,34 +63,24 @@ class Ref:
     def build_maps(self):
         W3, H3 = 3 * self.cp.faceW, 3 * self.cp.faceH
         m1 = np.empty((H3, W3), np.float32); m2 = np.empty((H3, W3), np.float32)
-        self.L.ref_set_camera(C.byref(self.cp))
-        self.L.ref_build_maps(_p(m1), _p(m2))
+        self._cam().ref_build_maps(_p(m1), _p(m2))
         return m1, m2
 
     def warp(self, fisheye, m1, m2, canvas=None):
         fisheye = _u8(fisheye)
         if canvas is None:
             canvas = np.zeros((3 * self.cp.faceH, 3 * self.cp.faceW), np.uint8)
-        self.L.ref_set_camera(C.byref(self.cp))
-        self.L.ref_warp(_p(fisheye), _p(m1), _p(m2), _p(canvas))
+        self._cam().ref_warp(_p(fisheye), _p(m1), _p(m2), _p(canvas))
         return canvas
 
     def extractor(self, nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST):
         return RefORBextractor(self, nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST)
 
-    def warp_extract_batch(self, fisheyes, m1, m2, mask, nfeatures, scaleFactor, nlevels, iniTh, minTh, nthreads):
-        fisheyes = _u8(fisheyes); mask = _u8(mask)
-        self.L.ref_set_camera(C.byref(self.cp))
-        self.L.ref_set_pins(0)                         # the timed baseline runs the stock code paths (glibc malloc / sincosf)
-        return self.L.ref_warp_extract_batch(_p(fisheyes), fisheyes.shape[0], _p(m1), _p(m2), _p(mask), int(nfeatures), C.c_float(scaleFactor), int(nlevels),
-                                             int(iniTh), int(minTh), int(nthreads))
-
     def search_by_projection_last(self, kCur, dCur, TcwCur, kLast, TcwLast, hasMP, Xw, dMP, mpObs, curTaken, th, checkOri=True):
         kCur = np.ascontiguousarray(kCur); kLast = np.ascontiguousarray(kLast)
         a = [_u8(dCur), _f32(TcwCur).reshape(16), _f32(TcwLast).reshape(16), _u8(hasMP), _f32(Xw), _u8(dMP), np.ascontiguousarray(mpObs, np.int32), _u8(curTaken)]
         match = np.empty(len(kCur), np.int32)
-        self.L.ref_set_camera(C.byref(self.cp))
-        n = self.L.ref_search_by_projection_last(len(kCur), _p(kCur), _p(a[0]), _p(a[1]), len(kLast), _p(kLast), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]),
+        n = self._cam().ref_search_by_projection_last(len(kCur), _p(kCur), _p(a[0]), _p(a[1]), len(kLast), _p(kLast), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]),
                                                  C.c_float(th), int(checkOri), _p(match))
         return n, match
 
@@ -96,14 +88,13 @@ class Ref:
         kF = np.ascontiguousarray(kF)
         a = [_u8(dF), _u8(inView), _f32(projXY), np.ascontiguousarray(level, np.int32), _f32(viewCos), _u8(dMP), np.ascontiguousarray(mpObs, np.int32), _u8(fTaken)]
         match = np.empty(len(kF), np.int32)
-        self.L.ref_set_camera(C.byref(self.cp))
-        n = self.L.ref_search_by_projection_local(len(kF), _p(kF), _p(a[0]), len(a[1]), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), C.c_float(th),
+        n = self._cam().ref_search_by_projection_local(len(kF), _p(kF), _p(a[0]), len(a[1]), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), C.c_float(th),
                                                   C.c_float(nnratio), _p(match))
         return n, match
 
     def ray_to_cubemap(self, xyz):
         xyz = _f32(xyz).reshape(-1, 3); uv = np.zeros((len(xyz), 2), np.float32); faces = np.zeros(len(xyz), np.int32)
-        self.L.ref_set_camera(C.byref(self.cp))
+        self._cam()
         for i in range(len(xyz)):
             u = C.c_float(); v = C.c_float()
             faces[i] = self.L.ref_ray_to_cubemap(C.c_float(xyz[i, 0]), C.c_float(xyz[i, 1]), C.c_float(xyz[i, 2]), C.byref(u), C.byref(v))
@@ -113,8 +104,7 @@ class Ref:
     def warp_extract_batch_out(self, fisheyes, m1, m2, mask, nfeatures, scaleFactor, nlevels, iniTh, minTh, nthreads, cap):
         fisheyes = _u8(fisheyes); mask = _u8(mask); F = fisheyes.shape[0]
         kps = np.zeros((F, cap), KP_DTYPE); desc = np.zeros((F, cap, 32), np.uint8); n = np.zeros(F, np.int32)
-        self.L.ref_set_camera(C.byref(self.cp)); self.L.ref_set_pins(0)
-        self.L.ref_warp_extract_batch_out.restype = C.c_long
+        self._cam().ref_set_pins(0)                    # the timed baseline runs the stock code paths (glibc malloc / sincosf)
         self.L.ref_warp_extract_batch_out(_p(fisheyes), F, _p(m1), _p(m2), _p(mask), int(nfeatures), C.c_float(scaleFactor), int(nlevels), int(iniTh), int(minTh), int(nthreads), int(cap),
                                           _p(kps), _p(desc), _p(n))
         return kps, desc, n
@@ -122,8 +112,7 @@ class Ref:
     # ---- LocalMapping feature operations (src/MapPoint.cpp:243-303, src/ORBMatcher.cpp:971-1240) on reference KeyFrame / MapPoint objects
     def distinctive_descriptor(self, desc):
         desc = _u8(desc).reshape(-1, 32); out = np.zeros(32, np.uint8)
-        self.L.ref_set_camera(C.byref(self.cp))
-        self.L.ref_distinctive_descriptor(len(desc), _p(desc), _p(out))
+        self._cam().ref_distinctive_descriptor(len(desc), _p(desc), _p(out))
         return out
 
     def fuse(self, kKF, dKF, Tcw, Xw, kObs, dMP, TcwObs, th=3.0):
@@ -131,8 +120,7 @@ class Ref:
         kKF = np.ascontiguousarray(kKF); kObs = np.ascontiguousarray(kObs); Xw = _f32(Xw); n = len(Xw)
         a = [_u8(dKF), _f32(Tcw).reshape(16), _u8(dMP), _f32(TcwObs).reshape(16)]
         valid = np.zeros(n, np.uint8); level = np.zeros(n, np.int32); idx = np.zeros(n, np.int32)
-        self.L.ref_set_camera(C.byref(self.cp))
-        nf = self.L.ref_fuse(len(kKF), _p(kKF), _p(a[0]), _p(a[1]), n, _p(Xw), _p(kObs), _p(a[2]), _p(a[3]), C.c_float(th), _p(valid), _p(level), _p(idx))
+        nf = self._cam().ref_fuse(len(kKF), _p(kKF), _p(a[0]), _p(a[1]), n, _p(Xw), _p(kObs), _p(a[2]), _p(a[3]), C.c_float(th), _p(valid), _p(level), _p(idx))
         return nf, valid, level, idx
 
     def search_for_triangulation(self, k1, d1, Tcw1, hasMP1, node1, k2, d2, Tcw2, hasMP2, node2, E12, checkOri=False):
@@ -140,16 +128,13 @@ class Ref:
         a = [_u8(d1), _f32(Tcw1).reshape(16), _u8(hasMP1), np.ascontiguousarray(node1, np.int32), _u8(d2), _f32(Tcw2).reshape(16), _u8(hasMP2), np.ascontiguousarray(node2, np.int32),
              _f32(E12).reshape(9)]
         Ow1 = np.zeros(3, np.float32); m = np.empty(len(k1), np.int32)
-        self.L.ref_set_camera(C.byref(self.cp))
-        n = self.L.ref_search_for_triangulation(len(k1), _p(k1), _p(a[0]), _p(a[1]), _p(a[2]), _p(a[3]), len(k2), _p(k2), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), _p(a[8]),
+        n = self._cam().ref_search_for_triangulation(len(k1), _p(k1), _p(a[0]), _p(a[1]), _p(a[2]), _p(a[3]), len(k2), _p(k2), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), _p(a[8]),
                                                 int(checkOri), _p(Ow1), _p(m))
         return n, m, Ow1
 
     def vector_sigma(self, kx, ky, normal_rig):
-        self.L.ref_vector_sigma.restype = C.c_float
         nr = _f32(normal_rig)
-        self.L.ref_set_camera(C.byref(self.cp))
-        return float(self.L.ref_vector_sigma(C.c_float(kx), C.c_float(ky), _p(nr)))
+        return float(self._cam().ref_vector_sigma(C.c_float(kx), C.c_float(ky), _p(nr)))
 
     def descriptor_distance(self, a, b):
         a = _u8(a); b = _u8(b)
@@ -224,7 +209,6 @@ class RefVocabulary:
 
     def __init__(self, path, variant="libref.so"):
         self.L = lib(variant)
-        self.L.ref_voc_load.restype = C.c_void_p
         self._h = C.c_void_p(self.L.ref_voc_load(str(path).encode()))
         if not self._h:
             raise RuntimeError("vocabulary load failed: " + str(path))

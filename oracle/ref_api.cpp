@@ -3,10 +3,11 @@
 // libref.so = the reference's OWN translation units, compiled UNMODIFIED from where they lie under /root/reference
 // (src/ORBExtractor.cpp, CamModelGeneral.cpp, Frame.cpp, ORBMatcher.cpp, KeyFrame.cpp, MapPoint.cpp, Map.cpp, KeyFrameDatabase.cpp and
 // ThirdParty/DBoW2/DBoW2/*.cpp) against the cv:: shim in oracle/cvshim (no OpenCV C++ exists in this container), plus this file.
-// This file holds only (1) flat C wrappers that call the reference classes the way the reference's own callers do (file:line cited),
+// This file holds only (1) flat C wrappers that call the reference classes the way the reference's own callers do (file:line cited), on
+// objects built from flat arrays by oracle/ref_scene.cpp (which libdropin.so shares, so both harnesses check the same scenes),
 // (2) the few caller-side lines of src/System.cpp that cannot be compiled here (System.cpp needs Pangolin): the map loop of
-// CreateUndistortRectifyMap (:301-324) and the five cv::remap calls (:327-355), (3) Converter::toDescriptorVector
-// (src/Converter.cpp:29-39; Converter.cpp needs Eigen), and (4) two optional PINS of behaviour the reference leaves to its environment:
+// CreateUndistortRectifyMap (:301-324) and the five cv::remap calls (:327-355), and (3) two optional PINS of behaviour the reference leaves to
+// its environment:
 //   PIN_ALLOC   std::list<ExtractorNode> nodes come from a monotonic arena, so the reference's `sort(pair<int,ExtractorNode*>)`
 //               tie-break by heap address (src/ORBExtractor.cpp:658) is "later-created node first" -- the order the oracle defines;
 //   PIN_SINCOS  sincosf (what gcc emits for cos/sin at src/ORBExtractor.cpp:83-84) is the fp64 det_sincos of oracle/cvprim.h instead
@@ -22,14 +23,12 @@
 #include <thread>
 #include <vector>
 
-#include "CamModelGeneral.h"
 #include "Converter.h"
-#include "Frame.h"
-#include "KeyFrame.h"
-#include "Map.h"
-#include "MapPoint.h"
 #include "ORBExtractor.h"
 #include "ORBMatcher.h"
+#include "ref_scene.h"
+
+using namespace scene;
 
 // ------------------------------------------------------------------------------------------------- pins
 enum { PIN_ALLOC = 1, PIN_SINCOS = 2 };
@@ -73,36 +72,13 @@ extern "C" void sincosf(float x, float* s, float* c) {
     real(x, s, c);
 }
 
-// src/Converter.cpp:29-39 (Converter.cpp itself needs Eigen / g2o): one Mat per descriptor row
-std::vector<cv::Mat> Converter::toDescriptorVector(const cv::Mat& Descriptors) {
-    std::vector<cv::Mat> vDesc;
-    vDesc.reserve(Descriptors.rows);
-    for (int j = 0; j < Descriptors.rows; j++) vDesc.push_back(Descriptors.row(j));
-    return vDesc;
-}
-
-struct RefCam { double c, d, e, u0, v0, p[5], invp[12]; int Iw, Ih, faceW, faceH; double fov; };   // same layout as orc::CamParams / oracle.CamParams
-
 extern "C" {
 
 void ref_set_pins(int mask) { g_pins.store(mask); }
 int ref_get_pins() { return g_pins.load(); }
 size_t ref_arena_used() { return g_arenaUsed.load(); }
 
-// System::System, src/System.cpp:63-89
-void ref_set_camera(const RefCam* cp) {
-    cv::Mat_<double> poly = cv::Mat::zeros(5, 1, CV_64F);
-    for (int i = 0; i < 5; ++i) poly.at<double>(i, 0) = cp->p[i];
-    cv::Mat_<double> invpoly = cv::Mat::zeros(12, 1, CV_64F);
-    for (int i = 0; i < 12; ++i) invpoly.at<double>(i, 0) = cp->invp[i];
-    double cdeu0v0[5] = {cp->c, cp->d, cp->e, cp->u0, cp->v0};
-    const int nFaceH = cp->faceH, nFaceW = cp->faceW;
-    double fx = static_cast<double>(nFaceW) / 2, fy = static_cast<double>(nFaceH) / 2;
-    double cx = static_cast<double>(nFaceW) / 2, cy = static_cast<double>(nFaceH) / 2;
-    std::streambuf* old = std::cout.rdbuf(nullptr);   // SetCosFovTh prints two lines
-    CamModelGeneral::GetCamera()->SetCamParams(cdeu0v0, poly, invpoly, cp->Iw, cp->Ih, fx, fy, cx, cy, nFaceW, nFaceH, cp->fov);
-    std::cout.rdbuf(old);
-}
+void ref_set_camera(const RefCam* cp) { set_camera(cp); }
 float ref_cos_fov_th() { return CamModelGeneral::GetCamera()->GetCosFovTh(); }
 
 // System::CreateUndistortRectifyMap, src/System.cpp:301-324 (the loop around CamModelGeneral::CubemapToFisheye)
@@ -167,34 +143,6 @@ void ref_orb_level_image(void* hv, int level, uint8_t* out) {
     for (int y = 0; y < L.rows; y++) std::memcpy(out + (size_t)y * L.cols, L.ptr<uchar>(y), (size_t)L.cols);
 }
 
-// timed CPU baseline (bench.py cpu_baseline.kind "reference"): warp + ORBextractor::operator() over nframes frames with nthreads
-// independent workers, each owning its extractor like one reference process per core. Returns the total keypoint count.
-long ref_warp_extract_batch(const uint8_t* fisheyes, int nframes, const float* map1, const float* map2, const uint8_t* mask, int nfeatures, float scaleFactor,
-                            int nlevels, int iniTh, int minTh, int nthreads) {
-    CamModelGeneral* cam = CamModelGeneral::GetCamera();
-    const int W3 = cam->GetCubeFaceWidth() * 3, H3 = cam->GetCubeFaceHeight() * 3, Iw = cam->GetFisheyeWidth(), Ih = cam->GetFisheyeHeight();
-    std::vector<long> totals(nthreads, 0);
-    auto work = [&](int t) {
-        ORBextractor ex(nfeatures, scaleFactor, nlevels, iniTh, minTh);
-        cv::Mat canvas = cv::Mat::zeros(H3, W3, CV_8UC1), mk(H3, W3, CV_8UC1, (void*)mask), desc;   // Examples/cubemap_lafida.cpp:111
-        cv::Mat m1(H3, W3, CV_32F, (void*)map1), m2(H3, W3, CV_32F, (void*)map2);
-        std::vector<cv::KeyPoint> kps;
-        for (int f = t; f < nframes; f += nthreads) {
-            cv::Mat fe(Ih, Iw, CV_8UC1, (void*)(fisheyes + (size_t)f * Iw * Ih));
-            warp_into(canvas, fe, m1, m2);
-            ex(canvas, mk, kps, desc);
-            totals[t] += (long)kps.size();
-        }
-    };
-    std::vector<std::thread> th;
-    for (int t = 1; t < nthreads; t++) th.emplace_back(work, t);
-    work(0);
-    for (auto& x : th) x.join();
-    long s = 0;
-    for (long v : totals) s += v;
-    return s;
-}
-
 // ---- Frame (src/Frame.cpp:104-156): extraction + ComputeKeyPointRays (:746-760) + AssignFeaturesToGrid (:158-176), exactly as Tracking builds it
 struct RefFrame { Frame* F; };
 void* ref_frame_from_image(void* orb, const uint8_t* img, const uint8_t* mask, int rows, int cols) {
@@ -206,17 +154,9 @@ void* ref_frame_from_image(void* orb, const uint8_t* img, const uint8_t* mask, i
 }
 void ref_frame_destroy(void* fv) { RefFrame* f = (RefFrame*)fv; delete f->F; delete f; }
 int ref_frame_n(void* fv) { return ((RefFrame*)fv)->F->N; }
-void ref_frame_get(void* fv, cv::KeyPoint* kps, uint8_t* desc, float* rays, int32_t* gridCount) {
-    Frame* F = ((RefFrame*)fv)->F;
-    const int n = F->N;
-    if (n && kps) std::memcpy((void*)kps, F->mvKeys.data(), (size_t)n * sizeof(cv::KeyPoint));
-    for (int i = 0; i < n; i++) {
-        if (desc) std::memcpy(desc + 32 * (size_t)i, F->mDescriptors.ptr<uchar>(i), 32);
-        if (rays) for (int c = 0; c < 3; c++) rays[3 * i + c] = F->mvKeyRays[i](c);
-    }
-    if (gridCount)
-        for (int f = 0; f < CUBEMAP_FACES; f++) for (int x = 0; x < CUBEFACE_GRID_COLS; x++) for (int y = 0; y < CUBEFACE_GRID_ROWS; y++)
-            gridCount[(f * CUBEFACE_GRID_COLS + x) * CUBEFACE_GRID_ROWS + y] = (int)F->mGrid[f][x][y].size();
+void ref_frame_get(void* fv, KpPOD* kps, uint8_t* desc, float* rays, int32_t* gridCount) {
+    const Frame& F = *((RefFrame*)fv)->F;
+    read_frame(F, F.N, kps, desc, rays, gridCount);
 }
 // grid cell contents in the reference's order: mGrid[face][col][row] (include/Frame.h:129)
 int ref_frame_grid_cell(void* fv, int face, int col, int row, int32_t* idx, int cap) {
@@ -232,63 +172,14 @@ int ref_frame_features_in_area(void* fv, float x, float y, float r, int minLevel
 }
 
 // ---- projection matchers of the reference on objects built from flat arrays (what Tracking holds after Frame::Frame)
-namespace {
-struct KpPOD { float x, y, size, angle, response; int octave, class_id; };
-cv::Mat mat_from(const float* T, int r, int c) { cv::Mat m(r, c, CV_32F); for (int i = 0; i < r * c; i++) m.at<float>(i / c, i % c) = T[i]; return m; }
-Frame* make_frame(int n, const KpPOD* kps, const uint8_t* desc, const float* Tcw, int nlevels, float scaleFactor) {
-    Frame* F = new Frame();
-    F->mnId = Frame::nNextId++;
-    F->N = n;
-    F->mvKeys.resize(n);
-    if (n) std::memcpy((void*)F->mvKeys.data(), kps, (size_t)n * sizeof(KpPOD));
-    F->mDescriptors = cv::Mat(n, 32, CV_8UC1);
-    for (int i = 0; i < n; i++) std::memcpy(F->mDescriptors.ptr<uchar>(i), desc + 32 * (size_t)i, 32);
-    F->mvKeyRays.resize(n);
-    for (int i = 0; i < n; i++) CamModelGeneral::GetCamera()->TransformCubemapToRays(F->mvKeyRays[i], F->mvKeys[i].pt);   // Frame::ComputeKeyPointRays
-    F->mvpMapPoints.assign(n, static_cast<MapPoint*>(NULL));
-    F->mvbOutlier.assign(n, false);
-    F->mnScaleLevels = nlevels; F->mfScaleFactor = scaleFactor; F->mfLogScaleFactor = log(scaleFactor);
-    F->mvScaleFactors.resize(nlevels); F->mvLevelSigma2.resize(nlevels); F->mvInvScaleFactors.resize(nlevels); F->mvInvLevelSigma2.resize(nlevels);
-    F->mvScaleFactors[0] = 1.0f; F->mvLevelSigma2[0] = 1.0f;
-    for (int i = 1; i < nlevels; i++) { F->mvScaleFactors[i] = F->mvScaleFactors[i - 1] * scaleFactor; F->mvLevelSigma2[i] = F->mvScaleFactors[i] * F->mvScaleFactors[i]; }
-    for (int i = 0; i < nlevels; i++) { F->mvInvScaleFactors[i] = 1.0f / F->mvScaleFactors[i]; F->mvInvLevelSigma2[i] = 1.0f / F->mvLevelSigma2[i]; }
-    if (Tcw) F->SetPose(mat_from(Tcw, 4, 4));
-    // Frame::AssignFeaturesToGrid is private: replay it (src/Frame.cpp:158-176) with the public PosInGrid
-    const int W3 = 3 * CamModelGeneral::GetCamera()->GetCubeFaceWidth();
-    Frame::mnMinX = 0.0f; Frame::mnMaxX = (float)W3; Frame::mnMinY = 0.0f; Frame::mnMaxY = (float)(3 * CamModelGeneral::GetCamera()->GetCubeFaceHeight());
-    Frame::mfGridElementLengthInv = static_cast<float>(3 * CUBEFACE_GRID_COLS) / static_cast<float>(Frame::mnMaxX - Frame::mnMinX);
-    Frame::mfGridElementLength = static_cast<float>(Frame::mnMaxX - Frame::mnMinX) / static_cast<float>(3 * CUBEFACE_GRID_COLS);
-    for (int i = 0; i < n; i++) {
-        CamModelGeneral::eFace face; int gx, gy;
-        if (F->PosInGrid(F->mvKeys[i], face, gx, gy)) F->mGrid[face][gx][gy].push_back(i);
-    }
-    return F;
-}
-}  // namespace
-
-// ORBMatcher(nnratio, checkOri).SearchByProjection(CurrentFrame, LastFrame, th, true)   src/ORBMatcher.cpp:130-251
-// matchCur[i2]: index i of the LastFrame feature whose MapPoint now sits in CurrentFrame.mvpMapPoints[i2], -1 empty, -2 a pre-existing MapPoint.
+// ORBMatcher(0.9, checkOri).SearchByProjection(CurrentFrame, LastFrame, th, true)   src/ORBMatcher.cpp:130-251
 int ref_search_by_projection_last(int nCur, const KpPOD* kCur, const uint8_t* dCur, const float* TcwCur, int nLast, const KpPOD* kLast, const float* TcwLast,
                                   const uint8_t* hasMP, const float* Xw, const uint8_t* dMP, const int32_t* mpObs, const uint8_t* curTaken, float th, int checkOri,
                                   int32_t* matchCur) {
-    Map map;
-    Frame* cur = make_frame(nCur, kCur, dCur, TcwCur, 8, 1.2f);
-    Frame* last = make_frame(nLast, kLast, dMP, TcwLast, 8, 1.2f);   // its descriptors double as the MapPoints' (MapPoint ctor copies row idxF)
-    KeyFrame* kfObs = new KeyFrame(*last, &map, NULL);
-    std::map<MapPoint*, int> idxOf; std::vector<MapPoint*> owned;
-    for (int i = 0; i < nLast; i++) {
-        if (!hasMP[i]) continue;
-        MapPoint* mp = new MapPoint(mat_from(Xw + 3 * i, 3, 1), &map, last, i);
-        if (mpObs[i] > 0) mp->AddObservation(kfObs, i);
-        last->mvpMapPoints[i] = mp; idxOf[mp] = i; owned.push_back(mp);
-    }
-    const float P0[3] = {0, 0, 1};
-    for (int i2 = 0; i2 < nCur; i2++) if (curTaken[i2]) { MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), kfObs, &map); mp->AddObservation(kfObs, 0); cur->mvpMapPoints[i2] = mp; idxOf[mp] = -2; owned.push_back(mp); }
+    ProjectionLastScene s(nCur, kCur, dCur, TcwCur, nLast, kLast, TcwLast, hasMP, Xw, dMP, mpObs, curTaken);
     ORBMatcher matcher(0.9f, checkOri != 0);
-    const int n = matcher.SearchByProjection(*cur, *last, th, true);
-    for (int i2 = 0; i2 < nCur; i2++) matchCur[i2] = cur->mvpMapPoints[i2] ? idxOf[cur->mvpMapPoints[i2]] : -1;
-    for (MapPoint* mp : owned) delete mp;
-    delete kfObs; delete cur; delete last;
+    const int n = matcher.SearchByProjection(*s.cur, *s.last, th, true);
+    s.read(matchCur);
     return n;
 }
 
@@ -296,13 +187,11 @@ int ref_search_by_projection_last(int nCur, const KpPOD* kCur, const uint8_t* dC
 int ref_search_by_projection_local(int nF, const KpPOD* kF, const uint8_t* dF, int nMP, const uint8_t* inView, const float* projXY, const int32_t* level, const float* viewCos,
                                    const uint8_t* dMP, const int32_t* mpObs, const uint8_t* fTaken, float th, float nnratio, int32_t* matchF) {
     Map map;
-    const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    Frame* F = make_frame(nF, kF, dF, I4, 8, 1.2f);
-    std::vector<KpPOD> kd(nMP); for (int m = 0; m < nMP; m++) { kd[m] = KpPOD{700, 700, 31, 0, 0, 0, -1}; }
-    Frame* holder = make_frame(nMP, kd.data(), dMP, I4, 8, 1.2f);   // only lends its descriptor rows to the MapPoint constructor
+    Frame* F = make_frame(nF, kF, dF, I4);
+    std::vector<KpPOD> kd(nMP, kHolderKp);
+    Frame* holder = make_frame(nMP, kd.data(), dMP, I4);   // only lends its descriptor rows to the MapPoint constructor
     KeyFrame* kfObs = new KeyFrame(*holder, &map, NULL);
     std::map<MapPoint*, int> idxOf; std::vector<MapPoint*> mps(nMP), owned;
-    const float P0[3] = {0, 0, 1};
     for (int m = 0; m < nMP; m++) {
         MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), &map, holder, m);
         if (mpObs[m] > 0) mp->AddObservation(kfObs, m);
@@ -333,7 +222,9 @@ void ref_expr_neg_Rt_t(const float* R9, const float* t3, float* out3) {
     for (int i = 0; i < 3; i++) out3[i] = o.at<float>(i);
 }
 
-// same with per-frame outputs (kps / desc: nframes x cap) for the extract+match CPU baseline
+// timed CPU baseline (bench.py cpu_baseline.kind "reference"): warp + ORBextractor::operator() over nframes frames with nthreads independent
+// workers, each owning its extractor like one reference process per core (Examples/cubemap_lafida.cpp:111). Per-frame outputs kps / desc:
+// nframes x cap, for the extract+match baseline. Returns the total key point count.
 long ref_warp_extract_batch_out(const uint8_t* fisheyes, int nframes, const float* map1, const float* map2, const uint8_t* mask, int nfeatures, float scaleFactor, int nlevels,
                                 int iniTh, int minTh, int nthreads, int cap, cv::KeyPoint* kpsOut, uint8_t* descOut, int* nOut) {
     CamModelGeneral* cam = CamModelGeneral::GetCamera();
@@ -393,60 +284,23 @@ int ref_descriptor_distance(const uint8_t* a, const uint8_t* b) {
     return ORBMatcher::DescriptorDistance(ma, mb);
 }
 
-}  // extern "C"
-
 // =========================================================================================== LocalMapping feature operations (SURVEY §8(f) rank 4)
-namespace {
-// KeyFrames at ascending addresses, so that std::map<KeyFrame*, size_t> iterates them in creation order (MapPoint::mObservations is keyed by pointer)
-struct KFArray {
-    char* buf; std::vector<KeyFrame*> kf;
-    KFArray(int n) : buf((char*)std::malloc((size_t)n * sizeof(KeyFrame) + 64)), kf(n, static_cast<KeyFrame*>(NULL)) {}
-    KeyFrame* make(int i, Frame& F, Map* map) { kf[i] = new (buf + (size_t)i * sizeof(KeyFrame)) KeyFrame(F, map, NULL); return kf[i]; }
-    ~KFArray() { for (KeyFrame* k : kf) if (k) k->~KeyFrame(); std::free(buf); }
-};
-}  // namespace
-
-extern "C" {
-
 // MapPoint::ComputeDistinctiveDescriptors on a MapPoint observed once in each of N key frames (observation i carries desc row i); out = mDescriptor
 void ref_distinctive_descriptor(int N, const uint8_t* desc, uint8_t* out32) {
-    Map map;
-    const float I4[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    const float P0[3] = {0, 0, 1};
-    KFArray A(N);
-    const KpPOD kp = {700, 700, 31, 0, 0, 0, -1};
-    for (int i = 0; i < N; i++) { Frame* F = make_frame(1, &kp, desc + 32 * (size_t)i, I4, 8, 1.2f); A.make(i, *F, &map); delete F; }
-    MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), A.kf[0], &map);
-    for (int i = 0; i < N; i++) mp->AddObservation(A.kf[i], 0);
-    mp->ComputeDistinctiveDescriptors();
-    const cv::Mat d = mp->GetDescriptor();
-    std::memcpy(out32, d.ptr<uchar>(0), 32);
-    delete mp;
+    const int32_t offset[2] = {0, N};
+    DistinctiveScene s(1, offset, desc);
+    s.mps[0]->ComputeDistinctiveDescriptors();
+    std::memcpy(out32, s.mps[0]->GetDescriptor().ptr<uchar>(0), 32);
 }
 
-// ORBMatcher(0.6).Fuse(pKF, vpMapPoints, th) on a key frame without MapPoints. MapPoint m: position Xw, observed once, by key point m of a second
-// key frame (pose TcwObs, key points kObs - their octave fixes the scale-invariance distances - and descriptors dMP) -> UpdateNormalAndDepth +
-// ComputeDistinctiveDescriptors give it normal, distances and descriptor the way LocalMapping does. Outputs: valid / level = the pre-tests and
-// PredictScale of Fuse evaluated with the reference's own getters; idxInKF[m] = key point of pKF the MapPoint (or what replaced it) sits on after
-// the call, -1 none. Returns nFused.
+// ORBMatcher(0.6).Fuse(pKF, vpMapPoints, th) on the scene of FuseScene. Outputs: valid / level = the pre-tests and PredictScale of Fuse evaluated
+// with the reference's own getters; idxInKF[m] = FuseScene::index_in_kf after the call. Returns nFused.
 int ref_fuse(int nKF, const KpPOD* kKF, const uint8_t* dKF, const float* Tcw, int nMP, const float* Xw, const KpPOD* kObs, const uint8_t* dMP, const float* TcwObs, float th,
              uint8_t* valid, int32_t* level, int32_t* idxInKF) {
-    Map map;
-    Frame* F = make_frame(nKF, kKF, dKF, Tcw, 8, 1.2f);
-    Frame* Fo = make_frame(nMP, kObs, dMP, TcwObs, 8, 1.2f);
-    KFArray A(2);
-    KeyFrame* pKF = A.make(0, *F, &map); KeyFrame* pObs = A.make(1, *Fo, &map);
-    delete F; delete Fo;
-    std::vector<MapPoint*> mps(nMP);
-    for (int m = 0; m < nMP; m++) {
-        MapPoint* mp = new MapPoint(mat_from(Xw + 3 * m, 3, 1), pObs, &map);
-        mp->AddObservation(pObs, m); pObs->AddMapPoint(mp, m);
-        mp->ComputeDistinctiveDescriptors(); mp->UpdateNormalAndDepth();
-        mps[m] = mp;
-    }
-    cv::Mat Ow = pKF->GetCameraCenter();
+    FuseScene s(nKF, kKF, dKF, Tcw, nMP, Xw, kObs, dMP, TcwObs);
+    cv::Mat Ow = s.pKF->GetCameraCenter();
     for (int m = 0; m < nMP; m++) {   // src/ORBMatcher.cpp:1145-1178 with the reference's own accessors
-        MapPoint* pMP = mps[m];
+        MapPoint* pMP = s.mps[m];
         valid[m] = 0; level[m] = 0;
         cv::Mat p3Dw = pMP->GetWorldPos();
         const float maxDistance = pMP->GetMaxDistanceInvariance();
@@ -456,44 +310,26 @@ int ref_fuse(int nKF, const KpPOD* kKF, const uint8_t* dKF, const float* Tcw, in
         if (dist3D < minDistance || dist3D > maxDistance) continue;
         cv::Mat Pn = pMP->GetNormal();
         if (PO.dot(Pn) < 0.5 * dist3D) continue;
-        valid[m] = 1; level[m] = pMP->PredictScale(dist3D, pKF);
+        valid[m] = 1; level[m] = pMP->PredictScale(dist3D, s.pKF);
     }
     ORBMatcher matcher(0.6f, true);
-    const int nFused = matcher.Fuse(pKF, mps, th);
-    for (int m = 0; m < nMP; m++) {
-        MapPoint* q = mps[m];
-        while (q->GetReplaced()) q = q->GetReplaced();
-        idxInKF[m] = q->GetIndexInKeyFrame(pKF);
-    }
-    for (MapPoint* mp : mps) delete mp;
+    const int nFused = matcher.Fuse(s.pKF, s.mps, th);
+    for (int m = 0; m < nMP; m++) idxInKF[m] = s.index_in_kf(m);
     return nFused;
 }
 
-// ORBMatcher(0.6, checkOri).SearchForTriangulation(pKF1, pKF2, E12, pairs). node1 / node2: vocabulary node of every feature (mFeatVec), hasMP: the key
-// point already has a MapPoint. Ow1out = pKF1->GetCameraCenter(). match12[i1] = i2 or -1. Returns nmatches.
+// ORBMatcher(0.6, checkOri).SearchForTriangulation(pKF1, pKF2, E12, pairs) on the scene of TriangulationScene. Ow1out = pKF1->GetCameraCenter().
+// match12[i1] = i2 or -1. Returns nmatches.
 int ref_search_for_triangulation(int n1, const KpPOD* k1, const uint8_t* d1, const float* Tcw1, const uint8_t* hasMP1, const int32_t* node1, int n2, const KpPOD* k2,
                                  const uint8_t* d2, const float* Tcw2, const uint8_t* hasMP2, const int32_t* node2, const float* E12, int checkOri, float* Ow1out,
                                  int32_t* match12) {
-    Map map;
-    Frame* F1 = make_frame(n1, k1, d1, Tcw1, 8, 1.2f);
-    Frame* F2 = make_frame(n2, k2, d2, Tcw2, 8, 1.2f);
-    KFArray A(2);
-    KeyFrame* kf1 = A.make(0, *F1, &map); KeyFrame* kf2 = A.make(1, *F2, &map);
-    delete F1; delete F2;
-    for (int i = 0; i < n1; i++) kf1->mFeatVec.addFeature(node1[i], i);
-    for (int i = 0; i < n2; i++) kf2->mFeatVec.addFeature(node2[i], i);
-    const float P0[3] = {0, 0, 1};
-    std::vector<MapPoint*> owned;
-    for (int i = 0; i < n1; i++) if (hasMP1[i]) { MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), kf1, &map); kf1->AddMapPoint(mp, i); owned.push_back(mp); }
-    for (int i = 0; i < n2; i++) if (hasMP2[i]) { MapPoint* mp = new MapPoint(mat_from(P0, 3, 1), kf2, &map); kf2->AddMapPoint(mp, i); owned.push_back(mp); }
-    cv::Mat Ow = kf1->GetCameraCenter();
+    TriangulationScene s(n1, k1, d1, Tcw1, hasMP1, node1, n2, k2, d2, Tcw2, hasMP2, node2);
+    cv::Mat Ow = s.kf1->GetCameraCenter();
     for (int i = 0; i < 3; i++) Ow1out[i] = Ow.at<float>(i);
     ORBMatcher matcher(0.6f, checkOri != 0);
     std::vector<std::pair<size_t, size_t> > pairs;
-    const int n = matcher.SearchForTriangulation(kf1, kf2, mat_from(E12, 3, 3), pairs);
-    for (int i = 0; i < n1; i++) match12[i] = -1;
-    for (size_t i = 0; i < pairs.size(); i++) match12[pairs[i].first] = (int32_t)pairs[i].second;
-    for (MapPoint* mp : owned) delete mp;
+    const int n = matcher.SearchForTriangulation(s.kf1, s.kf2, mat_from(E12, 3, 3), pairs);
+    s.read(pairs, match12);
     return n;
 }
 

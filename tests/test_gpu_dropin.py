@@ -10,38 +10,56 @@ import numpy as np
 import pytest
 
 from cubemapslam_b200 import config, synth
+from oracle.oracle import KP_DTYPE, _p
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "oracle", "_ref", "libdropin.so")
-KP = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"), ("octave", "<i4"), ("class_id", "<i4")])
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-@pytest.fixture(scope="module")
+@pytest.fixture
 def dropin(oracle):
+    """dropin(cfg): libdropin.so with the reference's CamModelGeneral, a process-wide singleton, set to cfg's camera. Every test sets its own
+    camera first, so none depends on what an earlier test left there."""
     if not os.path.exists(LIB):
         pytest.skip("oracle/_ref/libdropin.so is built in the build container (needs the reference tree)")
     L = C.CDLL(LIB)
-    cfg = config.lafida_450()
-    cp = oracle.cam_params(cfg)
-    L.dropin_set_camera(C.byref(cp))
-    return L, cfg, cp
+
+    def with_camera(cfg):
+        L.dropin_set_camera(C.byref(oracle.cam_params(cfg)))
+        return L
+    return with_camera
+
+
+def _in_fov(oracle, cfg, kpxy):
+    """Which key points have their ray inside the field of view: Optimizer skips the others (src/Optimizer.cpp:84-86, :323-325, :520), so the
+    tests drop them up front on both sides."""
+    kp = np.zeros(len(kpxy), KP_DTYPE); kp["x"] = kpxy[:, 0]; kp["y"] = kpxy[:, 1]
+    rays, _ = oracle.key_point_rays(kp, int(cfg["CubeFace.w"]), int(cfg["CubeFace.h"]))
+    a = np.float32(cfg["Camera.fov"]) / np.float32(2) * (np.float32(3.1415926535897932384626) / np.float32(180))
+    return rays[:, 2] >= np.float32(np.cos(np.float64(a)))
+
+
+def _inv_sigma2(octave):
+    """Frame::mvInvLevelSigma2[octave] of 8 levels with scale factor 1.2, in float32."""
+    sc = np.float32(1.0); tab = []
+    for _ in range(8):
+        tab.append(np.float32(1.0) / (sc * sc)); sc = sc * np.float32(1.2)
+    return np.array([tab[o] for o in octave], np.float32)
 
 
 def test_frame_constructor_runs_gpu_extractor(oracle, dropin):
     """Frame::Frame(im, mask, ts, extractor, voc) of the reference with the drop-in ORBextractor: keypoints / descriptors equal the oracle,
     and the reference's own ComputeKeyPointRays / AssignFeaturesToGrid ran on them."""
-    L, cfg, cp = dropin
+    cfg = config.lafida_450()
+    L = dropin(cfg)
+    cp = oracle.cam_params(cfg)
     mask = config.load_mask("gray_lafida_cubemap_mask_450")
     m1, m2 = oracle.build_maps(cp)
     for fi in (0, 3):
         canvas = oracle.warp(cp, synth.fisheye_frame(cfg, fi), m1, m2)
         cap = 2100
-        kps = np.zeros(cap, KP); desc = np.zeros((cap, 32), np.uint8); rays = np.zeros((cap, 3), np.float32); grid = np.zeros((5, 50, 50), np.int32)
+        kps = np.zeros(cap, KP_DTYPE); desc = np.zeros((cap, 32), np.uint8); rays = np.zeros((cap, 3), np.float32); grid = np.zeros((5, 50, 50), np.int32)
         n = L.dropin_frame_from_image(_p(canvas), _p(mask), 1350, 1350, 2000, C.c_float(1.2), 8, 20, 7, cap, _p(kps), _p(desc), _p(rays), _p(grid))
         rk, rd = oracle.ORBextractor(2000, 1.2, 8, 20, 7, 450, 450)(canvas, mask)
         assert n == len(rk) > 1000
@@ -52,14 +70,14 @@ def test_frame_constructor_runs_gpu_extractor(oracle, dropin):
 def test_search_by_bow_on_reference_objects(dropin):
     """ORBMatcher(0.7, true).SearchByBoW(pKF, F, matches) through the reference's KeyFrame / Frame / MapPoint objects: the GPU drop-in and the
     reference's own CPU body (src/ORBMatcher.cpp:409-539, same objects) must agree exactly."""
-    L, cfg, cp = dropin
+    L = dropin(config.lafida_450())
     for seed, n in ((0, 1500), (1, 700)):
         A, aA, B, aB, perm = synth.descriptor_pair(seed, n=n)
         rng = np.random.default_rng(40 + seed)
         nodeA = rng.integers(0, 60, n).astype(np.int32); nodeB = nodeA[perm].copy()
         nodeB[rng.random(n) < 0.1] = 61
         valid = (rng.random(n) < 0.8).astype(np.uint8)
-        kA = np.zeros(n, KP); kB = np.zeros(n, KP)
+        kA = np.zeros(n, KP_DTYPE); kB = np.zeros(n, KP_DTYPE)
         kA["x"] = 600; kA["y"] = 600; kB["x"] = 600; kB["y"] = 600; kA["angle"] = aA; kB["angle"] = aB
         mg = np.zeros(n, np.int32); mc = np.zeros(n, np.int32); ng = C.c_int32(); nc = C.c_int32()
         L.dropin_search_by_bow(n, _p(kA), _p(A), _p(valid), _p(nodeA), n, _p(kB), _p(B), _p(nodeB), C.c_float(0.7), 1, _p(mg), C.byref(ng), _p(mc), C.byref(nc))
@@ -68,15 +86,12 @@ def test_search_by_bow_on_reference_objects(dropin):
 
 
 def test_pose_optimization_on_reference_frame(oracle, dropin):
-    L, cfg, cp = dropin
+    cfg = config.lafida_450()
+    L = dropin(cfg)
     for seed in (5, 6):
         q = synth.pose_problem(n=300, faceW=450, seed=seed, outlier_frac=0.15)
-        # Optimizer::PoseOptimization skips correspondences whose key-point ray lies outside the field of view (src/Optimizer.cpp:84-86): feed both
-        # sides only correspondences that pass it, so that the oracle (which takes its edges as given) sees the same edge set
-        kp0 = np.zeros(len(q["Xw"]), KP); kp0["x"] = q["kpxy"][:, 0]; kp0["y"] = q["kpxy"][:, 1]
-        rays, _ = oracle.key_point_rays(kp0, 450, 450)
-        a = np.float32(cfg["Camera.fov"]) / np.float32(2) * (np.float32(3.1415926535897932384626) / np.float32(180))
-        keep = rays[:, 2] >= np.float32(np.cos(np.float64(a)))
+        # feed both sides only correspondences inside the field of view, so that the oracle (which takes its edges as given) sees the same edge set
+        keep = _in_fov(oracle, cfg, q["kpxy"])
         q = dict(q, Xw=q["Xw"][keep], kpxy=q["kpxy"][keep], inv_sigma2=q["inv_sigma2"][keep])
         n = len(q["Xw"])
         octave = np.zeros(n, np.int32)
@@ -91,22 +106,16 @@ def test_pose_optimization_on_reference_frame(oracle, dropin):
 def test_local_bundle_adjustment_on_reference_map(oracle, dropin):
     """Optimizer::LocalBundleAdjustment(pKF, &stop, pMap) on a Map built with the reference's KeyFrame / MapPoint / Map API; every key frame is
     covisible with the current one (every point is seen by all 6), so the local window is the whole problem and equals the oracle's input."""
-    L, cfg, cp = dropin
+    cfg = config.lafida_450()
+    L = dropin(cfg)
     p = synth.ba_problem(nKF=6, nMP=400, kmin=6, kmax=6, faceW=450, seed=21, radius=1.5)
-    # the reference skips observations whose key-point ray is outside the field of view (src/Optimizer.cpp:323-325): drop them up front on both sides
-    kp0 = np.zeros(len(p["eMP"]), KP); kp0["x"] = p["kpxy"][:, 0]; kp0["y"] = p["kpxy"][:, 1]
-    rays, _ = oracle.key_point_rays(kp0, 450, 450)
-    a = np.float32(cfg["Camera.fov"]) / np.float32(2) * (np.float32(3.1415926535897932384626) / np.float32(180))
-    keep = rays[:, 2] >= np.float32(np.cos(np.float64(a)))
+    keep = _in_fov(oracle, cfg, p["kpxy"])
     for key in ("eMP", "eKF", "kpxy", "inv_sigma2"):
         p[key] = np.ascontiguousarray(p[key][keep])
     nKF, nMP, nE = 6, 400, len(p["eMP"])
     rng = np.random.default_rng(2)
     octave = rng.integers(0, 8, nE).astype(np.int32)
-    sc = np.float32(1.0); tab = []
-    for i in range(8):
-        tab.append(np.float32(1.0) / (sc * sc)); sc = sc * np.float32(1.2)
-    inv_sigma2 = np.array([tab[o] for o in octave], np.float32)
+    inv_sigma2 = _inv_sigma2(octave)
     T = np.ascontiguousarray(p["Tcw"], np.float32).reshape(nKF, 16).copy(); pts = np.ascontiguousarray(p["pts"], np.float32).copy()
     erased = np.zeros(nE, np.uint8)
     window = L.dropin_local_ba(nKF, nMP, nE, _p(T), _p(pts), _p(p["eMP"]), _p(p["eKF"]), _p(np.ascontiguousarray(p["kpxy"], np.float32)), _p(octave), 3, _p(erased))
@@ -124,14 +133,10 @@ def test_local_bundle_adjustment_on_reference_map(oracle, dropin):
 
 
 @pytest.mark.parametrize("seed,th", [(0, 15.0), (1, 30.0)])
-def test_search_by_projection_on_reference_frames(oracle, seed, th):
+def test_search_by_projection_on_reference_frames(dropin, seed, th):
     """ORBMatcher(0.9, true).SearchByProjection(CurrentFrame, LastFrame, th, true) (src/Tracking.cpp:634) on reference Frame / MapPoint objects:
     the GPU drop-in and the reference's own CPU body, from identical starting states, leave identical mvpMapPoints and return the same count."""
-    if not os.path.exists(LIB):
-        pytest.skip("oracle/_ref/libdropin.so is built in the build container")
-    L = C.CDLL(LIB)
-    cp = oracle.cam_params(config.front_1024())
-    L.dropin_set_camera(C.byref(cp))
+    L = dropin(config.front_1024())
     s = synth.tracking_pair(seed, n=1500, faceW=650)
     nC, nL = len(s["kCur"]), len(s["kLast"])
     mg = np.zeros(nC, np.int32); mc = np.zeros(nC, np.int32); ng = C.c_int32(); nc = C.c_int32()
@@ -142,23 +147,13 @@ def test_search_by_projection_on_reference_frames(oracle, seed, th):
                                        C.c_float(th), 1, _p(mg), C.byref(ng), _p(mc), C.byref(nc))
     assert ng.value == nc.value > 300
     assert np.array_equal(mg, mc)
-    # fixture switches the singleton camera back for the other tests of this module
-    L.dropin_set_camera(C.byref(oracle.cam_params(config.lafida_450())))
-
-
-def _front(oracle):
-    if not os.path.exists(LIB):
-        pytest.skip("oracle/_ref/libdropin.so is built in the build container")
-    L = C.CDLL(LIB)
-    L.dropin_set_camera(C.byref(oracle.cam_params(config.front_1024())))
-    return L
 
 
 @pytest.mark.parametrize("seed,th", [(0, 3.0), (1, 6.0)])
-def test_fuse_on_reference_key_frames(oracle, seed, th):
+def test_fuse_on_reference_key_frames(dropin, seed, th):
     """ORBMatcher(0.6).Fuse(pKF, vpMapPoints, th) (src/LocalMapping.cpp:402,423) on reference KeyFrame / MapPoint objects: the GPU drop-in (search on
     the device, Replace / AddObservation bookkeeping through the reference's own methods) and the reference's CPU body leave identical maps."""
-    L = _front(oracle)
+    L = dropin(config.front_1024())
     s = synth.mapping_pair(seed, n=1500, faceW=650)
     n = len(s["Xw"])
     a = [np.ascontiguousarray(s["kCur"]), np.ascontiguousarray(s["dCur"]), np.ascontiguousarray(s["TcwCur"], np.float32), np.ascontiguousarray(s["Xw"], np.float32),
@@ -167,13 +162,12 @@ def test_fuse_on_reference_key_frames(oracle, seed, th):
     L.dropin_fuse(len(a[0]), _p(a[0]), _p(a[1]), _p(a[2]), n, _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), C.c_float(th), _p(ig), _p(bg), C.byref(ng), _p(ic), _p(bc), C.byref(nc))
     assert ng.value == nc.value > 150
     assert np.array_equal(ig, ic) and np.array_equal(bg, bc)
-    L.dropin_set_camera(C.byref(oracle.cam_params(config.lafida_450())))
 
 
 @pytest.mark.parametrize("seed,ori", [(0, False), (1, True)])
-def test_search_for_triangulation_on_reference_key_frames(oracle, seed, ori):
+def test_search_for_triangulation_on_reference_key_frames(dropin, seed, ori):
     """ORBMatcher(0.6, false).SearchForTriangulation(pKF1, pKF2, E12, pairs) (src/LocalMapping.cpp:262): drop-in == the reference's CPU body."""
-    L = _front(oracle)
+    L = dropin(config.front_1024())
     s = synth.mapping_pair(30 + seed, n=1500, faceW=650)
     n1, n2 = len(s["kCur"]), len(s["kLast"])
     a = [np.ascontiguousarray(s["kCur"]), np.ascontiguousarray(s["dCur"]), np.ascontiguousarray(s["TcwCur"], np.float32), np.ascontiguousarray(s["hasMPCur"]),
@@ -184,12 +178,11 @@ def test_search_for_triangulation_on_reference_key_frames(oracle, seed, ori):
                                       C.byref(ng), _p(mc), C.byref(nc))
     assert ng.value == nc.value > 100
     assert np.array_equal(mg, mc)
-    L.dropin_set_camera(C.byref(oracle.cam_params(config.lafida_450())))
 
 
-def test_batched_distinctive_descriptors_on_reference_map_points(oracle):
+def test_batched_distinctive_descriptors_on_reference_map_points(dropin):
     """cubemap_b200::DistinctiveDescriptors (one launch for all MapPoints of a key frame) == MapPoint::ComputeDistinctiveDescriptors per point."""
-    L = _front(oracle)
+    L = dropin(config.front_1024())
     rng = np.random.default_rng(3)
     P = 400; off = [0]; rows = []
     for p in range(P):
@@ -201,27 +194,21 @@ def test_batched_distinctive_descriptors_on_reference_map_points(oracle):
     desc = np.ascontiguousarray(np.stack(rows)); off = np.array(off, np.int32); eq = np.zeros(P, np.uint8)
     L.dropin_distinctive_batch(P, _p(off), _p(desc), _p(eq))
     assert eq.all()
-    L.dropin_set_camera(C.byref(oracle.cam_params(config.lafida_450())))
 
 
 def test_global_bundle_adjustment_on_reference_map(oracle, dropin):
     """Optimizer::GlobalBundleAdjustemnt(pMap, 20) (src/Tracking.cpp:514, src/LoopClosing.cpp:649; body src/Optimizer.cpp:461-621) through the drop-in on a
     Map built with the reference's API == the oracle's LM with one optimize(20), robust kernel on, no outlier stage."""
-    L, cfg, cp = dropin
+    cfg = config.lafida_450()
+    L = dropin(cfg)
     p = synth.ba_problem(nKF=7, nMP=350, kmin=3, kmax=7, faceW=450, seed=31, radius=1.5)
-    kp0 = np.zeros(len(p["eMP"]), KP); kp0["x"] = p["kpxy"][:, 0]; kp0["y"] = p["kpxy"][:, 1]
-    rays, _ = oracle.key_point_rays(kp0, 450, 450)
-    a = np.float32(cfg["Camera.fov"]) / np.float32(2) * (np.float32(3.1415926535897932384626) / np.float32(180))
-    keep = rays[:, 2] >= np.float32(np.cos(np.float64(a)))       # the reference skips observations outside the field of view (src/Optimizer.cpp:520)
+    keep = _in_fov(oracle, cfg, p["kpxy"])
     for key in ("eMP", "eKF", "kpxy", "inv_sigma2"):
         p[key] = np.ascontiguousarray(p[key][keep])
     nKF, nMP, nE = 7, 350, len(p["eMP"])
     rng = np.random.default_rng(4)
     octave = rng.integers(0, 8, nE).astype(np.int32)
-    sc = np.float32(1.0); tab = []
-    for i in range(8):
-        tab.append(np.float32(1.0) / (sc * sc)); sc = sc * np.float32(1.2)
-    inv_sigma2 = np.array([tab[o] for o in octave], np.float32)
+    inv_sigma2 = _inv_sigma2(octave)
     T = np.ascontiguousarray(p["Tcw"], np.float32).reshape(nKF, 16).copy(); pts = np.ascontiguousarray(p["pts"], np.float32).copy()
     L.dropin_global_ba(nKF, nMP, nE, _p(T), _p(pts), _p(p["eMP"]), _p(p["eKF"]), _p(np.ascontiguousarray(p["kpxy"], np.float32)), _p(octave), 20)
     fixed = np.zeros(nKF, np.uint8); fixed[0] = 1                 # only mnId == 0 is fixed
