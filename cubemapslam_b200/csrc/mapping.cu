@@ -79,7 +79,7 @@ struct FuseArgs {
 __global__ void __launch_bounds__(256) k_fuse_search(FuseArgs A) {
     const int m = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (m >= A.nMP) return;
-    unsigned best = 0xffffffffu;   // dist << 20 | position in the visiting order
+    unsigned best = 256u << 20;   // dist << 20 | position in the visiting order; starts at the reference's bestDist = 256, so a complement never wins
     int bestI = -1;
     if (A.valid[m]) {
         float xc[3];

@@ -8,6 +8,7 @@ import pytest
 from cubemapslam_b200 import config, synth
 
 from oracle import ref
+from tests import test_gpu_mapping_limits as L
 from tests.refrecord import LIVE, RefRecord, same
 
 REC = RefRecord("oracle_mapping")
@@ -86,17 +87,7 @@ def test_fuse_on_face_boundaries(oracle, cam):
     returned face - it only asks IsInImage(u, v) (src/ORBMatcher.cpp:1150-1154). MapPoints exactly on a face seam (|x/z| == 1 etc.) and behind the
     camera exercise that path: oracle == compiled reference."""
     cp, r = cam
-    s = synth.mapping_pair(5, n=1200, faceW=650)
-    rng = np.random.default_rng(11)
-    Xw = s["Xw"].copy()
-    n = len(Xw)
-    d = rng.uniform(2.0, 9.0, n).astype(np.float32); y = rng.uniform(-0.9, 0.9, n).astype(np.float32) * d
-    k = np.arange(n) % 6
-    Xw[k == 0] = np.stack([d, y, d], 1)[k == 0]           # x / z == 1: front test passes, u == W fails the in-face test
-    Xw[k == 1] = np.stack([-d, y, d], 1)[k == 1]          # x / z == -1
-    Xw[k == 2] = np.stack([y, d, d], 1)[k == 2]           # y / z == 1
-    Xw[k == 3] = np.stack([d, y, -d], 1)[k == 3]          # behind: right face, z / x == -1
-    Xw[k == 4] = 0                                        # the origin: no face at all -> (-1, -1)
+    s, Xw, _ = L.face_boundary_points()
     I4 = np.eye(4, dtype=np.float32)
     nf, valid, level, idx = REC("fuse_face_boundaries", lambda: r.fuse(s["kCur"], s["dCur"], I4, Xw, s["kLast"], s["dLast"], I4, 4.0))
     g = oracle.FrameGrid(s["kCur"], 650, 650)
@@ -104,3 +95,65 @@ def test_fuse_on_face_boundaries(oracle, cam):
     fused = bd <= 50
     assert nf == int(fused.sum())
     assert np.array_equal(np.where(fused, bi, -1), idx)
+
+
+# ---- the scenes of tests/test_gpu_mapping_limits.py that have a reference counterpart
+@pytest.fixture(scope="module")
+def cam450(oracle):
+    cp = oracle.cam_params(config.lafida_450())
+    return cp, ref.Ref(cp) if LIVE else None
+
+
+def test_fuse_ties_and_complements(oracle, cam):
+    """Ties at the least distance across cells, 32-cell chunks and seam rectangles (the first visited wins, not the lowest index), and
+    complement-only windows: the reference fuses the first visited tied key point and nothing in a complement window."""
+    cp, r = cam
+    S = L.tie_scene(oracle); a = S.arrays()
+    nf, valid, level, idx = REC("fuse_ties", lambda: r.fuse(a["kKF"], a["dKF"], a["Tcw"], a["Xw"], S.kobs(), a["dMP"], a["Tcw"], a["th"]))
+    ms = [c["m"] for c in S.cases]
+    assert (valid[ms] == 1).all() and np.array_equal(level[ms], a["level"][ms])   # the reference predicts the levels the GPU test uses
+    bi, bd = oracle.FrameGrid(a["kKF"], 650, 650).fuse_search(a["dKF"], a["Tcw"], a["scale"], a["isg"], valid, a["Xw"], level, a["dMP"], a["th"])
+    fused = bd <= 50
+    assert nf == int(fused.sum())
+    assert np.array_equal(np.where(fused, bi, -1), idx)
+    for c in S.cases:
+        assert idx[c["m"]] == (c["expect"] if c["dist"] <= 50 else -1), c
+
+
+@pytest.mark.parametrize("seed,th", [(0, 3.0), (2, 12.0)])
+def test_fuse_search_450(oracle, cam450, seed, th):
+    cp, r = cam450
+    s = synth.mapping_pair(seed, n=1500, faceW=450)
+    nf, valid, level, idx = REC("fuse450_%d" % seed, lambda: r.fuse(s["kCur"], s["dCur"], s["TcwCur"], s["Xw"], s["kLast"], s["dLast"], s["TcwLast"], th))
+    bi, bd = oracle.FrameGrid(s["kCur"], 450, 450).fuse_search(s["dCur"], s["TcwCur"], s["scale"], s["inv_level_sigma2"], valid, s["Xw"], level, s["dLast"], th)
+    fused = bd <= 50
+    assert nf == int(fused.sum()) and nf > 150
+    assert np.array_equal(np.where(fused, bi, -1), idx)
+
+
+def test_search_for_triangulation_450(oracle, cam450):
+    """Three synthetic pairs, a pure rotation (camera centre exactly 0, E12 = 0) and an epipole on a face seam, at face width 450: KF1's
+    pose [I | -Ow1] gives the reference exactly the camera centre the GPU test uses."""
+    cp, r = cam450
+    for i, p in enumerate(L.triangulation_pairs(oracle)):
+        s = p["s"]; ori = i % 2 == 1
+        T1 = s["TcwCur"] if i < 3 else np.eye(4, dtype=np.float32)
+        if i == 4:
+            T1 = T1.copy(); T1[:3, 3] = -p["Ow"]
+        n2, m2, Ow1 = REC("triangulation450_%d" % i, lambda: r.search_for_triangulation(s["kCur"], s["dCur"], T1, s["hasMPCur"], s["nodeCur"], s["kLast"], s["dLast"],
+                                                                                            p["T2"], s["hasMPObs"], s["nodeObs"], p["E"], ori), digest=(1,))
+        assert i < 3 or np.array_equal(Ow1, p["Ow"]), i
+        n1, m1 = L.oracle_triangulation(oracle, dict(p, Ow=Ow1), 450, ori)
+        assert n1 == n2, i
+        assert same(np.asarray(m1, np.int32), m2), i
+
+
+def test_distinctive_descriptor_ties(oracle, cam):
+    """Least-median ties first at rows 0, 31, 32, 127, 128, 129 (distinct descriptors, so the returned bytes name the row), all-identical
+    sets and random sets of N = 1, 2, 3, 127, 128, 129 and small even N."""
+    cp, r = cam
+    sets = L.distinctive_sets(max_n=129)
+    rbest = REC("distinctive_ties", lambda: np.stack([r.distinctive_descriptor(d) for d in sets]))
+    for d, rb in zip(sets, rbest):
+        best = oracle.distinctive_descriptors(d, np.array([0, len(d)], np.int32))[0]
+        assert np.array_equal(rb, d[best])
