@@ -49,7 +49,7 @@ Handle::~Handle() {
 }  // namespace cslam
 
 extern "C" const char* cslam_last_error(void) { return cslam::g_err; }
-extern "C" int cslam_version(void) { return 100; }
+extern "C" int cslam_version(void) { return 101; }
 extern "C" int cslam_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

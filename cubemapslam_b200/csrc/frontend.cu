@@ -1194,8 +1194,35 @@ using namespace cslam;
 enum { KIND_WARP = 0, KIND_PYRAMID, KIND_FAST, KIND_DISTRIBUTE, KIND_DESCRIBE, KIND_COUNT, KIND_END = KernelTimer::END };
 static const char* kKindNames[KIND_COUNT] = {"k_warp", "k_pyramid", "k_fast", "k_distribute", "k_describe"};
 
-// error flag: set by k_fast, k_distribute and k_describe when a fixed-capacity buffer overflows. arena: device staging of the host entry
-// points (fisheye frames, key points, descriptors, counts).
+// A host batch as the caller passed it: input frames (fisheye frames, or canvases of pitch inPitch) and the output buffers; pin*: the
+// buffer is page-locked, so the copy engines use it directly
+struct HostBatch {
+    const uint8_t* in; int inPitch; bool fromWarp;
+    cslam_keypoint* kps; uint8_t* desc; int32_t* n;
+    bool pinIn, pinK, pinD, pinN;
+};
+// Where a host batch is staged and which error flag its kernels write. The device buffers hold the whole batch (frame f at f times the
+// per-frame size); the page-locked ones stand in for the caller's pageable buffers. up / down: the streams of the fisheye uploads and of the
+// downloads, ordered to each chunk's kernels by evUp / evRun; nullptr: the chunk's own stream (the synchronous entry points).
+struct HostStage {
+    uint8_t* dfe; cslam_keypoint* dk; uint8_t* dd; int32_t* dn;
+    uint8_t* hIn; cslam_keypoint* hKps; uint8_t* hDesc; int32_t* hN;
+    int* errFlag;
+    cudaStream_t up, down; cudaEvent_t evUp, evRun;
+};
+// A pending ticket of cslam_frontend_submit (ticket 0: the slot is free). Its device staging, error flag and events are made the first time
+// the slot is used, each page-locked staging buffer the first time the slot meets a pageable buffer of its kind. Not from the arena: the next
+// entry point's reset() would hand the pieces out again while the ticket's copies still use them.
+struct PendingSlot {
+    int64_t ticket = 0;
+    HostStage s = {};
+    int* errHost = nullptr;          // page-locked copy of *s.errFlag, written after the ticket's last kernel
+    cudaEvent_t evDone = nullptr;    // after the ticket's downloads and its error flag's copy
+    HostBatch b = {}; int batch = 0;
+};
+
+// error flag: set by k_fast, k_distribute and k_describe when a fixed-capacity buffer overflows. arena: device staging of the synchronous
+// host entry points (fisheye frames, key points, descriptors, counts).
 struct cslam_frontend : cslam::Handle {
     cslam_cam_params cam;
     cslam_orb_params orb;
@@ -1209,18 +1236,23 @@ struct cslam_frontend : cslam::Handle {
     uint32_t* d_candCount = nullptr; // maxBatch x nlevels
     uint32_t* d_kept = nullptr; uint32_t* d_keptCount = nullptr;
     uint8_t* h_pin_in = nullptr; cslam_keypoint* h_pin_kps = nullptr; uint8_t* h_pin_desc = nullptr; int32_t* h_pin_n = nullptr;
-    static const int MAX_LANES = 4;
-    cudaStream_t lane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evLane[MAX_LANES] = {nullptr, nullptr, nullptr, nullptr}; cudaEvent_t evFork = nullptr;
+    // kernel lanes 0..MAX_LANES-1, forked from the handle's stream and joined back by every call; then the copy lanes of submitted
+    // batches, which are never joined: UP_LANE (uploads, wait for nothing) and DOWN_LANE (downloads, wait for their chunk's kernels)
+    static const int MAX_LANES = 4, UP_LANE = MAX_LANES, DOWN_LANE = MAX_LANES + 1, ALL_LANES = MAX_LANES + 2;
+    cudaStream_t lane[ALL_LANES] = {}; cudaEvent_t evLane[MAX_LANES] = {}; cudaEvent_t evFork = nullptr;
     static constexpr int DEV_LANES = 2;     // lanes used by cslam_frontend_run_dev
     static constexpr int HOST_CHUNKS = 8;   // most chunks a host-buffer batch is cut into
+    PendingSlot slot[CSLAM_FRONTEND_MAX_PENDING];
+    int64_t lastTicket = 0;
     KernelTimer timer;           // optional per-kernel timing (cslam_frontend_set_timing); a timed batch runs as one lane and one chunk
     bool cornersDirty = false;   // level buffers hold a caller canvas pyramid (non-zero corner regions) from cslam_orb_extract
     int pyrWin[MAX_LEVELS] = {};   // k_pyramid instantiation (PYR_WIN or PYR_WIN_MAX) of each level >= 1
-    ~cslam_frontend() {   // the lanes' work is joined into the handle's stream, which destroy_handle has waited for; the lanes are waited for too
-        for (int i = 0; i < MAX_LANES; i++) {
+    ~cslam_frontend() {   // the kernel lanes are joined into the handle's stream, which destroy_handle has waited for; every lane is waited for too
+        for (int i = 0; i < ALL_LANES; i++)
             if (lane[i]) { cudaStreamSynchronize(lane[i]); cudaStreamDestroy(lane[i]); }
-            if (evLane[i]) cudaEventDestroy(evLane[i]);
-        }
+        for (int i = 0; i < MAX_LANES; i++) if (evLane[i]) cudaEventDestroy(evLane[i]);
+        for (PendingSlot& p : slot)
+            for (cudaEvent_t e : {p.s.evUp, p.s.evRun, p.evDone}) if (e) cudaEventDestroy(e);
         if (evFork) cudaEventDestroy(evFork);
     }
 };
@@ -1457,8 +1489,9 @@ extern "C" int cslam_frontend_create(cslam_frontend** out, int device, const csl
         for (v = 0; v <= vmax; ++v) fe->umax[v] = cv_round_d(std::sqrt(hp2 - v * v));
         for (v = HALF_PATCH, v0 = 0; v >= vmin; --v) { while (fe->umax[v0] == fe->umax[v0 + 1]) ++v0; fe->umax[v] = v0; ++v0; }
     }
-    for (int i = 0; i < cslam_frontend::MAX_LANES; i++)
-        if (cudaStreamCreateWithFlags(&fe->lane[i], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&fe->evLane[i], cudaEventDisableTiming) != cudaSuccess) { set_error("lane stream creation failed"); return fail(CSLAM_E_CUDA); }
+    for (int i = 0; i < cslam_frontend::ALL_LANES; i++)
+        if (cudaStreamCreateWithFlags(&fe->lane[i], cudaStreamNonBlocking) != cudaSuccess ||
+            (i < cslam_frontend::MAX_LANES && cudaEventCreateWithFlags(&fe->evLane[i], cudaEventDisableTiming) != cudaSuccess)) { set_error("lane stream creation failed"); return fail(CSLAM_E_CUDA); }
     if (cudaEventCreateWithFlags(&fe->evFork, cudaEventDisableTiming) != cudaSuccess) { set_error("event creation failed"); return fail(CSLAM_E_CUDA); }
     {
         uint32_t icRows[32] = {};
@@ -1622,11 +1655,23 @@ extern "C" int cslam_frontend_kp_capacity(const cslam_frontend* fe) { return fe 
 extern "C" void* cslam_frontend_stream(const cslam_frontend* fe) { return fe ? (void*)fe->stream : nullptr; }
 extern "C" int64_t cslam_frontend_launches(const cslam_frontend* fe) { return fe ? fe->launches : 0; }
 
-extern "C" int cslam_frontend_sync(cslam_frontend* fe) {
-    if (!fe) return CSLAM_E_BADARG;
-    const int rc = fe->sync("front end: a fixed-capacity buffer overflowed on the device (candidates / nodes / keypoints)");
+static const char* kOverflowMessage = "front end: a fixed-capacity buffer overflowed on the device (candidates / nodes / keypoints)";
+
+// the end of every synchronous call: waits for the handle's stream (every call's kernels and the synchronous calls' copies) and reports the
+// handle's own flag, never a ticket's
+static int sync_stream(cslam_frontend* fe) {
+    const int rc = fe->sync(kOverflowMessage);
     fe->timer.collect();
     return rc;
+}
+
+// waits for all enqueued work, the pending tickets' copies included
+extern "C" int cslam_frontend_sync(cslam_frontend* fe) {
+    if (!fe) return CSLAM_E_BADARG;
+    CSLAM_CUDA(cudaSetDevice(fe->device));
+    CSLAM_CUDA(cudaStreamSynchronize(fe->lane[cslam_frontend::UP_LANE]));
+    CSLAM_CUDA(cudaStreamSynchronize(fe->lane[cslam_frontend::DOWN_LANE]));
+    return sync_stream(fe);
 }
 
 // Frame range [f0, f0+cnt) of the per-batch buffers, for one lane
@@ -1653,7 +1698,9 @@ static int launch_warp(cslam_frontend* fe, cudaStream_t st, const uint8_t* d_fis
     return 0;
 }
 
-static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, cslam_keypoint* d_kps, uint8_t* d_desc, int32_t* d_nout, bool useSkip) {
+// errFlag: where k_fast, k_distribute and k_describe report an overflow (the handle's flag, or a pending ticket's)
+static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, cslam_keypoint* d_kps, uint8_t* d_desc, int32_t* d_nout, bool useSkip,
+                          int* errFlag) {
     const int nl = fe->L.nlevels;
     const DevLevels L = shifted(fe, f0);
     uint32_t* candCount = fe->d_candCount + (size_t)f0 * nl;
@@ -1669,19 +1716,19 @@ static int launch_extract(cslam_frontend* fe, cudaStream_t st, int f0, int cnt, 
         const LevelGeom& g = L.g[l];
         dim3 grid(cdiv(g.nColsEff, CG), cdiv(g.nRowsEff, FAST_R), cnt);
         mark(fe, st, KIND_FAST);
-        k_fast<<<grid, 256, fast_smem(g).total, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, fe->errFlag,
+        k_fast<<<grid, 256, fast_smem(g).total, st>>>(L.img[l], g, fe->orb.ini_th_fast, fe->orb.min_th_fast, L.cand[l], candCount + l, nl, errFlag,
                                      L.fcols[l], useSkip ? L.skip[l] : nullptr, useSkip ? L.live[l] : nullptr, L.liveOff[l]);
     }
     CSLAM_CUDA(cudaGetLastError());
     DistributeArgs da;
     da.L = L; da.candCount = candCount; da.kept = fe->d_kept + (size_t)f0 * nl * fe->M; da.keptCount = fe->d_keptCount + (size_t)f0 * nl;
     da.mask = fe->d_mask; da.maskPitch = fe->maskPitch;
-    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.M = fe->M; da.errFlag = fe->errFlag;
+    da.imgW = fe->CW; da.imgH = fe->CH; da.faceW = fe->W; da.faceH = fe->H; da.M = fe->M; da.errFlag = errFlag;
     mark(fe, st, KIND_DISTRIBUTE);
     k_distribute<<<dim3(nl, cnt), DIST_THREADS, dist_smem(fe->M).total, st>>>(da);
     DescribeArgs ds;
     ds.L = L; ds.kept = da.kept; ds.keptCount = da.keptCount; ds.M = fe->M; ds.kps = d_kps; ds.desc = d_desc; ds.nOut = d_nout; ds.kpCap = fe->kpCap;
-    ds.errFlag = fe->errFlag;
+    ds.errFlag = errFlag;
     mark(fe, st, KIND_DESCRIBE);
     k_describe<<<dim3(cdiv(fe->kpCap, DESC_WARPS), cnt), DESC_WARPS * 32, 0, st>>>(ds);
     mark(fe, st, KIND_END);
@@ -1740,13 +1787,20 @@ static int lanes_for(const cslam_frontend* fe, int batch, int want) {
     return std::max(1, std::min(std::min(want, cslam_frontend::MAX_LANES), batch));
 }
 
-// frames [f0, f0+cnt) of a host fisheye batch, through h_pin_in unless the caller's buffer is page-locked, to `dfe` and warped into level 0
-static int warp_host(cslam_frontend* fe, cudaStream_t st, const uint8_t* in, bool pinIn, uint8_t* dfe, int f0, int cnt) {
+// chunks of a host batch on `nlanes` lanes. The batch is cut into more chunks than there are lanes (chunk c runs on lane c % nlanes): the first
+// upload - the only one nothing overlaps within the call - is then 1/8 of the batch instead of 1/4, and the copy engines stay busy behind the
+// kernels of earlier chunks
+static int host_chunks(const cslam_frontend* fe, int batch, int nlanes) {
+    return fe->timer.on() ? 1 : std::max(nlanes, std::min(cslam_frontend::HOST_CHUNKS, std::max(1, batch / 8)));
+}
+
+// frames [f0, f0+cnt) of a host fisheye batch, through the page-locked hIn unless the caller's buffer is page-locked, to `dfe` on `st`
+static int upload_fisheye(cslam_frontend* fe, cudaStream_t st, const uint8_t* in, bool pinIn, uint8_t* hIn, uint8_t* dfe, int f0, int cnt) {
     const size_t fb = (size_t)fe->cam.Iw * fe->cam.Ih, off = (size_t)f0 * fb;
     const uint8_t* src = in + off;
-    if (!pinIn) { std::memcpy(fe->h_pin_in + off, src, (size_t)cnt * fb); src = fe->h_pin_in + off; }
+    if (!pinIn) { std::memcpy(hIn + off, src, (size_t)cnt * fb); src = hIn + off; }
     CSLAM_CUDA(cudaMemcpyAsync(dfe + off, src, (size_t)cnt * fb, cudaMemcpyHostToDevice, st));
-    return launch_warp(fe, st, dfe + off, f0, cnt);
+    return 0;
 }
 
 extern "C" int cslam_warp(cslam_frontend* fe, const uint8_t* fisheye, int batch, uint8_t* canvas, int canvas_pitch) {
@@ -1756,7 +1810,8 @@ extern "C" int cslam_warp(cslam_frontend* fe, const uint8_t* fisheye, int batch,
     uint8_t* dfe = nullptr;
     if ((rc = prepare_level0(fe, true)) || (rc = fe->arena.take(&dfe, (size_t)batch * fe->cam.Iw * fe->cam.Ih))) return rc;
     rc = enqueue(fe, batch, 1, 1, [&](cudaStream_t st, int f0, int cnt) -> int {
-        if (int rc = warp_host(fe, st, fisheye, is_pinned(fisheye), dfe, f0, cnt)) return rc;
+        int rc = upload_fisheye(fe, st, fisheye, is_pinned(fisheye), fe->h_pin_in, dfe, f0, cnt);
+        if (rc || (rc = launch_warp(fe, st, dfe + (size_t)f0 * fe->cam.Iw * fe->cam.Ih, f0, cnt))) return rc;
         // the reference writes only the five face ROIs; corner tiles of the caller's canvas are left untouched
         const int W = fe->W, pitch = fe->L.g[0].pitch;
         for (int f = f0; f < f0 + cnt; f++)
@@ -1768,39 +1823,58 @@ extern "C" int cslam_warp(cslam_frontend* fe, const uint8_t* fisheye, int batch,
         return 0;
     });
     if (rc) { cudaStreamSynchronize(fe->stream); return rc; }
-    return cslam_frontend_sync(fe);
+    return sync_stream(fe);
 }
 
-// host entry points: H2D -> kernels -> D2H per chunk; caller buffers are used directly when they are page-locked. The caller has reset the arena.
-static int run_host(cslam_frontend* fe, const uint8_t* in, int inPitch, bool fromWarp, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
+static HostBatch host_batch(const uint8_t* in, int inPitch, bool fromWarp, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
+    return HostBatch{in, inPitch, fromWarp, kps, desc, n_out, is_pinned(in), is_pinned(kps), is_pinned(desc), is_pinned(n_out)};
+}
+
+// One chunk, frames [f0, f0+cnt), of a host batch: upload, k_warp (or the caller's canvases straight into level 0), launch_extract, download.
+// The one sequence of cslam_frontend_run, cslam_orb_extract and cslam_frontend_submit; caller buffers are used directly when they are
+// page-locked. The kernels run on `st`, the copies on s.up / s.down when those are set.
+static int host_chunk(cslam_frontend* fe, const HostBatch& b, const HostStage& s, cudaStream_t st, int f0, int cnt) {
     const size_t nk = (size_t)fe->kpCap;
-    uint8_t* dfe = nullptr; cslam_keypoint* dk = nullptr; uint8_t* dd = nullptr; int32_t* dn = nullptr;
-    int rc;
-    if ((rc = prepare_level0(fe, fromWarp)) || (fromWarp && (rc = fe->arena.take(&dfe, (size_t)batch * fe->cam.Iw * fe->cam.Ih))) ||
-        (rc = fe->arena.take(&dk, batch * nk)) || (rc = fe->arena.take(&dd, batch * nk * 32)) || (rc = fe->arena.take(&dn, (size_t)batch))) return rc;
-    const int nlanes = lanes_for(fe, batch, 4);
-    // the batch is cut into more chunks than there are streams (chunk c runs on stream c % nlanes): the first upload - the only one nothing overlaps -
-    // is then 1/8 of the batch instead of 1/4, and the copy engines stay busy behind the kernels of earlier chunks
-    const int nchunks = fe->timer.on() ? 1 : std::max(nlanes, std::min(cslam_frontend::HOST_CHUNKS, std::max(1, batch / 8)));
-    const bool pinIn = is_pinned(in), pinK = is_pinned(kps), pinD = is_pinned(desc), pinN = is_pinned(n_out);
-    rc = enqueue(fe, batch, nlanes, nchunks, [&](cudaStream_t st, int f0, int cnt) -> int {
+    cudaStream_t up = s.up ? s.up : st, down = s.down ? s.down : st;
+    int rc = 0;
+    if (b.fromWarp) {
+        if ((rc = upload_fisheye(fe, up, b.in, b.pinIn, s.hIn, s.dfe, f0, cnt))) return rc;
+        if (up != st) { CSLAM_CUDA(cudaEventRecord(s.evUp, up)); CSLAM_CUDA(cudaStreamWaitEvent(st, s.evUp, 0)); }
+        if ((rc = launch_warp(fe, st, s.dfe + (size_t)f0 * fe->cam.Iw * fe->cam.Ih, f0, cnt))) return rc;
+    } else {   // level 0 is shared by every call: it is written in the order of the kernels, on `st`
         const int pitch = fe->L.g[0].pitch;
-        int rc = 0;
-        if (fromWarp) rc = warp_host(fe, st, in, pinIn, dfe, f0, cnt);
-        else CSLAM_CUDA(cudaMemcpy2DAsync(fe->L.img[0] + (size_t)f0 * pitch * fe->CH, pitch, in + (size_t)f0 * inPitch * fe->CH, inPitch, fe->CW, (size_t)fe->CH * cnt,
-                                          cudaMemcpyHostToDevice, st));
-        if (rc || (rc = launch_extract(fe, st, f0, cnt, dk + (size_t)f0 * nk, dd + (size_t)f0 * nk * 32, dn + f0, fromWarp))) return rc;
-        CSLAM_CUDA(cudaMemcpyAsync((pinK ? kps : fe->h_pin_kps) + (size_t)f0 * nk, dk + (size_t)f0 * nk, (size_t)cnt * nk * sizeof(cslam_keypoint), cudaMemcpyDeviceToHost, st));
-        CSLAM_CUDA(cudaMemcpyAsync((pinD ? desc : fe->h_pin_desc) + (size_t)f0 * nk * 32, dd + (size_t)f0 * nk * 32, (size_t)cnt * nk * 32, cudaMemcpyDeviceToHost, st));
-        CSLAM_CUDA(cudaMemcpyAsync((pinN ? n_out : fe->h_pin_n) + f0, dn + f0, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        return 0;
-    });
+        CSLAM_CUDA(cudaMemcpy2DAsync(fe->L.img[0] + (size_t)f0 * pitch * fe->CH, pitch, b.in + (size_t)f0 * b.inPitch * fe->CH, b.inPitch, fe->CW,
+                                     (size_t)fe->CH * cnt, cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = launch_extract(fe, st, f0, cnt, s.dk + (size_t)f0 * nk, s.dd + (size_t)f0 * nk * 32, s.dn + f0, b.fromWarp, s.errFlag))) return rc;
+    if (down != st) { CSLAM_CUDA(cudaEventRecord(s.evRun, st)); CSLAM_CUDA(cudaStreamWaitEvent(down, s.evRun, 0)); }
+    CSLAM_CUDA(cudaMemcpyAsync((b.pinK ? b.kps : s.hKps) + (size_t)f0 * nk, s.dk + (size_t)f0 * nk, (size_t)cnt * nk * sizeof(cslam_keypoint), cudaMemcpyDeviceToHost, down));
+    CSLAM_CUDA(cudaMemcpyAsync((b.pinD ? b.desc : s.hDesc) + (size_t)f0 * nk * 32, s.dd + (size_t)f0 * nk * 32, (size_t)cnt * nk * 32, cudaMemcpyDeviceToHost, down));
+    CSLAM_CUDA(cudaMemcpyAsync((b.pinN ? b.n : s.hN) + f0, s.dn + f0, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, down));
+    return 0;
+}
+
+// the pageable outputs of a finished host batch, out of their page-locked staging
+static void copy_out(const cslam_frontend* fe, const HostBatch& b, const HostStage& s, int batch) {
+    const size_t tot = (size_t)batch * fe->kpCap;
+    if (!b.pinK) std::memcpy(b.kps, s.hKps, tot * sizeof(cslam_keypoint));
+    if (!b.pinD) std::memcpy(b.desc, s.hDesc, tot * 32);
+    if (!b.pinN) std::memcpy(b.n, s.hN, batch * sizeof(int32_t));
+}
+
+// the synchronous host entry points, staged through the arena and h_pin_*; the caller has reset the arena
+static int run_host(cslam_frontend* fe, const HostBatch& b, int batch) {
+    const size_t nk = (size_t)fe->kpCap;
+    HostStage s = {};
+    s.hIn = fe->h_pin_in; s.hKps = fe->h_pin_kps; s.hDesc = fe->h_pin_desc; s.hN = fe->h_pin_n; s.errFlag = fe->errFlag;
+    int rc;
+    if ((rc = prepare_level0(fe, b.fromWarp)) || (b.fromWarp && (rc = fe->arena.take(&s.dfe, (size_t)batch * fe->cam.Iw * fe->cam.Ih))) ||
+        (rc = fe->arena.take(&s.dk, batch * nk)) || (rc = fe->arena.take(&s.dd, batch * nk * 32)) || (rc = fe->arena.take(&s.dn, (size_t)batch))) return rc;
+    const int nlanes = lanes_for(fe, batch, cslam_frontend::MAX_LANES);
+    rc = enqueue(fe, batch, nlanes, host_chunks(fe, batch, nlanes), [&](cudaStream_t st, int f0, int cnt) { return host_chunk(fe, b, s, st, f0, cnt); });
     if (rc) { cudaStreamSynchronize(fe->stream); return rc; }
-    if ((rc = cslam_frontend_sync(fe))) return rc;
-    const size_t tot = (size_t)batch * nk;
-    if (!pinK) std::memcpy(kps, fe->h_pin_kps, tot * sizeof(cslam_keypoint));
-    if (!pinD) std::memcpy(desc, fe->h_pin_desc, tot * 32);
-    if (!pinN) std::memcpy(n_out, fe->h_pin_n, batch * sizeof(int32_t));
+    if ((rc = sync_stream(fe))) return rc;
+    copy_out(fe, b, s, batch);
     return CSLAM_OK;
 }
 
@@ -1809,14 +1883,86 @@ extern "C" int cslam_orb_extract(cslam_frontend* fe, const uint8_t* canvas, int 
     if (rc) return rc;
     if (canvas_pitch < fe->CW) { set_error("cslam_orb_extract: canvas pitch %d is below the canvas width %d", canvas_pitch, fe->CW); return CSLAM_E_BADARG; }
     fe->arena.reset();
-    return run_host(fe, canvas, canvas_pitch, false, batch, kps, desc, n_out);
+    return run_host(fe, host_batch(canvas, canvas_pitch, false, kps, desc, n_out), batch);
 }
 
 extern "C" int cslam_frontend_run(cslam_frontend* fe, const uint8_t* fisheye, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out) {
     int rc = check_batch(fe, "cslam_frontend_run", batch, {fisheye, kps, desc, n_out});
     if (rc) return rc;
     fe->arena.reset();
-    return run_host(fe, fisheye, 0, true, batch, kps, desc, n_out);
+    return run_host(fe, host_batch(fisheye, 0, true, kps, desc, n_out), batch);
+}
+
+// The staging of a pending slot for the buffers of `b`: device buffers, error flag and events on the slot's first use, each page-locked
+// buffer the first time the slot meets a pageable buffer of its kind. Sized for max_batch, so a slot never grows.
+static int slot_stage(cslam_frontend* fe, PendingSlot& p, const HostBatch& b) {
+    HostStage& s = p.s;
+    const size_t B = fe->maxBatch, nk = fe->kpCap, fb = (size_t)fe->cam.Iw * fe->cam.Ih;
+    int rc = 0;
+    if (!p.evDone) {   // made last: a first use that failed half-way starts again
+        if ((rc = dev_alloc(fe->owned, &s.dfe, B * fb, false)) || (rc = dev_alloc(fe->owned, &s.dk, B * nk, false)) ||
+            (rc = dev_alloc(fe->owned, &s.dd, B * nk * 32, false)) || (rc = dev_alloc(fe->owned, &s.dn, B, false)) ||
+            (rc = dev_alloc(fe->owned, &s.errFlag, 1, false)) || (rc = pinned_alloc(fe->pinned, &p.errHost, 1))) return rc;
+        s.up = fe->lane[cslam_frontend::UP_LANE]; s.down = fe->lane[cslam_frontend::DOWN_LANE];
+        CSLAM_CUDA(cudaEventCreateWithFlags(&s.evUp, cudaEventDisableTiming));
+        CSLAM_CUDA(cudaEventCreateWithFlags(&s.evRun, cudaEventDisableTiming));
+        CSLAM_CUDA(cudaEventCreateWithFlags(&p.evDone, cudaEventDisableTiming));
+    }
+    if ((!b.pinIn && !s.hIn && (rc = pinned_alloc(fe->pinned, &s.hIn, B * fb))) || (!b.pinK && !s.hKps && (rc = pinned_alloc(fe->pinned, &s.hKps, B * nk))) ||
+        (!b.pinD && !s.hDesc && (rc = pinned_alloc(fe->pinned, &s.hDesc, B * nk * 32))) || (!b.pinN && !s.hN && (rc = pinned_alloc(fe->pinned, &s.hN, B)))) return rc;
+    return 0;
+}
+
+// Enqueues slot p's batch. Its kernels run on the kernel lanes, forked from the handle's stream and joined back: they follow every earlier
+// call's kernels, which share the pyramid levels, candidate and kept lists and counters, and every later call's kernels follow them. The
+// uploads (UP_LANE) wait for nothing: the slot's staging is free once its previous ticket was waited. The downloads (DOWN_LANE) wait for their
+// chunk's kernels only, so the next call's kernels do not wait for them. The ticket's error flag is copied after its last kernel.
+static int enqueue_ticket(cslam_frontend* fe, PendingSlot& p, int batch) {
+    const HostStage& s = p.s;
+    CSLAM_CUDA(cudaMemsetAsync(s.errFlag, 0, sizeof(int), fe->stream));
+    const int nlanes = lanes_for(fe, batch, cslam_frontend::MAX_LANES);
+    const int rc = enqueue(fe, batch, nlanes, host_chunks(fe, batch, nlanes), [&](cudaStream_t st, int f0, int cnt) { return host_chunk(fe, p.b, s, st, f0, cnt); });
+    if (rc) return rc;
+    CSLAM_CUDA(cudaEventRecord(s.evRun, fe->stream));
+    CSLAM_CUDA(cudaStreamWaitEvent(s.down, s.evRun, 0));
+    CSLAM_CUDA(cudaMemcpyAsync(p.errHost, s.errFlag, sizeof(int), cudaMemcpyDeviceToHost, s.down));
+    CSLAM_CUDA(cudaEventRecord(p.evDone, s.down));
+    return 0;
+}
+
+extern "C" int cslam_frontend_submit(cslam_frontend* fe, const uint8_t* fisheye, int batch, cslam_keypoint* kps, uint8_t* desc, int32_t* n_out,
+                                     int64_t* ticket) {
+    int rc = check_batch(fe, "cslam_frontend_submit", batch, {fisheye, kps, desc, n_out, ticket});
+    if (rc) return rc;
+    if (!fe->d_wtiles) { set_error("cslam_frontend_submit: this front end was created without fisheye geometry (Iw/Ih = 0): no warp"); return CSLAM_E_BADARG; }
+    PendingSlot* p = nullptr;
+    for (PendingSlot& q : fe->slot) if (!q.ticket) { p = &q; break; }
+    if (!p) { set_error("cslam_frontend_submit: %d tickets are pending; wait for one first", CSLAM_FRONTEND_MAX_PENDING); return CSLAM_E_BADARG; }
+    p->b = host_batch(fisheye, 0, true, kps, desc, n_out); p->batch = batch;
+    if ((rc = slot_stage(fe, *p, p->b))) return rc;
+    if ((rc = prepare_level0(fe, true)) || (rc = enqueue_ticket(fe, *p, batch))) {
+        cudaStreamSynchronize(fe->stream); cudaStreamSynchronize(p->s.up); cudaStreamSynchronize(p->s.down);
+        return rc;
+    }
+    p->ticket = *ticket = ++fe->lastTicket;
+    return CSLAM_OK;
+}
+
+extern "C" int cslam_frontend_wait(cslam_frontend* fe, int64_t ticket) {
+    PendingSlot* p = nullptr;
+    if (fe && ticket > 0)
+        for (PendingSlot& q : fe->slot) if (q.ticket == ticket) p = &q;
+    if (!p) { set_error("cslam_frontend_wait: ticket %lld is not pending", (long long)ticket); return CSLAM_E_BADARG; }
+    p->ticket = 0;   // waited, whatever the outcome
+    CSLAM_CUDA(cudaSetDevice(fe->device));
+    CSLAM_CUDA(cudaEventSynchronize(p->evDone));
+    if (fe->timer.on()) {   // the timer's events are on the kernel lanes, joined into the handle's stream
+        CSLAM_CUDA(cudaStreamSynchronize(fe->stream));
+        fe->timer.collect();
+    }
+    if (*p->errHost) { set_error("%s", kOverflowMessage); return *p->errHost; }
+    copy_out(fe, p->b, p->s, p->batch);
+    return CSLAM_OK;
 }
 
 // returns without synchronising, so it takes nothing from the arena
@@ -1827,7 +1973,7 @@ extern "C" int cslam_frontend_run_dev(cslam_frontend* fe, const uint8_t* fisheye
     const size_t nk = (size_t)fe->kpCap, fsz = (size_t)fe->cam.Iw * fe->cam.Ih;
     return enqueue(fe, batch, nlanes, nlanes, [&](cudaStream_t st, int f0, int cnt) -> int {
         const int rc = launch_warp(fe, st, fisheye_dev + (size_t)f0 * fsz, f0, cnt);
-        return rc ? rc : launch_extract(fe, st, f0, cnt, kps_dev + (size_t)f0 * nk, desc_dev + (size_t)f0 * nk * 32, n_out_dev + f0, true);
+        return rc ? rc : launch_extract(fe, st, f0, cnt, kps_dev + (size_t)f0 * nk, desc_dev + (size_t)f0 * nk * 32, n_out_dev + f0, true, fe->errFlag);
     });
 }
 

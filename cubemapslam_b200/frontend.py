@@ -2,7 +2,8 @@
 
   System::CvtFisheyeToCubeMap_reverseQuery_withInterpolation  (reference src/System.cpp:327-355)  -> FrontEnd.warp
   ORBextractor::operator()                                     (reference src/ORBExtractor.cpp:838-926) -> FrontEnd.extract
-FrontEnd.run / run_dev fuse both for batches (BASELINE config 2). PyTorch is only used by callers for device memory."""
+FrontEnd.run / run_dev fuse both for batches (BASELINE config 2); submit_raw / wait are run_raw in two halves, so that one batch computes while the
+next uploads and the previous downloads. PyTorch is only used by callers for device memory."""
 import ctypes as C
 
 import numpy as np
@@ -22,6 +23,7 @@ class FrontEnd(_capi.Handle):
         self.CW, self.CH = 3 * self.cam.face_w, 3 * self.cam.face_h
         if mask.shape != (self.CH, self.CW):
             raise ValueError("mask must be %dx%d (same size as the cubemap canvas, reference src/ORBExtractor.cpp:848)" % (self.CH, self.CW))
+        self._pending = {}   # ticket -> the arrays of a submitted batch, kept alive until it is waited or the handle is closed
         super().__init__(int(device), C.byref(self.cam), C.byref(self.orb), ptr(mask), mask.shape[1], int(max_batch))
         self.max_batch = max_batch
         self.kp_cap = lib().cslam_frontend_kp_capacity(self._h)
@@ -65,6 +67,26 @@ class FrontEnd(_capi.Handle):
     def run_raw(self, fisheye, kps, desc, n):
         """Batched host call into caller-provided (pinned) buffers; no per-frame splitting."""
         check(lib().cslam_frontend_run(self._h, ptr(fisheye), int(fisheye.shape[0]), ptr(kps), ptr(desc), ptr(n)))
+
+    def submit_raw(self, fisheye, kps, desc, n):
+        """run_raw's batch, enqueued without waiting: returns the ticket to wait() on. The four arrays are referenced here until then, as the
+        GPU reads a page-locked input and writes the outputs until the ticket is waited."""
+        t = C.c_int64()
+        check(lib().cslam_frontend_submit(self._h, ptr(fisheye), int(fisheye.shape[0]), ptr(kps), ptr(desc), ptr(n), C.byref(t)))
+        self._pending[t.value] = (fisheye, kps, desc, n)
+        return t.value
+
+    def wait(self, ticket):
+        """Waits for a submitted batch; its buffers then hold what run_raw writes. Raises for the ticket's own errors; the ticket is waited
+        either way."""
+        try:
+            check(lib().cslam_frontend_wait(self._h, C.c_int64(int(ticket))))
+        finally:
+            self._pending.pop(int(ticket), None)
+
+    def close(self):
+        super().close()   # waits for the pending tickets' device work
+        self._pending = {}
 
     # ---- device-resident path (addresses as ints, e.g. torch.Tensor.data_ptr())
     def run_dev(self, fisheye_dev, batch, kps_dev, desc_dev, n_dev):

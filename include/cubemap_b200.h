@@ -8,7 +8,8 @@
  * Conventions: every function returns 0 on success or a negative CSLAM_E_* code (cslam_last_error() gives the
  * text, thread-local); no exceptions cross the ABI; the caller owns every buffer it passes; the library owns
  * device memory and streams; "_dev" entry points take DEVICE pointers and run asynchronously on the handle's
- * stream (cslam_*_sync to wait), all others take HOST pointers and are synchronous. There is no CPU fallback:
+ * stream (cslam_*_sync to wait); cslam_frontend_submit takes HOST pointers and returns before the GPU is done
+ * (cslam_frontend_wait to collect); all others take HOST pointers and are synchronous. There is no CPU fallback:
  * without a CUDA device creation fails with CSLAM_E_NODEVICE.
  */
 #ifndef CUBEMAP_B200_H
@@ -77,6 +78,32 @@ int cslam_frontend_run(cslam_frontend* fe, const uint8_t* fisheye, int batch, cs
 /* Same with device-resident input and output (asynchronous on the front end's stream). */
 int cslam_frontend_run_dev(cslam_frontend* fe, const uint8_t* fisheye_dev, int batch, cslam_keypoint* kps_dev,
                            uint8_t* desc_dev, int32_t* n_out_dev);
+/* cslam_frontend_run in two halves, so that one batch computes while the next uploads and the previous downloads:
+ * submit batch i+1, then wait for batch i.
+ * - Buffers: the arguments and layout of cslam_frontend_run. When wait(ticket) returns 0 they hold exactly the bytes
+ *   cslam_frontend_run writes for the same frames; rows past n_out[f] are unspecified.
+ * - submit checks everything before it enqueues anything (null buffers, batch outside 1..max_batch, a front end made
+ *   without fisheye geometry, the pending limit), then enqueues the batch and returns without waiting for the GPU. On
+ *   any error no ticket is issued and nothing is enqueued.
+ * - Input: a pageable `fisheye` is copied into library staging before submit returns, so it may be reused at once; a
+ *   page-locked one is read by the copy engine until wait returns.
+ * - Output: kps, desc and n_out, pageable or page-locked, are written until wait returns (pageable ones inside wait).
+ * - At most CSLAM_FRONTEND_MAX_PENDING tickets are submitted and not yet waited; one more submit is CSLAM_E_BADARG.
+ * - Tickets are positive and increase per front end. Pending tickets may be waited in any order; waiting on a ticket
+ *   that was never issued or was already waited is CSLAM_E_BADARG.
+ * - A fixed-capacity overflow in a ticket's kernels is returned by that ticket's wait (CSLAM_E_CAPACITY), never by
+ *   another ticket's wait nor by cslam_frontend_sync. The ticket is waited either way.
+ * - Calls take effect in call order: any other call made while tickets are pending gives the bytes it gives on a fresh
+ *   front end. cslam_frontend_get_level / _get_candidates show the most recently enqueued batch; cslam_frontend_sync
+ *   waits for all enqueued work, pending tickets included, and reports only the front end's own errors.
+ * - With timing on, a submitted batch runs as one lane and one chunk, like a timed cslam_frontend_run; its kernels are
+ *   accumulated when it is waited.
+ * - cslam_frontend_destroy with tickets pending waits for their device work, writes nothing more to pageable outputs,
+ *   and frees everything. */
+#define CSLAM_FRONTEND_MAX_PENDING 2
+int cslam_frontend_submit(cslam_frontend* fe, const uint8_t* fisheye, int batch, cslam_keypoint* kps, uint8_t* desc,
+                          int32_t* n_out, int64_t* ticket);
+int cslam_frontend_wait(cslam_frontend* fe, int64_t ticket);
 /* Debug / stage-parity access (host copies of the last batch's intermediates). level image is apron-less. */
 int cslam_frontend_level_size(const cslam_frontend* fe, int level, int* w, int* h);
 int cslam_frontend_get_level(cslam_frontend* fe, int frame, int level, uint8_t* out /* h*w */);
