@@ -20,17 +20,16 @@ def available(variant="libref.so"):
     return os.path.exists(os.path.join(_HERE, "_ref", variant))
 
 
-def build():
+def build(target="ref"):
     """Only possible where the reference tree is present (the build container)."""
     if os.path.isdir(os.environ.get("REF", "/root/reference")):
-        subprocess.check_call(["make", "-s", "-j8", "-C", _HERE, "ref"])
+        subprocess.check_call(["make", "-s", "-j8", "-C", _HERE, target])
 
 
 def lib(variant="libref.so"):
     if variant not in _LIBS:
         path = os.path.join(_HERE, "_ref", variant)
-        if not os.path.exists(path):
-            build()
+        build("_ref/" + variant)       # where the reference tree exists, make brings the library up to date with its sources' contents
         L = C.CDLL(path)
         for name, t in (("ref_orb_create", C.c_void_p), ("ref_frame_from_image", C.c_void_p), ("ref_voc_load", C.c_void_p), ("ref_cos_fov_th", C.c_float),
                         ("ref_vector_sigma", C.c_float), ("ref_arena_used", C.c_size_t), ("ref_warp_extract_batch_out", C.c_long)):
@@ -91,6 +90,13 @@ class Ref:
         n = self._cam().ref_search_by_projection_local(len(kF), _p(kF), _p(a[0]), len(a[1]), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), C.c_float(th),
                                                   C.c_float(nnratio), _p(match))
         return n, match
+
+    def frame_index(self, kps):
+        """Rays, mGrid sizes (5 x 50 x 50) and the cell contents in (face, col, row) order of a Frame holding the given key points."""
+        kps = np.ascontiguousarray(kps); n = len(kps)
+        rays = np.zeros((n, 3), np.float32); count = np.zeros((5, 50, 50), np.int32); idx = np.zeros(max(n, 1), np.int32)
+        self._cam().ref_frame_index(n, _p(kps), _p(rays), _p(count), _p(idx))
+        return rays, count, idx[:int(count.sum())].copy()
 
     def ray_to_cubemap(self, xyz):
         xyz = _f32(xyz).reshape(-1, 3); uv = np.zeros((len(xyz), 2), np.float32); faces = np.zeros(len(xyz), np.int32)

@@ -171,6 +171,18 @@ int ref_frame_features_in_area(void* fv, float x, float y, float r, int minLevel
     return (int)v.size();
 }
 
+// Frame::ComputeKeyPointRays + AssignFeaturesToGrid of GIVEN key points (scene::make_frame): rays, mGrid sizes, and the mGrid cell contents
+// concatenated in (face, col, row) order. Every key point must lie on a face (ComputeKeyPointRays exits otherwise), and its cell corner on
+// the same face (PosInGrid asserts otherwise).
+void ref_frame_index(int n, const KpPOD* kps, float* rays, int32_t* gridCount, int32_t* cellIdx) {
+    Frame* F = make_frame(n, kps, NULL, NULL);
+    read_frame(*F, n, NULL, NULL, rays, gridCount);
+    int m = 0;
+    for (int f = 0; f < CUBEMAP_FACES; f++) for (int x = 0; x < CUBEFACE_GRID_COLS; x++) for (int y = 0; y < CUBEFACE_GRID_ROWS; y++)
+        for (size_t j = 0; j < F->mGrid[f][x][y].size(); j++) cellIdx[m++] = (int32_t)F->mGrid[f][x][y][j];
+    delete F;
+}
+
 // ---- projection matchers of the reference on objects built from flat arrays (what Tracking holds after Frame::Frame)
 // ORBMatcher(0.9, checkOri).SearchByProjection(CurrentFrame, LastFrame, th, true)   src/ORBMatcher.cpp:130-251
 int ref_search_by_projection_last(int nCur, const KpPOD* kCur, const uint8_t* dCur, const float* TcwCur, int nLast, const KpPOD* kLast, const float* TcwLast,

@@ -7,6 +7,7 @@ import pytest
 from cubemapslam_b200 import config, synth
 
 from oracle import ref
+from tests import test_gpu_tracking_limits as L
 from tests.refrecord import LIVE, RefRecord, same
 
 REC = RefRecord("oracle_frame_index")
@@ -83,3 +84,22 @@ def test_features_in_area_all_wraparound_cases(oracle, frame):
     assert same(lens, rlens) and same(np.concatenate(got).astype(np.int32), rall)
     assert lens[-1] == 0
     assert (lens[:-1] > 0).sum() > 0.2 * (len(queries) - 1)
+
+
+@pytest.mark.parametrize("W,name,over", [(650, "front_cam_params", {}), (450, "lafida_cam0_params", {"CubeFace_w": 450, "CubeFace_h": 450}), (610, "front_cam_params", {"CubeFace_w": 610, "CubeFace_h": 610})])
+def test_rays_and_grid_of_given_key_points(oracle, W, name, over):
+    """The frames of tests/test_gpu_tracking_limits.py (seams, the float below each seam, cell edges, a 300-key-point cell, n = 0 / 257 /
+    4096) through the reference's Frame: rays bit for bit, mGrid sizes and contents. Key points off the faces are left out here
+    (ComputeKeyPointRays exits on them), and so are key points whose cell corner lies on another face (the debug build's PosInGrid asserts;
+    x = 1949.9999 at W = 650 is one): the GPU file compares those with the oracle only."""
+    cp = oracle.cam_params(config.camera(name, **over))
+    r = ref.Ref(cp) if LIVE else None
+    for i, (k, n) in enumerate(L.index_frames(W, with_off=False)):
+        k = k[:min(n, 4096)]
+        assert all(L.ref_safe(x, y, W) for x, y in zip(k["x"], k["y"])), i
+        rrays, rcount, ridx = REC("given_%d_%d" % (W, i), lambda: r.frame_index(k), digest=(0, 1, 2))
+        rays, _ = oracle.key_point_rays(k, W, W)
+        start, idx = oracle.FrameGrid(k, W, W).csr()
+        assert same(rays, rrays), i
+        assert same(np.diff(start).reshape(5, 50, 50).astype(np.int32), rcount), i
+        assert same(idx.astype(np.int32), ridx), i

@@ -7,6 +7,7 @@ import pytest
 from cubemapslam_b200 import config, synth
 
 from oracle import ref
+from tests import test_gpu_tracking_limits as L
 from tests.refrecord import LIVE, RefRecord, same
 
 REC = RefRecord("oracle_projection")
@@ -73,3 +74,60 @@ def test_search_by_projection_local_map(oracle, cam, seed, th, nn):
     n2, m2 = REC("local_map_%d" % seed, run, digest=(1,))
     assert n1 == n2 and n1 > 200
     assert same(np.asarray(m1, np.int32), m2)
+
+
+# ---- the scenes of tests/test_gpu_tracking_limits.py: ties, thresholds, gates, projections, taken slots, histograms and sizes
+CAMS = {650: dict(name="front_cam_params", Camera_Ih=1024, Camera_v0=512.0), 450: dict(name="lafida_cam0_params", CubeFace_w=450, CubeFace_h=450),
+        610: dict(name="front_cam_params", Camera_Ih=1024, Camera_v0=512.0, CubeFace_w=610, CubeFace_h=610)}
+
+
+@pytest.fixture(scope="module", params=sorted(CAMS))
+def cam_w(request, oracle):
+    W = request.param
+    c = dict(CAMS[W]); name = c.pop("name")
+    cp = oracle.cam_params(config.camera(name, **c))
+    r = ref.Ref(cp) if LIVE else None
+    cth = float(REC("cos_fov_th_%d" % W, lambda: r.cos_fov_th()))
+    assert np.float32(cth) == L.cos_fov_th()                  # the GPU file's field-of-view threshold is the camera's
+    return W, r, np.float32(cth)
+
+
+def reference_can_take(a):
+    """Every key point on a face with its cell corner on the same face: ComputeKeyPointRays exits and the debug build's PosInGrid asserts
+    otherwise."""
+    return all(L.ref_safe(x, y, a["W"]) for x, y in zip(a["k"]["x"], a["k"]["y"])) and all(L.ref_safe(x, y, a["W"]) for x, y in zip(a["kl"]["x"], a["kl"]["y"]))
+
+
+@pytest.mark.parametrize("ori", [True, False])
+def test_search_by_projection_last_limits(oracle, cam_w, ori):
+    W, r, cth = cam_w
+    for i, P in enumerate(L.last_batch(oracle, W)):
+        a = P.arrays()
+        assert reference_can_take(a), i
+
+        def run():
+            n2, m2 = r.search_by_projection_last(a["k"], a["d"], a["T"], a["kl"], a["T"], a["valid"], a["Xw"], a["dq"], a["obs"], a["taken"], L.TH_LAST, ori)
+            return n2, np.where(m2 == -2, -1, m2)
+        n2, m2 = REC("limits_last_%d_%d_%d" % (W, i, ori), run, digest=(1,))
+        n1, m1 = L.oracle_search(oracle, a, 0, cth, ori)
+        assert n1 == n2, (i, n1, n2)
+        assert same(np.asarray(m1, np.int32), m2), i
+
+
+@pytest.mark.parametrize("nn", L.NNRATIOS)
+def test_search_by_projection_local_limits(oracle, cam_w, nn):
+    W, r, _ = cam_w
+    pairs = [(P, L.TH_LOCAL) for P in L.local_batch(oracle, W, nn)]
+    if nn == 0.8:
+        pairs += [(L.radius_pair(oracle, W, th), th) for th in (1.0, float(np.nextafter(np.float32(1), np.float32(2))))]
+    for i, (P, th) in enumerate(pairs):
+        a = P.arrays()
+        assert reference_can_take(a), i
+
+        def run():
+            n2, m2 = r.search_by_projection_local(a["k"], a["d"], a["valid"], a["proj"], a["level"], a["vcos"], a["dq"], a["obs"], a["taken"], th, nn)
+            return n2, np.where(m2 == -2, -1, m2)
+        n2, m2 = REC("limits_local_%d_%s_%d" % (W, nn, i), run, digest=(1,))
+        n1, m1 = L.oracle_search(oracle, a, 1, nn=nn, th=th)
+        assert n1 == n2, (i, n1, n2)
+        assert same(np.asarray(m1, np.int32), m2), i
