@@ -8,6 +8,13 @@
 //                 output word id, leaf node, FeatureVector node (level L - levelsup)
 // k_bow_vector    CTA per frame: the BowVector std::map restated as sort by (word, feature index) + in-order segment sums (double, the order
 //                 addWeight sees) + the L1 normalisation summed in word order like BowVector::normalize -> bit-identical doubles
+// k_bow_vector_fv CTA of 1024 threads per frame, up to 16384 features (the initialisation extractor's key frames reach 3*nFeatures + 3*nlevels,
+//                 9024 at 3000 features): the BowVector as k_bow_vector builds it, then the FeatureVector (std::map<NodeId, std::vector<unsigned>>)
+//                 as a second sort of the same live features by (node, feature index), written as CSR: node ascending, indices ascending.
+//                 Keys are 64-bit, id << 14 | index: a word id needs 20 bits and an index 14, one more than the 32-bit keys of k_bow_vector hold.
+//                 One CTA per frame keeps both sorts and every segment on chip: 16384 keys x 8 B + 16384 ranks x 4 B = 192 KB of shared
+//                 memory, inside the 227 KB an sm_90 CTA may use, and no cross-CTA merge. A call is two launches (k_bow_descend, k_bow_vector_fv)
+//                 whatever the number of frames.
 #include <cstring>
 #include <vector>
 #include "common.cuh"
@@ -91,6 +98,84 @@ __global__ void __launch_bounds__(256) k_bow_vector(VocDev V, const int32_t* __r
     if (norm > 0.0) for (int i = tid; i < nWords; i += 256) bowVal[o + i] = bowVal[o + i] / norm;
 }
 
+// exclusive scan of the segment starts of the sorted keys (segment = key >> FV_IDX_BITS; all-ones keys are dead and sort last): rank[p] = output
+// slot of the segment starting at p, all-ones elsewhere. Returns the number of segments. blockDim.x = 1024.
+constexpr int FV_IDX_BITS = 14;
+constexpr unsigned long long FV_DEAD = ~0ull;
+__device__ int fv_segment_ranks(const unsigned long long* key, uint32_t* rank, int n2, uint32_t* wsum, uint32_t& carry) {
+    const int tid = threadIdx.x;
+    if (tid == 0) carry = 0;
+    __syncthreads();
+    for (int base = 0; base < n2; base += 1024) {
+        const int p = base + tid;
+        const uint32_t x = (p < n2 && key[p] != FV_DEAD && (p == 0 || (key[p - 1] >> FV_IDX_BITS) != (key[p] >> FV_IDX_BITS))) ? 1u : 0u;
+        uint32_t s = x;
+#pragma unroll
+        for (int sh = 1; sh < 32; sh <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, s, sh); if ((tid & 31) >= sh) s += t; }
+        if ((tid & 31) == 31) wsum[tid >> 5] = s;
+        __syncthreads();
+        uint32_t pre = carry;
+        for (int w = 0; w < (tid >> 5); w++) pre += wsum[w];
+        if (p < n2) rank[p] = x ? pre + s - 1 : 0xffffffffu;
+        __syncthreads();
+        if (tid == 1023) carry = pre + s;
+        __syncthreads();
+    }
+    return (int)carry;
+}
+
+// BowVector + FeatureVector of frames of up to 16384 features from k_bow_descend's word / leaf / node. Per frame f: bow_word / bow_val at
+// f*stride (bowCount[f] entries), fv_node at f*stride (fvCount[f] nodes), fv_start at f*(stride+1) (fvCount[f] + 1 offsets into fv_feat),
+// fv_feat at f*stride (the live features, grouped by node).
+__global__ void __launch_bounds__(1024) k_bow_vector_fv(VocDev V, const int32_t* __restrict__ n, int stride, int n2, const int32_t* __restrict__ word,
+                                                        const int32_t* __restrict__ leaf, const int32_t* __restrict__ node, int32_t* __restrict__ bowWord,
+                                                        double* __restrict__ bowVal, int32_t* __restrict__ bowCount, int32_t* __restrict__ fvNode,
+                                                        int32_t* __restrict__ fvStart, int32_t* __restrict__ fvFeat, int32_t* __restrict__ fvCount) {
+    extern __shared__ unsigned long long key64[];   // n2 keys, then n2 ranks
+    uint32_t* rank = reinterpret_cast<uint32_t*>(key64 + n2);
+    __shared__ uint32_t wsum[32], carry;
+    __shared__ double norm;
+    const int f = blockIdx.x, tid = threadIdx.x, nf = min(n[f], stride);
+    const size_t o = (size_t)f * stride, os = (size_t)f * (stride + 1);
+    // 1. BowVector: sort by (word, index); stopped words (node -1) are dead keys
+    for (int i = tid; i < n2; i += 1024)
+        key64[i] = (i < nf && node[o + i] >= 0) ? ((unsigned long long)(uint32_t)word[o + i] << FV_IDX_BITS) | (unsigned)i : FV_DEAD;
+    __syncthreads();
+    block_bitonic_sort(key64, n2);
+    const int nWords = fv_segment_ranks(key64, rank, n2, wsum, carry);
+    // in-order segment sums, feature by feature (BowVector::addWeight); a word is one leaf, so every addend of a segment is that leaf's weight
+    for (int p = tid; p < n2; p += 1024) {
+        if (rank[p] == 0xffffffffu) continue;
+        const unsigned long long w = key64[p] >> FV_IDX_BITS;
+        const double wt = V.weight[leaf[o + (key64[p] & ((1u << FV_IDX_BITS) - 1))]];
+        double s = 0;
+        for (int q = p; q < n2 && key64[q] != FV_DEAD && (key64[q] >> FV_IDX_BITS) == w; q++) s += wt;
+        bowWord[o + rank[p]] = (int32_t)w; bowVal[o + rank[p]] = s;
+    }
+    __syncthreads();
+    if (tid == 0) {   // BowVector::normalize(L1): norm += fabs(value) in word order
+        double s = 0;
+        for (int i = 0; i < nWords; i++) s += fabs(bowVal[o + i]);
+        norm = s; bowCount[f] = nWords;
+    }
+    __syncthreads();
+    if (norm > 0.0) for (int i = tid; i < nWords; i += 1024) bowVal[o + i] = bowVal[o + i] / norm;
+    // 2. FeatureVector: the same live features sorted by (node, index) -> CSR
+    for (int i = tid; i < n2; i += 1024)
+        key64[i] = (i < nf && node[o + i] >= 0) ? ((unsigned long long)(uint32_t)node[o + i] << FV_IDX_BITS) | (unsigned)i : FV_DEAD;
+    __syncthreads();
+    block_bitonic_sort(key64, n2);
+    const int nNodes = fv_segment_ranks(key64, rank, n2, wsum, carry);
+    for (int p = tid; p < n2; p += 1024) {
+        const unsigned long long kp = key64[p];
+        if (kp == FV_DEAD) continue;
+        fvFeat[o + p] = (int32_t)(kp & ((1u << FV_IDX_BITS) - 1));
+        if (rank[p] != 0xffffffffu) { fvNode[o + rank[p]] = (int32_t)(kp >> FV_IDX_BITS); fvStart[os + rank[p]] = p; }
+        if (p + 1 == n2 || key64[p + 1] == FV_DEAD) fvStart[os + nNodes] = p + 1;   // the last live feature closes the last node
+    }
+    if (tid == 0) { fvCount[f] = nNodes; if (nNodes == 0) fvStart[os] = 0; }
+}
+
 }  // namespace cslam
 
 using namespace cslam;
@@ -134,6 +219,7 @@ extern "C" int cslam_vocabulary_create(cslam_vocabulary** out, int device, int k
         cudaMemcpy(dW, w.data(), (size_t)N * 8, cudaMemcpyHostToDevice) != cudaSuccess) { set_error("vocabulary upload failed"); return fail(CSLAM_E_CUDA); }
     v->V.k = k; v->V.L = L; v->V.nNodes = N; v->V.childStart = dStart; v->V.childList = dList; v->V.desc = dDesc; v->V.weight = dW; v->V.wordId = dWid;
     cudaFuncSetAttribute(k_bow_vector, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4096 * 4);
+    cudaFuncSetAttribute(k_bow_vector_fv, cudaFuncAttributeMaxDynamicSharedMemorySize, CSLAM_BOW_FV_MAX_FEATURES * 12);
     *out = v;
     return CSLAM_OK;
 }
@@ -167,5 +253,44 @@ extern "C" int cslam_bow_transform(cslam_vocabulary* v, const uint8_t* desc, con
     CSLAM_CUDA(cudaMemcpyAsync(bow_word, dBowWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
     CSLAM_CUDA(cudaMemcpyAsync(bow_val, dBowVal, nf * 8, cudaMemcpyDeviceToHost, v->stream));
     CSLAM_CUDA(cudaMemcpyAsync(bow_count, dBowCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
+    return v->sync();
+}
+
+extern "C" int cslam_bow_transform_fv_dev(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* word, int32_t* leaf,
+                                          int32_t* node, int32_t* bow_word, double* bow_val, int32_t* bow_count, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feat,
+                                          int32_t* fv_count) {
+    if (!v || !desc || !n || !word || !leaf || !node || !bow_word || !bow_val || !bow_count || !fv_node || !fv_start || !fv_feat || !fv_count || nframes <= 0 || stride <= 0 ||
+        stride > CSLAM_BOW_FV_MAX_FEATURES) { set_error("cslam_bow_transform_fv_dev: bad argument (stride must be in [1, %d])", CSLAM_BOW_FV_MAX_FEATURES); return CSLAM_E_BADARG; }
+    CSLAM_CUDA(cudaSetDevice(v->device));
+    k_bow_descend<<<dim3(cdiv(stride, 128), nframes), 128, 0, v->stream>>>(v->V, desc, n, stride, levelsup, word, leaf, node);
+    const int n2 = pow2_at_least(stride);
+    k_bow_vector_fv<<<nframes, 1024, (size_t)n2 * 12, v->stream>>>(v->V, n, stride, n2, word, leaf, node, bow_word, bow_val, bow_count, fv_node, fv_start, fv_feat, fv_count);
+    v->launches += 2;
+    CSLAM_CUDA(cudaGetLastError());
+    return CSLAM_OK;
+}
+
+extern "C" int cslam_bow_transform_fv(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* bow_word, double* bow_val,
+                                      int32_t* bow_count, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feat, int32_t* fv_count) {
+    if (!v || !desc || !n || !bow_word || !bow_val || !bow_count || !fv_node || !fv_start || !fv_feat || !fv_count || nframes <= 0 || nframes > v->maxFrames || stride <= 0 ||
+        stride > CSLAM_BOW_FV_MAX_FEATURES) {
+        set_error("cslam_bow_transform_fv: bad argument (nframes must be in [1, max_frames], stride in [1, %d])", CSLAM_BOW_FV_MAX_FEATURES); return CSLAM_E_BADARG;
+    }
+    CSLAM_CUDA(cudaSetDevice(v->device));
+    v->arena.reset();
+    const size_t nf = (size_t)nframes * stride, ns = (size_t)nframes * (stride + 1);
+    const uint8_t* dFeat; const int32_t* dN; int32_t *dWord, *dLeaf, *dNode, *dBowWord, *dBowCount, *dFvNode, *dFvStart, *dFvFeat, *dFvCount; double* dBowVal; int rc;
+    if ((rc = v->arena.upload(&dFeat, desc, nf * 32)) || (rc = v->arena.upload(&dN, n, nframes)) || (rc = v->arena.take(&dWord, nf)) || (rc = v->arena.take(&dLeaf, nf)) ||
+        (rc = v->arena.take(&dNode, nf)) || (rc = v->arena.take(&dBowWord, nf)) || (rc = v->arena.take(&dBowVal, nf)) || (rc = v->arena.take(&dBowCount, nframes)) ||
+        (rc = v->arena.take(&dFvNode, nf)) || (rc = v->arena.take(&dFvStart, ns)) || (rc = v->arena.take(&dFvFeat, nf)) || (rc = v->arena.take(&dFvCount, nframes)) ||
+        (rc = cslam_bow_transform_fv_dev(v, dFeat, dN, stride, nframes, levelsup, dWord, dLeaf, dNode, dBowWord, dBowVal, dBowCount, dFvNode, dFvStart, dFvFeat, dFvCount)))
+        return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(bow_word, dBowWord, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(bow_val, dBowVal, nf * 8, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(bow_count, dBowCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(fv_node, dFvNode, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(fv_start, dFvStart, ns * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(fv_feat, dFvFeat, nf * 4, cudaMemcpyDeviceToHost, v->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(fv_count, dFvCount, (size_t)nframes * 4, cudaMemcpyDeviceToHost, v->stream));
     return v->sync();
 }

@@ -40,14 +40,15 @@ __device__ __forceinline__ void three_maxima(const int* hist, int* keep) {
     for (int i = 0; i < HISTO_BINS; i++) keep[i] = (i == ind1 || i == ind2 || i == ind3);
 }
 
-// Block-wide ascending bitonic sort of n2 u32 keys in shared memory, n2 a power of two; every thread of the block calls it
-__device__ inline void block_bitonic_sort(uint32_t* key, int n2) {
+// Block-wide ascending bitonic sort of n2 unsigned keys (u32 or u64) in shared memory, n2 a power of two; every thread of the block calls it
+template <class K>
+__device__ inline void block_bitonic_sort(K* key, int n2) {
     for (int k = 2; k <= n2; k <<= 1)
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int t = threadIdx.x; t < n2; t += blockDim.x) {
                 const int ixj = t ^ j;
                 if (ixj > t) {
-                    const uint32_t a = key[t], b = key[ixj];
+                    const K a = key[t], b = key[ixj];
                     const bool up = (t & k) == 0;
                     if ((a > b) == up) { key[t] = b; key[ixj] = a; }
                 }

@@ -189,6 +189,22 @@ int cslam_bow_transform(cslam_vocabulary* v, const uint8_t* desc, const int32_t*
                         int32_t* bow_word, double* bow_val, int32_t* bow_count);
 int cslam_bow_transform_dev(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* word, int32_t* leaf, int32_t* node,
                             int32_t* bow_word, double* bow_val, int32_t* bow_count);
+/* The same transform with the FeatureVector built too, for frames of up to CSLAM_BOW_FV_MAX_FEATURES features (the initialisation extractor's key
+ * frames have up to 3*nFeatures + 3*nlevels: 9024 at 3000 features), whatever the handle's max_features; cslam_vocabulary_create still takes
+ * max_features <= 4096, which bounds only cslam_bow_transform. The host form takes nframes <= max_frames; stride > CSLAM_BOW_FV_MAX_FEATURES is
+ * CSLAM_E_BADARG in both forms. Two launches per call, whatever nframes. Outputs per frame f (n[f] is clamped to stride):
+ *   bow_word / bow_val at f*stride: the BowVector in map order (bow_count[f] entries), as cslam_bow_transform writes it;
+ *   fv_node at f*stride: the FeatureVector's nodes ascending (fv_count[f] entries);
+ *   fv_start at f*(stride+1): fv_count[f] + 1 offsets; node fv_node[j] holds fv_feat[fv_start[j] .. fv_start[j+1]) of the row at f*stride,
+ *   feature indices ascending - the std::map<NodeId, std::vector<unsigned>> FeatureVector::addFeature builds. A stopped word's feature
+ *   (weight 0) is in neither vector. A leaf shallower than L - levelsup puts its features in node 0.
+ * The _dev form also writes the per-feature word, leaf and node (f*stride) that cslam_bow_transform_dev writes. */
+#define CSLAM_BOW_FV_MAX_FEATURES 16384
+int cslam_bow_transform_fv(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* bow_word, double* bow_val,
+                           int32_t* bow_count, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feat, int32_t* fv_count);
+int cslam_bow_transform_fv_dev(cslam_vocabulary* v, const uint8_t* desc, const int32_t* n, int stride, int nframes, int levelsup, int32_t* word, int32_t* leaf,
+                               int32_t* node, int32_t* bow_word, double* bow_val, int32_t* bow_count, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feat,
+                               int32_t* fv_count);
 
 /* ---------------------------------------------------------------------------------------------- tracker
  * The matcher on the steady-state frame path and the per-frame indexing it needs (SURVEY.md 8(f) rows 1 and 3):
