@@ -7,11 +7,11 @@
 namespace cslam {
 
 // k_frame_index (track.cu) on the caller's stream, counted on the caller's launch counter: rays (optional) and the cell CSR of `nframes`
-// frames of key points. prepare_frame_index() sets the kernel's shared-memory limit on the current device; every handle that launches it
-// calls it once, at create.
+// frames of key points, kpStride <= maxStride (<= 65535: the CSR holds u16 positions and indices). prepare_frame_index() sets the kernel's
+// shared-memory limit on the current device; every handle that launches it calls it once, at create.
 int prepare_frame_index();
 int frame_index(cudaStream_t stream, int64_t& launches, const cslam_keypoint* kps, const int32_t* n, int nframes, int kpStride, int faceW, int faceH, float* rays,
-                uint16_t* cellStart, uint16_t* cellIdx);
+                uint16_t* cellStart, uint16_t* cellIdx, int maxStride = 4096);
 
 // The GetFeaturesInArea window table in constant memory (without -rdc every translation unit that includes this holds its own copy)
 static __constant__ AreaRect c_area[5][9][3] = AREA_TABLE_INIT;

@@ -15,6 +15,8 @@
 // k_search_by_bow     one CTA per pair; both FeatureVectors are rebuilt on the fly by an in-CTA bitonic sort of
 //                     (node, index); one warp walks the KF features of a node in order (the reference's "already
 //                     matched" skip makes that order matter), lanes scan the F features of the node.
+// k_search_by_bow_fv  the same search for key frames past 4096 features, from FeatureVectors given as CSRs (no sort): one warp per KF node,
+//                     the F node found by binary search; the "already matched" state is an int16 per F feature in shared memory.
 #include <cstring>
 #include <vector>
 #include "common.cuh"
@@ -270,19 +272,10 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
                 const int iF = keyF[p] & 0xfff;
                 if (mF[iF] >= 0) continue;
                 if (kfkfMode && !fValid[(size_t)pair * nF + iF]) continue;
-                const int d = hamming256(k0, k1, __ldg(F4 + 2 * iF), __ldg(F4 + 2 * iF + 1));
-                if (d < best1) { best2 = best1; best1 = d; bpos = p; }
-                else if (d < best2) best2 = d;
+                bow_take(hamming256(k0, k1, __ldg(F4 + 2 * iF), __ldg(F4 + 2 * iF + 1)), p, best1, best2, bpos);
             }
-#pragma unroll
-            for (int o = 16; o; o >>= 1) {
-                const int ob1 = __shfl_xor_sync(0xffffffffu, best1, o), ob2 = __shfl_xor_sync(0xffffffffu, best2, o), op = __shfl_xor_sync(0xffffffffu, bpos, o);
-                // merge two partial scans: the winner is the smaller distance, ties go to the earlier list position
-                const bool otherWins = ob1 < best1 || (ob1 == best1 && op < bpos);
-                if (otherWins) { best2 = min(best1, ob2); best1 = ob1; bpos = op; }
-                else best2 = min(best2, ob1);
-            }
-            if ((kfkfMode ? best1 < 50 : best1 <= 50) && (float)best1 < __fmul_rn(nnratio, (float)best2)) {
+            bow_warp_merge(best1, best2, bpos);
+            if (bow_accept(best1, best2, nnratio, kfkfMode)) {
                 const int iF = keyF[bpos] & 0xfff;
                 if (lane == 0) {
                     mF[iF] = iK;
@@ -311,6 +304,80 @@ __global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow(const uint8_t* __
         for (int i = tid; i < nKF; i += BOW_THREADS) out[i] = -1;
         __syncthreads();
         for (int j = tid; j < nF; j += BOW_THREADS) if (mF[j] >= 0) out[mF[j]] = j;
+    }
+    if (tid == 0) nmatches[pair] = total;
+}
+
+// SearchByBoW of key frames up to CSLAM_BOW_FV_MAX_FEATURES features, from FeatureVectors given as CSRs (cslam_bow_transform_fv's layout).
+// One CTA per pair; warp w takes the KF FeatureVector's nodes w, w + 8, ... and finds each node in F's by binary search. Within a node the KF
+// features go in list order and lanes scan the node's F features in list order, as in k_search_by_bow. An F feature sits in one node only,
+// so the warps never share one. Shared memory: the matched KF feature per F feature (int16, -1 = free), 2 * F.stride bytes.
+struct FvSide {
+    const uint8_t* desc; const float* ang; const uint8_t* valid;   // valid: nullptr on the F side of (KeyFrame, Frame)
+    const int32_t* n; int stride;                                  // features of pair p: min(n[p], stride) rows at p*stride
+    const int32_t* node; const int32_t* start; const int32_t* feat; const int32_t* count;   // FeatureVector of pair p, count[p] nodes
+};
+__global__ void __launch_bounds__(BOW_THREADS) k_search_by_bow_fv(FvSide K, FvSide F, float nnratio, int checkOri, int32_t* __restrict__ match,
+                                                                  int32_t* __restrict__ nmatches) {
+    // F.valid == nullptr: (KeyFrame, Frame), match per F feature; else (KeyFrame, KeyFrame), strict TH_LOW, match per KF feature
+    extern __shared__ int16_t taken[];
+    __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total;
+    const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = BOW_THREADS / 32;
+    const bool kfkf = F.valid != nullptr;
+    const int nK = min(K.n[pair], K.stride), nF = min(F.n[pair], F.stride), cK = K.count[pair], cF = F.count[pair];
+    const uint4* K4 = reinterpret_cast<const uint4*>(K.desc + (size_t)pair * K.stride * 32);
+    const uint4* F4 = reinterpret_cast<const uint4*>(F.desc + (size_t)pair * F.stride * 32);
+    const float* aK = K.ang + (size_t)pair * K.stride; const float* aF = F.ang + (size_t)pair * F.stride;
+    const uint8_t* vK = K.valid + (size_t)pair * K.stride; const uint8_t* vF = kfkf ? F.valid + (size_t)pair * F.stride : nullptr;
+    const int32_t* nodeK = K.node + (size_t)pair * K.stride; const int32_t* nodeF = F.node + (size_t)pair * F.stride;
+    const int32_t* startK = K.start + (size_t)pair * (K.stride + 1); const int32_t* startF = F.start + (size_t)pair * (F.stride + 1);
+    const int32_t* featK = K.feat + (size_t)pair * K.stride; const int32_t* featF = F.feat + (size_t)pair * F.stride;
+    for (int j = tid; j < nF; j += BOW_THREADS) taken[j] = -1;
+    if (tid < HISTO_BINS) hist[tid] = 0;
+    if (tid == 0) total = 0;
+    __syncthreads();
+    for (int g = warp; g < cK; g += nwarps) {
+        const int gF = fv_find(nodeF, cF, __ldg(nodeK + g));
+        if (gF < 0) continue;
+        const int fs = __ldg(startF + gF), fe = __ldg(startF + gF + 1), ke = __ldg(startK + g + 1);
+        for (int q = __ldg(startK + g); q < ke; q++) {
+            const int iK = __ldg(featK + q);
+            if (!vK[iK]) continue;
+            const uint4 k0 = __ldg(K4 + 2 * iK), k1 = __ldg(K4 + 2 * iK + 1);
+            int best1 = 256, best2 = 256, bpos = 0x7fffffff;
+            for (int p = fs + lane; p < fe; p += 32) {
+                const int iF = __ldg(featF + p);
+                if (taken[iF] >= 0 || (kfkf && !vF[iF])) continue;
+                bow_take(hamming256(k0, k1, __ldg(F4 + 2 * iF), __ldg(F4 + 2 * iF + 1)), p, best1, best2, bpos);
+            }
+            bow_warp_merge(best1, best2, bpos);
+            if (bow_accept(best1, best2, nnratio, kfkf) && lane == 0) {
+                const int iF = __ldg(featF + bpos);
+                taken[iF] = (int16_t)iK;
+                if (checkOri) atomicAdd(&hist[rot_bin(aK[iK], aF[iF])], 1);
+                atomicAdd(&total, 1);
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    if (checkOri) {
+        if (tid == 0) three_maxima(hist, keep);
+        __syncthreads();
+        for (int j = tid; j < nF; j += BOW_THREADS) {
+            const int m = taken[j];
+            if (m >= 0 && !keep[rot_bin(aK[m], aF[j])]) { taken[j] = -1; atomicSub(&total, 1); }
+        }
+        __syncthreads();
+    }
+    if (!kfkf) {
+        int32_t* out = match + (size_t)pair * F.stride;
+        for (int j = tid; j < F.stride; j += BOW_THREADS) out[j] = j < nF ? taken[j] : -1;
+    } else {
+        int32_t* out = match + (size_t)pair * K.stride;
+        for (int i = tid; i < K.stride; i += BOW_THREADS) out[i] = -1;
+        __syncthreads();
+        for (int j = tid; j < nF; j += BOW_THREADS) if (taken[j] >= 0) out[taken[j]] = j;
     }
     if (tid == 0) nmatches[pair] = total;
 }
@@ -637,4 +704,57 @@ extern "C" int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, co
     CSLAM_CUDA(cudaMemcpyAsync(match12, dMatch, k1 * 4, cudaMemcpyDeviceToHost, m->stream));
     CSLAM_CUDA(cudaMemcpyAsync(nmatches, dNm, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
     return m->sync();
+}
+
+// ------------------------------------------------------------------------------------------------- SearchByBoW from FeatureVector CSRs
+// Both forms of SearchByBoW for key frames of up to CSLAM_BOW_FV_MAX_FEATURES features, whatever the handle's max_features. Host buffers,
+// staged through the arena; every CSR is checked before anything is enqueued.
+static int bow_fv_host(cslam_matcher* m, const char* fn, int npairs, FvSide K, FvSide F, float nnratio, int check_ori, int32_t* match, int32_t* nmatches) {
+    const bool kfkf = F.valid != nullptr;
+    if (!m || npairs <= 0 || npairs > m->maxPairs || K.stride <= 0 || F.stride <= 0 || K.stride > CSLAM_BOW_FV_MAX_FEATURES || F.stride > CSLAM_BOW_FV_MAX_FEATURES ||
+        !K.desc || !K.ang || !K.valid || !K.n || !K.node || !K.start || !K.feat || !K.count || !F.desc || !F.ang || !F.n || !F.node || !F.start || !F.feat || !F.count ||
+        !match || !nmatches) {
+        set_error("%s: bad argument (pairs in [1, %d], strides in [1, %d])", fn, m ? m->maxPairs : 0, CSLAM_BOW_FV_MAX_FEATURES);
+        return CSLAM_E_BADARG;
+    }
+    int bad = 0;
+    const char* why = fv_csr_check(npairs, K.stride, K.n, K.node, K.start, K.feat, K.count, &bad);
+    const char* side = kfkf ? "key frame 1" : "key frame";
+    if (!why) { why = fv_csr_check(npairs, F.stride, F.n, F.node, F.start, F.feat, F.count, &bad); side = kfkf ? "key frame 2" : "frame"; }
+    if (why) { set_error("%s: malformed FeatureVector of the %s of pair %d: %s", fn, side, bad, why); return CSLAM_E_BADARG; }
+    CSLAM_CUDA(cudaSetDevice(m->device));
+    m->arena.reset();
+    DevArena& a = m->arena;
+    const size_t k = (size_t)npairs * K.stride, f = (size_t)npairs * F.stride, out = kfkf ? k : f;
+    FvSide dK = K, dF = F;
+    int32_t *dMatch, *dN; int rc;
+    if ((rc = a.upload(&dK.desc, K.desc, k * 32)) || (rc = a.upload(&dK.ang, K.ang, k)) || (rc = a.upload(&dK.valid, K.valid, k)) || (rc = a.upload(&dK.n, K.n, npairs)) ||
+        (rc = a.upload(&dK.node, K.node, k)) || (rc = a.upload(&dK.start, K.start, k + npairs)) || (rc = a.upload(&dK.feat, K.feat, k)) ||
+        (rc = a.upload(&dK.count, K.count, npairs)) || (rc = a.upload(&dF.desc, F.desc, f * 32)) || (rc = a.upload(&dF.ang, F.ang, f)) ||
+        (kfkf && (rc = a.upload(&dF.valid, F.valid, f))) || (rc = a.upload(&dF.n, F.n, npairs)) || (rc = a.upload(&dF.node, F.node, f)) ||
+        (rc = a.upload(&dF.start, F.start, f + npairs)) || (rc = a.upload(&dF.feat, F.feat, f)) || (rc = a.upload(&dF.count, F.count, npairs)) ||
+        (rc = a.take(&dMatch, out)) || (rc = a.take(&dN, npairs))) return rc;
+    k_search_by_bow_fv<<<npairs, BOW_THREADS, (size_t)F.stride * sizeof(int16_t), m->stream>>>(dK, dF, nnratio, check_ori, dMatch, dN);
+    m->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    CSLAM_CUDA(cudaMemcpyAsync(match, dMatch, out * 4, cudaMemcpyDeviceToHost, m->stream));
+    CSLAM_CUDA(cudaMemcpyAsync(nmatches, dN, (size_t)npairs * 4, cudaMemcpyDeviceToHost, m->stream));
+    return m->sync();
+}
+
+extern "C" int cslam_search_by_bow_fv(cslam_matcher* m, int npairs, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid, const int32_t* n_kf, int kf_stride,
+                                      const int32_t* kf_fv_node, const int32_t* kf_fv_start, const int32_t* kf_fv_feat, const int32_t* kf_fv_count, const uint8_t* descF,
+                                      const float* angF, const int32_t* n_f, int f_stride, const int32_t* f_fv_node, const int32_t* f_fv_start, const int32_t* f_fv_feat,
+                                      const int32_t* f_fv_count, float nnratio, int check_ori, int32_t* match_f, int32_t* nmatches) {
+    return bow_fv_host(m, "cslam_search_by_bow_fv", npairs, {descKF, angKF, kf_valid, n_kf, kf_stride, kf_fv_node, kf_fv_start, kf_fv_feat, kf_fv_count},
+                       {descF, angF, nullptr, n_f, f_stride, f_fv_node, f_fv_start, f_fv_feat, f_fv_count}, nnratio, check_ori, match_f, nmatches);
+}
+
+extern "C" int cslam_search_by_bow_kf_fv(cslam_matcher* m, int npairs, const uint8_t* desc1, const float* ang1, const uint8_t* valid1, const int32_t* n1, int stride1,
+                                         const int32_t* fv_node1, const int32_t* fv_start1, const int32_t* fv_feat1, const int32_t* fv_count1, const uint8_t* desc2,
+                                         const float* ang2, const uint8_t* valid2, const int32_t* n2, int stride2, const int32_t* fv_node2, const int32_t* fv_start2,
+                                         const int32_t* fv_feat2, const int32_t* fv_count2, float nnratio, int check_ori, int32_t* match12, int32_t* nmatches) {
+    if (!valid2) { set_error("cslam_search_by_bow_kf_fv: bad argument (valid2 is required)"); return CSLAM_E_BADARG; }
+    return bow_fv_host(m, "cslam_search_by_bow_kf_fv", npairs, {desc1, ang1, valid1, n1, stride1, fv_node1, fv_start1, fv_feat1, fv_count1},
+                       {desc2, ang2, valid2, n2, stride2, fv_node2, fv_start2, fv_feat2, fv_count2}, nnratio, check_ori, match12, nmatches);
 }

@@ -1,7 +1,9 @@
 // Device-side ORB-matching rules shared by the matcher kernels (match.cu, track.cu, mapping.cu, bow.cu): one definition each, so the
 // reference's exact rounding and tie-breaking live in one place.
 #pragma once
+#include <algorithm>
 #include <cstdint>
+#include <vector>
 
 namespace cslam {
 
@@ -64,6 +66,61 @@ __device__ __forceinline__ int node_lower_bound(const uint32_t* key, int n, uint
     int lo = 0, hi = n;
     while (lo < hi) { const int mid = (lo + hi) >> 1; if (key[mid] < target) lo = mid + 1; else hi = mid; }
     return lo;
+}
+
+// SearchByBoW's candidate scan (src/ORBMatcher.cpp:455-475): feature at list position p with distance d against the running (best1, best2,
+// position of best1). Strict `<`, so of equal distances the first position scanned wins; a lane scans its positions in increasing order.
+__device__ __forceinline__ void bow_take(int d, int p, int& best1, int& best2, int& bpos) {
+    if (d < best1) { best2 = best1; best1 = d; bpos = p; }
+    else if (d < best2) best2 = d;
+}
+// Merges the 32 lanes' partial scans: the winner is the smaller distance, ties go to the earlier list position. Every lane ends with the result.
+__device__ __forceinline__ void bow_warp_merge(int& best1, int& best2, int& bpos) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        const int ob1 = __shfl_xor_sync(0xffffffffu, best1, o), ob2 = __shfl_xor_sync(0xffffffffu, best2, o), op = __shfl_xor_sync(0xffffffffu, bpos, o);
+        const bool otherWins = ob1 < best1 || (ob1 == best1 && op < bpos);
+        if (otherWins) { best2 = min(best1, ob2); best1 = ob1; bpos = op; }
+        else best2 = min(best2, ob1);
+    }
+}
+// SearchByBoW's acceptance: TH_LOW = 50 with `<=` for (KeyFrame, Frame) (:477) and `<` for (KeyFrame, KeyFrame) (:619), then the ratio test in float
+__device__ __forceinline__ bool bow_accept(int best1, int best2, float nnratio, bool strictThLow) {
+    return (strictThLow ? best1 < 50 : best1 <= 50) && (float)best1 < __fmul_rn(nnratio, (float)best2);
+}
+
+// A FeatureVector given as a CSR (cslam_bow_transform_fv's layout: nodes strictly ascending): the position of `node` among node[0, count),
+// or -1 when the FeatureVector does not hold it
+__device__ __forceinline__ int fv_find(const int32_t* __restrict__ node, int count, int32_t target) {
+    int lo = 0, hi = count;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (__ldg(node + mid) < target) lo = mid + 1; else hi = mid; }
+    return lo < count && __ldg(node + lo) == target ? lo : -1;
+}
+
+// Host check of `npairs` FeatureVectors in that CSR layout, pair p at node / feat + p*stride, start + p*(stride+1), with n[p] features (clamped
+// to stride) and count[p] nodes. Returns nullptr, or what is wrong with pair *bad. Each feature may sit in one node only: the searches treat
+// the nodes as independent.
+static inline const char* fv_csr_check(int npairs, int stride, const int32_t* n, const int32_t* node, const int32_t* start, const int32_t* feat,
+                                       const int32_t* count, int* bad) {
+    std::vector<uint8_t> seen(stride);
+    for (int p = 0; p < npairs; p++) {
+        *bad = p;
+        if (n[p] < 0) return "negative feature count";
+        const int nn = n[p] < stride ? n[p] : stride, c = count[p];
+        if (c < 0 || c > stride) return "node count outside [0, stride]";
+        const int32_t* st = start + (size_t)p * (stride + 1); const int32_t* nd = node + (size_t)p * stride; const int32_t* ft = feat + (size_t)p * stride;
+        if (st[0] < 0) return "fv_start below 0";
+        for (int j = 0; j < c; j++) if (st[j + 1] < st[j]) return "fv_start decreases";
+        if (st[c] > nn) return "fv_start exceeds the feature count";
+        if (c && nd[0] < 0) return "negative node id";
+        for (int j = 0; j + 1 < c; j++) if (nd[j + 1] <= nd[j]) return "nodes not strictly ascending";
+        std::fill(seen.begin(), seen.end(), 0);
+        for (int k = st[0]; k < st[c]; k++) {
+            if (ft[k] < 0 || ft[k] >= nn) return "feature index outside [0, feature count)";
+            if (seen[ft[k]]++) return "feature listed twice";
+        }
+    }
+    return nullptr;
 }
 
 // Node ids the keys hold apart: [-1, 2^20 - 1). -1 (a stopped word's feature, in no FeatureVector node) packs to group 0xfffff, which the

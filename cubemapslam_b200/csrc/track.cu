@@ -343,8 +343,8 @@ int cslam::prepare_frame_index() {
     return CSLAM_OK;
 }
 int cslam::frame_index(cudaStream_t stream, int64_t& launches, const cslam_keypoint* kps, const int32_t* n, int nframes, int kpStride, int faceW, int faceH, float* rays,
-                       uint16_t* cellStart, uint16_t* cellIdx) {
-    if (!kps || !n || !cellStart || !cellIdx || nframes <= 0 || kpStride <= 0 || kpStride > 4096 || faceW <= 0 || faceW != faceH) { set_error("cslam_frame_index: bad argument"); return CSLAM_E_BADARG; }
+                       uint16_t* cellStart, uint16_t* cellIdx, int maxStride) {
+    if (!kps || !n || !cellStart || !cellIdx || nframes <= 0 || kpStride <= 0 || kpStride > maxStride || faceW <= 0 || faceW != faceH) { set_error("cslam_frame_index: bad argument"); return CSLAM_E_BADARG; }
     k_frame_index<<<nframes, 256, NCELLS * 4, stream>>>(kps, n, kpStride, faceW, faceH, rays, cellStart, cellIdx); launches++;
     CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;

@@ -3,6 +3,7 @@
   ORBMatcher(nnratio, checkOri)          constructor arguments kept
   DescriptorDistance(a, b)               src/ORBMatcher.cpp:951-967
   SearchByBoW(KF, F)                     src/ORBMatcher.cpp:409-539   (arrays instead of KeyFrame*/Frame&)
+  SearchByBoW_fv / SearchByBoW_KF_fv     the same searches for key frames of up to Vocabulary.MAX_FV_FEATURES features, FeatureVectors as CSRs
   match_bruteforce                       BASELINE config 3 (definition: DESIGN.md §matcher)
 All calls are batched over `npairs` independent pairs (leading axis)."""
 import ctypes as C
@@ -10,6 +11,7 @@ import ctypes as C
 import numpy as np
 
 from ._capi import Handle, check, lib, ptr
+from .vocabulary import Vocabulary
 
 TH_HIGH = 100
 TH_LOW = 50
@@ -107,3 +109,37 @@ class ORBMatcher(Handle):
     def search_by_bow_dev(self, descKF, angKF, kf_valid, node_kf, nKF, descF, angF, node_f, nF, npairs, match_f, nmatches):
         check(lib().cslam_search_by_bow_dev(self._h, ptr(descKF), ptr(angKF), ptr(kf_valid), ptr(node_kf), int(nKF), ptr(descF), ptr(angF), ptr(node_f),
                                             int(nF), int(npairs), C.c_float(self.nnratio), int(self.check_ori), ptr(match_f), ptr(nmatches)))
+
+    def SearchByBoW_fv(self, descKF, angKF, kf_valid, n_kf, fv_kf, descF, angF, n_f, fv_f):
+        """cslam_search_by_bow_fv: SearchByBoW(KeyFrame*, Frame&) for strides up to Vocabulary.MAX_FV_FEATURES, whatever max_features.
+        Per-feature arrays are (P, stride, ...), n_* (P,); fv_* = (node, start, feat, count), batched as pack_fv returns them (the layout
+        cslam_bow_transform_fv writes). Returns (nmatches (P,), match_f (P, f_stride)), -1 past n_f."""
+        return self._bow_fv(lib().cslam_search_by_bow_fv, descKF, angKF, kf_valid, n_kf, fv_kf, descF, angF, None, n_f, fv_f)
+
+    def SearchByBoW_KF_fv(self, desc1, ang1, valid1, n1, fv1, desc2, ang2, valid2, n2, fv2):
+        """cslam_search_by_bow_kf_fv: SearchByBoW(KeyFrame*, KeyFrame*) likewise. Returns (nmatches (P,), match12 (P, stride1))."""
+        return self._bow_fv(lib().cslam_search_by_bow_kf_fv, desc1, ang1, valid1, n1, fv1, desc2, ang2, valid2, n2, fv2)
+
+    def _bow_fv(self, fn, d1, a1, v1, n1, fv1, d2, a2, v2, n2, fv2):
+        d1 = np.ascontiguousarray(d1, np.uint8); d2 = np.ascontiguousarray(d2, np.uint8)
+        P, s1, s2 = d1.shape[0], d1.shape[1], d2.shape[1]
+        a1 = np.ascontiguousarray(a1, np.float32); a2 = np.ascontiguousarray(a2, np.float32); v1 = np.ascontiguousarray(v1, np.uint8)
+        n1 = np.ascontiguousarray(n1, np.int32); n2 = np.ascontiguousarray(n2, np.int32)
+        f1 = [np.ascontiguousarray(x, np.int32) for x in fv1]; f2 = [np.ascontiguousarray(x, np.int32) for x in fv2]
+        out = np.empty((P, s1 if v2 is not None else s2), np.int32); nm = np.empty(P, np.int32)
+        v2 = None if v2 is None else np.ascontiguousarray(v2, np.uint8)
+        side2 = [ptr(d2), ptr(a2)] + ([ptr(v2)] if v2 is not None else [])
+        check(fn(self._h, P, ptr(d1), ptr(a1), ptr(v1), ptr(n1), s1, *[ptr(x) for x in f1], *side2, ptr(n2), s2, *[ptr(x) for x in f2],
+                 C.c_float(self.nnratio), int(self.check_ori), ptr(out), ptr(nm)))
+        return nm, out
+
+
+def pack_fv(fvs, stride):
+    """Per-frame FeatureVectors [(node (j,), start (j + 1,), feat (start[-1],)), ...] (Vocabulary.transform_fv's last three outputs) ->
+    the batched CSR (node (P, stride), start (P, stride + 1), feat (P, stride), count (P,)) of the _fv entries."""
+    assert stride <= Vocabulary.MAX_FV_FEATURES
+    P = len(fvs)
+    node = np.zeros((P, stride), np.int32); start = np.zeros((P, stride + 1), np.int32); feat = np.zeros((P, stride), np.int32); count = np.zeros(P, np.int32)
+    for p, (nd, st, ft) in enumerate(fvs):
+        j = len(nd); count[p] = j; node[p, :j] = nd; start[p, :j + 1] = st; feat[p, :len(ft)] = ft
+    return node, start, feat, count

@@ -10,6 +10,7 @@
 #include <cstring>
 #include <vector>
 
+#include "FeatureVector_csr_b200.h"
 #include "cubemap_b200.h"
 
 // the reference's own CPU bodies, exported by dropin/ORBMatcher_cpu_forward.cpp
@@ -23,11 +24,6 @@ cslam_matcher* b200_matcher() {   // ORBMatcher objects live on three threads in
     return m;
 }
 void b200_fatal() { std::fprintf(stderr, "ORBMatcher (cubemap_b200): %s\n", cslam_last_error()); std::exit(EXIT_FAILURE); }
-// DBoW2::FeatureVector = std::map<NodeId, std::vector<unsigned int>>; features absent from it get sentinels that never meet
-void node_ids(const DBoW2::FeatureVector& fv, std::vector<int32_t>& node) {
-    for (DBoW2::FeatureVector::const_iterator it = fv.begin(); it != fv.end(); ++it)
-        for (size_t k = 0; k < it->second.size(); k++) node[it->second[k]] = (int32_t)it->first;
-}
 void gather(const cv::Mat& desc, const std::vector<cv::KeyPoint>& keys, int n, std::vector<uint8_t>& d, std::vector<float>& a) {
     d.resize((size_t)n * 32); a.resize(n);
     for (int i = 0; i < n; i++) { std::memcpy(&d[(size_t)i * 32], desc.ptr<uchar>(i), 32); a[i] = keys[i].angle; }
@@ -109,37 +105,41 @@ int ORBMatcher::SearchByProjection(KeyFrame* pKF, cv::Mat Scw, const std::vector
     return cslam_cpu_SearchByProjection(this, pKF, Scw, vpPoints, vpMatched, th);
 }
 
-// reference src/ORBMatcher.cpp:409-539 (Tracking::TrackReferenceKeyFrame :577, Relocalization :1045)
+// reference src/ORBMatcher.cpp:409-539 (Tracking::TrackReferenceKeyFrame :577, Relocalization :1045). Both FeatureVectors go to the device as
+// they are (cslam_search_by_bow_fv), so key frames of the initialisation extractor (up to 3*nFeatures + 3*nlevels key points) are taken too.
 int ORBMatcher::SearchByBoW(KeyFrame* pKF, Frame& F, std::vector<MapPoint*>& vpMapPointMatches) {
     const std::vector<MapPoint*> vpMapPointsKF = pKF->GetMapPointMatches();
-    const int nKF = (int)vpMapPointsKF.size(), nF = F.N;
+    const int32_t nKF = (int32_t)vpMapPointsKF.size(), nF = F.N;
     vpMapPointMatches = std::vector<MapPoint*>(nF, static_cast<MapPoint*>(NULL));
+    if (nKF == 0 || nF == 0) return 0;
     std::vector<uint8_t> dK, dF, valid(nKF); std::vector<float> aK, aF;
     gather(pKF->mDescriptors, pKF->mvKeys, nKF, dK, aK); gather(F.mDescriptors, F.mvKeys, nF, dF, aF);
     for (int i = 0; i < nKF; i++) valid[i] = vpMapPointsKF[i] && !vpMapPointsKF[i]->isBad();
-    std::vector<int32_t> nodeK(nKF, 0x7ffff), nodeF(nF, 0x7fffe), matchF(nF);
-    node_ids(pKF->mFeatVec, nodeK); node_ids(F.mFeatVec, nodeF);
-    int32_t n = 0;
-    if (cslam_search_by_bow(b200_matcher(), dK.data(), aK.data(), valid.data(), nodeK.data(), nKF, dF.data(), aF.data(), nodeF.data(), nF, 1, mfNNratio,
-                            mbCheckOrientation, matchF.data(), &n) != CSLAM_OK) b200_fatal();
+    const cubemap_b200::FeatureVectorCsr fK(pKF->mFeatVec, nKF), fF(F.mFeatVec, nF);
+    std::vector<int32_t> matchF(nF); int32_t n = 0;
+    if (cslam_search_by_bow_fv(b200_matcher(), 1, dK.data(), aK.data(), valid.data(), &nKF, nKF, fK.node.data(), fK.start.data(), fK.feat.data(), &fK.count, dF.data(),
+                               aF.data(), &nF, nF, fF.node.data(), fF.start.data(), fF.feat.data(), &fF.count, mfNNratio, mbCheckOrientation, matchF.data(), &n) != CSLAM_OK)
+        b200_fatal();
     for (int j = 0; j < nF; j++) if (matchF[j] >= 0) vpMapPointMatches[j] = vpMapPointsKF[matchF[j]];
     return n;
 }
 
-// reference src/ORBMatcher.cpp:541-674 (LoopClosing::ComputeSim3 :238)
+// reference src/ORBMatcher.cpp:541-674 (LoopClosing::ComputeSim3 :238), through cslam_search_by_bow_kf_fv likewise
 int ORBMatcher::SearchByBoW(KeyFrame* pKF1, KeyFrame* pKF2, std::vector<MapPoint*>& vpMatches12) {
     const std::vector<MapPoint*> mp1 = pKF1->GetMapPointMatches(), mp2 = pKF2->GetMapPointMatches();
-    const int n1 = (int)mp1.size(), n2 = (int)mp2.size();
+    const int32_t n1 = (int32_t)mp1.size(), n2 = (int32_t)mp2.size();
     vpMatches12 = std::vector<MapPoint*>(n1, static_cast<MapPoint*>(NULL));
+    if (n1 == 0 || n2 == 0) return 0;
     std::vector<uint8_t> d1, d2, v1(n1), v2(n2); std::vector<float> a1, a2;
     gather(pKF1->mDescriptors, pKF1->mvKeys, n1, d1, a1); gather(pKF2->mDescriptors, pKF2->mvKeys, n2, d2, a2);
     for (int i = 0; i < n1; i++) v1[i] = mp1[i] && !mp1[i]->isBad();
     for (int i = 0; i < n2; i++) v2[i] = mp2[i] && !mp2[i]->isBad();
-    std::vector<int32_t> nd1(n1, 0x7ffff), nd2(n2, 0x7fffe), m12(n1);
-    node_ids(pKF1->mFeatVec, nd1); node_ids(pKF2->mFeatVec, nd2);
-    int32_t n = 0;
-    if (cslam_search_by_bow_kf(b200_matcher(), d1.data(), a1.data(), v1.data(), nd1.data(), n1, d2.data(), a2.data(), v2.data(), nd2.data(), n2, 1, mfNNratio,
-                               mbCheckOrientation, m12.data(), &n) != CSLAM_OK) b200_fatal();
+    const cubemap_b200::FeatureVectorCsr f1(pKF1->mFeatVec, n1), f2(pKF2->mFeatVec, n2);
+    std::vector<int32_t> m12(n1); int32_t n = 0;
+    if (cslam_search_by_bow_kf_fv(b200_matcher(), 1, d1.data(), a1.data(), v1.data(), &n1, n1, f1.node.data(), f1.start.data(), f1.feat.data(), &f1.count, d2.data(),
+                                  a2.data(), v2.data(), &n2, n2, f2.node.data(), f2.start.data(), f2.feat.data(), &f2.count, mfNNratio, mbCheckOrientation, m12.data(),
+                                  &n) != CSLAM_OK)
+        b200_fatal();
     for (int i = 0; i < n1; i++) if (m12[i] >= 0) vpMatches12[i] = mp2[m12[i]];
     return n;
 }

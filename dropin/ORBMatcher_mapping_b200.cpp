@@ -11,6 +11,7 @@
 #include <cstring>
 #include <vector>
 
+#include "FeatureVector_csr_b200.h"
 #include "cubemap_b200.h"
 
 int cslam_cpu_Fuse(ORBMatcher* m, KeyFrame* pKF, cv::Mat Scw, const std::vector<MapPoint*>& vpPoints, float th, std::vector<MapPoint*>& vpReplacePoint);
@@ -25,12 +26,6 @@ void b200_fatal() { std::fprintf(stderr, "ORBMatcher (cubemap_b200): %s\n", csla
 void gather_desc(const cv::Mat& desc, int n, std::vector<uint8_t>& d) {
     d.resize((size_t)n * 32);
     for (int i = 0; i < n; i++) std::memcpy(&d[(size_t)i * 32], desc.ptr<uchar>(i), 32);
-}
-// vocabulary node of every feature; features the FeatureVector does not list get a node no other key frame uses
-void node_ids(const DBoW2::FeatureVector& fv, int n, int32_t absent, std::vector<int32_t>& node) {
-    node.assign(n, absent);
-    for (DBoW2::FeatureVector::const_iterator it = fv.begin(); it != fv.end(); ++it)
-        for (size_t k = 0; k < it->second.size(); k++) node[it->second[k]] = (int32_t)it->first;
 }
 }  // namespace
 
@@ -70,9 +65,9 @@ int ORBMatcher::Fuse(KeyFrame* pKF, const std::vector<MapPoint*>& vpMapPoints, c
     for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) T[4 * r + c] = Tcw.at<float>(r, c);
     std::vector<int32_t> bestIdx(nMPs), bestDist(nMPs);
     static_assert(sizeof(cv::KeyPoint) == sizeof(cslam_keypoint), "cv::KeyPoint layout");
-    if (cslam_fuse_search(b200_mapper(), reinterpret_cast<const cslam_keypoint*>(pKF->mvKeys.data()), dKF.data(), nKF, T, nMPs, valid.data(), Xw.data(), level.data(), dMP.data(), th,
-                          pKF->mvScaleFactors.data(), pKF->mvInvLevelSigma2.data(), pKF->mnScaleLevels, cam->GetCubeFaceWidth(), cam->GetCubeFaceHeight(), bestIdx.data(),
-                          bestDist.data()) != CSLAM_OK) b200_fatal();
+    if (cslam_fuse_search_large(b200_mapper(), reinterpret_cast<const cslam_keypoint*>(pKF->mvKeys.data()), dKF.data(), nKF, T, nMPs, valid.data(), Xw.data(), level.data(), dMP.data(), th,
+                                pKF->mvScaleFactors.data(), pKF->mvInvLevelSigma2.data(), pKF->mnScaleLevels, cam->GetCubeFaceWidth(), cam->GetCubeFaceHeight(),
+                                bestIdx.data(), bestDist.data()) != CSLAM_OK) b200_fatal();
     // (3) the order-dependent bookkeeping, verbatim in effect (src/ORBMatcher.cpp:1217-1236)
     int nFused = 0;
     for (int i = 0; i < nMPs; i++) {
@@ -101,9 +96,9 @@ int ORBMatcher::SearchForTriangulation(KeyFrame* pKF1, KeyFrame* pKF2, cv::Mat E
     const int32_t n1 = pKF1->N, n2 = pKF2->N;
     vMatchedPairs.clear();
     if (n1 == 0 || n2 == 0) return 0;
-    std::vector<uint8_t> d1, d2, has1(n1, 0), has2(n2, 0); std::vector<int32_t> node1, node2; std::vector<float> r1((size_t)n1 * 3), r2((size_t)n2 * 3);
+    std::vector<uint8_t> d1, d2, has1(n1, 0), has2(n2, 0); std::vector<float> r1((size_t)n1 * 3), r2((size_t)n2 * 3);
     gather_desc(pKF1->mDescriptors, n1, d1); gather_desc(pKF2->mDescriptors, n2, d2);
-    node_ids(pKF1->mFeatVec, n1, (1 << 20) - 3, node1); node_ids(pKF2->mFeatVec, n2, (1 << 20) - 2, node2);
+    const cubemap_b200::FeatureVectorCsr f1(pKF1->mFeatVec, n1), f2(pKF2->mFeatVec, n2);
     for (int i = 0; i < n1; i++) { has1[i] = pKF1->GetMapPoint(i) != NULL; for (int c = 0; c < 3; c++) r1[3 * (size_t)i + c] = pKF1->mvKeyRays[i](c); }
     for (int i = 0; i < n2; i++) { has2[i] = pKF2->GetMapPoint(i) != NULL; for (int c = 0; c < 3; c++) r2[3 * (size_t)i + c] = pKF2->mvKeyRays[i](c); }
     const cv::Mat Cw = pKF1->GetCameraCenter(), T2 = pKF2->GetPose();
@@ -112,10 +107,11 @@ int ORBMatcher::SearchForTriangulation(KeyFrame* pKF1, KeyFrame* pKF2, cv::Mat E
     for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) Tcw2[4 * r + c] = T2.at<float>(r, c);
     for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) E[3 * r + c] = E12.at<float>(r, c);
     std::vector<int32_t> match(n1); int32_t nm = 0;
-    if (cslam_search_for_triangulation(b200_mapper(), 1, reinterpret_cast<const cslam_keypoint*>(pKF1->mvKeys.data()), d1.data(), r1.data(), has1.data(), node1.data(), &n1, n1,
-                                       reinterpret_cast<const cslam_keypoint*>(pKF2->mvKeys.data()), d2.data(), r2.data(), has2.data(), node2.data(), &n2, n2, Ow1, Tcw2, E,
-                                       pKF2->mvScaleFactors.data(), pKF2->mvLevelSigma2.data(), pKF2->mnScaleLevels, cam->GetCubeFaceWidth(), cam->GetCubeFaceHeight(),
-                                       mbCheckOrientation, match.data(), &nm) != CSLAM_OK) b200_fatal();
+    if (cslam_search_for_triangulation_fv(b200_mapper(), 1, reinterpret_cast<const cslam_keypoint*>(pKF1->mvKeys.data()), d1.data(), r1.data(), has1.data(), &n1, n1,
+                                          f1.node.data(), f1.start.data(), f1.feat.data(), &f1.count, reinterpret_cast<const cslam_keypoint*>(pKF2->mvKeys.data()),
+                                          d2.data(), r2.data(), has2.data(), &n2, n2, f2.node.data(), f2.start.data(), f2.feat.data(), &f2.count, Ow1, Tcw2, E,
+                                          pKF2->mvScaleFactors.data(), pKF2->mvLevelSigma2.data(), pKF2->mnScaleLevels, cam->GetCubeFaceWidth(),
+                                          cam->GetCubeFaceHeight(), mbCheckOrientation, match.data(), &nm) != CSLAM_OK) b200_fatal();
     vMatchedPairs.reserve(nm);
     for (int i = 0; i < n1; i++) if (match[i] >= 0) vMatchedPairs.push_back(std::make_pair((size_t)i, (size_t)match[i]));
     return nm;

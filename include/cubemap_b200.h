@@ -173,6 +173,24 @@ int cslam_search_by_bow_kf(cslam_matcher* m, const uint8_t* desc1, const float* 
                            const uint8_t* desc2, const float* ang2, const uint8_t* valid2, const int32_t* node2, int n2, int npairs,
                            float nnratio, int check_ori, int32_t* match12, int32_t* nmatches);
 
+/* Both SearchByBoW forms for key frames of up to CSLAM_BOW_FV_MAX_FEATURES features (the initialisation extractor's key frames reach 9024 at 3000
+ * features), whatever the handle's max_features; npairs <= max_pairs. Same matching rules and outputs as cslam_search_by_bow / _kf, but each
+ * side's FeatureVector comes in as a CSR, exactly as cslam_bow_transform_fv writes it, so its outputs feed these entries unchanged: pair p
+ * holds min(n[p], stride) features in the rows at p*stride (descriptors, angles, valid), fv_count[p] nodes strictly ascending in fv_node at
+ * p*stride, fv_count[p] + 1 offsets in fv_start at p*(stride+1), and node fv_node[j] holds fv_feat[fv_start[j] .. fv_start[j+1]) of the row
+ * at p*stride, in list order (a DBoW2::FeatureVector as it is). A feature in no node is never matched. Host buffers, synchronous.
+ * CSLAM_E_BADARG, before anything runs: a stride outside [1, CSLAM_BOW_FV_MAX_FEATURES], n[p] < 0, fv_count[p] outside [0, stride], fv_start
+ * below 0, decreasing or past min(n[p], stride), a feature index outside [0, min(n[p], stride)) or listed twice, nodes not strictly ascending.
+ * Outputs: match_f / match12 at p*f_stride / p*stride1 for every row of the stride (-1 past the count); nmatches[p]. */
+int cslam_search_by_bow_fv(cslam_matcher* m, int npairs, const uint8_t* descKF, const float* angKF, const uint8_t* kf_valid, const int32_t* n_kf, int kf_stride,
+                           const int32_t* kf_fv_node, const int32_t* kf_fv_start, const int32_t* kf_fv_feat, const int32_t* kf_fv_count, const uint8_t* descF,
+                           const float* angF, const int32_t* n_f, int f_stride, const int32_t* f_fv_node, const int32_t* f_fv_start, const int32_t* f_fv_feat,
+                           const int32_t* f_fv_count, float nnratio, int check_ori, int32_t* match_f, int32_t* nmatches);
+int cslam_search_by_bow_kf_fv(cslam_matcher* m, int npairs, const uint8_t* desc1, const float* ang1, const uint8_t* valid1, const int32_t* n1, int stride1,
+                              const int32_t* fv_node1, const int32_t* fv_start1, const int32_t* fv_feat1, const int32_t* fv_count1, const uint8_t* desc2,
+                              const float* ang2, const uint8_t* valid2, const int32_t* n2, int stride2, const int32_t* fv_node2, const int32_t* fv_start2,
+                              const int32_t* fv_feat2, const int32_t* fv_count2, float nnratio, int check_ori, int32_t* match12, int32_t* nmatches);
+
 /* ---------------------------------------------------------------------------------------------- vocabulary (DBoW2 transform)
  * ORBVocabulary::transform(features, BowVector&, FeatureVector&, levelsup) as Frame::ComputeBoW / KeyFrame::ComputeBoW call it (src/Frame.cpp:719-726;
  * ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1262). The tree is given as flat arrays for nodes 1..n_nodes in ORBvoc.txt's line order (what
@@ -338,6 +356,10 @@ int cslam_distinctive_descriptors(cslam_mapper* m, const uint8_t* desc, const in
 int cslam_fuse_search(cslam_mapper* m, const cslam_keypoint* k_kf, const uint8_t* d_kf, int n_kf, const float* Tcw /* 4x4 row-major */, int n_mp, const uint8_t* mp_valid,
                       const float* mp_xw /* n_mp x 3 */, const int32_t* mp_level, const uint8_t* mp_desc /* n_mp x 32 */, float th, const float* scale_factors,
                       const float* inv_level_sigma2, int nlevels, int face_w, int face_h, int32_t* best_idx, int32_t* best_dist);
+/* The same search for key frames of up to CSLAM_BOW_FV_MAX_FEATURES key points (n_kf); cslam_fuse_search is this with n_kf <= 4096. */
+int cslam_fuse_search_large(cslam_mapper* m, const cslam_keypoint* k_kf, const uint8_t* d_kf, int n_kf, const float* Tcw, int n_mp, const uint8_t* mp_valid,
+                            const float* mp_xw, const int32_t* mp_level, const uint8_t* mp_desc, float th, const float* scale_factors,
+                            const float* inv_level_sigma2, int nlevels, int face_w, int face_h, int32_t* best_idx, int32_t* best_dist);
 
 /* ORBMatcher::SearchForTriangulation(pKF1, pKF2, E12, vMatchedPairs) (reference src/ORBMatcher.cpp:971-1124) for `npairs` key-frame pairs in one
  * launch (LocalMapping::CreateNewMapPoints matches the new key frame against ~20 neighbours). Pair p reads rows [p*stride, p*stride + n[p]) of
@@ -350,6 +372,15 @@ int cslam_search_for_triangulation(cslam_mapper* m, int npairs, const cslam_keyp
                                    const int32_t* n1, int stride1, const cslam_keypoint* k2, const uint8_t* d2, const float* rays2, const uint8_t* has_mp2, const int32_t* node2,
                                    const int32_t* n2, int stride2, const float* Ow1, const float* Tcw2, const float* E12, const float* scale_factors,
                                    const float* level_sigma2, int nlevels, int face_w, int face_h, int check_orientation, int32_t* match12, int32_t* nmatches);
+/* The same search for key frames of up to CSLAM_BOW_FV_MAX_FEATURES features, with each key frame's FeatureVector as a CSR in
+ * cslam_bow_transform_fv's layout instead of per-feature node ids (fv_* as for cslam_search_by_bow_fv, rejected the same way). The features
+ * of a node are scanned in list order. match12: every row of stride1 per pair, -1 past n1[p]. */
+int cslam_search_for_triangulation_fv(cslam_mapper* m, int npairs, const cslam_keypoint* k1, const uint8_t* d1, const float* rays1, const uint8_t* has_mp1,
+                                      const int32_t* n1, int stride1, const int32_t* fv_node1, const int32_t* fv_start1, const int32_t* fv_feat1,
+                                      const int32_t* fv_count1, const cslam_keypoint* k2, const uint8_t* d2, const float* rays2, const uint8_t* has_mp2,
+                                      const int32_t* n2, int stride2, const int32_t* fv_node2, const int32_t* fv_start2, const int32_t* fv_feat2,
+                                      const int32_t* fv_count2, const float* Ow1, const float* Tcw2, const float* E12, const float* scale_factors,
+                                      const float* level_sigma2, int nlevels, int face_w, int face_h, int check_orientation, int32_t* match12, int32_t* nmatches);
 
 #ifdef __cplusplus
 }
