@@ -122,7 +122,85 @@ struct TrackArgs {
     const float* qProj; const int32_t* qLevel; const float* qViewCos;     // mode 1
     int mode, W, H, checkOri; float th, nnratio, cosFovTh; float scale[16];
     int32_t* match; int32_t* nmatches; int* errFlag;
+    uint32_t* lmList; uint16_t* lmCount;   // k_local_candidates -> k_local_commit: LM_K packed entries and the candidate count per (frame, MapPoint)
 };
+
+// Mode 1's window of the MapPoint in row `row` (scale: A.scale or a copy): RadiusByViewingCos (src/ORBMatcher.cpp:380-386), times th unless th == 1, times the scale of
+// the predicted level; levels [level - 1, level]
+__device__ __forceinline__ void local_window(const TrackArgs& A, const float* scale, size_t row, float& u, float& v, float& radius, int& minL, int& maxL) {
+    u = A.qProj[row * 2]; v = A.qProj[row * 2 + 1];
+    const int lvl = A.qLevel[row];
+    float r = A.qViewCos[row] > 0.998 ? 2.5f : 4.0f;   // float compared with the double literal 0.998
+    if (A.th != 1.0f) r = __fmul_rn(r, A.th);
+    radius = __fmul_rn(r, scale[lvl]); minL = lvl - 1; maxL = lvl;
+}
+
+// Frame::GetFeaturesInArea for one query, walked by the calling warp: the window's cells in the reference's visiting order (area_cells; entries
+// ascending inside a cell), the level and radius gates, and the Hamming distance to the query's descriptor qd. The candidates go to cIdx / cDist
+// in visiting order; returns their number (warp-uniform). More than TRK_CAND candidates, or more than 16 in one cell, sets CSLAM_E_CAPACITY.
+__device__ __forceinline__ int window_candidates(const cslam_keypoint* kC, const uint4* dC, const uint16_t* CS, const uint16_t* CI, float u, float v, float radius, int minL,
+                                                 int maxL, int W, int H, float inv, const uint4* qd, uint16_t* cIdx, uint16_t* cDist, int* errFlag) {
+    const int lane = threadIdx.x & 31;
+    int ncand = 0;
+    AreaQuery aq;
+    if (!area_query(u, v, radius, W, H, inv, aq)) return 0;
+    const bool checkLevels = (minL > 0) || (maxL >= 0);
+    const uint4 a0 = __ldg(qd), a1 = __ldg(qd + 1);
+    for (int k = 0; k < 3; k++) {
+        AreaCells rc;
+        if (!area_cells(aq, k, rc)) break;
+        for (int cb = 0; cb < rc.n; cb += 32) {   // lanes = consecutive cells (ix major, iy minor), entries kept in cell order
+            const int ci = cb + lane;
+            int s = 0, e = 0;
+            if (ci < rc.n) { const int cell = rc.cell(ci); s = CS[cell]; e = CS[cell + 1]; }
+            // walk the (few) entries of the 32 cells in order
+            const int maxLen = __reduce_max_sync(0xffffffffu, e - s);
+            if (maxLen == 0) continue;
+            // per lane: filter its cell's entries, then order-preserving append
+            int myKeep = 0; uint16_t keepIdx[16];   // a 13-px cell with more than 16 passing key points is reported, never truncated silently
+            bool slow = false;
+            for (int a = s; a < e; a++) {
+                const int idx = CI[a];
+                const cslam_keypoint kp = kC[idx];
+                if (checkLevels) { if (kp.octave < minL) continue; if (maxL >= 0 && kp.octave > maxL) continue; }
+                if (fabsf(__fsub_rn(kp.x, u)) < radius && fabsf(__fsub_rn(kp.y, v)) < radius) { if (myKeep < 16) keepIdx[myKeep] = (uint16_t)idx; else slow = true; myKeep++; }
+            }
+            if (__any_sync(0xffffffffu, slow)) { if (lane == 0) *errFlag = CSLAM_E_CAPACITY; myKeep = min(myKeep, 16); }
+            int off = myKeep;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, off, o); if (lane >= o) off += t; }
+            const int tot = __shfl_sync(0xffffffffu, off, 31);
+            off -= myKeep;
+            for (int j = 0; j < myKeep; j++) {
+                const int pos = ncand + off + j;
+                if (pos < TRK_CAND) {
+                    const int idx = keepIdx[j];
+                    cIdx[pos] = (uint16_t)idx;
+                    cDist[pos] = (uint16_t)hamming256(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
+                } else *errFlag = CSLAM_E_CAPACITY;
+            }
+            ncand = min(ncand + tot, TRK_CAND);
+        }
+    }
+    return ncand;
+}
+
+// The reference's scalar scan over one query's candidates in visiting order, skipping taken slots: `dist < bestDist` shifts the best to
+// second place; with `second` (mode 1) `else if (dist < bestDist2)` replaces the second. No candidate: dist 256, level -1.
+struct Best { int dist, level, dist2, level2, idx; };
+__device__ __forceinline__ Best best_two(const uint16_t* cIdx, const uint16_t* cDist, int nc, const uint8_t* slotObs, const cslam_keypoint* kC, bool second) {
+    Best b = {256, -1, 256, -1, -1};
+    for (int c = 0; c < nc; c++) {
+        const int idx = cIdx[c];
+        if (slotObs[idx]) continue;
+        const int dist = cDist[c];
+        if (dist < b.dist) { b.dist2 = b.dist; b.dist = dist; b.level2 = b.level; b.level = kC[idx].octave; b.idx = idx; }
+        else if (second && dist < b.dist2) { b.level2 = kC[idx].octave; b.dist2 = dist; }
+    }
+    return b;
+}
+// mode 1's ratio test (src/ORBMatcher.cpp:111-112): only when the best and the second best are at the same level
+__device__ __forceinline__ bool ratio_ok(const Best& b, float nnratio) { return !(b.level == b.level2 && (float)b.dist > __fmul_rn(nnratio, (float)b.dist2)); }
 
 __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackArgs A) {
     __shared__ uint16_t candIdx[TRK_WARPS][TRK_CAND];
@@ -160,54 +238,8 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
                 if (ok) ok = ray_to_cubemap(xc[0], xc[1], xc[2], A.W, A.H, u, v);
                 const int oct = A.kLast[(size_t)p * A.qStride + q].octave;
                 radius = __fmul_rn(A.th, A.scale[oct]); minL = oct - 1; maxL = oct + 1;
-            } else {
-                u = A.qProj[((size_t)p * A.qStride + q) * 2]; v = A.qProj[((size_t)p * A.qStride + q) * 2 + 1];
-                const int lvl = A.qLevel[(size_t)p * A.qStride + q];
-                float r = A.qViewCos[(size_t)p * A.qStride + q] > 0.998 ? 2.5f : 4.0f;   // float compared with the double literal 0.998
-                if (A.th != 1.0f) r = __fmul_rn(r, A.th);
-                radius = __fmul_rn(r, A.scale[lvl]); minL = lvl - 1; maxL = lvl;
-            }
-            AreaQuery aq;
-            if (ok && area_query(u, v, radius, A.W, A.H, inv, aq)) {
-                const bool checkLevels = (minL > 0) || (maxL >= 0);
-                const uint4 a0 = __ldg(dQ + 2 * q), a1 = __ldg(dQ + 2 * q + 1);
-                for (int k = 0; k < 3; k++) {
-                    AreaCells rc;
-                    if (!area_cells(aq, k, rc)) break;
-                    for (int cb = 0; cb < rc.n; cb += 32) {   // lanes = consecutive cells (ix major, iy minor), entries kept in cell order
-                        const int ci = cb + lane;
-                        int s = 0, e = 0;
-                        if (ci < rc.n) { const int cell = rc.cell(ci); s = CS[cell]; e = CS[cell + 1]; }
-                        // walk the (few) entries of the 32 cells in order
-                        const int maxLen = __reduce_max_sync(0xffffffffu, e - s);
-                        if (maxLen == 0) continue;
-                        // per lane: filter its cell's entries, then order-preserving append
-                        int myKeep = 0; uint16_t keepIdx[16];   // a 13-px cell with more than 16 passing key points is reported, never truncated silently
-                        bool slow = false;
-                        for (int a = s; a < e; a++) {
-                            const int idx = CI[a];
-                            const cslam_keypoint kp = kC[idx];
-                            if (checkLevels) { if (kp.octave < minL) continue; if (maxL >= 0 && kp.octave > maxL) continue; }
-                            if (fabsf(__fsub_rn(kp.x, u)) < radius && fabsf(__fsub_rn(kp.y, v)) < radius) { if (myKeep < 16) keepIdx[myKeep] = (uint16_t)idx; else slow = true; myKeep++; }
-                        }
-                        if (__any_sync(0xffffffffu, slow)) { if (lane == 0) *A.errFlag = CSLAM_E_CAPACITY; myKeep = min(myKeep, 16); }
-                        int off = myKeep;
-#pragma unroll
-                        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, off, o); if (lane >= o) off += t; }
-                        const int tot = __shfl_sync(0xffffffffu, off, 31);
-                        off -= myKeep;
-                        for (int j = 0; j < myKeep; j++) {
-                            const int pos = ncand + off + j;
-                            if (pos < TRK_CAND) {
-                                const int idx = keepIdx[j];
-                                candIdx[warp][pos] = (uint16_t)idx;
-                                candDist[warp][pos] = (uint16_t)hamming256(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1));
-                            } else *A.errFlag = CSLAM_E_CAPACITY;
-                        }
-                        ncand = min(ncand + tot, TRK_CAND);
-                    }
-                }
-            }
+            } else local_window(A, A.scale, (size_t)p * A.qStride + q, u, v, radius, minL, maxL);
+            if (ok) ncand = window_candidates(kC, dC, CS, CI, u, v, radius, minL, maxL, A.W, A.H, inv, dQ + 2 * q, candIdx[warp], candDist[warp], A.errFlag);
         }
         if (lane == 0) candN[warp] = ncand;
         __syncthreads();
@@ -216,16 +248,10 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
             for (int w = 0; w < TRK_WARPS; w++) {
                 const int qq = q0 + w, nc = candN[w];
                 if (qq >= nQ || nc == 0) continue;
-                int bestDist = 256, bestLevel = -1, bestDist2 = 256, bestLevel2 = -1, bestIdx = -1;
-                for (int c = 0; c < nc; c++) {
-                    const int idx = candIdx[w][c];
-                    if (slotObs[idx]) continue;
-                    const int dist = candDist[w][c];
-                    if (dist < bestDist) { bestDist2 = bestDist; bestDist = dist; bestLevel2 = bestLevel; bestLevel = kC[idx].octave; bestIdx = idx; }
-                    else if (A.mode == 1 && dist < bestDist2) { bestLevel2 = kC[idx].octave; bestDist2 = dist; }
-                }
-                if (bestDist > 100) continue;   // TH_HIGH
-                if (A.mode == 1 && bestLevel == bestLevel2 && (float)bestDist > __fmul_rn(A.nnratio, (float)bestDist2)) continue;
+                const Best b = best_two(candIdx[w], candDist[w], nc, slotObs, kC, A.mode == 1);
+                if (b.dist > 100) continue;   // TH_HIGH
+                if (A.mode == 1 && !ratio_ok(b, A.nnratio)) continue;
+                const int bestIdx = b.idx;
                 M[bestIdx] = qq; slotObs[bestIdx] = A.qObs[(size_t)p * A.qStride + qq];
                 total++;
                 if (A.mode == 0 && A.checkOri) {
@@ -244,6 +270,122 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
         __syncthreads();
         for (int i = tid; i < logN; i += blockDim.x)
             if (!keep[logBin[i]]) { M[logIdx[i]] = -2; atomicSub(&total, 1); }   // -2: assigned, then cleared (the reference NULLs the slot)
+        __syncthreads();
+    }
+    if (tid == 0) A.nmatches[p] = total;
+}
+
+// ------------------------------------------------------------------------------------------------- local maps past 4096 MapPoints
+// cslam_search_by_projection_local_large in two launches (DESIGN.md, "Local maps past 4096 MapPoints"):
+//   k_local_candidates: one warp per (frame, MapPoint) over the whole device walks the window (window_candidates) and keeps the first LM_K
+//     candidates in (distance, visiting position) order, packed, plus the full candidate count.
+//   k_local_commit: one CTA per frame applies the reference's rules in MapPoint order. The first two untaken entries of that order are the
+//     scan's best and second best, so a MapPoint needs nothing else unless fewer than two of its stored entries are untaken while it has more
+//     than LM_K candidates: then the committing warp walks the window again and runs the scan itself (best_two).
+static const int LM_K = 8;        // stored entries per MapPoint: a performance choice, the answer does not depend on it
+static const int LM_CHUNK = 256;  // MapPoints per staged chunk of the commit
+
+// entry = feature (12 bits) | distance << 12 (9 bits) | octave << 21 (a signed byte)
+__device__ __forceinline__ uint32_t lm_pack(int idx, int dist, int octave) { return (uint32_t)idx | (uint32_t)dist << 12 | (uint32_t)(octave & 0xff) << 21; }
+
+__global__ void __launch_bounds__(TRK_WARPS * 32) k_local_candidates(TrackArgs A, int nframes) {
+    __shared__ uint16_t candIdx[TRK_WARPS][TRK_CAND];
+    __shared__ uint16_t candDist[TRK_WARPS][TRK_CAND];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int q = blockIdx.x * TRK_WARPS + warp;
+    const float inv = __fdiv_rn((float)(3 * GRID_G), (float)(3 * A.W));
+    uint16_t* cI = candIdx[warp]; uint16_t* cD = candDist[warp];
+    for (int p = blockIdx.y; p < nframes; p += gridDim.y) {
+        if (q >= min(A.nQ[p], A.qStride)) continue;
+        const size_t row = (size_t)p * A.qStride + q;
+        const cslam_keypoint* kC = A.kCur + (size_t)p * A.curStride;
+        int nc = 0;
+        __syncwarp();   // the previous frame's reads of cI / cD are done
+        if (A.qValid[row]) {
+            float u, v, radius; int minL, maxL;
+            local_window(A, A.scale, row, u, v, radius, minL, maxL);
+            nc = window_candidates(kC, reinterpret_cast<const uint4*>(A.dCur + (size_t)p * A.curStride * 32), A.cellStart + (size_t)p * (NCELLS + 1),
+                                   A.cellIdx + (size_t)p * A.curStride, u, v, radius, minL, maxL, A.W, A.H, inv, reinterpret_cast<const uint4*>(A.qDesc) + 2 * row, cI, cD,
+                                   A.errFlag);
+        }
+        __syncwarp();
+        // selection by key = distance << 8 | position (unique), LM_K rounds of a warp minimum above the previous round's key
+        int last = -1;
+        for (int j = 0; j < min(nc, LM_K); j++) {
+            unsigned mn = 0xffffffffu;
+            for (int c = lane; c < nc; c += 32) { const unsigned key = (unsigned)cD[c] << 8 | (unsigned)c; if ((int)key > last && key < mn) mn = key; }
+            mn = __reduce_min_sync(0xffffffffu, mn);
+            last = (int)mn;
+            if (lane == 0) { const int pos = mn & 0xff, idx = cI[pos]; A.lmList[row * LM_K + j] = lm_pack(idx, cD[pos], kC[idx].octave); }
+        }
+        if (lane == 0) A.lmCount[row] = (uint16_t)nc;
+    }
+}
+
+// chunk c of a frame's MapPoints (rows row0 + c * LM_CHUNK ...) into one buffer of the commit, by threads t0, t0 + nt, ...
+__device__ __forceinline__ void lm_stage(const TrackArgs& A, size_t row0, int nQ, int c, int t0, int nt, uint32_t* list, uint16_t* cnt, uint8_t* obs) {
+    const int q0 = c * LM_CHUNK, n = min(LM_CHUNK, nQ - q0);
+    for (int i = t0; i < n * LM_K; i += nt) list[i] = A.lmList[(row0 + q0) * LM_K + i];
+    for (int i = t0; i < n; i += nt) { cnt[i] = A.lmCount[row0 + q0 + i]; obs[i] = A.qObs[row0 + q0 + i]; }
+}
+
+// The reference's scan over the whole window of the MapPoint in row `row` of frame p, walked again by the calling warp. scale: A.scale in
+// shared memory (indexed by level, a kernel parameter array would be copied to local memory)
+__device__ __forceinline__ Best lm_rewalk(const TrackArgs& A, const float* scale, int p, size_t row, const uint8_t* slotObs, uint16_t* candIdx, uint16_t* candDist) {
+    const cslam_keypoint* kC = A.kCur + (size_t)p * A.curStride;
+    float u, v, radius; int minL, maxL;
+    local_window(A, scale, row, u, v, radius, minL, maxL);
+    const int nc = window_candidates(kC, reinterpret_cast<const uint4*>(A.dCur + (size_t)p * A.curStride * 32), A.cellStart + (size_t)p * (NCELLS + 1),
+                                     A.cellIdx + (size_t)p * A.curStride, u, v, radius, minL, maxL, A.W, A.H, __fdiv_rn((float)(3 * GRID_G), (float)(3 * A.W)),
+                                     reinterpret_cast<const uint4*>(A.qDesc) + 2 * row, candIdx, candDist, A.errFlag);
+    __syncwarp();
+    return best_two(candIdx, candDist, nc, slotObs, kC, true);
+}
+
+__global__ void __launch_bounds__(TRK_WARPS * 32, 1) k_local_commit(TrackArgs A) {
+    __shared__ uint32_t list[2][LM_CHUNK * LM_K];   // double-buffered: warp 0 commits one chunk while the other warps stage the next
+    __shared__ uint16_t cnt[2][LM_CHUNK];
+    __shared__ uint8_t obs[2][LM_CHUNK];
+    __shared__ uint8_t slotObs[4096];
+    __shared__ uint16_t candIdx[TRK_CAND], candDist[TRK_CAND];   // warp 0's window walk when the stored entries run out
+    __shared__ float sScale[16];
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nCur = min(A.nCur[p], A.curStride), nQ = max(0, min(A.nQ[p], A.qStride)), nChunks = (nQ + LM_CHUNK - 1) / LM_CHUNK;
+    const cslam_keypoint* kC = A.kCur + (size_t)p * A.curStride;
+    int32_t* M = A.match + (size_t)p * A.curStride;
+    const size_t row0 = (size_t)p * A.qStride;
+    for (int i = tid; i < A.curStride; i += blockDim.x) { M[i] = -1; if (i < nCur) slotObs[i] = A.curTaken[(size_t)p * A.curStride + i]; }
+    if (tid < 16) sScale[tid] = A.scale[tid];
+    if (nChunks > 0) lm_stage(A, row0, nQ, 0, tid, blockDim.x, list[0], cnt[0], obs[0]);
+    __syncthreads();
+    int total = 0;   // warp 0
+    for (int c = 0; c < nChunks; c++) {
+        const int b = c & 1, q0 = c * LM_CHUNK, n = min(LM_CHUNK, nQ - q0);
+        if (warp != 0) {
+            if (c + 1 < nChunks) lm_stage(A, row0, nQ, c + 1, tid - 32, blockDim.x - 32, list[b ^ 1], cnt[b ^ 1], obs[b ^ 1]);
+        } else {
+            for (int j = 0; j < n; j++) {
+                const int nc = cnt[b][j];
+                if (nc == 0) continue;
+                const int ns = min(nc, LM_K);
+                const uint32_t e = lane < ns ? list[b][j * LM_K + lane] : 0u;
+                const unsigned fr = __ballot_sync(0xffffffffu, lane < ns && !slotObs[e & 0xfff]);
+                Best best = {256, -1, 256, -1, -1};
+                if (__popc(fr) < 2 && nc > LM_K) {   // the untaken entries may lie past the stored ones: the reference's scan over the whole window
+                    best = lm_rewalk(A, sScale, p, row0 + q0 + j, slotObs, candIdx, candDist);
+                    __syncwarp();   // every lane has read candIdx / candDist before the next walk overwrites them
+                } else if (fr) {
+                    const uint32_t e1 = __shfl_sync(0xffffffffu, e, __ffs(fr) - 1);
+                    best.idx = e1 & 0xfff; best.dist = (e1 >> 12) & 0x1ff; best.level = (int8_t)(e1 >> 21);
+                    const unsigned rest = fr & (fr - 1);
+                    if (rest) { const uint32_t e2 = __shfl_sync(0xffffffffu, e, __ffs(rest) - 1); best.dist2 = (e2 >> 12) & 0x1ff; best.level2 = (int8_t)(e2 >> 21); }
+                }
+                if (best.dist > 100 || !ratio_ok(best, A.nnratio)) continue;   // TH_HIGH, ratio test
+                if (lane == 0) { M[best.idx] = q0 + j; slotObs[best.idx] = obs[b][j]; }
+                total++;
+                __syncwarp();   // the slot's new state is visible to every lane before the next MapPoint
+            }
+        }
         __syncthreads();
     }
     if (tid == 0) A.nmatches[p] = total;
@@ -451,6 +593,50 @@ extern "C" int cslam_search_by_projection_local(cslam_tracker* t, int nframes, c
         (rc = cslam_frame_index_dev(t, kF, nF, nframes, f_stride, face_w, face_h, nullptr, cs, ci)) ||
         (rc = cslam_search_by_projection_local_dev(t, nframes, kF, dF, nF, f_stride, cs, ci, taken, nQ, mp_stride, valid, proj, lvl, vcos, dQ, obs, face_w, face_h, th, nnratio,
                                                    scale_factor, nlevels, match, nmOut))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
+    return cslam_tracker_sync(t);
+}
+
+// Local maps of up to CSLAM_LOCAL_MAP_MAX_POINTS MapPoints per frame, whatever the handle's max_features (frames stay <= max_features): the
+// arguments and outputs of cslam_search_by_projection_local, with -1 in every slot row past a frame's count. Every argument is checked before
+// anything is enqueued; the per-call scratch (LM_K + 1/2 words per MapPoint row) comes from the handle's arena.
+extern "C" int cslam_search_by_projection_local_large(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride,
+                                                      const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy,
+                                                      const int32_t* level, const float* view_cos, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h,
+                                                      float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f, int32_t* nmatches) {
+    static const char* fn = "cslam_search_by_projection_local_large";
+    if (!t || nframes <= 0 || nframes > t->maxFrames || f_stride <= 0 || f_stride > t->maxFeat || mp_stride <= 0 || mp_stride > CSLAM_LOCAL_MAP_MAX_POINTS ||
+        face_w <= 0 || face_w != face_h || nlevels < 1 || nlevels > 16 || !k_f || !d_f || !n_f || !f_taken || !n_mp || !in_view || !proj_xy || !level || !view_cos ||
+        !d_mp || !mp_obs || !match_f || !nmatches) {
+        set_error("%s: bad argument (frames in [1, %d], f_stride in [1, %d], mp_stride in [1, %d], nlevels in [1, 16], square faces)", fn, t ? t->maxFrames : 0,
+                  t ? t->maxFeat : 0, CSLAM_LOCAL_MAP_MAX_POINTS);
+        return CSLAM_E_BADARG;
+    }
+    for (int f = 0; f < nframes; f++)   // the window radius reads the scale of the predicted level
+        for (int q = 0; q < std::min(n_mp[f], mp_stride); q++) {
+            const size_t r = (size_t)f * mp_stride + q;
+            if (in_view[r] && (level[r] < 0 || level[r] >= nlevels)) { set_error("%s: frame %d MapPoint %d: level %d outside [0, %d)", fn, f, q, level[r], nlevels); return CSLAM_E_BADARG; }
+        }
+    CSLAM_CUDA(cudaSetDevice(t->device));
+    t->arena.reset();
+    const size_t nc = (size_t)nframes * f_stride, nm = (size_t)nframes * mp_stride;
+    DevArena& a = t->arena;
+    const cslam_keypoint* kF; const uint8_t *dF, *taken, *valid, *dQ, *obs; const int32_t *nF, *nQ, *lvl; const float *proj, *vcos; uint16_t *cs, *ci, *lmCount;
+    uint32_t* lmList; int32_t *match, *nmOut; int rc;
+    if ((rc = a.upload(&kF, k_f, nc)) || (rc = a.upload(&dF, d_f, nc * 32)) || (rc = a.upload(&nF, n_f, nframes)) || (rc = a.upload(&taken, f_taken, nc)) ||
+        (rc = a.upload(&nQ, n_mp, nframes)) || (rc = a.upload(&valid, in_view, nm)) || (rc = a.upload(&proj, proj_xy, nm * 2)) || (rc = a.upload(&lvl, level, nm)) ||
+        (rc = a.upload(&vcos, view_cos, nm)) || (rc = a.upload(&dQ, d_mp, nm * 32)) || (rc = a.upload(&obs, mp_obs, nm)) || (rc = a.take(&cs, (size_t)nframes * (NCELLS + 1))) ||
+        (rc = a.take(&ci, nc)) || (rc = a.take(&lmList, nm * LM_K)) || (rc = a.take(&lmCount, nm)) || (rc = a.take(&match, nc)) || (rc = a.take(&nmOut, nframes)) ||
+        (rc = cslam_frame_index_dev(t, kF, nF, nframes, f_stride, face_w, face_h, nullptr, cs, ci))) return rc;
+    TrackArgs A; std::memset(&A, 0, sizeof(A));
+    A.kCur = kF; A.dCur = dF; A.nCur = nF; A.cellStart = cs; A.cellIdx = ci; A.curTaken = taken; A.curStride = f_stride;
+    A.nQ = nQ; A.qStride = mp_stride; A.qValid = valid; A.qDesc = dQ; A.qObs = obs; A.qProj = proj; A.qLevel = lvl; A.qViewCos = vcos;
+    A.mode = 1; A.W = face_w; A.H = face_h; A.th = th; A.nnratio = nnratio; fill_scales(A, scale_factor, nlevels);
+    A.match = match; A.nmatches = nmOut; A.errFlag = t->errFlag; A.lmList = lmList; A.lmCount = lmCount;
+    k_local_candidates<<<dim3(cdiv(mp_stride, TRK_WARPS), std::min(nframes, 65535)), TRK_WARPS * 32, 0, t->stream>>>(A, nframes); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    k_local_commit<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }

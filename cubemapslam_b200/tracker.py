@@ -4,6 +4,7 @@
   Frame::GetFeaturesInArea cell rectangles            (src/Frame.cpp:251-716)                     -> area_rects (host utility)
   ORBMatcher::SearchByProjection(Frame&, const Frame&, th, mono)        (src/ORBMatcher.cpp:130-251) -> Tracker.SearchByProjection_last
   ORBMatcher::SearchByProjection(Frame&, vector<MapPoint*>&, th)        (src/ORBMatcher.cpp:51-128)  -> Tracker.SearchByProjection_local
+                                                                        local maps past 4096 MapPoints -> Tracker.SearchByProjection_local_large
 All calls are batched over independent frames (leading axis)."""
 import ctypes as C
 
@@ -12,6 +13,7 @@ import numpy as np
 from ._capi import KP_DTYPE, Handle, check, lib, ptr
 
 NCELLS = 5 * 50 * 50
+CSLAM_LOCAL_MAP_MAX_POINTS = 1 << 20   # MapPoints per frame of SearchByProjection_local_large
 
 
 def area_rects(x, y, r, face_w, face_h):
@@ -62,6 +64,17 @@ class Tracker(Handle):
         return (int(nm[0]), match[0]) if single else (nm, match)
 
     def SearchByProjection_local(self, kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor=1.2, nlevels=8, nF=None, nMP=None):
+        return self._local("cslam_search_by_projection_local", kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor, nlevels,
+                           nF, nMP)
+
+    def SearchByProjection_local_large(self, kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor=1.2, nlevels=8, nF=None,
+                                       nMP=None):
+        """SearchByProjection_local for local maps of up to CSLAM_LOCAL_MAP_MAX_POINTS MapPoints per frame, whatever max_features (frames stay
+        within it). Same arguments and results; match rows past a frame's count are -1."""
+        return self._local("cslam_search_by_projection_local_large", kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor,
+                           nlevels, nF, nMP)
+
+    def _local(self, entry, kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor, nlevels, nF, nMP):
         kF = np.ascontiguousarray(kF, KP_DTYPE); single = kF.ndim == 1
         k = kF[None] if single else kF
         P, fs = k.shape
@@ -71,8 +84,8 @@ class Tracker(Handle):
         nf = np.full(P, fs, np.int32) if nF is None else np.ascontiguousarray(nF, np.int32).reshape(P)
         nm_ = np.full(P, ms, np.int32) if nMP is None else np.ascontiguousarray(nMP, np.int32).reshape(P)
         match = np.empty((P, fs), np.int32); nm = np.empty(P, np.int32)
-        check(lib().cslam_search_by_projection_local(self._h, P, ptr(k), ptr(a[0]), ptr(nf), fs, ptr(a[7]), ptr(nm_), ms, ptr(a[1]), ptr(a[2]), ptr(a[3]), ptr(a[4]), ptr(a[5]), ptr(a[6]),
-                                                     int(face_w), int(face_h), C.c_float(th), C.c_float(nnratio), C.c_float(scale_factor), int(nlevels), ptr(match), ptr(nm)))
+        check(getattr(lib(), entry)(self._h, P, ptr(k), ptr(a[0]), ptr(nf), fs, ptr(a[7]), ptr(nm_), ms, ptr(a[1]), ptr(a[2]), ptr(a[3]), ptr(a[4]), ptr(a[5]), ptr(a[6]),
+                                      int(face_w), int(face_h), C.c_float(th), C.c_float(nnratio), C.c_float(scale_factor), int(nlevels), ptr(match), ptr(nm)))
         return (int(nm[0]), match[0]) if single else (nm, match)
 
     def search_by_projection_last_dev(self, npairs, kCur, dCur, nCur, cur_stride, cell_start, cell_idx, curTaken, TcwCur, kLast, nLast, last_stride, hasMP, Xw, dMP, mpObs,

@@ -76,7 +76,9 @@ int ORBMatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMap
     CamModelGeneral* cam = CamModelGeneral::GetCamera();
     const int nF = F.N, nM = (int)vpMapPoints.size();
     if (nF == 0 || nM == 0) return 0;
-    if (nM > 4096) { std::fprintf(stderr, "ORBMatcher (cubemap_b200): more than 4096 local MapPoints in one SearchByProjection call\n"); std::exit(EXIT_FAILURE); }
+    if (nM > CSLAM_LOCAL_MAP_MAX_POINTS) {
+        std::fprintf(stderr, "ORBMatcher (cubemap_b200): more than %d local MapPoints in one SearchByProjection call\n", CSLAM_LOCAL_MAP_MAX_POINTS); std::exit(EXIT_FAILURE);
+    }
     std::vector<uint8_t> dF, dMP((size_t)nM * 32, 0), inView(nM, 0), obs(nM, 0), taken(nF, 0); std::vector<float> aF, proj((size_t)nM * 2, 0.f), vcos(nM, 0.f); std::vector<int32_t> lvl(nM, 0);
     gather(F.mDescriptors, F.mvKeys, nF, dF, aF);
     for (int m = 0; m < nM; m++) {
@@ -89,9 +91,13 @@ int ORBMatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMap
     }
     for (int i = 0; i < nF; i++) taken[i] = F.mvpMapPoints[i] && F.mvpMapPoints[i]->Observations() > 0;
     std::vector<int32_t> match(nF); int32_t n = 0, nf = nF, nm = nM;
-    if (cslam_search_by_projection_local(b200_tracker(), 1, reinterpret_cast<const cslam_keypoint*>(F.mvKeys.data()), dF.data(), &nf, nF, taken.data(), &nm, nM, inView.data(), proj.data(),
-                                         lvl.data(), vcos.data(), dMP.data(), obs.data(), cam->GetCubeFaceWidth(), cam->GetCubeFaceHeight(), th, mfNNratio, F.mfScaleFactor,
-                                         F.mnScaleLevels, match.data(), &n) != CSLAM_OK) b200_fatal();
+    // Every size goes to the _large entry (Tracking::UpdateLocalPoints takes every point of every local key frame, past 4096 as the map grows).
+    // It is also the faster one below 4096: median host-call latency on an H100 80GB HBM3 (700 W), one frame of 4096 key points, face 650,
+    // th 5, two runs of tools/local_map_latency.py: 0.82-0.85 ms against 1.77-1.79 ms for cslam_search_by_projection_local at 1024
+    // MapPoints, 2.06-2.14 against 6.43-6.70 ms at 4096.
+    if (cslam_search_by_projection_local_large(b200_tracker(), 1, reinterpret_cast<const cslam_keypoint*>(F.mvKeys.data()), dF.data(), &nf, nF, taken.data(), &nm, nM,
+                                               inView.data(), proj.data(), lvl.data(), vcos.data(), dMP.data(), obs.data(), cam->GetCubeFaceWidth(),
+                                               cam->GetCubeFaceHeight(), th, mfNNratio, F.mfScaleFactor, F.mnScaleLevels, match.data(), &n) != CSLAM_OK) b200_fatal();
     for (int i = 0; i < nF; i++) if (match[i] >= 0) F.mvpMapPoints[i] = vpMapPoints[match[i]];
     return n;
 }
