@@ -14,7 +14,9 @@ struct PoseOptArgs {
     const int* offset; float* Tcw; const float* Xw; const float* kpxy; const float* invSigma2;
     int faceW, faceH; uint8_t* outlier; int32_t* inliers; double* pose64; double* err; uint8_t* level;
     const int32_t* count; int stride;   // offset == nullptr: frame f owns correspondences [f*stride, f*stride + count[f])
+    double* log; int32_t* nlog;         // optional LM log (test hook, nullptr in production): PO_LOG_ROWS rows of (chi2, lambda, trials, accepted) per frame
 };
+constexpr int PO_LOG_ROWS = 40;         // 4 rounds x optimize(10)
 
 // The kernel is a long sequential schedule of block-wide phases. Every phase is an out-of-line device function (all threads call it
 // convergently; barriers inside): ptxas handles each phase on its own instead of one enormous inlined body (which took ~20 minutes).
@@ -143,8 +145,8 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
     if (tid == 0) { S.pose0 = pose_from_Tcw32(A.Tcw + 16 * f); S.pose = S.pose0; }
     for (int i = tid; i < n; i += T) { A.outlier[beg + i] = 0; A.level[beg + i] = 0; A.err[2 * (beg + i)] = 0; A.err[2 * (beg + i) + 1] = 0; }
     __syncthreads();
-    if (n < 3) { if (tid == 0) { A.inliers[f] = 0; if (A.pose64) pose_to_fp64(S.pose0, A.pose64 + 7 * f); } return; }
-    int nBadEdges = 0;
+    if (n < 3) { if (tid == 0) { A.inliers[f] = 0; if (A.pose64) pose_to_fp64(S.pose0, A.pose64 + 7 * f); if (A.nlog) A.nlog[f] = 0; } return; }
+    int nBadEdges = 0, nRows = 0;
     bool robust = true;
     for (int it = 0; it < 4; it++) {
         if (tid == 0) S.pose = S.pose0;
@@ -160,12 +162,14 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
                 po_build_system(F, &S, robust);
                 if (tid == 0 && iter == 0) {
                     double m = 0; int k = 0;
-                    for (int a = 0; a < 6; a++) { m = fmax(m, fabs(S.Hs[k])); k += 6 - a; }
+                    // std::max(fabs(H_jj), m) of computeLambdaInit (optimization_algorithm_levenberg.cpp:176): a NaN diagonal makes m NaN
+                    // until a later diagonal replaces it, which fmax would skip
+                    for (int a = 0; a < 6; a++) { const double d = fabs(S.Hs[k]); m = d < m ? m : d; k += 6 - a; }
                     S.lambda = 1e-5 * m; S.ni = 2;
                 }
                 if (iter == 0) nBad = 0;
                 __syncthreads();
-                double rho = 0; int qmax = 0;
+                double rho = 0; int qmax = 0; bool accepted = false;
                 do {
                     if (tid == 0) po_trial_thread0(&S);
                     __syncthreads();
@@ -183,9 +187,15 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
                         else { S.lambda *= S.ni; S.ni *= 2; S.pose = S.backup; }
                     }
                     if (good) currentChi = tempChi;
+                    accepted |= good;
                     __syncthreads();
                     qmax++;
                 } while (rho < 0 && qmax < 10);
+                if (A.log && tid == 0) {   // the oracle's IterLog row of this LM iteration
+                    double* r = A.log + ((size_t)f * PO_LOG_ROWS + nRows) * 4;
+                    r[0] = currentChi; r[1] = S.lambda; r[2] = qmax; r[3] = accepted ? 1 : 0;
+                }
+                nRows++;
                 if (qmax == 10 || rho == 0) break;
                 if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
                 if (nBad >= 3) break;
@@ -197,6 +207,7 @@ __global__ void __launch_bounds__(256) k_pose_opt(PoseOptArgs A) {
     }
     if (tid == 0) {
         A.inliers[f] = n - nBadEdges;
+        if (A.nlog) A.nlog[f] = nRows;
         pose_to_Tcw32(S.pose, A.Tcw + 16 * f);
         if (A.pose64) pose_to_fp64(S.pose, A.pose64 + 7 * f);
     }
@@ -215,18 +226,33 @@ static int launch_pose_opt(cslam_optimizer* o, int nframes, size_t nCorr, PoseOp
     return CSLAM_OK;
 }
 
-extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw, const float* kp_xy, const float* inv_sigma2,
-                                       int face_w, int face_h, uint8_t* outlier, int32_t* inliers, double* pose_fp64) {
-    if (!o || nframes <= 0 || !offset || !Tcw || !inliers) { set_error("cslam_pose_optimization: bad argument"); return CSLAM_E_BADARG; }
+// Both host entry points: every key point of a frame the optimizer runs on (>= 3 correspondences) must lie on a face, checked before anything
+// is enqueued. The reference calls exit() in computeError there (include/g2o_cubemap_vertices_edges.h:52-58); the kernel would take it as the
+// lower face. log / nlog (nframes x PO_LOG_ROWS x 4, nframes) may be null.
+static int pose_opt_host(const char* fn, cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw, const float* kp_xy,
+                         const float* inv_sigma2, int face_w, int face_h, uint8_t* outlier, int32_t* inliers, double* pose_fp64, double* log, int32_t* nlog) {
+    if (!o || nframes <= 0 || !offset || !Tcw || !inliers) { set_error("%s: bad argument", fn); return CSLAM_E_BADARG; }
     if (face_w != face_h || face_w <= 0) { set_error("cube faces must be square"); return CSLAM_E_BADARG; }
+    for (int f = 0; f < nframes; f++) {
+        if (offset[f + 1] - offset[f] < 3) continue;
+        for (int e = offset[f]; e < offset[f + 1]; e++)
+            if (face_of_pixel_f(kp_xy[2 * e], kp_xy[2 * e + 1], face_w, face_h) < 0) {
+                set_error("%s: frame %d, correspondence %d: keypoint (%g,%g) is on no cube face (the reference calls exit() here)", fn, f, e - offset[f],
+                          kp_xy[2 * e], kp_xy[2 * e + 1]);
+                return CSLAM_E_BADARG;
+            }
+    }
     CSLAM_CUDA(cudaSetDevice(o->device));
     o->arena.reset();
     const int n = offset[nframes];
     PoseOptArgs A; std::memset(&A, 0, sizeof(A));
     int* d_off; float *d_T, *d_X, *d_kp, *d_w; uint8_t* d_out; int32_t* d_inl; double* d_p64;
+    double* d_log = nullptr; int32_t* d_nlog = nullptr;
     int rc;
     if ((rc = o->arena.take(&d_off, nframes + 1)) || (rc = o->arena.take(&d_T, (size_t)nframes * 16)) || (rc = o->arena.take(&d_X, (size_t)n * 3)) || (rc = o->arena.take(&d_kp, (size_t)n * 2)) ||
         (rc = o->arena.take(&d_w, n)) || (rc = o->arena.take(&d_out, n)) || (rc = o->arena.take(&d_inl, nframes)) || (rc = o->arena.take(&d_p64, (size_t)nframes * 7))) return rc;
+    // rows past a frame's count read 0
+    if (log && ((rc = o->arena.take(&d_log, (size_t)nframes * PO_LOG_ROWS * 4, true)) || (rc = o->arena.take(&d_nlog, nframes)))) return rc;
     CSLAM_CUDA(cudaMemcpyAsync(d_off, offset, (nframes + 1) * 4, cudaMemcpyHostToDevice, o->stream));
     CSLAM_CUDA(cudaMemcpyAsync(d_T, Tcw, (size_t)nframes * 64, cudaMemcpyHostToDevice, o->stream));
     if (n) {
@@ -235,7 +261,7 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
         CSLAM_CUDA(cudaMemcpyAsync(d_w, inv_sigma2, (size_t)n * 4, cudaMemcpyHostToDevice, o->stream));
     }
     A.offset = d_off; A.Tcw = d_T; A.Xw = d_X; A.kpxy = d_kp; A.invSigma2 = d_w; A.faceW = face_w; A.faceH = face_h; A.outlier = d_out; A.inliers = d_inl;
-    A.pose64 = d_p64;
+    A.pose64 = d_p64; A.log = d_log; A.nlog = d_nlog;
     if ((rc = launch_pose_opt(o, nframes, n, A))) return rc;
     // frames with < 3 correspondences are returned untouched (src/Optimizer.cpp:133-134): copy back only the others
     std::vector<float> Tout((size_t)nframes * 16);
@@ -243,9 +269,24 @@ extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const in
     if (n && outlier) CSLAM_CUDA(cudaMemcpyAsync(outlier, d_out, n, cudaMemcpyDeviceToHost, o->stream));
     CSLAM_CUDA(cudaMemcpyAsync(inliers, d_inl, nframes * 4, cudaMemcpyDeviceToHost, o->stream));
     if (pose_fp64) CSLAM_CUDA(cudaMemcpyAsync(pose_fp64, d_p64, (size_t)nframes * 56, cudaMemcpyDeviceToHost, o->stream));
+    if (log) {
+        CSLAM_CUDA(cudaMemcpyAsync(log, d_log, (size_t)nframes * PO_LOG_ROWS * 4 * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+        CSLAM_CUDA(cudaMemcpyAsync(nlog, d_nlog, (size_t)nframes * 4, cudaMemcpyDeviceToHost, o->stream));
+    }
     if ((rc = o->sync())) return rc;
     for (int f = 0; f < nframes; f++) if (offset[f + 1] - offset[f] >= 3) std::memcpy(Tcw + 16 * f, Tout.data() + 16 * f, 64);
     return CSLAM_OK;
+}
+
+extern "C" int cslam_pose_optimization(cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw, const float* kp_xy, const float* inv_sigma2,
+                                       int face_w, int face_h, uint8_t* outlier, int32_t* inliers, double* pose_fp64) {
+    return pose_opt_host("cslam_pose_optimization", o, nframes, offset, Tcw, Xw, kp_xy, inv_sigma2, face_w, face_h, outlier, inliers, pose_fp64, nullptr, nullptr);
+}
+extern "C" int cslam_pose_optimization_log(cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw, const float* kp_xy,
+                                           const float* inv_sigma2, int face_w, int face_h, uint8_t* outlier, int32_t* inliers, double* pose_fp64, double* log,
+                                           int32_t* nlog) {
+    if (!log || !nlog) { set_error("cslam_pose_optimization_log: bad argument"); return CSLAM_E_BADARG; }
+    return pose_opt_host("cslam_pose_optimization_log", o, nframes, offset, Tcw, Xw, kp_xy, inv_sigma2, face_w, face_h, outlier, inliers, pose_fp64, log, nlog);
 }
 
 // Device-resident variant for pipelines (config 5): fixed stride, per-frame counts, all pointers on the device, asynchronous on the optimizer's stream.

@@ -10,6 +10,9 @@ import numpy as np
 from ._capi import BAProblem, BAResult, Handle, check, lib, ptr
 
 
+POSE_LOG_ROWS = 40   # rows of cslam_pose_optimization_log's per-frame LM log: 4 rounds x optimize(10)
+
+
 class Optimizer(Handle):
     KIND = "optimizer"
 
@@ -56,8 +59,10 @@ class Optimizer(Handle):
         check(lib().cslam_pose_optimization_dev(self._h, int(nframes), int(stride), ptr(count), ptr(Tcw), ptr(Xw), ptr(kpxy), ptr(inv_sigma2), int(faceW), int(faceH), ptr(outlier),
                                                 ptr(inliers)))
 
-    def PoseOptimization(self, Tcw, Xw, kpxy, inv_sigma2, faceW, faceH, offset=None):
-        """Single frame (Tcw 4x4, Xw n x 3, ...) or a batch (Tcw F x 4 x 4, offset F+1 into the concatenated correspondences)."""
+    def PoseOptimization(self, Tcw, Xw, kpxy, inv_sigma2, faceW, faceH, offset=None, log=False):
+        """Single frame (Tcw 4x4, Xw n x 3, ...) or a batch (Tcw F x 4 x 4, offset F+1 into the concatenated correspondences).
+        log=True also returns the LM log: per frame up to POSE_LOG_ROWS rows of (chi2, lambda, trials, accepted), one per LM iteration with
+        every round's rows in order (nlog rows per frame; a single frame gets its rows only)."""
         Tcw = np.ascontiguousarray(Tcw, np.float32)
         single = Tcw.ndim == 2
         T = Tcw.reshape(-1, 16).copy()
@@ -68,8 +73,19 @@ class Optimizer(Handle):
         offset = np.ascontiguousarray(offset, np.int32)
         F = T.shape[0]; n = int(offset[-1])
         outlier = np.zeros(max(n, 1), np.uint8); inl = np.zeros(F, np.int32); pose64 = np.zeros((F, 7))
-        check(lib().cslam_pose_optimization(self._h, F, ptr(offset), ptr(T), ptr(Xw), ptr(kpxy), ptr(inv_sigma2), int(faceW), int(faceH), ptr(outlier), ptr(inl),
-                                            ptr(pose64)))
+        if log:
+            lg = np.zeros((F, POSE_LOG_ROWS, 4)); nlog = np.zeros(F, np.int32)
+            check(lib().cslam_pose_optimization_log(self._h, F, ptr(offset), ptr(T), ptr(Xw), ptr(kpxy), ptr(inv_sigma2), int(faceW), int(faceH), ptr(outlier),
+                                                    ptr(inl), ptr(pose64), ptr(lg), ptr(nlog)))
+        else:
+            check(lib().cslam_pose_optimization(self._h, F, ptr(offset), ptr(T), ptr(Xw), ptr(kpxy), ptr(inv_sigma2), int(faceW), int(faceH), ptr(outlier),
+                                                ptr(inl), ptr(pose64)))
         if single:
-            return dict(inliers=int(inl[0]), Tcw=T.reshape(4, 4), outlier=outlier[:n], pose64=pose64[0])
-        return dict(inliers=inl, Tcw=T.reshape(F, 4, 4), outlier=outlier[:n], pose64=pose64)
+            r = dict(inliers=int(inl[0]), Tcw=T.reshape(4, 4), outlier=outlier[:n], pose64=pose64[0])
+            if log:
+                r.update(log=lg[0, :nlog[0]], nlog=int(nlog[0]))
+            return r
+        r = dict(inliers=inl, Tcw=T.reshape(F, 4, 4), outlier=outlier[:n], pose64=pose64)
+        if log:
+            r.update(log=lg, nlog=nlog)
+        return r

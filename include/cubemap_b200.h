@@ -336,8 +336,18 @@ int cslam_pose_optimization(cslam_optimizer* o, int nframes, const int32_t* offs
                             const float* kp_xy, const float* inv_sigma2, int face_w, int face_h, uint8_t* outlier,
                             int32_t* inliers, double* pose_fp64);
 
+/* cslam_pose_optimization plus its LM log (for tests): log is nframes x 40 x 4 doubles, one row (chi2 after the iteration, lambda, trials,
+ * accepted 0/1) per LM iteration of the 4 rounds x optimize(10), every round's rows in order, zero past nlog[f] rows. In both host forms,
+ * a frame of >= 3 correspondences with a key point on no cube face is CSLAM_E_BADARG (the reference calls exit() there); the message names
+ * the frame and the correspondence (index within the frame) and nothing is written. */
+int cslam_pose_optimization_log(cslam_optimizer* o, int nframes, const int32_t* offset, float* Tcw, const float* Xw,
+                                const float* kp_xy, const float* inv_sigma2, int face_w, int face_h, uint8_t* outlier,
+                                int32_t* inliers, double* pose_fp64, double* log, int32_t* nlog);
+
 /* Device-resident PoseOptimization for pipelines: frame f owns correspondences [f*stride, f*stride + count[f]); all pointers on the device;
- * asynchronous on the optimizer's stream (cslam_optimizer_stream / cslam_optimizer_sync). */
+ * asynchronous on the optimizer's stream (cslam_optimizer_stream / cslam_optimizer_sync). Precondition, not checked (the key points are on
+ * the device): every key point lies on a cube face, as the front end's key points that cslam_tracker_gather_pose_inputs_dev
+ * passes on always do; the host forms reject one that does not. */
 int cslam_pose_optimization_dev(cslam_optimizer* o, int nframes, int stride, const int32_t* count, float* Tcw, const float* Xw, const float* kp_xy, const float* inv_sigma2,
                                 int face_w, int face_h, uint8_t* outlier, int32_t* inliers);
 void* cslam_optimizer_stream(const cslam_optimizer* o);

@@ -358,6 +358,8 @@ struct PoseOpt {
     std::vector<int> actE; double lambda = -1, ni = 2; int nBad = 0;
     double Hm[36], b[6], x[6];
     std::vector<IterLog> log;
+    std::vector<int> logRound, logStop;          // per log row: round, why the iteration ended its round (0 none, 1 qmax == 10, 2 rho == 0, 3 nBad >= 3)
+    std::vector<uint8_t> roundOutlier;           // 4 x n: the outlier flags after each round's classification
     double chi2(int e) const { return obs[e].w * (err[2 * e] * err[2 * e] + err[2 * e + 1] * err[2 * e + 1]); }
     void computeError(int e) { double Xc[3]; se3_map(pose, &Xw[3 * e], Xc); edge_error(obs[e], f, Xc, &err[2 * e]); }
     void computeActiveErrors() { for (int e : actE) computeError(e); }
@@ -398,15 +400,16 @@ struct PoseOpt {
             } else { lambda *= ni; ni *= 2; pose = backup; }
             qmax++;
         } while (rho < 0 && qmax < 10);
-        log.push_back({currentChi, lambda, qmax, accepted});
-        if (qmax == 10 || rho == 0) return 1;
+        log.push_back({currentChi, lambda, qmax, accepted}); logStop.push_back(0);
+        if (qmax == 10 || rho == 0) { logStop.back() = qmax == 10 ? 1 : 2; return 1; }
         if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
-        if (nBad >= 3) return 1;
+        if (nBad >= 3) { logStop.back() = 3; return 1; }
         return 0;
     }
     // returns inliers; outlier[e] as mvbOutlier (src/Optimizer.cpp:133-189)
     int run(uint8_t* outlier) {
-        err.assign((size_t)n * 2, 0); level.assign(n, 0); robust = true; log.clear(); pose = pose0;
+        err.assign((size_t)n * 2, 0); level.assign(n, 0); robust = true; log.clear(); logRound.clear(); logStop.clear(); pose = pose0;
+        roundOutlier.assign((size_t)4 * n, 0);
         for (int e = 0; e < n; e++) outlier[e] = 0;
         for (int k = 0; k < 6; k++) x[k] = 0;
         if (n < 3) return 0;
@@ -415,11 +418,13 @@ struct PoseOpt {
             pose = pose0;
             actE.clear(); for (int e = 0; e < n; e++) if (level[e] == 0) actE.push_back(e);
             if (!actE.empty()) { bool ok = true; for (int i = 0; i < 10 && ok; i++) ok = (lmIteration(i) == 0); }
+            logRound.resize(log.size(), it);
             nBadEdges = 0;
             for (int e = 0; e < n; e++) {
                 if (outlier[e]) computeError(e);
                 const float c = (float)chi2(e);
                 if (c > 5.991f) { outlier[e] = 1; level[e] = 1; nBadEdges++; } else { outlier[e] = 0; level[e] = 0; }
+                roundOutlier[(size_t)it * n + e] = outlier[e];
             }
             if (it == 2) robust = false;
             if (n < 10) break;

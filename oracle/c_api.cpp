@@ -241,21 +241,37 @@ int orc_local_ba(int nKF, int nMP, int nE, float* Tcw, const uint8_t* kfFixed, f
     for (int i = 0; i < n && i < logCap; i++) { log[4 * i] = ba.log[i].chi2; log[4 * i + 1] = ba.log[i].lambda; log[4 * i + 2] = ba.log[i].trials; log[4 * i + 3] = ba.log[i].accepted; }
     return n;
 }
+// rowInfo (optional): logCap x 2 ints, (round, stop) per log row as PoseOpt::logRound / logStop; roundOutlier (optional): 4 x n flags.
+// Returns -1 (nothing written) when a frame of >= 3 correspondences has a key point on no face.
 int orc_pose_opt(int n, float* Tcw, const float* Xw, const float* kpxy, const float* invSigma2, int faceW, int faceH, uint8_t* outlier,
-                 double* pose_out64, double* log, int logCap, int* nIters) {
+                 double* pose_out64, double* log, int logCap, int* nIters, int* rowInfo, uint8_t* roundOutlier) {
     PoseOpt po; po.n = n; po.W = faceW; po.H = faceH; po.f = faceW / 2.0;
     po.pose0 = se3_from_Tcw32(Tcw); po.Xw.resize((size_t)n * 3); po.obs.resize(n);
     for (int e = 0; e < n; e++) { for (int i = 0; i < 3; i++) po.Xw[3 * e + i] = (double)Xw[3 * e + i]; po.obs[e] = make_obs(kpxy[2 * e], kpxy[2 * e + 1], invSigma2[e], faceW, faceH); }
+    // a key point on no face: the reference's computeError calls exit() (only reached with >= 3 correspondences); nothing is written
+    if (n >= 3) for (int e = 0; e < n; e++) if (po.obs[e].face < 0) return -1;
     int inl = po.run(outlier);
     if (n >= 3) se3_to_Tcw32(po.pose, Tcw);   // src/Optimizer.cpp:133-134 returns before SetPose
     if (pose_out64) { pose_out64[0] = po.pose.t[0]; pose_out64[1] = po.pose.t[1]; pose_out64[2] = po.pose.t[2];
         pose_out64[3] = po.pose.r.x; pose_out64[4] = po.pose.r.y; pose_out64[5] = po.pose.r.z; pose_out64[6] = po.pose.r.w; }
     int m = (int)po.log.size();
     for (int i = 0; i < m && i < logCap; i++) { log[4 * i] = po.log[i].chi2; log[4 * i + 1] = po.log[i].lambda; log[4 * i + 2] = po.log[i].trials; log[4 * i + 3] = po.log[i].accepted; }
+    if (rowInfo) for (int i = 0; i < m && i < logCap; i++) { rowInfo[2 * i] = po.logRound[i]; rowInfo[2 * i + 1] = po.logStop[i]; }
+    if (roundOutlier && n >= 3) std::memcpy(roundOutlier, po.roundOutlier.data(), (size_t)4 * n);
     if (nIters) *nIters = m;
     return inl;
 }
 // exposed pieces for unit tests
+// PoseOptimization's classification value (float)chi2 of every edge, from errors computed at the pose pose7 (t, q) (src/Optimizer.cpp:156-163)
+void orc_pose_edge_chi2(const double* pose7, int n, const float* Xw, const float* kpxy, const float* invSigma2, int faceW, int faceH, float* chi2) {
+    SE3 T; T.t[0] = pose7[0]; T.t[1] = pose7[1]; T.t[2] = pose7[2]; T.r.x = pose7[3]; T.r.y = pose7[4]; T.r.z = pose7[5]; T.r.w = pose7[6];
+    for (int e = 0; e < n; e++) {
+        const EdgeObs o = make_obs(kpxy[2 * e], kpxy[2 * e + 1], invSigma2[e], faceW, faceH);
+        const double X[3] = {(double)Xw[3 * e], (double)Xw[3 * e + 1], (double)Xw[3 * e + 2]};
+        double Xc[3], er[2]; se3_map(T, X, Xc); edge_error(o, faceW / 2.0, Xc, er);
+        chi2[e] = (float)(o.w * (er[0] * er[0] + er[1] * er[1]));
+    }
+}
 void orc_se3_exp(const double* u, double* out7) { SE3 s = se3_exp(u); out7[0] = s.t[0]; out7[1] = s.t[1]; out7[2] = s.t[2]; out7[3] = s.r.x; out7[4] = s.r.y; out7[5] = s.r.z; out7[6] = s.r.w; }
 void orc_edge_eval(const float* Tcw, const double* X, float kx, float ky, int faceW, int faceH, double* err2, double* Jp12, double* Jx6, int* face) {
     SE3 T = se3_from_Tcw32(Tcw); EdgeObs o = make_obs(kx, ky, 1.f, faceW, faceH); double Xc[3], R[3][3], Jp[2][6], Jx[2][3];

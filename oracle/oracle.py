@@ -369,9 +369,23 @@ def pose_opt(Tcw, Xw, kpxy, inv_sigma2, faceW, faceH):
     Tcw = _f32(Tcw).copy().reshape(16); Xw = _f32(Xw); kpxy = _f32(kpxy); inv_sigma2 = _f32(inv_sigma2)
     n = Xw.shape[0]
     outlier = np.zeros(max(n, 1), np.uint8); pose64 = np.zeros(7); log = np.zeros((64, 4)); nit = C.c_int()
+    info = np.zeros((64, 2), np.int32); rounds = np.zeros((4, max(n, 1)), np.uint8)
     inl = lib().orc_pose_opt(n, _p(Tcw), _p(Xw), _p(kpxy), _p(inv_sigma2), int(faceW), int(faceH), _p(outlier), _p(pose64), _p(log), 64,
-                             C.byref(nit))
-    return dict(inliers=inl, Tcw=Tcw.reshape(4, 4), outlier=outlier[:n], pose64=pose64, log=log[:nit.value])
+                             C.byref(nit), _p(info), _p(rounds))
+    if inl < 0:
+        raise ValueError("pose_opt: a key point lies on no cube face (the reference calls exit())")
+    m = nit.value
+    # round / stop per log row (stop: 0 none, 1 qmax == 10, 2 rho == 0, 3 nBad >= 3); round_outlier: flags after each round
+    return dict(inliers=inl, Tcw=Tcw.reshape(4, 4), outlier=outlier[:n], pose64=pose64, log=log[:m], round=info[:m, 0].copy(), stop=info[:m, 1].copy(),
+                round_outlier=rounds[:, :n].copy())
+
+
+def pose_edge_chi2(pose64, Xw, kpxy, inv_sigma2, faceW, faceH):
+    """PoseOptimization's (float)chi2 of every correspondence with its error computed at the pose pose64 (t, q)."""
+    pose64 = np.ascontiguousarray(pose64, np.float64); Xw = _f32(Xw); kpxy = _f32(kpxy); inv_sigma2 = _f32(inv_sigma2)
+    n = Xw.shape[0]; out = np.zeros(max(n, 1), np.float32)
+    lib().orc_pose_edge_chi2(_p(pose64), n, _p(Xw), _p(kpxy), _p(inv_sigma2), int(faceW), int(faceH), _p(out))
+    return out[:n]
 
 
 def se3_exp(u):
