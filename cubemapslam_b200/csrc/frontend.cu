@@ -309,17 +309,30 @@ __device__ __forceinline__ uint32_t arc_score_x2(const uint32_t (&R)[16], uint32
     return __vimax3_u16x2(t1, t2, T) - T;
 }
 
+// Compass bound of the arc score of 2 pixels in u16x2 lanes, from ring pixels 0, 4, 8, 12 alone (same lane encoding as arc_score_x2).
+// 9 contiguous ring pixels always hold two neighbouring compass points 4j and 4j+4, so A <= max_j min(R[4j], R[4j+4]), which by
+// distributivity is min(max(R0, R8), max(R4, R12)); dually B >= max(min(R0, R8), min(R4, R12)). Only the centre is masked: with cl = c
+// with low bytes 0 and ch = c with low bytes 0xff, max(A, cl) - cl and ch - min(B, ch) are d << 8 | (0..255) for the bright and dark
+// margins d = max(A - c, 0), max(c - B, 0) of the high bytes, whatever the low bytes hold. Returned per lane: max(those, acc); with
+// acc = T1 = t << 8 | 0xff (or a previous result) that is T1 exactly where neither margin exceeds t: where the arc score is provably <= t.
+__device__ __forceinline__ uint32_t compass_x2(uint32_t r0, uint32_t r4, uint32_t r8, uint32_t r12, uint32_t c, uint32_t acc) {
+    const uint32_t A = __vminu2(__vmaxu2(r0, r8), __vmaxu2(r4, r12));
+    const uint32_t Bm = __vmaxu2(__vminu2(r0, r8), __vminu2(r4, r12));
+    const uint32_t cl = c & 0xff00ff00u, ch = c | 0x00ff00ffu;
+    return __vimax3_u16x2(__vmaxu2(A, cl) - cl, ch - __vminu2(Bm, ch), acc);   // lanes never borrow
+}
+
 // q = i / d for 0 <= i < 65536/..: d-uniform fast division (tile loops have i < 8192, d <= 64)
 __device__ __forceinline__ int fdiv_small(int i, uint32_t magic) { return (int)(((uint32_t)i * magic) >> 20); }
 __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d - 1) / d; }
 
 // Layout of one CTA: one tile column (CG cells wide) of FAST_R consecutive cell rows of one frame, walked tile by tile (a tile = CG cells of
 // one cell row, exactly the reference's per-cell ROIs). Phases of each tile:
-//  A  branch-free exact arc score of every detection pixel (4 pixels per work item) -> S (u16, (s - mt) << 8, 0 where s <= mt; mt = minTh clamped to
-//     1..255, see below).
-//     On the warp path (`live` given) only the tile's live work items are scored: every other item's 7x7 windows hold one constant
-//     (DevLevels::live), so its scores are 0, which the zeroed S already holds. Each warp appends the items it scored non-zero to the
-//     tile's nz list (one shared atomic per warp)
+//  A0 compass pretest of every work item (4 pixels): an item goes to the tile's pass list (one shared atomic per warp) unless the compass
+//     bound (compass_x2) proves all 4 of its scores <= mt (mt = minTh clamped to 1..255, see below). On the warp path (`live` given) only
+//     the tile's live work items are tested: every other item's 7x7 windows hold one constant (DevLevels::live), so its scores are 0
+//  A  branch-free exact arc score of every pass-list item -> S (u16, (s - mt) << 8, 0 where s <= mt). An item left out scores 0, which the
+//     zeroed S already holds. Each warp appends the items it scored non-zero to the tile's nz list (one shared atomic per warp)
 //  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the nz list -> shared list; a keypoint at
 //     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
 //  C  the selected entries (the per-cell fallback filter) appended to the strip's output buffer, one shared atomic per warp; the buffer is
@@ -368,8 +381,10 @@ struct FastCols {
 // Dynamic shared memory of a k_fast CTA (byte offsets), sized from the level's cell geometry; CELL_MAX bounds it (fast_smem_max)
 struct FastSmem {
     int items;                 // the tile column's FastCols::item table
+    int pass;                  // the current tile's items the compass bound could not prove corner-free (u16, encoded as the live list):
+                               // phase A's work list. Its own region, like the nz list
     int nz;                    // the current tile's items phase A scored non-zero (u16, encoded as the live list): phase B's work list.
-                               // Its own region: warps append ahead of other warps' live-list reads, and the other buffers hold the next tile
+                               // Its own region: warps append ahead of other warps' pass-list reads, and the other buffers hold the next tile
     int tile, tileBytes;     // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
                                // then hCell + 6 rows of FAST_TS
     int s2, klist;             // score map (hCell + 2 rows of FAST_SW pair-words); NMS survivors, kmax entries
@@ -384,7 +399,8 @@ __host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
     const int nzCap = max(g.liveCap, ((CG * g.wCell + 6) >> 2) * g.hCell);
     m.items = 0;
     m.nz = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);   // a constant offset: no register holds its address
-    m.tile = m.nz + 16 * ((nzCap + 7) / 8);
+    m.pass = m.nz + 16 * ((nzCap + 7) / 8);
+    m.tile = m.pass + 16 * ((nzCap + 7) / 8);
     m.s2 = m.tile + 2 * m.tileBytes;
     m.live = m.s2 + (g.hCell + 2) * FAST_SW * 4;
     m.klist = m.live + 2 * m.liveBytes;
@@ -417,7 +433,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
     __shared__ int rowVisit[FAST_R];                    // the strip row's tile has work (not skipped, detection rows > 0)
     __shared__ uint32_t sout[FAST_OUT];   // the strip's selected candidates, packed as in cand
     __shared__ int cnt20[CG];
-    __shared__ int nK, nNZ, nOut, flushN;
+    __shared__ int nK, nPass, nNZ, nOut, flushN;
     __shared__ uint32_t flushBase;
     const int frame = blockIdx.z, row0 = blockIdx.y * FAST_R, nr = min(FAST_R, g.nRowsEff - row0);
     const int tid = threadIdx.x, lane = tid & 31;
@@ -479,11 +495,13 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         }
     };
     // Barriers of one tile (buffer b = tile parity in the strip):
-    //  top   S2 cleared, nK / nNZ / cnt20 reset: the previous tile's phases B and C are done with them (its end barrier)
+    //  top   S2 cleared, nK / nPass / nNZ / cnt20 reset: the previous tile's phases A, B and C are done with them (its end barrier), or it
+    //        ended at BP with nPass = 0 and read nothing else after B1
     //  wait  this thread's copies of the tile landed; B1 (__syncthreads_or) makes every thread's copies visible
     //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phase A, before its B2
-    //  A (reads the live list of b; appends to the nz list, nNZ) -> B2 -> B (S2, item table, nz list, nNZ) -> B3 -> C (klist, nK, cnt20;
-    //  appends to the output buffer) -> end barrier
+    //  A0 (reads the live list of b; appends to the pass list, nPass) -> BP -> A (pass list, nPass; appends to the nz list, nNZ) -> B2 ->
+    //  B (S2, item table, nz list, nNZ) -> B3 -> C (klist, nK, cnt20; appends to the output buffer) -> end barrier
+    //  a tile whose pass list is empty has no corner: after BP it goes on to the next tile as the !any path does after B1
     //  after the end barrier: flush when the buffer could not hold another tile's kmax entries, and at the end of the strip (one barrier
     //  more; the next appends follow the next tile's B1)
     for (int b = 0;; b ^= 1) {
@@ -501,7 +519,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
             }
         }
         if (tid < CG) cnt20[tid] = 0;
-        if (tid == 0) { nK = 0; nNZ = 0; }
+        if (tid == 0) { nK = 0; nPass = 0; nNZ = 0; }
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         // caller canvases: an all-zero tile has no corners at any threshold (OR of the columns this thread staged)
         uint32_t acc = live ? 1u : 0u;
@@ -519,6 +537,45 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
             cur = next;
             continue;
         }
+        // ---- A0: the compass words of score_item (rows 0, 3 and 6 of the item: ring 0, 4 / 12 and centre, 8) and their bound.
+        // compass_x2 ignores the low bytes, so the words of centres 0 and 2 need not be funnel shifts: a word shifted left by 8 bits puts
+        // its bytes 0 and 2 in the high bytes of its lanes (a multiply by 256, on the FMA pipe rather than the integer pipe). Ring 0 / 8
+        // of centres 0, 2 are bytes 0, 2 of the row-0 / row-6 word, ring 4 the same of ring 4's word of centres 1, 3 (V4), ring 12 bytes 1, 3
+        // of the word left of the centre row (m), and the centres bytes 0, 2 of the centre word.
+        {
+            const int w0 = X.w0;
+            const uint32_t T1 = T | 0x00ff00ffu;
+            auto passes = [&](int e) {   // e: the item, encoded as the live list
+                const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + (e >> 6) * FAST_TS + 4 * (w0 + (e & 63)));
+                const int RS = FAST_TS / 4;
+                const uint32_t* r3 = r0 + 3 * RS; const uint32_t* r6 = r0 + 6 * RS;
+                const uint32_t uc = r0[0], m = r3[-1], c = r3[0], p = r3[1], dc = r6[0];
+                const uint32_t V4 = __funnelshift_r(c, p, 24);
+                const uint32_t b02 = compass_x2(uc * 256u, V4 * 256u, dc * 256u, m, c * 256u, T1);
+                return compass_x2(uc, V4, dc, __funnelshift_r(m, c, 8), c, b02) != T1;
+            };
+            // items that can score go to the pass list in the same encoding (ptxas aggregates the atomic: one ATOMS per warp)
+            uint16_t* const passS = reinterpret_cast<uint16_t*>(fsm + SM.pass);
+            if (live) {
+                for (uint32_t it = tid; it < nLive; it += 256) {
+                    const int e = liveS[it];
+                    if (passes(e)) passS[atomicAdd(&nPass, 1)] = (uint16_t)e;
+                }
+            } else {
+                const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
+                for (int it = tid; it < nw * ny; it += 256) {
+                    const int y = fdiv_small(it, mgItems), e = y << 6 | (it - y * nw);
+                    if (passes(e)) passS[atomicAdd(&nPass, 1)] = (uint16_t)e;
+                }
+            }
+        }
+        __syncthreads();   // BP
+        const int npass = nPass;
+        if (npass == 0) {   // no item can score: nothing reads S2, the lists, the counters or buffer b after BP
+            if (next == nr) break;
+            cur = next;
+            continue;
+        }
         // ---- A
         {
             const int w0 = X.w0;
@@ -528,42 +585,44 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
                 const int RS = FAST_TS / 4;
                 // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
                 // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
-                // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle
+                // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle.
+                // arc_score_x2 reads only the high bytes, so where U[k] is no loaded word it is V[k] shifted left by 8 bits (V[k]'s low
+                // bytes are U's pixels): a multiply by 256 on the FMA pipe instead of a funnel shift on the integer pipe
                 uint32_t V[16], U[16], Cv, Cu;
                 {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
                     const uint32_t m = r0[-1], c = r0[0], p = r0[1];
                     V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
-                    U[15] = __funnelshift_r(m, c, 16); U[0] = V[15]; U[1] = c;
+                    U[15] = V[15] * 256u; U[0] = V[15]; U[1] = c;
                 }
                 {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
                     const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
-                    U[14] = __funnelshift_r(m, c, 8); U[2] = __funnelshift_r(c, p, 8);
+                    U[14] = V[14] * 256u; U[2] = V[2] * 256u;
                 }
                 {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
                     const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
-                    U[13] = m; U[3] = __funnelshift_r(c, p, 16);
+                    U[13] = m; U[3] = V[3] * 256u;
                 }
                 {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
                     const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
-                    U[12] = m; U[4] = __funnelshift_r(c, p, 16); Cu = __funnelshift_r(m, c, 24);
+                    U[12] = m; U[4] = V[4] * 256u; Cu = c * 256u;
                 }
                 {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
                     const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
-                    U[11] = m; U[5] = __funnelshift_r(c, p, 16);
+                    U[11] = m; U[5] = V[5] * 256u;
                 }
                 {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
                     const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
-                    U[10] = __funnelshift_r(m, c, 8); U[6] = __funnelshift_r(c, p, 8);
+                    U[10] = V[10] * 256u; U[6] = V[6] * 256u;
                 }
                 {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
                     const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
                     V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
-                    U[9] = __funnelshift_r(m, c, 16); U[8] = V[9]; U[7] = c;
+                    U[9] = V[9] * 256u; U[8] = V[9]; U[7] = c;
                 }
                 const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
                 // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
@@ -575,26 +634,16 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
                         make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
                 return nz;
             };
-            // items scored non-zero go to the tile's nz list, encoded as the live list (y<<6 | (wi - w0)). ptxas aggregates the atomic: one
-            // ATOMS per warp (tools/kfast_sass.py). The entry is formed again after the score rather than held across it (register pressure)
+            // items scored non-zero go to the tile's nz list, in the same encoding. ptxas aggregates the atomic: one ATOMS per warp
+            // (tools/kfast_sass.py). The entry is read again after the score rather than held across it (register pressure)
+            const uint16_t* const passS = reinterpret_cast<const uint16_t*>(fsm + SM.pass);
             uint16_t* const nzS = reinterpret_cast<uint16_t*>(fsm + SM.nz);
-            if (live) {
-                for (uint32_t it = tid; it < nLive; it += 256) {
-                    const int e = liveS[it];
-                    if (score_item(e >> 6, w0 + (e & 63))) nzS[atomicAdd(&nNZ, 1)] = liveS[it];
-                }
-            } else {
-                const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
-                for (int it = tid; it < nw * ny; it += 256) {
-                    const int y = fdiv_small(it, mgItems);
-                    if (score_item(y, w0 + (it - y * nw))) {
-                        const int y2 = fdiv_small(it, mgItems);
-                        nzS[atomicAdd(&nNZ, 1)] = (uint16_t)(y2 << 6 | (it - y2 * nw));
-                    }
-                }
+            for (int it = tid; it < npass; it += 256) {
+                const int e = passS[it];
+                if (score_item(e >> 6, w0 + (e & 63))) nzS[atomicAdd(&nNZ, 1)] = passS[it];
             }
         }
-        __syncthreads();
+        __syncthreads();   // B2
         // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
         // non-zero only inside an item phase A scored non-zero, so B walks the tile's nz list; one thread reads the item's 3 x 4 pair-word
         // neighbourhood once.
@@ -658,7 +707,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         if (nOut > FAST_OUT - SM.kmax) flush();
         cur = next;
     }
-    if (nOut > 0) flush();   // after the last tile's end barrier or B1
+    if (nOut > 0) flush();   // after the last tile's end barrier, B1 or BP
 }
 
 // ------------------------------------------------------------------------------------------------- k_distribute

@@ -9,6 +9,10 @@ of fast_tile_x in frontend.cu). Per level, summed over --frames frames, one JSON
                    before the nz list (within 1 % of the real live lists, DESIGN.md section 4)
   nz_items         live items with a pixel of the detection area whose score is above minThFAST: what phase B scores now
   nz_fraction      nz_items / live_items
+  compass_items    live items with a pixel of the detection area that the compass bound cannot prove corner-free (compass_x2 in
+                   frontend.cu): what phase A0 passes on to phase A (it also tests the item's pixels outside the detection area, so
+                   the kernel's pass lists can be slightly longer)
+  compass_fraction compass_items / live_items
   zero_warp_groups share of 32-item groups of a tile's live items (one warp's items in one pass) that hold no nz item: what phase B's
                    early return for an all-zero item already skipped as a whole warp
 
@@ -45,14 +49,28 @@ def fast_scores(img):
     return out
 
 
+def compass_pass(img, minth):
+    """True where the compass bound of the arc score exceeds mt = minth clamped to 1..255: min(max(R0, R8), max(R4, R12)) > c + mt or
+    max(min(R0, R8), min(R4, R12)) < c - mt (0 within 3 of the border)."""
+    h, w = img.shape
+    mt = min(max(minth, 1), 255)
+    c = img[3:h - 3, 3:w - 3].astype(np.int16)
+    r0, r4, r8, r12 = (img[3 + dy:h - 3 + dy, 3 + dx:w - 3 + dx].astype(np.int16) for dx, dy in (RING[0], RING[4], RING[8], RING[12]))
+    ua = np.minimum(np.maximum(r0, r8), np.maximum(r4, r12))
+    lb = np.maximum(np.minimum(r0, r8), np.minimum(r4, r12))
+    out = np.zeros((h, w), bool)
+    out[3:h - 3, 3:w - 3] = (ua - c > mt) | (c - lb > mt)
+    return out
+
+
 def single_valued(img):
     """True where the 7x7 window centred on the pixel holds one value."""
     from scipy.ndimage import maximum_filter, minimum_filter
     return maximum_filter(img, size=7, mode="nearest") == minimum_filter(img, size=7, mode="nearest")
 
 
-def tile_items(score, flat, minth, minB, maxBX, maxBY, wCell, hCell, nColsEff, nRowsEff):
-    """Per k_fast tile, its items in list order (detection row, then item): (live, nz) boolean vectors."""
+def tile_items(score, flat, cpass, minth, minB, maxBX, maxBY, wCell, hCell, nColsEff, nRowsEff):
+    """Per k_fast tile, its items in list order (detection row, then item): (live, nz, compass) boolean vectors."""
     for cy in range(nRowsEff):
         iniY = minB + cy * hCell
         ny = min(iniY + hCell + 6, maxBY) - iniY - 6
@@ -72,7 +90,8 @@ def tile_items(score, flat, minth, minB, maxBX, maxBY, wCell, hCell, nColsEff, n
             cc = np.clip(cols, 0, score.shape[1] - 1)
             lv = ~flat[ys][:, cc] & valid
             nz = (score[ys][:, cc] > minth) & valid
-            yield lv.reshape(ny, -1, 4).any(2).ravel(), nz.reshape(ny, -1, 4).any(2).ravel()
+            cp = cpass[ys][:, cc] & valid
+            yield tuple(m.reshape(ny, -1, 4).any(2).ravel() for m in (lv, nz, cp))
 
 
 def main():
@@ -88,20 +107,21 @@ def main():
     cp = orc.cam_params(cfg)
     m1, m2 = orc.build_maps(cp)
     mask = bench.load_mask()
-    levels = [dict(live_items=0, nz_items=0, groups=0, zero_groups=0) for _ in range(o.nlevels)]
+    levels = [dict(live_items=0, nz_items=0, compass_items=0, groups=0, zero_groups=0) for _ in range(o.nlevels)]
     for f in range(args.frames):
         ex = orc.ORBextractor(o.nfeatures, o.scale_factor, o.nlevels, o.ini_th_fast, o.min_th_fast, cp.faceW, cp.faceH)
         ex(orc.warp(cp, synth.fisheye_frame(cfg, f), m1, m2), mask)
         for l in range(o.nlevels):
             img = ex.level_image(l)
             h, w = img.shape
-            score, flat = fast_scores(img), single_valued(img)
+            score, flat, cpass = fast_scores(img), single_valued(img), compass_pass(img, o.min_th_fast)
             L = levels[l]
             L["side"] = w
-            for live, nz in tile_items(score, flat, o.min_th_fast, *_grid(w, h)):
+            for live, nz, comp in tile_items(score, flat, cpass, o.min_th_fast, *_grid(w, h)):
                 nzl = nz[live]                                       # the live list, in k_fast's order
                 L["live_items"] += int(live.sum())
                 L["nz_items"] += int(nzl.sum())
+                L["compass_items"] += int(comp[live].sum())
                 for g in range(0, len(nzl), 32):
                     L["groups"] += 1
                     L["zero_groups"] += int(not nzl[g:g + 32].any())
@@ -109,10 +129,13 @@ def main():
     for L in levels:
         out.append({"side": L["side"], "live_items": L["live_items"] // args.frames, "nz_items": L["nz_items"] // args.frames,
                     "nz_fraction": round(L["nz_items"] / max(L["live_items"], 1), 4),
+                    "compass_items": L["compass_items"] // args.frames,
+                    "compass_fraction": round(L["compass_items"] / max(L["live_items"], 1), 4),
                     "zero_warp_groups": round(L["zero_groups"] / max(L["groups"], 1), 4)})
-    tl = sum(L["live_items"] for L in levels); tn = sum(L["nz_items"] for L in levels)
+    tl, tn, tc = (sum(L[k] for L in levels) for k in ("live_items", "nz_items", "compass_items"))
     print(json.dumps({"frames": args.frames, "min_th_fast": o.min_th_fast, "per_frame": out,
-                      "total": {"live_items": tl // args.frames, "nz_items": tn // args.frames, "nz_fraction": round(tn / max(tl, 1), 4)}}))
+                      "total": {"live_items": tl // args.frames, "nz_items": tn // args.frames, "nz_fraction": round(tn / max(tl, 1), 4),
+                                "compass_items": tc // args.frames, "compass_fraction": round(tc / max(tl, 1), 4)}}))
 
 
 if __name__ == "__main__":

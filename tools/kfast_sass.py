@@ -13,6 +13,8 @@ object:
                                        the u16 live list (staged in shared memory); `append`: the instructions of its body that append a non-zero
                                        item to the nz list (the atomic ptxas aggregates per warp and the u16 store: VOTEU, FLO, POPC, S2R, SHFL,
                                        ATOMS, STS.U16 and the uniform address arithmetic)
+  phase_a0                             each compass-pretest loop (a loop without a barrier whose body issues fewer than 64 VIMNMX3 / VIMNMX, a
+                                       shared-memory atomic and a u16 store: the pass-list append), with `live` and `append` as for phase_a
   phase_b                              each NMS loop (a loop with a shared-memory atomic, VIMNMX3 and no barrier)
   compaction                           the other loops with a shared-memory atomic and no barrier (NMS survivors, phase C)
   each loop                            [start, end] byte offsets, the body's instruction count and its opcode histogram
@@ -101,7 +103,7 @@ def main():
             cubin = os.path.join(tmp, "frontend.cubin")
             res = compile_cubin(cubin)
         insns = k_fast_sass(cubin)
-    strip, phase_a, phase_b, compaction, staging = [], [], [], [], []
+    strip, phase_a0, phase_a, phase_b, compaction, staging = [], [], [], [], [], []
     for lo, hi in loops(insns):
         b = body(insns, lo, hi)
         h = hist(b)
@@ -110,20 +112,21 @@ def main():
         if minmax >= 64 and h.get("BAR", 0):
             entry["bar"], entry["atomg"] = h.get("BAR", 0), h.get("ATOMG", 0)
             strip.append(entry)
-        elif minmax >= 64:
+        elif minmax >= 64 or (h.get("ATOMS", 0) and not h.get("BAR", 0) and any(op.startswith("STS.U16") for op, _ in b)):
             entry["live"] = any(op.startswith("LDS") and ".U16" in op for op, _ in b)
             entry["append"] = sum(1 for op, _ in b if op.split(".")[0] in APPEND or op.startswith("STS.U16"))
-            phase_a.append(entry)
+            (phase_a if minmax >= 64 else phase_a0).append(entry)
         elif h.get("ATOMS", 0) and not h.get("BAR", 0):
             (phase_b if h.get("VIMNMX3", 0) else compaction).append(entry)
         elif h.get("LDGSTS", 0):
             staging.append(entry)
-    first_a = min((int(e["range"][0], 16) for e in strip + phase_a), default=insns[-1][0] + 1)
+    first_a = min((int(e["range"][0], 16) for e in strip + phase_a0 + phase_a), default=insns[-1][0] + 1)
     pro = [op for a, op, _ in insns if a < first_a and op != "NOP"]
     pro_h = Counter(op.split(".")[0] for op in pro)
     out = dict(res)
     out["prologue"] = {"instructions": len(pro), "I2F": pro_h.get("I2F", 0), "MUFU": pro_h.get("MUFU", 0), "F2I": pro_h.get("F2I", 0)}
     out["strip"] = strip
+    out["phase_a0"] = phase_a0
     out["phase_a"] = phase_a
     out["phase_b"] = phase_b
     out["compaction"] = compaction
