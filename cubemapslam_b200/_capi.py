@@ -37,7 +37,7 @@ class BAProblem(C.Structure):
 
 class BAResult(C.Structure):
     _fields_ = [("outlier", C.c_void_p), ("pose_fp64", C.c_void_p), ("points_fp64", C.c_void_p), ("lm_log", C.c_void_p),
-                ("log_cap", C.c_int32), ("iterations", C.c_int32), ("trials", C.c_int32)]
+                ("log_cap", C.c_int32), ("iterations", C.c_int32), ("trials", C.c_int32), ("stop_after_trials", C.c_int32)]
 
 
 _lib = None

@@ -26,6 +26,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <cstring>
+#include <limits>
 #include <vector>
 #include "optimizer.cuh"
 
@@ -53,7 +54,8 @@ struct BADev {
     const int4* tuples;              // (a1, a2, landmark, -): the landmark rides along so that k_ba_schur has no tuple -> edge -> landmark load chain
     double *Hpp, *bp, *Hll, *bl, *Hpl, *Dinv, *db, *xp, *xl;
     double *S, *bpr;                 // the reduced camera system [S n*n | g n | bpr n] in BAHost::red; k_ba_solve reads g as row n of S
-    double* scal;                    // [0] chi2, [1] scale, [2] max diag (as bits), [3] solve flag, [4] lambda of the current trial
+    double* scal;                    // [0] chi2, [1] scale, [2] max diag (as bits), [3] solve flag, [4] lambda of the current trial,
+                                     // [5] 1 + largest key of a NaN diagonal, [6] 1 + largest key (as bits; 0 = none; see k_ba_diag_keys)
     double* part; unsigned* ticket;  // block partials + arrival counter of the deterministic grid reductions
     double* posePart; unsigned* poseTicket;   // k_ba_lin_poses: slice sums [nQ][POSE_SPLIT][27] + arrival counter per pose
     int robust; double delta, dsqr;
@@ -224,16 +226,35 @@ __global__ void __launch_bounds__(256) k_ba_lin_poses(BADev D) {
     if (threadIdx.x < 6) D.bp[6 * p + threadIdx.x] = red[0][21 + threadIdx.x];
 }
 
-// computeLambdaInit: max |H_jj| over all active free vertices (integer atomicMax of the bit pattern: order independent)
-__global__ void __launch_bounds__(256) k_ba_maxdiag(BADev D) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    double m = 0;
-    if (i < D.nP * 6) m = fabs(D.Hpp[36 * (i / 6) + 7 * (i % 6)]);
+// computeLambdaInit (optimization_algorithm_levenberg.cpp:166-178) runs m = std::max(fabs(H_jj), m) in index-mapping order: free poses, then
+// active points, each vertex's diagonal in order. std::max returns its first argument when a comparison involves NaN, so a NaN diagonal sets
+// m = NaN and the next diagonal replaces it: m is the maximum over the diagonals after the LAST NaN one, or NaN when that NaN is the last
+// diagonal. Key of diagonal j: 6 p + j for free pose p, 6 nP + 3 l + j for active landmark l (the global index keeps the order) = the thread
+// index i below. Two order-free steps, atomicMax of bit patterns of non-negative doubles: the largest NaN key and the largest key
+// (k_ba_diag_keys), then the largest |H_jj| above the NaN key (k_ba_maxdiag).
+__device__ __forceinline__ bool diag_of_key(const BADev& D, int i, double* d) {
+    if (i < D.nP * 6) { *d = D.Hpp[36 * (i / 6) + 7 * (i % 6)]; return true; }
     const int j = i - D.nP * 6;
-    if (j >= 0 && j < D.nMP * 3) { const int l = j / 3; if (D.ptAct[l]) m = fabs(D.Hll[9 * l + 4 * (j % 3)]); }
+    if (j < D.nMP * 3 && D.ptAct[j / 3]) { *d = D.Hll[9 * (j / 3) + 4 * (j % 3)]; return true; }
+    return false;
+}
+__device__ __forceinline__ void warp_max_to(double m, double* dst) {   // m >= 0
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(reinterpret_cast<unsigned long long*>(&D.scal[2]), (unsigned long long)__double_as_longlong(m));
+    if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(reinterpret_cast<unsigned long long*>(dst), (unsigned long long)__double_as_longlong(m));
+}
+__global__ void __launch_bounds__(256) k_ba_diag_keys(BADev D) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    double d = 0;
+    const bool act = diag_of_key(D, i, &d);
+    warp_max_to(act && isnan(d) ? i + 1.0 : 0.0, &D.scal[5]);
+    warp_max_to(act ? i + 1.0 : 0.0, &D.scal[6]);
+}
+__global__ void __launch_bounds__(256) k_ba_maxdiag(BADev D) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    double d = 0;
+    const bool act = diag_of_key(D, i, &d) && i + 1.0 > D.scal[5];
+    warp_max_to(act ? fabs(d) : 0.0, &D.scal[2]);
 }
 
 // Dinv = (Hll + lambda I)^-1 (3x3 cofactors, like Eigen), db = Dinv * bl
@@ -686,7 +707,8 @@ __global__ void __launch_bounds__(SOLVE_T) k_ba_solve(BADev D, double* __restric
     for (int i = tid; i < n; i += SOLVE_T) D.xp[i] = y[i];
 }
 
-// xl = Dinv (bl - Hpl^T xp)   (block_solver.hpp:461-481)
+// xl = Dinv (bl - Hpl^T xp)   (block_solver.hpp:461-481). A failed reduced solve (scal[3] != 0) left xp unwritten: the trial is a zero step
+// (xl = 0 here, xp taken as 0 by k_ba_update and k_ba_scale), as the LM loop models LinearSolver failure.
 __global__ void __launch_bounds__(128) k_ba_backsub(BADev D) {
     const int l = (blockIdx.x * blockDim.x + threadIdx.x) / LM_LANES, sub = threadIdx.x % LM_LANES;
     const bool in = l < D.nMP, act = in && D.ptAct[l];
@@ -706,7 +728,7 @@ __global__ void __launch_bounds__(128) k_ba_backsub(BADev D) {
 #pragma unroll
     for (int j = 0; j < 3; j++) { cl[j] += __shfl_xor_sync(0xffffffffu, cl[j], 1); cl[j] += __shfl_xor_sync(0xffffffffu, cl[j], 2); }
     if (!in || sub) return;
-    if (!act) { D.xl[3 * l] = 0; D.xl[3 * l + 1] = 0; D.xl[3 * l + 2] = 0; return; }
+    if (!act || D.scal[3] != 0.0) { D.xl[3 * l] = 0; D.xl[3 * l + 1] = 0; D.xl[3 * l + 2] = 0; return; }
 #pragma unroll
     for (int j = 0; j < 3; j++) cl[j] = D.bl[3 * l + j] - cl[j];
     const double* Di = D.Dinv + DINV_LD * (size_t)l;
@@ -719,7 +741,7 @@ __device__ __noinline__ Pose pose_oplus_ba(const Pose& est, const double* u) { r
 // push() + oplus (base_vertex.h:96-99, types_six_dof_expmap.h:73-76, types_sba.h:52-56)
 __global__ void __launch_bounds__(256) k_ba_update(BADev D) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < D.nKF) { const Pose T = D.pose[i]; D.poseBak[i] = T; const int p = D.poseIdx[i]; if (p >= 0) D.pose[i] = pose_oplus_ba(T, D.xp + 6 * p); }
+    if (i < D.nKF) { const Pose T = D.pose[i]; D.poseBak[i] = T; const int p = D.poseIdx[i]; if (p >= 0 && D.scal[3] == 0.0) D.pose[i] = pose_oplus_ba(T, D.xp + 6 * p); }
     if (i < D.nMP) {
         const double x = D.X[3 * i], y = D.X[3 * i + 1], z = D.X[3 * i + 2];
         D.Xbak[3 * i] = x; D.Xbak[3 * i + 1] = y; D.Xbak[3 * i + 2] = z;
@@ -733,13 +755,14 @@ __global__ void __launch_bounds__(256) k_ba_restore(BADev D) {
     if (i < D.nMP) { D.X[3 * i] = D.Xbak[3 * i]; D.X[3 * i + 1] = D.Xbak[3 * i + 1]; D.X[3 * i + 2] = D.Xbak[3 * i + 2]; }
 }
 
-// computeScale: sum_j x_j (lambda x_j + b_j); the pose part is added by rank 0 only (replicated), landmarks by their owner
+// computeScale: sum_j x_j (lambda x_j + b_j); the pose part is added by rank 0 only (replicated), landmarks by their owner. After a failed
+// solve x = 0 goes through the same formula (a NaN lambda or b still gives NaN, as in the LM loop)
 __global__ void __launch_bounds__(256) k_ba_scale(BADev D, double* out) {
     __shared__ double sh[32];
     const double lambda = D.scal[4];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     double v = 0;
-    if (i < D.n && D.rank == 0) v = D.xp[i] * (lambda * D.xp[i] + D.bpr[i]);
+    if (i < D.n && D.rank == 0) { const double x = D.scal[3] == 0.0 ? D.xp[i] : 0.0; v = x * (lambda * x + D.bpr[i]); }
     const int j = i - D.n;
     if (j >= 0 && j < 3 * D.nMP) { const int l = j / 3; if (D.ptAct[l]) v = D.xl[j] * (lambda * D.xl[j] + D.bl[j]); }
     double tot;
@@ -1002,13 +1025,14 @@ struct BAHost {
     double* HppFull = nullptr;        // multi-GPU: all-reduced copy of the pose blocks for computeLambdaInit
     size_t xstride = 0;               // one-shot path: doubles between the two payload buffers of an exchange region
     int* d_xerr = nullptr;
-    double lambda = -1, ni = 2; int nBad = 0; int iterations = 0, trials = 0;
+    double lambda = -1, ni = 2; int nBad = 0; int iterations = 0, trials = 0, stopAfterTrials = 0;
     bool errorsCurrent = false; double lastChi = 0;   // D.err / chi2 belong to the current state (set by an accepted trial)
     const volatile uint8_t* stop = nullptr;
     bool useOneShot = false;
     cudaGraphExec_t trialGraph = nullptr; int64_t launchesPerTrial = 0;
     ~BAHost() { drop_graph(); }
-    bool terminate() const { return stop ? (*stop != 0) : false; }
+    // pbStopFlag; stopAfterTrials (a test hook, 0 = off): as if the flag became non-zero right after that trial of the call
+    bool terminate() const { return (stop && *stop != 0) || (stopAfterTrials > 0 && trials >= stopAfterTrials); }
     size_t payload() const { return (size_t)D.n * D.n + 2 * (size_t)D.n; }
     void tick(int kind) { o->timer.record(o->stream, kind); }
     void drop_graph() { if (trialGraph) { cudaGraphExecDestroy(trialGraph); trialGraph = nullptr; } }
@@ -1192,16 +1216,20 @@ struct BAHost {
     int lambda_init(double* lam) {
         int rc;
         CSLAM_CUDA(cudaMemsetAsync(D.scal + 2, 0, sizeof(double), o->stream));
+        CSLAM_CUDA(cudaMemsetAsync(D.scal + 5, 0, 2 * sizeof(double), o->stream));
         BADev M = D;
         if (o->nranks > 1 && D.nP > 0) {   // computeLambdaInit needs the full pose blocks: sum a COPY of the partial blocks once per optimize()
             CSLAM_CUDA(cudaMemcpyAsync(HppFull, D.Hpp, (size_t)D.nP * 36 * 8, cudaMemcpyDeviceToDevice, o->stream));
             if ((rc = allreduce("pose blocks", HppFull, (size_t)D.nP * 36, NCCL_SUM))) return rc;
             M.Hpp = HppFull;
         }
+        k_ba_diag_keys<<<grid(D.nP * 6 + D.nMP * 3), 256, 0, o->stream>>>(M); o->launches++;
+        if ((rc = allreduce_small(D.scal + 5, 2, true))) return rc;
         k_ba_maxdiag<<<grid(D.nP * 6 + D.nMP * 3), 256, 0, o->stream>>>(M); o->launches++;
         if ((rc = allreduce_small(D.scal + 2, 1, true))) return rc;
-        if ((rc = fetch(D.scal, 4))) return rc;
-        *lam = 1e-5 * o->h_scal[2];
+        if ((rc = fetch(D.scal, 7))) return rc;
+        const double nanKey = o->h_scal[5], lastKey = o->h_scal[6];
+        *lam = nanKey > 0 && nanKey == lastKey ? std::numeric_limits<double>::quiet_NaN() : 1e-5 * o->h_scal[2];
         return 0;
     }
     // One LM trial on the stream: lambda -> device, BlockSolver::solve (Dinv, Schur, [exchange], reduced solve, back substitution), push + oplus,
@@ -1211,6 +1239,7 @@ struct BAHost {
         CSLAM_CUDA(cudaMemcpyAsync(D.scal + 4, o->h_scal + 8, sizeof(double), cudaMemcpyHostToDevice, o->stream));   // h_scal[8] = lambda
         tick(BK_DINV);
         k_ba_dinv<<<grid(D.nMP), 256, 0, o->stream>>>(D); o->launches++;
+        CSLAM_CUDA(cudaMemsetAsync(D.scal + 3, 0, sizeof(double), o->stream));   // solve flag (no reduced system, n = 0, cannot fail)
         if (D.n > 0) {
             const bool multi = o->nranks > 1, oneShot = multi && useOneShot;
             const unsigned ep = oneShot ? ++o->epoch : 0;
@@ -1230,7 +1259,6 @@ struct BAHost {
                     k_ba_add_lambda<<<grid(D.n), 256, 0, o->stream>>>(red, D.n, lambda); o->launches++;
                 }
             }
-            CSLAM_CUDA(cudaMemsetAsync(D.scal + 3, 0, sizeof(double), o->stream));
             tick(BK_SOLVE);
             const size_t panel = 2 * (size_t)LD_NB * ldp * 8, ybytes = (size_t)D.n * 8;
             const int stage = panel + ybytes <= 200 * 1024 ? 1 : 0;
@@ -1302,16 +1330,17 @@ struct BAHost {
             rho = currentChi - tempChi;
             const double scale = o->h_scal[1] + 1e-3;
             rho /= scale;
-            if (rho > 0 && std::isfinite(tempChi) && ok2) {
+            // levenberg.cpp:126-149 as it stands: a failed solve is a zero step with tempChi = DBL_MAX, and rho is whatever that gives (NaN
+            // for an infinite currentChi or a NaN scale, which ends the trial loop on a rejected trial)
+            if (rho > 0 && std::isfinite(tempChi)) {
                 double alpha = 1. - std::pow((2 * rho - 1), 3);
                 alpha = std::min(alpha, 2. / 3.);
                 lambda *= std::max(1. / 3., alpha); ni = 2; currentChi = tempChi; accepted = 1;
-                errorsCurrent = true; lastChi = tempChi;
+                errorsCurrent = true; lastChi = o->h_scal[0];   // the trial's chi2 of this state (tempChi is DBL_MAX after a failed solve)
             } else {
                 errorsCurrent = false;   // pop(): the state is the old one again, the error array holds the trial's
                 lambda *= ni; ni *= 2;
                 k_ba_restore<<<grid(std::max(D.nKF, D.nMP)), 256, 0, o->stream>>>(D); o->launches++;
-                if (!ok2) rho = -1;
             }
             qmax++;
         } while (rho < 0 && qmax < 10 && !terminate());
@@ -1387,7 +1416,7 @@ extern "C" int cslam_local_ba(cslam_optimizer* o, cslam_ba_problem* p, const vol
     o->arena.reset();
     if (r) { r->iterations = 0; r->trials = 0; if (r->outlier) std::memset(r->outlier, 0, p->n_edges); }
     if (stop_flag && *stop_flag) return CSLAM_OK;   // src/Optimizer.cpp:359-361
-    BAHost H; H.o = o; H.p = p; H.res = r; H.stop = stop_flag; H.nEg = p->n_edges;
+    BAHost H; H.o = o; H.p = p; H.res = r; H.stop = stop_flag; H.nEg = p->n_edges; H.stopAfterTrials = r ? r->stop_after_trials : 0;
     BADev& D = H.D; std::memset(&D, 0, sizeof(D));
     D.nKF = p->n_kf; D.nMP = p->n_mp; D.f = p->face_w / 2.0; D.rank = o->rank; D.nranks = o->nranks;
     D.robust = 1; D.delta = huber_delta(); D.dsqr = D.delta * D.delta;

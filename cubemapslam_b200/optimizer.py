@@ -41,7 +41,8 @@ class Optimizer(Handle):
         id128 = np.ascontiguousarray(id128, np.uint8)
         check(lib().cslam_optimizer_init_nccl(self._h, ptr(id128), int(rank), int(nranks)))
 
-    def LocalBundleAdjustment(self, Tcw, kf_fixed, pts, eMP, eKF, kpxy, inv_sigma2, faceW, faceH, its1=5, its2=10, stop_flag=None):
+    def LocalBundleAdjustment(self, Tcw, kf_fixed, pts, eMP, eKF, kpxy, inv_sigma2, faceW, faceH, its1=5, its2=10, stop_flag=None, stop_after_trials=0):
+        """stop_after_trials=k (a test hook, 0 = off): the call behaves as if stop_flag became non-zero right after its k-th LM trial."""
         Tcw = np.ascontiguousarray(Tcw, np.float32).reshape(-1, 16).copy(); pts = np.ascontiguousarray(pts, np.float32).copy()
         kf_fixed = np.ascontiguousarray(kf_fixed, np.uint8); eMP = np.ascontiguousarray(eMP, np.int32); eKF = np.ascontiguousarray(eKF, np.int32)
         kpxy = np.ascontiguousarray(kpxy, np.float32); inv_sigma2 = np.ascontiguousarray(inv_sigma2, np.float32)
@@ -49,7 +50,7 @@ class Optimizer(Handle):
         p = BAProblem(nKF, nMP, nE, ptr(Tcw).value, ptr(kf_fixed).value, ptr(pts).value, ptr(eMP).value, ptr(eKF).value, ptr(kpxy).value,
                       ptr(inv_sigma2).value, int(faceW), int(faceH))
         outlier = np.zeros(max(nE, 1), np.uint8); pose64 = np.zeros((nKF, 7)); pts64 = np.zeros((max(nMP, 1), 3)); log = np.zeros((64, 4))
-        r = BAResult(ptr(outlier).value, ptr(pose64).value, ptr(pts64).value, ptr(log).value, 64, 0, 0)
+        r = BAResult(ptr(outlier).value, ptr(pose64).value, ptr(pts64).value, ptr(log).value, 64, 0, 0, int(stop_after_trials))
         sf = ptr(stop_flag) if stop_flag is not None else None
         check(lib().cslam_local_ba(self._h, C.byref(p), sf, int(its1), int(its2), C.byref(r)))
         return dict(Tcw=Tcw.reshape(nKF, 4, 4), pts=pts, outlier=outlier[:nE], pose64=pose64, pts64=pts64[:nMP], log=log[:r.iterations], iters=r.iterations,

@@ -93,7 +93,7 @@ struct Window {
         p.Tcw = Tcw.data(); p.kf_fixed = fixed.data(); p.points = pts.data(); p.edge_mp = eMP.data(); p.edge_kf = eKF.data(); p.kp_xy = kp.data();
         p.inv_sigma2 = w.data(); p.face_w = cam->GetCubeFaceWidth(); p.face_h = cam->GetCubeFaceHeight();
         outlier.assign(eMP.size() + 1, 0);
-        cslam_ba_result r; r.outlier = outlier.data(); r.pose_fp64 = NULL; r.points_fp64 = NULL; r.lm_log = NULL; r.log_cap = 0;
+        cslam_ba_result r; r.outlier = outlier.data(); r.pose_fp64 = NULL; r.points_fp64 = NULL; r.lm_log = NULL; r.log_cap = 0; r.stop_after_trials = 0;
         return cslam_local_ba(b200_optimizer(), &p, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), its1, its2, &r);
     }
 };

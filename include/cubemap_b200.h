@@ -312,6 +312,7 @@ typedef struct cslam_ba_result {
     int32_t log_cap;
     int32_t iterations;      /* out: LM iterations run (both optimize() calls) */
     int32_t trials;          /* out: total LM trials (linear solves) */
+    int32_t stop_after_trials; /* test hook: behave as if *stop_flag became non-zero right after this trial of the call; 0 = off */
 } cslam_ba_result;
 
 typedef struct cslam_optimizer cslam_optimizer;

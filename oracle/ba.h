@@ -198,13 +198,15 @@ struct LocalBA {
     std::vector<int> level;                      // 0 active / 1 outlier
     bool robust = true; Huber hub = make_huber();
     const volatile uint8_t* stopFlag = nullptr;
+    int stopAfterTrials = 0, trialsDone = 0;     // test hook: behave as if *stopFlag became non-zero right after trial k of the call (0 = off)
     std::vector<IterLog> log;
+    std::vector<int> logRound, logStop;          // per log row: round (0, 1), why the iteration ended its round (0 none, 1 qmax == 10, 2 rho == 0, 3 nBad >= 3, 4 stop flag)
     // active set
     std::vector<int> poseIdx, ptIdx, actE; int nP = 0, nL = 0;
     // linear system
     std::vector<double> Hpp, Hll, Hpl, bp, bl, x; double lambda = -1, ni = 2; int nBad = 0;
 
-    bool terminate() const { return stopFlag ? (*stopFlag != 0) : false; }
+    bool terminate() const { return (stopFlag && *stopFlag != 0) || (stopAfterTrials > 0 && trialsDone >= stopAfterTrials); }
     double chi2(int e) const { return obs[e].w * (err[2 * e] * err[2 * e] + err[2 * e + 1] * err[2 * e + 1]); }
 
     void initializeOptimization() {  // sparse_optimizer.cpp:206-267 + buildIndexMapping :166-190
@@ -247,7 +249,7 @@ struct LocalBA {
             }
         }
     }
-    double computeLambdaInit() const {
+    double computeLambdaInit() const {   // std::max(fabs(H_jj), m) in index-mapping order: a NaN diagonal resets the maximum (last one: NaN)
         double m = 0;
         for (int p = 0; p < nP; p++) for (int j = 0; j < 6; j++) m = std::max(std::fabs(Hpp[36 * p + 7 * j]), m);
         for (int l = 0; l < nL; l++) for (int j = 0; j < 3; j++) m = std::max(std::fabs(Hll[9 * l + 4 * j]), m);
@@ -318,12 +320,13 @@ struct LocalBA {
                 alpha = std::min(alpha, 2. / 3.);
                 lambda *= std::max(1. / 3., alpha); ni = 2; currentChi = tempChi; accepted = 1;
             } else { lambda *= ni; ni *= 2; pose = poseBackup; X = Xbackup; }   // pop
-            qmax++;
+            qmax++; trialsDone++;
         } while (rho < 0 && qmax < 10 && !terminate());
-        log.push_back({currentChi, lambda, qmax, accepted});
-        if (qmax == 10 || rho == 0) return 1;
+        log.push_back({currentChi, lambda, qmax, accepted}); logStop.push_back(0);
+        if (qmax == 10 || rho == 0) { logStop.back() = qmax == 10 ? 1 : 2; return 1; }
         if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
-        if (nBad >= 3) return 1;
+        if (nBad >= 3) { logStop.back() = 3; return 1; }
+        if (terminate()) logStop.back() = 4;
         return 0;
     }
     int optimize(int iterations) {  // sparse_optimizer.cpp:354-419
@@ -335,15 +338,17 @@ struct LocalBA {
     bool depthPositive(int e) const { double Xc[3]; se3_map(pose[eKF[e]], &X[3 * eMP[e]], Xc); return Xc[2] > 0.0; }
     // src/Optimizer.cpp:359-416 ; outlier[e]=1 for observations the reference would erase
     void run(uint8_t* outlier, int its1 = 5, int its2 = 10) {
-        err.assign((size_t)nE * 2, 0); level.assign(nE, 0); robust = true; log.clear();
+        err.assign((size_t)nE * 2, 0); level.assign(nE, 0); robust = true; log.clear(); logRound.clear(); logStop.clear(); trialsDone = 0;
         for (int e = 0; e < nE; e++) outlier[e] = 0;
         if (terminate()) return;
         initializeOptimization(); optimize(its1);
+        logRound.resize(log.size(), 0);
         bool bDoMore = !terminate();
         if (bDoMore) {
             for (int e = 0; e < nE; e++) if (chi2(e) > 5.991 || !depthPositive(e)) level[e] = 1;
             robust = false;
             initializeOptimization(); optimize(its2);
+            logRound.resize(log.size(), 1);
         }
         for (int e = 0; e < nE; e++) if (chi2(e) > 5.991 || !depthPositive(e)) outlier[e] = 1;
     }

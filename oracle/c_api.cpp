@@ -220,16 +220,19 @@ int orc_voc_transform(void* vv, const uint8_t* feats, int n, int levelsup, int* 
 // poses: nKF x 16 float32 (Tcw row-major, in/out); points: nMP x 3 float32 (in/out); edges: mp, kf, kp xy, invSigma2.
 // pose_out64: nKF x 7 (tx,ty,tz,qx,qy,qz,qw) fp64 state before the float32 cast; pts_out64: nMP x 3.
 // log: up to logCap rows of (chi2, lambda, trials, accepted). Returns the number of LM iterations run.
+// stopAfterTrials: the run behaves as if *stopFlag became non-zero right after that trial of the call (0 = off). Optional outputs: rowInfo
+// logCap x 2 ints (round, stop) per log row as LocalBA::logRound / logStop; level: nE edge levels after round 1; chi2: nE, the chi2 of
+// every edge's last computed error at the end.
 int orc_local_ba(int nKF, int nMP, int nE, float* Tcw, const uint8_t* kfFixed, float* pts, const int* eMP, const int* eKF, const float* kpxy,
                  const float* invSigma2, int faceW, int faceH, const uint8_t* stopFlag, int its1, int its2, uint8_t* outlier,
-                 double* pose_out64, double* pts_out64, double* log, int logCap) {
+                 double* pose_out64, double* pts_out64, double* log, int logCap, int stopAfterTrials, int* rowInfo, uint8_t* level, double* chi2) {
     LocalBA ba; ba.nKF = nKF; ba.nMP = nMP; ba.nE = nE; ba.W = faceW; ba.H = faceH; ba.f = faceW / 2.0;
     ba.pose.resize(nKF); ba.fixed.assign(kfFixed, kfFixed + nKF);
     for (int k = 0; k < nKF; k++) ba.pose[k] = se3_from_Tcw32(Tcw + 16 * k);
     ba.X.resize((size_t)nMP * 3); for (size_t i = 0; i < (size_t)nMP * 3; i++) ba.X[i] = (double)pts[i];
     ba.eMP.assign(eMP, eMP + nE); ba.eKF.assign(eKF, eKF + nE); ba.obs.resize(nE);
     for (int e = 0; e < nE; e++) ba.obs[e] = make_obs(kpxy[2 * e], kpxy[2 * e + 1], invSigma2[e], faceW, faceH);
-    ba.stopFlag = stopFlag;
+    ba.stopFlag = stopFlag; ba.stopAfterTrials = stopAfterTrials;
     ba.run(outlier, its1, its2);
     for (int k = 0; k < nKF; k++) {
         se3_to_Tcw32(ba.pose[k], Tcw + 16 * k);
@@ -239,7 +242,21 @@ int orc_local_ba(int nKF, int nMP, int nE, float* Tcw, const uint8_t* kfFixed, f
     for (size_t i = 0; i < (size_t)nMP * 3; i++) { pts[i] = (float)ba.X[i]; if (pts_out64) pts_out64[i] = ba.X[i]; }
     int n = (int)ba.log.size();
     for (int i = 0; i < n && i < logCap; i++) { log[4 * i] = ba.log[i].chi2; log[4 * i + 1] = ba.log[i].lambda; log[4 * i + 2] = ba.log[i].trials; log[4 * i + 3] = ba.log[i].accepted; }
+    if (rowInfo) for (int i = 0; i < n && i < logCap; i++) { rowInfo[2 * i] = ba.logRound[i]; rowInfo[2 * i + 1] = ba.logStop[i]; }
+    if (level) for (int e = 0; e < nE && !ba.level.empty(); e++) level[e] = (uint8_t)ba.level[e];
+    if (chi2) for (int e = 0; e < nE && !ba.err.empty(); e++) chi2[e] = ba.chi2(e);
     return n;
+}
+// LocalBA's classification value chi2 of every edge, from errors computed at the fp64 state pose7 (nKF x 7: t, q) and X (nMP x 3)
+void orc_ba_edge_chi2(int nE, const double* pose7, const double* X, const int* eMP, const int* eKF, const float* kpxy, const float* invSigma2,
+                      int faceW, int faceH, double* chi2) {
+    for (int e = 0; e < nE; e++) {
+        const double* p = pose7 + 7 * eKF[e];
+        SE3 T; T.t[0] = p[0]; T.t[1] = p[1]; T.t[2] = p[2]; T.r.x = p[3]; T.r.y = p[4]; T.r.z = p[5]; T.r.w = p[6];
+        const EdgeObs o = make_obs(kpxy[2 * e], kpxy[2 * e + 1], invSigma2[e], faceW, faceH);
+        double Xc[3], er[2]; se3_map(T, X + 3 * eMP[e], Xc); edge_error(o, faceW / 2.0, Xc, er);
+        chi2[e] = o.w * (er[0] * er[0] + er[1] * er[1]);
+    }
 }
 // rowInfo (optional): logCap x 2 ints, (round, stop) per log row as PoseOpt::logRound / logStop; roundOutlier (optional): 4 x n flags.
 // Returns -1 (nothing written) when a frame of >= 3 correspondences has a key point on no face.

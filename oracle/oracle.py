@@ -354,15 +354,28 @@ class Vocabulary:
 
 
 # ----------------------------------------------------------------------------- bundle adjustment
-def local_ba(Tcw, kf_fixed, pts, eMP, eKF, kpxy, inv_sigma2, faceW, faceH, its1=5, its2=10, stop_flag=None):
+def local_ba(Tcw, kf_fixed, pts, eMP, eKF, kpxy, inv_sigma2, faceW, faceH, its1=5, its2=10, stop_flag=None, stop_after_trials=0):
     Tcw = _f32(Tcw).copy(); pts = _f32(pts).copy()
     kf_fixed = _u8(kf_fixed); eMP = _i32(eMP); eKF = _i32(eKF); kpxy = _f32(kpxy); inv_sigma2 = _f32(inv_sigma2)
     nKF, nMP, nE = Tcw.shape[0], pts.shape[0], eMP.shape[0]
-    outlier = np.zeros(nE, np.uint8); pose64 = np.zeros((nKF, 7)); pts64 = np.zeros((nMP, 3)); log = np.zeros((64, 4))
+    outlier = np.zeros(max(nE, 1), np.uint8); pose64 = np.zeros((nKF, 7)); pts64 = np.zeros((max(nMP, 1), 3)); log = np.zeros((64, 4))
+    info = np.zeros((64, 2), np.int32); level = np.zeros(max(nE, 1), np.uint8); chi2 = np.zeros(max(nE, 1))
     sf = _p(stop_flag) if stop_flag is not None else None
     n = lib().orc_local_ba(nKF, nMP, nE, _p(Tcw), _p(kf_fixed), _p(pts), _p(eMP), _p(eKF), _p(kpxy), _p(inv_sigma2), int(faceW), int(faceH),
-                           sf, int(its1), int(its2), _p(outlier), _p(pose64), _p(pts64), _p(log), 64)
-    return dict(Tcw=Tcw.reshape(nKF, 4, 4), pts=pts, outlier=outlier, pose64=pose64, pts64=pts64, log=log[:n], iters=n)
+                           sf, int(its1), int(its2), _p(outlier), _p(pose64), _p(pts64), _p(log), 64, int(stop_after_trials), _p(info), _p(level), _p(chi2))
+    # round / stop per log row (stop: 0 budget left or exhausted, 1 qmax == 10, 2 rho == 0, 3 nBad >= 3, 4 stop flag); level: edge levels after
+    # round 1; chi2: every edge's chi2 from its last computed error (what the classification reads)
+    return dict(Tcw=Tcw.reshape(nKF, 4, 4), pts=pts, outlier=outlier[:nE], pose64=pose64, pts64=pts64[:nMP], log=log[:n], iters=n,
+                round=info[:n, 0].copy(), stop=info[:n, 1].copy(), level=level[:nE], chi2=chi2[:nE])
+
+
+def ba_edge_chi2(pose64, pts64, eMP, eKF, kpxy, inv_sigma2, faceW, faceH):
+    """LocalBA's chi2 of every edge with its error computed at the fp64 state (pose64: nKF x 7 t, q; pts64: nMP x 3)."""
+    pose64 = np.ascontiguousarray(pose64, np.float64); pts64 = np.ascontiguousarray(pts64, np.float64)
+    eMP = _i32(eMP); eKF = _i32(eKF); kpxy = _f32(kpxy); inv_sigma2 = _f32(inv_sigma2)
+    n = eMP.shape[0]; out = np.zeros(max(n, 1))
+    lib().orc_ba_edge_chi2(n, _p(pose64), _p(pts64), _p(eMP), _p(eKF), _p(kpxy), _p(inv_sigma2), int(faceW), int(faceH), _p(out))
+    return out[:n]
 
 
 def pose_opt(Tcw, Xw, kpxy, inv_sigma2, faceW, faceH):

@@ -13,6 +13,34 @@ rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE"
 torch.cuda.set_device(local)
 dist.init_process_group("nccl", device_id=torch.device("cuda", local))
 small = len(sys.argv) > 1 and sys.argv[1] == "small"
+if len(sys.argv) > 1 and sys.argv[1] == "nan_lambda":
+    # the face-plane scenes of tests/local_ba_limits_scenes.py (NaN lambda, and the maxima after a NaN diagonal) on every rank; rank 0 compares
+    # the sharded result with a single-GPU run. The ranks sum chi2 and the pose blocks in another order than one GPU does, so only the LM
+    # decisions and the outliers are exact; chi2 and lambda agree to 1e-8 (NaN where NaN), poses and points to 1e-5 overall
+    from tests import local_ba_limits_scenes as S
+    o = Optimizer(device=local)
+    idt = torch.zeros(128, dtype=torch.uint8, device="cuda")
+    if rank == 0:
+        idt.copy_(torch.from_numpy(Optimizer.nccl_unique_id()))
+    dist.broadcast(idt, 0)
+    o.init_nccl(idt.cpu().numpy(), rank, world)
+    ref = Optimizer(device=local) if rank == 0 else None
+    n, same = 0, True
+    for W in S.WIDTHS:
+        for where in ("first", "middle", "last"):
+            a = S.args(S.plane_fixed(W, where))
+            g = o.LocalBundleAdjustment(*a)
+            if rank == 0:
+                r = ref.LocalBundleAdjustment(*a)
+                rl = lambda a, b: float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-30))
+                same &= bool(g["iters"] == r["iters"] and np.array_equal(g["log"][:, 2:], r["log"][:, 2:]) and np.array_equal(g["outlier"], r["outlier"])
+                             and np.allclose(g["log"][:, :2], r["log"][:, :2], rtol=1e-8, atol=0, equal_nan=True)
+                             and rl(g["pose64"], r["pose64"]) < 1e-5 and rl(g["pts64"], r["pts64"]) < 1e-5)
+            n += 1
+    if rank == 0:
+        print(json.dumps({"n_gpus": world, "scenes": n, "all_match": same}))
+    dist.destroy_process_group()
+    sys.exit(0)
 dense = len(sys.argv) > 1 and sys.argv[1] == "dense"
 prof = "prof" in sys.argv[1:]
 p = (synth.ba_problem(nKF=12, nMP=1500, kmin=2, kmax=8, faceW=450, seed=3, radius=1.5) if small else
