@@ -13,6 +13,7 @@
 // memory; (B) one thread commits the 8 MapPoints in order with the reference's scalar best / second-best rule against the `taken` flags.
 // Distances dominate the work and stay parallel; the commit touches a few dozen shorts per MapPoint. Hamming distance, rotation bin and
 // three-maxima filter: orb_match.cuh.
+#include <climits>
 #include <cstring>
 #include <vector>
 #include "area_table.cuh"
@@ -391,6 +392,178 @@ __global__ void __launch_bounds__(TRK_WARPS * 32, 1) k_local_commit(TrackArgs A)
     if (tid == 0) A.nmatches[p] = total;
 }
 
+// ------------------------------------------------------------------------------------------------- SearchForInitialization
+// cslam_search_for_initialization in four launches after F2's frame index (DESIGN.md, "SearchForInitialization"):
+//   k_init_candidates (count): one warp per F1 key point counts its window's candidates (level-0 F2 key points inside the strict |dx|, |dy| < r gate);
+//   k_init_scan: the counts become list offsets; the host reads the total and takes exactly that much scratch from the arena;
+//   k_init_candidates (fill): the same walk stores every candidate as (F2 index, Hamming distance) in visiting order - no window or cell cap;
+//   k_init_commit: one CTA applies the reference's rules in i1 order over the stored lists, then the rotation-consistency filter.
+static const int INIT_WARPS = 8;
+static const int INIT_CHUNK = 64;        // queries per staged chunk of the commit
+static const int INIT_STAGE = 8192;      // entries staged per chunk; a list past them is read from global memory (the answer does not depend on it)
+
+// entry = F2 index (14 bits) | distance << 14 (9 bits); the position in the list is the visiting position
+__device__ __forceinline__ uint32_t init_pack(int idx, int dist) { return (uint32_t)idx | (uint32_t)dist << 14; }
+
+// The window of query i1 walked by the calling warp (area_query / area_cells, the reference's visiting order, entries ascending inside a cell),
+// with the level and radius gates of window_candidates. list == nullptr: returns the number of candidates (warp-uniform). Otherwise writes them
+// to list[0, count) in visiting order. Lanes take consecutive cells; each lane counts its cell's passing entries, a warp scan places them, and
+// the lane walks its cell again to write: nothing is held per lane, so no cell or window size is too large.
+__device__ int init_window(const cslam_keypoint* kC, const uint4* dC, const uint16_t* CS, const uint16_t* CI, float u, float v, float radius, int minL, int maxL,
+                           int W, int H, float inv, const uint4* qd, uint32_t* list) {
+    const int lane = threadIdx.x & 31;
+    int ncand = 0;
+    AreaQuery aq;
+    if (!area_query(u, v, radius, W, H, inv, aq)) return 0;
+    const bool checkLevels = (minL > 0) || (maxL >= 0);
+    uint4 a0 = make_uint4(0, 0, 0, 0), a1 = a0;
+    if (list) { a0 = __ldg(qd); a1 = __ldg(qd + 1); }
+    for (int k = 0; k < 3; k++) {
+        AreaCells rc;
+        if (!area_cells(aq, k, rc)) break;
+        for (int cb = 0; cb < rc.n; cb += 32) {
+            const int ci = cb + lane;
+            int s = 0, e = 0;
+            if (ci < rc.n) { const int cell = rc.cell(ci); s = CS[cell]; e = CS[cell + 1]; }
+            if (__reduce_max_sync(0xffffffffu, e - s) == 0) continue;
+            int mine = 0;
+            for (int pass = 0; pass < (list ? 2 : 1); pass++) {
+                int off = 0, tot = 0;
+                if (pass == 1) {
+                    off = mine;
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, off, o); if (lane >= o) off += t; }
+                    off -= mine;
+                }
+                for (int a = s; a < e; a++) {
+                    const int idx = CI[a];
+                    const cslam_keypoint kp = kC[idx];
+                    if (checkLevels) { if (kp.octave < minL) continue; if (maxL >= 0 && kp.octave > maxL) continue; }
+                    if (!(fabsf(__fsub_rn(kp.x, u)) < radius && fabsf(__fsub_rn(kp.y, v)) < radius)) continue;
+                    if (pass == 0) mine++;
+                    else list[ncand + off + tot++] = init_pack(idx, hamming256(a0, a1, __ldg(dC + 2 * idx), __ldg(dC + 2 * idx + 1)));
+                }
+            }
+            ncand += __reduce_add_sync(0xffffffffu, (unsigned)mine);
+        }
+    }
+    return ncand;
+}
+
+// count pass (list == nullptr): cnt[i1] = candidates of query i1; fill pass: list + off[i1] gets them. Only level-0 F1 key points search
+// (`if (level1 > 0) continue`; the host rejects negative octaves), in F2's level-0 key points (GetFeaturesInArea(.., level1, level1)).
+__global__ void __launch_bounds__(INIT_WARPS * 32) k_init_candidates(const cslam_keypoint* __restrict__ k1, const uint8_t* __restrict__ d1, const float* __restrict__ pos,
+                                                                     int n1, const cslam_keypoint* __restrict__ k2, const uint8_t* __restrict__ d2, const uint16_t* __restrict__ CS,
+                                                                     const uint16_t* __restrict__ CI, int W, int H, float radius, uint32_t* __restrict__ cnt,
+                                                                     const uint32_t* __restrict__ off, uint32_t* __restrict__ list) {
+    const int i1 = blockIdx.x * INIT_WARPS + (threadIdx.x >> 5);
+    if (i1 >= n1) return;
+    int nc = 0;
+    if (k1[i1].octave == 0) {
+        const float inv = __fdiv_rn((float)(3 * GRID_G), (float)(3 * W));
+        nc = init_window(k2, reinterpret_cast<const uint4*>(d2), CS, CI, pos[2 * i1], pos[2 * i1 + 1], radius, 0, 0, W, H, inv,
+                         reinterpret_cast<const uint4*>(d1) + 2 * i1, list ? list + off[i1] : nullptr);
+    }
+    if (!list && (threadIdx.x & 31) == 0) cnt[i1] = (uint32_t)nc;
+}
+
+// exclusive scan of cnt[0, n) in place into off[0, n]; one CTA of 1024 threads, n <= CSLAM_BOW_FV_MAX_FEATURES
+__global__ void __launch_bounds__(1024) k_init_scan(uint32_t* __restrict__ off, int n) {
+    __shared__ uint32_t wsum[32];
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    const int per = (n + 1023) / 1024, b = tid * per, e = min(n, b + per);
+    uint32_t s = 0;
+    for (int i = b; i < e; i++) s += off[i];
+    uint32_t x = s;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += t; }
+    if (lane == 31) wsum[w] = x;
+    __syncthreads();
+    uint32_t pre = x - s;
+    for (int ww = 0; ww < w; ww++) pre += wsum[ww];
+    for (int i = b; i < e; i++) { const uint32_t c = off[i]; off[i] = pre; pre += c; }
+    if (tid == 1023) off[n] = pre;
+}
+
+// staging of chunk c (queries c*INIT_CHUNK ...) by threads t0, t0 + nt, ...: its offsets, and its first INIT_STAGE entries
+__device__ __forceinline__ void init_stage(const uint32_t* off, const uint32_t* list, int n1, int c, int t0, int nt, uint32_t* sOff, uint32_t* sList) {
+    const int q0 = c * INIT_CHUNK, nq = min(INIT_CHUNK, n1 - q0);
+    for (int i = t0; i <= nq; i += nt) sOff[i] = off[q0 + i];
+    const uint32_t e0 = off[q0], ne = umin(off[q0 + nq] - e0, (uint32_t)INIT_STAGE);
+    for (uint32_t i = t0; i < ne; i += nt) sList[i] = list[e0 + i];
+}
+
+// Shared memory of k_init_commit: vMatchedDistance (u16, 0xffff = INT_MAX) and vnMatches21 (i16) per F2 key point, vnMatches12 (i16) and the
+// rotation bin (u8, 0xff: never pushed) per F1 key point, then two staging buffers of offsets and entries
+static const size_t INIT_SMEM = (size_t)CSLAM_BOW_FV_MAX_FEATURES * (2 + 2 + 2 + 1) + 2 * (INIT_CHUNK + 1) * 4 + 2 * INIT_STAGE * 4;
+
+// The reference's scan of query i1 ends with best and second best = the first two eligible entries (vMatchedDistance[i2] > dist) in (distance,
+// visiting position) order: both comparisons are strict, and the eligibility of an entry cannot change while i1 is scanned. Warp 0 takes them
+// as two warp minima of the key distance << 16 | position, applies the acceptance rules of orb_match.cuh and commits, query after query.
+__global__ void __launch_bounds__(INIT_WARPS * 32, 1) k_init_commit(const cslam_keypoint* __restrict__ k1, int n1, const cslam_keypoint* __restrict__ k2, int n2,
+                                                                    const uint32_t* __restrict__ off, const uint32_t* __restrict__ list, float nnratio, int checkOri,
+                                                                    int32_t* __restrict__ match12, int32_t* __restrict__ nmatches) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint32_t* sList = reinterpret_cast<uint32_t*>(smem);                           // [2][INIT_STAGE]
+    uint32_t* sOff = sList + 2 * INIT_STAGE;                                          // [2][INIT_CHUNK + 1]
+    uint16_t* mdist = reinterpret_cast<uint16_t*>(sOff + 2 * (INIT_CHUNK + 1));      // [n2]
+    int16_t* owner = reinterpret_cast<int16_t*>(mdist + CSLAM_BOW_FV_MAX_FEATURES);   // [n2]
+    int16_t* m12 = owner + CSLAM_BOW_FV_MAX_FEATURES;                                  // [n1]
+    uint8_t* bin = reinterpret_cast<uint8_t*>(m12 + CSLAM_BOW_FV_MAX_FEATURES);       // [n1]
+    __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nChunks = (n1 + INIT_CHUNK - 1) / INIT_CHUNK;
+    for (int i = tid; i < n2; i += blockDim.x) { mdist[i] = 0xffff; owner[i] = -1; }
+    for (int i = tid; i < n1; i += blockDim.x) { m12[i] = -1; bin[i] = 0xff; }
+    if (tid < HISTO_BINS) hist[tid] = 0;
+    if (tid == 0) total = 0;
+    if (nChunks > 0) init_stage(off, list, n1, 0, tid, blockDim.x, sOff, sList);
+    __syncthreads();
+    for (int c = 0; c < nChunks; c++) {
+        const int b = c & 1, q0 = c * INIT_CHUNK, nq = min(INIT_CHUNK, n1 - q0);
+        if (warp != 0) {
+            if (c + 1 < nChunks) init_stage(off, list, n1, c + 1, tid - 32, blockDim.x - 32, sOff + (b ^ 1) * (INIT_CHUNK + 1), sList + (b ^ 1) * INIT_STAGE);
+        } else {
+            const uint32_t* so = sOff + b * (INIT_CHUNK + 1); const uint32_t* sl = sList + b * INIT_STAGE;
+            for (int j = 0; j < nq; j++) {
+                const uint32_t s = so[j] - so[0], n = so[j + 1] - so[j];
+                if (n == 0) continue;
+                const uint32_t* L = s + n <= (uint32_t)INIT_STAGE ? sl + s : list + so[j];
+                uint32_t m1 = 0xffffffffu, m2 = 0xffffffffu;   // this lane's two smallest eligible keys
+                for (uint32_t p = lane; p < n; p += 32) {
+                    const uint32_t e = L[p], dist = e >> 14;
+                    if (mdist[e & 0x3fff] <= dist) continue;   // `if (vMatchedDistance[i2] <= dist) continue`
+                    const uint32_t key = dist << 16 | p;
+                    if (key < m1) { m2 = m1; m1 = key; } else if (key < m2) m2 = key;
+                }
+                const uint32_t best = __reduce_min_sync(0xffffffffu, m1);
+                const uint32_t second = __reduce_min_sync(0xffffffffu, m1 == best ? m2 : m1);
+                const int bestDist = best == 0xffffffffu ? INT_MAX : (int)(best >> 16), bestDist2 = second == 0xffffffffu ? INT_MAX : (int)(second >> 16);
+                if (!bow_accept(bestDist, bestDist2, nnratio, false)) continue;   // bestDist <= TH_LOW, bestDist < (float)bestDist2 * mfNNratio
+                if (lane == 0) {
+                    const int i1 = q0 + j, i2 = L[best & 0xffff] & 0x3fff;
+                    const int prev = owner[i2];
+                    if (prev >= 0) { m12[prev] = -1; total--; }
+                    m12[i1] = (int16_t)i2; owner[i2] = (int16_t)i1; mdist[i2] = (uint16_t)bestDist; total++;
+                    if (checkOri) bin[i1] = (uint8_t)rot_bin(k1[i1].angle, k2[i2].angle);
+                }
+                __syncwarp();   // the new vMatchedDistance is visible to every lane before the next query
+            }
+        }
+        __syncthreads();
+    }
+    if (checkOri) {
+        // ComputeThreeMaxima over the bin sizes: an i1 whose F2 key point a later i1 took stays in its bin and counts
+        for (int i = tid; i < n1; i += blockDim.x) if (bin[i] != 0xff) atomicAdd(&hist[bin[i]], 1);
+        __syncthreads();
+        if (tid == 0) three_maxima(hist, keep);
+        __syncthreads();
+        for (int i = tid; i < n1; i += blockDim.x) if (bin[i] != 0xff && !keep[bin[i]] && m12[i] >= 0) { m12[i] = -1; atomicSub(&total, 1); }
+        __syncthreads();
+    }
+    for (int i = tid; i < n1; i += blockDim.x) match12[i] = m12[i];
+    if (tid == 0) *nmatches = total;
+}
+
 // What Tracking does between SearchByProjection and PoseOptimization (src/Optimizer.cpp:80-131 reads mvpMapPoints / mvKeys / mvKeyRays):
 // the matched slots of a frame, in slot order, become the (world point, key point, 1/sigma^2) correspondences of the pose-only BA.
 __global__ void __launch_bounds__(256) k_gather_pose_inputs(const int32_t* __restrict__ match, const cslam_keypoint* __restrict__ kCur, const int32_t* __restrict__ nCur, int curStride,
@@ -638,5 +811,49 @@ extern "C" int cslam_search_by_projection_local_large(cslam_tracker* t, int nfra
     k_local_commit<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
     CSLAM_CUDA(cudaGetLastError());
     CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
+    return cslam_tracker_sync(t);
+}
+
+// One pair of frames of up to CSLAM_BOW_FV_MAX_FEATURES key points each, whatever the handle's max_features. Every argument is checked before
+// anything is enqueued. The candidate lists are sized to the call: the count pass's total is read back (one stream synchronisation) and exactly
+// that much scratch is taken from the handle's arena.
+extern "C" int cslam_search_for_initialization(cslam_tracker* t, const cslam_keypoint* k1, const uint8_t* d1, int n1, const float* prev_xy, const cslam_keypoint* k2,
+                                               const uint8_t* d2, int n2, int face_w, int face_h, int window_size, float nnratio, int check_ori, int32_t* match12,
+                                               int32_t* nmatches) {
+    static const char* fn = "cslam_search_for_initialization";
+    if (!t || n1 < 0 || n1 > CSLAM_BOW_FV_MAX_FEATURES || n2 < 0 || n2 > CSLAM_BOW_FV_MAX_FEATURES || !nmatches || (n1 > 0 && (!k1 || !d1 || !prev_xy || !match12)) ||
+        (n2 > 0 && (!k2 || !d2)) || face_w <= 0 || face_w != face_h || window_size <= 0 || 2 * window_size > face_w) {
+        set_error("%s: bad argument (n1, n2 in [0, %d], square faces, window_size in (0, face_w / 2], no NULL buffer)", fn, CSLAM_BOW_FV_MAX_FEATURES);
+        return CSLAM_E_BADARG;
+    }
+    for (int i = 0; i < n1; i++)   // a negative level would make GetFeaturesInArea search every level
+        if (k1[i].octave < 0) { set_error("%s: F1 key point %d has octave %d", fn, i, k1[i].octave); return CSLAM_E_BADARG; }
+    for (int i = 0; i < n1; i++) match12[i] = -1;
+    *nmatches = 0;
+    if (n1 == 0 || n2 == 0) return CSLAM_OK;
+    CSLAM_CUDA(cudaSetDevice(t->device));
+    t->arena.reset();
+    DevArena& a = t->arena;
+    const cslam_keypoint *dK1, *dK2; const uint8_t *dD1, *dD2; const float* dPos; const int32_t* dN2; uint16_t *cs, *ci; uint32_t *off, *list; int32_t *match, *nm; int rc;
+    if ((rc = a.upload(&dK1, k1, n1)) || (rc = a.upload(&dD1, d1, (size_t)n1 * 32)) || (rc = a.upload(&dPos, prev_xy, (size_t)n1 * 2)) || (rc = a.upload(&dK2, k2, n2)) ||
+        (rc = a.upload(&dD2, d2, (size_t)n2 * 32)) || (rc = a.upload(&dN2, &n2, 1)) || (rc = a.take(&cs, NCELLS + 1)) || (rc = a.take(&ci, n2)) ||
+        (rc = a.take(&off, (size_t)n1 + 1)) || (rc = a.take(&match, n1)) || (rc = a.take(&nm, 1)) ||
+        (rc = frame_index(t->stream, t->launches, dK2, dN2, 1, n2, face_w, face_h, nullptr, cs, ci, CSLAM_BOW_FV_MAX_FEATURES))) return rc;
+    const float r = (float)window_size;
+    const int blocks = cdiv(n1, INIT_WARPS);
+    k_init_candidates<<<blocks, INIT_WARPS * 32, 0, t->stream>>>(dK1, dD1, dPos, n1, dK2, dD2, cs, ci, face_w, face_h, r, off, nullptr, nullptr); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    k_init_scan<<<1, 1024, 0, t->stream>>>(off, n1); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    uint32_t totalEntries = 0;
+    CSLAM_CUDA(cudaMemcpyAsync(&totalEntries, off + n1, 4, cudaMemcpyDeviceToHost, t->stream));
+    CSLAM_CUDA(cudaStreamSynchronize(t->stream));
+    if ((rc = a.take(&list, totalEntries))) return rc;
+    k_init_candidates<<<blocks, INIT_WARPS * 32, 0, t->stream>>>(dK1, dD1, dPos, n1, dK2, dD2, cs, ci, face_w, face_h, r, nullptr, off, list); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    CSLAM_CUDA(cudaFuncSetAttribute(k_init_commit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)INIT_SMEM));
+    k_init_commit<<<1, INIT_WARPS * 32, INIT_SMEM, t->stream>>>(dK1, n1, dK2, n2, off, list, nnratio, check_ori, match, nm); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    CSLAM_CUDA(cudaMemcpyAsync(match12, match, (size_t)n1 * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nm, 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }

@@ -5,7 +5,8 @@
   ORBMatcher::SearchByProjection(Frame&, const Frame&, th, mono)        (src/ORBMatcher.cpp:130-251) -> Tracker.SearchByProjection_last
   ORBMatcher::SearchByProjection(Frame&, vector<MapPoint*>&, th)        (src/ORBMatcher.cpp:51-128)  -> Tracker.SearchByProjection_local
                                                                         local maps past 4096 MapPoints -> Tracker.SearchByProjection_local_large
-All calls are batched over independent frames (leading axis)."""
+  ORBMatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) (src/ORBMatcher.cpp:676-794) -> Tracker.SearchForInitialization
+All calls but SearchForInitialization (one pair per call) are batched over independent frames (leading axis)."""
 import ctypes as C
 
 import numpy as np
@@ -14,6 +15,7 @@ from ._capi import KP_DTYPE, Handle, check, lib, ptr
 
 NCELLS = 5 * 50 * 50
 CSLAM_LOCAL_MAP_MAX_POINTS = 1 << 20   # MapPoints per frame of SearchByProjection_local_large
+CSLAM_BOW_FV_MAX_FEATURES = 16384      # key points per frame of SearchForInitialization
 
 
 def area_rects(x, y, r, face_w, face_h):
@@ -87,6 +89,19 @@ class Tracker(Handle):
         check(getattr(lib(), entry)(self._h, P, ptr(k), ptr(a[0]), ptr(nf), fs, ptr(a[7]), ptr(nm_), ms, ptr(a[1]), ptr(a[2]), ptr(a[3]), ptr(a[4]), ptr(a[5]), ptr(a[6]),
                                       int(face_w), int(face_h), C.c_float(th), C.c_float(nnratio), C.c_float(scale_factor), int(nlevels), ptr(match), ptr(nm)))
         return (int(nm[0]), match[0]) if single else (nm, match)
+
+    def SearchForInitialization(self, k1, d1, prev_xy, k2, d2, face_w, face_h, window_size=100, nnratio=0.9, check_ori=True):
+        """One pair of frames of up to CSLAM_BOW_FV_MAX_FEATURES key points each, whatever max_features. prev_xy: (n1, 2) window centres
+        (vbPrevMatched). Returns (nmatches, match12, prev_xy updated with F2's key point of every surviving match)."""
+        k1 = np.ascontiguousarray(k1, KP_DTYPE); k2 = np.ascontiguousarray(k2, KP_DTYPE)
+        d1 = np.ascontiguousarray(d1, np.uint8); d2 = np.ascontiguousarray(d2, np.uint8); xy = np.ascontiguousarray(prev_xy, np.float32).reshape(-1, 2)
+        match = np.empty(len(k1), np.int32); nm = np.zeros(1, np.int32)
+        check(lib().cslam_search_for_initialization(self._h, ptr(k1), ptr(d1), len(k1), ptr(xy), ptr(k2), ptr(d2), len(k2), int(face_w), int(face_h), int(window_size),
+                                                    C.c_float(nnratio), int(check_ori), ptr(match), ptr(nm)))
+        out = xy.copy()
+        live = match >= 0
+        out[live, 0] = k2["x"][match[live]]; out[live, 1] = k2["y"][match[live]]
+        return int(nm[0]), match, out
 
     def search_by_projection_last_dev(self, npairs, kCur, dCur, nCur, cur_stride, cell_start, cell_idx, curTaken, TcwCur, kLast, nLast, last_stride, hasMP, Xw, dMP, mpObs,
                                       face_w, face_h, cos_fov_th, th, check_ori, match, nmatches, scale_factor=1.2, nlevels=8):

@@ -35,6 +35,9 @@ cslam_tracker* b200_tracker() {
 }
 }  // namespace
 
+// the calling thread's tracker handle, shared with dropin/ORBMatcher_init_b200.cpp
+cslam_tracker* cubemap_b200_thread_tracker() { return b200_tracker(); }
+
 // reference src/ORBMatcher.cpp:130-251 (Tracking::TrackWithMotionModel :634, with the retry at twice the window :641). The reference walks
 // LastFrame's MapPoints on the host; here their world positions / descriptors / observation flags are gathered and the projection, the
 // cube-face window lookup (Frame::GetFeaturesInArea), the Hamming search and the rotation-consistency filter run on the device.

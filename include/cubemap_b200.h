@@ -282,6 +282,19 @@ int cslam_search_by_projection_local_large(cslam_tracker* t, int nframes, const 
                                            const int32_t* level, const float* view_cos, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h,
                                            float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f, int32_t* nmatches);
 
+/* ORBMatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize) (src/ORBMatcher.cpp:676-794, Tracking::CubemapInitialization
+ * :428-429) for one pair of frames of up to CSLAM_BOW_FV_MAX_FEATURES key points each, whatever the handle's max_features (the initialisation
+ * extractor's frames hold 3*nFeatures + 3*nlevels: 9024 at 3000 features). Every level-0 key point i1 of F1 searches the level-0 key points of F2
+ * in the window GetFeaturesInArea(prev_xy[i1], window_size) with the reference's rules, in i1 order; then the rotation-consistency filter.
+ *   k1 / d1 / prev_xy: F1's key points, descriptors (n1 x 32) and window centres (n1 x 2 float: vbPrevMatched); k2 / d2: F2's (n2).
+ *   match12[i1]: i2, or -1 (n1 entries); nmatches: the function's return value. The caller updates vbPrevMatched from match12.
+ * CSLAM_E_BADARG before anything is enqueued: n1 or n2 outside [0, CSLAM_BOW_FV_MAX_FEATURES], a NULL pointer (k1, d1, prev_xy, match12 when
+ * n1 > 0; k2, d2 when n2 > 0; nmatches), faces that are not square, an F1 octave below 0, window_size outside (0, face_w / 2].
+ * Host buffers, synchronous. No window or cell capacity applies: the candidate lists are sized per call. */
+int cslam_search_for_initialization(cslam_tracker* t, const cslam_keypoint* k1, const uint8_t* d1, int n1, const float* prev_xy, const cslam_keypoint* k2,
+                                    const uint8_t* d2, int n2, int face_w, int face_h, int window_size, float nnratio, int check_ori, int32_t* match12,
+                                    int32_t* nmatches);
+
 /* What Tracking does between SearchByProjection and PoseOptimization (src/Optimizer.cpp:80-131): the matched slots of each frame, in slot order and
  * with the ray.z >= cos_fov_th test when rays are given, become (world point, key point, 1/sigma^2) correspondences at stride cur_stride; count_out[p] of them.
  * inv_sigma2_levels_dev: mvInvLevelSigma2 (one float per pyramid level) on the device. Device pointers, asynchronous on the tracker's stream. */
