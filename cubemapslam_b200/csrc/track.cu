@@ -7,14 +7,13 @@
 //   ORBMatcher::SearchByProjection(Frame&, const Frame&, th, mono)   src/ORBMatcher.cpp:130-251 (Tracking::TrackWithMotionModel :634)
 //   ORBMatcher::SearchByProjection(Frame&, vector<MapPoint*>&, th)   src/ORBMatcher.cpp:51-128  (Tracking::SearchLocalPoints :841)
 //
-// k_search_by_projection: one CTA per (frame pair / frame + local map). The reference's loop over MapPoints is sequential - a feature taken by
+// k_search_by_projection (the LastFrame search): one CTA per frame pair. The reference's loop over MapPoints is sequential - a feature taken by
 // an earlier MapPoint (with observations) is invisible to later ones - so the kernel works in rounds of 8 MapPoints: (A) each warp projects
 // its MapPoint, walks the window's cells in the reference's visiting order and stores the (feature, Hamming distance) candidates in shared
 // memory; (B) one thread commits the 8 MapPoints in order with the reference's scalar best / second-best rule against the `taken` flags.
 // Distances dominate the work and stay parallel; the commit touches a few dozen shorts per MapPoint. Hamming distance, rotation bin and
-// three-maxima filter: orb_match.cuh.
+// three-maxima filter: orb_match.cuh. The local-map search walks the same windows in two launches (k_local_candidates, k_local_commit).
 #include <climits>
-#include <cstring>
 #include <vector>
 #include "area_table.cuh"
 #include "common.cuh"
@@ -111,24 +110,27 @@ __global__ void __launch_bounds__(256) k_frame_index(const cslam_keypoint* __res
 }
 
 // ------------------------------------------------------------------------------------------------- projection matchers
-struct TrackArgs {
-    // current frame (the one searched)
+// What both projection searches read: the searched frame, the query rows (MapPoints), the window parameters and the outputs
+struct ProjArgs {
     const cslam_keypoint* kCur; const uint8_t* dCur; const int32_t* nCur; const uint16_t* cellStart; const uint16_t* cellIdx; const uint8_t* curTaken; int curStride;
-    // query side: LastFrame features (mode 0) or local MapPoints (mode 1)
     const int32_t* nQ; int qStride;
-    const uint8_t* qValid;      // mode 0: has a MapPoint that is not an outlier; mode 1: mbTrackInView && !isBad
+    const uint8_t* qValid;      // LastFrame: has a MapPoint that is not an outlier; local map: mbTrackInView && !isBad
     const uint8_t* qDesc;       // MapPoint descriptors
     const uint8_t* qObs;        // Observations() > 0
-    const float* qXw; const cslam_keypoint* kLast; const float* TcwCur;   // mode 0
-    const float* qProj; const int32_t* qLevel; const float* qViewCos;     // mode 1
-    int mode, W, H, checkOri; float th, nnratio, cosFovTh; float scale[16];
+    int W, H; float th; float scale[16];
     int32_t* match; int32_t* nmatches; int* errFlag;
+};
+// k_search_by_projection: the LastFrame's MapPoints, projected with the current pose
+struct LastArgs : ProjArgs { const float* qXw; const cslam_keypoint* kLast; const float* TcwCur; int checkOri; float cosFovTh; };
+// k_local_candidates / k_local_commit: the local map as Frame::isInFrustum left it
+struct LocalArgs : ProjArgs {
+    const float* qProj; const int32_t* qLevel; const float* qViewCos; float nnratio;
     uint32_t* lmList; uint16_t* lmCount;   // k_local_candidates -> k_local_commit: LM_K packed entries and the candidate count per (frame, MapPoint)
 };
 
-// Mode 1's window of the MapPoint in row `row` (scale: A.scale or a copy): RadiusByViewingCos (src/ORBMatcher.cpp:380-386), times th unless th == 1, times the scale of
+// The window of the local MapPoint in row `row` (scale: A.scale or a copy): RadiusByViewingCos (src/ORBMatcher.cpp:380-386), times th unless th == 1, times the scale of
 // the predicted level; levels [level - 1, level]
-__device__ __forceinline__ void local_window(const TrackArgs& A, const float* scale, size_t row, float& u, float& v, float& radius, int& minL, int& maxL) {
+__device__ __forceinline__ void local_window(const LocalArgs& A, const float* scale, size_t row, float& u, float& v, float& radius, int& minL, int& maxL) {
     u = A.qProj[row * 2]; v = A.qProj[row * 2 + 1];
     const int lvl = A.qLevel[row];
     float r = A.qViewCos[row] > 0.998 ? 2.5f : 4.0f;   // float compared with the double literal 0.998
@@ -187,7 +189,7 @@ __device__ __forceinline__ int window_candidates(const cslam_keypoint* kC, const
 }
 
 // The reference's scalar scan over one query's candidates in visiting order, skipping taken slots: `dist < bestDist` shifts the best to
-// second place; with `second` (mode 1) `else if (dist < bestDist2)` replaces the second. No candidate: dist 256, level -1.
+// second place; with `second` (the local-map search) `else if (dist < bestDist2)` replaces the second. No candidate: dist 256, level -1.
 struct Best { int dist, level, dist2, level2, idx; };
 __device__ __forceinline__ Best best_two(const uint16_t* cIdx, const uint16_t* cDist, int nc, const uint8_t* slotObs, const cslam_keypoint* kC, bool second) {
     Best b = {256, -1, 256, -1, -1};
@@ -200,16 +202,16 @@ __device__ __forceinline__ Best best_two(const uint16_t* cIdx, const uint16_t* c
     }
     return b;
 }
-// mode 1's ratio test (src/ORBMatcher.cpp:111-112): only when the best and the second best are at the same level
+// the local-map search's ratio test (src/ORBMatcher.cpp:111-112): only when the best and the second best are at the same level
 __device__ __forceinline__ bool ratio_ok(const Best& b, float nnratio) { return !(b.level == b.level2 && (float)b.dist > __fmul_rn(nnratio, (float)b.dist2)); }
 
-__global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackArgs A) {
+__global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(LastArgs A) {
     __shared__ uint16_t candIdx[TRK_WARPS][TRK_CAND];
     __shared__ uint16_t candDist[TRK_WARPS][TRK_CAND];
     __shared__ int candN[TRK_WARPS];
     __shared__ uint8_t slotObs[4096];
     __shared__ int hist[HISTO_BINS], keep[HISTO_BINS], total, logN;
-    __shared__ uint16_t logIdx[4096];   // mode 0: every accepted assignment (current slot, rotation bin), replayed by the orientation filter
+    __shared__ uint16_t logIdx[4096];   // every accepted assignment (current slot, rotation bin), replayed by the orientation filter
     __shared__ uint8_t logBin[4096];
     const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nCur = min(A.nCur[p], A.curStride), nQ = min(A.nQ[p], A.qStride);
@@ -225,22 +227,19 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
     __syncthreads();
     const float inv = __fdiv_rn((float)(3 * GRID_G), (float)(3 * A.W));
     float Tc[12];
-    if (A.mode == 0) for (int i = 0; i < 12; i++) Tc[i] = A.TcwCur[(size_t)p * 16 + i];
+    for (int i = 0; i < 12; i++) Tc[i] = A.TcwCur[(size_t)p * 16 + i];
     for (int q0 = 0; q0 < nQ; q0 += TRK_WARPS) {
         // ---- (A) candidates of MapPoint q = q0 + warp, in the reference's visiting order
         const int q = q0 + warp;
         int ncand = 0;
         if (q < nQ && A.qValid[(size_t)p * A.qStride + q]) {
-            float u = 0, v = 0, radius = 0; int minL = 0, maxL = 0; bool ok = true;
-            if (A.mode == 0) {
-                float xc[3];
-                transform_cw(Tc, A.qXw + ((size_t)p * A.qStride + q) * 3, xc);   // `Rcw*x3Dw+tcw`
-                if (xc[2] < A.cosFovTh) ok = false;
-                if (ok) ok = ray_to_cubemap(xc[0], xc[1], xc[2], A.W, A.H, u, v);
+            float xc[3], u = 0, v = 0;
+            transform_cw(Tc, A.qXw + ((size_t)p * A.qStride + q) * 3, xc);   // `Rcw*x3Dw+tcw`
+            if (!(xc[2] < A.cosFovTh) && ray_to_cubemap(xc[0], xc[1], xc[2], A.W, A.H, u, v)) {
                 const int oct = A.kLast[(size_t)p * A.qStride + q].octave;
-                radius = __fmul_rn(A.th, A.scale[oct]); minL = oct - 1; maxL = oct + 1;
-            } else local_window(A, A.scale, (size_t)p * A.qStride + q, u, v, radius, minL, maxL);
-            if (ok) ncand = window_candidates(kC, dC, CS, CI, u, v, radius, minL, maxL, A.W, A.H, inv, dQ + 2 * q, candIdx[warp], candDist[warp], A.errFlag);
+                ncand = window_candidates(kC, dC, CS, CI, u, v, __fmul_rn(A.th, A.scale[oct]), oct - 1, oct + 1, A.W, A.H, inv, dQ + 2 * q, candIdx[warp],
+                                          candDist[warp], A.errFlag);
+            }
         }
         if (lane == 0) candN[warp] = ncand;
         __syncthreads();
@@ -249,13 +248,12 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
             for (int w = 0; w < TRK_WARPS; w++) {
                 const int qq = q0 + w, nc = candN[w];
                 if (qq >= nQ || nc == 0) continue;
-                const Best b = best_two(candIdx[w], candDist[w], nc, slotObs, kC, A.mode == 1);
+                const Best b = best_two(candIdx[w], candDist[w], nc, slotObs, kC, false);
                 if (b.dist > 100) continue;   // TH_HIGH
-                if (A.mode == 1 && !ratio_ok(b, A.nnratio)) continue;
                 const int bestIdx = b.idx;
                 M[bestIdx] = qq; slotObs[bestIdx] = A.qObs[(size_t)p * A.qStride + qq];
                 total++;
-                if (A.mode == 0 && A.checkOri) {
+                if (A.checkOri) {
                     const int bin = rot_bin(A.kLast[(size_t)p * A.qStride + qq].angle, kC[bestIdx].angle);
                     hist[bin]++;
                     if (logN < 4096) { logIdx[logN] = (uint16_t)bestIdx; logBin[logN] = (uint8_t)bin; logN++; } else *A.errFlag = CSLAM_E_CAPACITY;
@@ -264,7 +262,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
         }
         __syncthreads();
     }
-    if (A.mode == 0 && A.checkOri) {
+    if (A.checkOri) {
         // the reference keeps per-bin lists of CURRENT feature indices (a slot overwritten by a later, observation-less MapPoint is listed twice)
         // and clears every slot listed in a non-dominant bin, decrementing nmatches per list entry: the assignment log is replayed.
         if (tid == 0) three_maxima(hist, keep);
@@ -276,8 +274,8 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_search_by_projection(TrackAr
     if (tid == 0) A.nmatches[p] = total;
 }
 
-// ------------------------------------------------------------------------------------------------- local maps past 4096 MapPoints
-// cslam_search_by_projection_local_large in two launches (DESIGN.md, "Local maps past 4096 MapPoints"):
+// ------------------------------------------------------------------------------------------------- the local-map search
+// cslam_search_by_projection_local, _local_dev and _local_large in two launches (DESIGN.md, "The local-map search"):
 //   k_local_candidates: one warp per (frame, MapPoint) over the whole device walks the window (window_candidates) and keeps the first LM_K
 //     candidates in (distance, visiting position) order, packed, plus the full candidate count.
 //   k_local_commit: one CTA per frame applies the reference's rules in MapPoint order. The first two untaken entries of that order are the
@@ -289,7 +287,7 @@ static const int LM_CHUNK = 256;  // MapPoints per staged chunk of the commit
 // entry = feature (12 bits) | distance << 12 (9 bits) | octave << 21 (a signed byte)
 __device__ __forceinline__ uint32_t lm_pack(int idx, int dist, int octave) { return (uint32_t)idx | (uint32_t)dist << 12 | (uint32_t)(octave & 0xff) << 21; }
 
-__global__ void __launch_bounds__(TRK_WARPS * 32) k_local_candidates(TrackArgs A, int nframes) {
+__global__ void __launch_bounds__(TRK_WARPS * 32) k_local_candidates(LocalArgs A, int nframes) {
     __shared__ uint16_t candIdx[TRK_WARPS][TRK_CAND];
     __shared__ uint16_t candDist[TRK_WARPS][TRK_CAND];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -324,7 +322,7 @@ __global__ void __launch_bounds__(TRK_WARPS * 32) k_local_candidates(TrackArgs A
 }
 
 // chunk c of a frame's MapPoints (rows row0 + c * LM_CHUNK ...) into one buffer of the commit, by threads t0, t0 + nt, ...
-__device__ __forceinline__ void lm_stage(const TrackArgs& A, size_t row0, int nQ, int c, int t0, int nt, uint32_t* list, uint16_t* cnt, uint8_t* obs) {
+__device__ __forceinline__ void lm_stage(const LocalArgs& A, size_t row0, int nQ, int c, int t0, int nt, uint32_t* list, uint16_t* cnt, uint8_t* obs) {
     const int q0 = c * LM_CHUNK, n = min(LM_CHUNK, nQ - q0);
     for (int i = t0; i < n * LM_K; i += nt) list[i] = A.lmList[(row0 + q0) * LM_K + i];
     for (int i = t0; i < n; i += nt) { cnt[i] = A.lmCount[row0 + q0 + i]; obs[i] = A.qObs[row0 + q0 + i]; }
@@ -332,7 +330,7 @@ __device__ __forceinline__ void lm_stage(const TrackArgs& A, size_t row0, int nQ
 
 // The reference's scan over the whole window of the MapPoint in row `row` of frame p, walked again by the calling warp. scale: A.scale in
 // shared memory (indexed by level, a kernel parameter array would be copied to local memory)
-__device__ __forceinline__ Best lm_rewalk(const TrackArgs& A, const float* scale, int p, size_t row, const uint8_t* slotObs, uint16_t* candIdx, uint16_t* candDist) {
+__device__ __forceinline__ Best lm_rewalk(const LocalArgs& A, const float* scale, int p, size_t row, const uint8_t* slotObs, uint16_t* candIdx, uint16_t* candDist) {
     const cslam_keypoint* kC = A.kCur + (size_t)p * A.curStride;
     float u, v, radius; int minL, maxL;
     local_window(A, scale, row, u, v, radius, minL, maxL);
@@ -343,7 +341,7 @@ __device__ __forceinline__ Best lm_rewalk(const TrackArgs& A, const float* scale
     return best_two(candIdx, candDist, nc, slotObs, kC, true);
 }
 
-__global__ void __launch_bounds__(TRK_WARPS * 32, 1) k_local_commit(TrackArgs A) {
+__global__ void __launch_bounds__(TRK_WARPS * 32, 1) k_local_commit(LocalArgs A) {
     __shared__ uint32_t list[2][LM_CHUNK * LM_K];   // double-buffered: warp 0 commits one chunk while the other warps stage the next
     __shared__ uint16_t cnt[2][LM_CHUNK];
     __shared__ uint8_t obs[2][LM_CHUNK];
@@ -352,10 +350,9 @@ __global__ void __launch_bounds__(TRK_WARPS * 32, 1) k_local_commit(TrackArgs A)
     __shared__ float sScale[16];
     const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nCur = min(A.nCur[p], A.curStride), nQ = max(0, min(A.nQ[p], A.qStride)), nChunks = (nQ + LM_CHUNK - 1) / LM_CHUNK;
-    const cslam_keypoint* kC = A.kCur + (size_t)p * A.curStride;
     int32_t* M = A.match + (size_t)p * A.curStride;
     const size_t row0 = (size_t)p * A.qStride;
-    for (int i = tid; i < A.curStride; i += blockDim.x) { M[i] = -1; if (i < nCur) slotObs[i] = A.curTaken[(size_t)p * A.curStride + i]; }
+    for (int i = tid; i < nCur; i += blockDim.x) { M[i] = -1; slotObs[i] = A.curTaken ? A.curTaken[(size_t)p * A.curStride + i] : 0; }
     if (tid < 16) sScale[tid] = A.scale[tid];
     if (nChunks > 0) lm_stage(A, row0, nQ, 0, tid, blockDim.x, list[0], cnt[0], obs[0]);
     __syncthreads();
@@ -629,7 +626,7 @@ extern "C" int cslam_tracker_create(cslam_tracker** out, int device, int max_fra
     if (!out || max_frames <= 0 || max_features <= 0 || max_features > 4096) { set_error("cslam_tracker_create: bad argument (max_features <= 4096)"); return CSLAM_E_BADARG; }
     cslam_tracker* t = new cslam_tracker; t->maxFrames = max_frames; t->maxFeat = max_features;
     // chunks: room for every array the host calls stage at the handle's limits, at most 64 MB
-    const size_t perFeature = 2 * sizeof(cslam_keypoint) + 2 * 32 + 3 + 2 * 4 + 3 * 4 + 2 * 4 + 4 + 3 * 4 + 2, perFrame = 3 * 4 + 16 * 4 + (NCELLS + 1) * 2;
+    const size_t perFeature = 2 * sizeof(cslam_keypoint) + 2 * 32 + 3 + 2 * 4 + 3 * 4 + 2 * 4 + 4 + 3 * 4 + 2 + LM_K * 4 + 2, perFrame = 3 * 4 + 16 * 4 + (NCELLS + 1) * 2;
     int rc;
     if ((rc = t->open(device, std::min<size_t>((size_t)64 << 20, (size_t)max_frames * max_features * perFeature + (size_t)max_frames * perFrame), true)) ||
         (rc = prepare_frame_index())) { destroy_handle(t); return rc; }
@@ -687,7 +684,7 @@ extern "C" int cslam_frame_index(cslam_tracker* t, const cslam_keypoint* kps, co
     return cslam_tracker_sync(t);
 }
 
-static void fill_scales(TrackArgs& A, float scale_factor, int nlevels) {
+static void fill_scales(ProjArgs& A, float scale_factor, int nlevels) {
     A.scale[0] = 1.0f;
     for (int i = 1; i < 16; i++) A.scale[i] = i < nlevels ? A.scale[i - 1] * scale_factor : A.scale[i - 1];
 }
@@ -699,12 +696,26 @@ extern "C" int cslam_search_by_projection_last_dev(cslam_tracker* t, int npairs,
                                                    int32_t* match_cur, int32_t* nmatches) {
     if (!t || npairs <= 0 || cur_stride <= 0 || cur_stride > 4096 || last_stride <= 0 || face_w != face_h || nlevels < 1 || nlevels > 16) { set_error("cslam_search_by_projection_last: bad argument"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
-    TrackArgs A; std::memset(&A, 0, sizeof(A));
-    A.kCur = k_cur; A.dCur = d_cur; A.nCur = n_cur; A.cellStart = cell_start; A.cellIdx = cell_idx; A.curTaken = cur_taken; A.curStride = cur_stride;
-    A.nQ = n_last; A.qStride = last_stride; A.qValid = has_mp; A.qDesc = d_mp; A.qObs = mp_obs; A.qXw = Xw; A.kLast = k_last; A.TcwCur = Tcw_cur;
-    A.mode = 0; A.W = face_w; A.H = face_h; A.checkOri = check_ori; A.th = th; A.nnratio = 0; A.cosFovTh = cos_fov_th; fill_scales(A, scale_factor, nlevels);
-    A.match = match_cur; A.nmatches = nmatches; A.errFlag = t->errFlag;
+    LastArgs A{{k_cur, d_cur, n_cur, cell_start, cell_idx, cur_taken, cur_stride, n_last, last_stride, has_mp, d_mp, mp_obs, face_w, face_h, th, {}, match_cur, nmatches,
+                t->errFlag}, Xw, k_last, Tcw_cur, check_ori, cos_fov_th};
+    fill_scales(A, scale_factor, nlevels);
     k_search_by_projection<<<npairs, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    return CSLAM_OK;
+}
+
+// The local-map search on device arrays, with the caller's scratch: LM_K entries and a candidate count per (frame, MapPoint) row. Every entry
+// reaches the kernels through it; it never resets the arena, so the host entries' staged arrays stay live.
+static int local_search(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride, const uint16_t* cell_start,
+                        const uint16_t* cell_idx, const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy,
+                        const int32_t* level, const float* view_cos, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio,
+                        float scale_factor, int nlevels, int32_t* match_f, int32_t* nmatches, uint32_t* lmList, uint16_t* lmCount) {
+    LocalArgs A{{k_f, d_f, n_f, cell_start, cell_idx, f_taken, f_stride, n_mp, mp_stride, in_view, d_mp, mp_obs, face_w, face_h, th, {}, match_f, nmatches, t->errFlag},
+                proj_xy, level, view_cos, nnratio, lmList, lmCount};
+    fill_scales(A, scale_factor, nlevels);
+    k_local_candidates<<<dim3(cdiv(mp_stride, TRK_WARPS), std::min(nframes, 65535)), TRK_WARPS * 32, 0, t->stream>>>(A, nframes); t->launches++;
+    CSLAM_CUDA(cudaGetLastError());
+    k_local_commit<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
     CSLAM_CUDA(cudaGetLastError());
     return CSLAM_OK;
 }
@@ -716,18 +727,29 @@ extern "C" int cslam_search_by_projection_local_dev(cslam_tracker* t, int nframe
                                                     int32_t* nmatches) {
     if (!t || nframes <= 0 || f_stride <= 0 || f_stride > 4096 || mp_stride <= 0 || face_w != face_h || nlevels < 1 || nlevels > 16) { set_error("cslam_search_by_projection_local: bad argument"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
-    TrackArgs A; std::memset(&A, 0, sizeof(A));
-    A.kCur = k_f; A.dCur = d_f; A.nCur = n_f; A.cellStart = cell_start; A.cellIdx = cell_idx; A.curTaken = f_taken; A.curStride = f_stride;
-    A.nQ = n_mp; A.qStride = mp_stride; A.qValid = in_view; A.qDesc = d_mp; A.qObs = mp_obs; A.qProj = proj_xy; A.qLevel = level; A.qViewCos = view_cos;
-    A.mode = 1; A.W = face_w; A.H = face_h; A.checkOri = 0; A.th = th; A.nnratio = nnratio; fill_scales(A, scale_factor, nlevels);
-    A.match = match_f; A.nmatches = nmatches; A.errFlag = t->errFlag;
-    k_search_by_projection<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    return CSLAM_OK;
+    t->arena.reset();
+    const size_t rows = (size_t)nframes * mp_stride;
+    uint32_t* lmList; uint16_t* lmCount; int rc;
+    if ((rc = t->arena.take(&lmList, rows * LM_K)) || (rc = t->arena.take(&lmCount, rows))) return rc;
+    return local_search(t, nframes, k_f, d_f, n_f, f_stride, cell_start, cell_idx, f_taken, n_mp, mp_stride, in_view, proj_xy, level, view_cos, d_mp, mp_obs, face_w, face_h,
+                        th, nnratio, scale_factor, nlevels, match_f, nmatches, lmList, lmCount);
 }
 
-// host entry points (one pair / frame per call batch; staging inside): what the drop-in ORBMatcher::SearchByProjection definitions call. Every
-// array is uploaded at its exact size: the kernels read no row past a frame's count.
+// The searched frames of a host entry, staged in the arena: key points, descriptors, counts and taken flags uploaded, the grid indexed (one
+// launch), the match rows and counts taken. Every array is uploaded at its exact size: the kernels read no row past a frame's count.
+struct StagedFrames { const cslam_keypoint* k; const uint8_t* d; const int32_t* n; const uint8_t* taken; uint16_t *cellStart, *cellIdx; int32_t *match, *nmatches; };
+static int stage_frames(cslam_tracker* t, int nframes, int stride, const cslam_keypoint* k, const uint8_t* d, const int32_t* n, const uint8_t* taken, int face_w, int face_h,
+                        StagedFrames& s) {
+    const size_t nc = (size_t)nframes * stride;
+    DevArena& a = t->arena;
+    int rc;
+    if ((rc = a.upload(&s.k, k, nc)) || (rc = a.upload(&s.d, d, nc * 32)) || (rc = a.upload(&s.n, n, nframes)) || (rc = a.upload(&s.taken, taken, nc)) ||
+        (rc = a.take(&s.cellStart, (size_t)nframes * (NCELLS + 1))) || (rc = a.take(&s.cellIdx, nc)) || (rc = a.take(&s.match, nc)) || (rc = a.take(&s.nmatches, nframes)))
+        return rc;
+    return cslam_frame_index_dev(t, s.k, s.n, nframes, stride, face_w, face_h, nullptr, s.cellStart, s.cellIdx);
+}
+
+// host entry points (one pair / frame per call batch; staging inside): what the drop-in ORBMatcher::SearchByProjection definitions call
 extern "C" int cslam_search_by_projection_last(cslam_tracker* t, int npairs, const cslam_keypoint* k_cur, const uint8_t* d_cur, const int32_t* n_cur, int cur_stride,
                                                const uint8_t* cur_taken, const float* Tcw_cur, const cslam_keypoint* k_last, const int32_t* n_last, int last_stride,
                                                const uint8_t* has_mp, const float* Xw, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float cos_fov_th, float th,
@@ -735,54 +757,28 @@ extern "C" int cslam_search_by_projection_last(cslam_tracker* t, int npairs, con
     if (!t || npairs <= 0 || npairs > t->maxFrames || cur_stride > t->maxFeat || last_stride > t->maxFeat) { set_error("cslam_search_by_projection_last: sizes out of range"); return CSLAM_E_BADARG; }
     CSLAM_CUDA(cudaSetDevice(t->device));
     t->arena.reset();
-    const size_t nc = (size_t)npairs * cur_stride, nl = (size_t)npairs * last_stride;
+    const size_t nl = (size_t)npairs * last_stride;
     DevArena& a = t->arena;
-    const cslam_keypoint *kC, *kL; const uint8_t *dC, *taken, *valid, *dQ, *obs; const int32_t *nC, *nL; const float *Tcw, *dXw; uint16_t *cs, *ci; int32_t *match, *nm; int rc;
-    if ((rc = a.upload(&kC, k_cur, nc)) || (rc = a.upload(&dC, d_cur, nc * 32)) || (rc = a.upload(&nC, n_cur, npairs)) || (rc = a.upload(&taken, cur_taken, nc)) ||
-        (rc = a.upload(&Tcw, Tcw_cur, (size_t)npairs * 16)) || (rc = a.upload(&kL, k_last, nl)) || (rc = a.upload(&nL, n_last, npairs)) || (rc = a.upload(&valid, has_mp, nl)) ||
-        (rc = a.upload(&dXw, Xw, nl * 3)) || (rc = a.upload(&dQ, d_mp, nl * 32)) || (rc = a.upload(&obs, mp_obs, nl)) || (rc = a.take(&cs, (size_t)npairs * (NCELLS + 1))) ||
-        (rc = a.take(&ci, nc)) || (rc = a.take(&match, nc)) || (rc = a.take(&nm, npairs)) ||
-        (rc = cslam_frame_index_dev(t, kC, nC, npairs, cur_stride, face_w, face_h, nullptr, cs, ci)) ||
-        (rc = cslam_search_by_projection_last_dev(t, npairs, kC, dC, nC, cur_stride, cs, ci, taken, Tcw, kL, nL, last_stride, valid, dXw, dQ, obs, face_w, face_h, cos_fov_th, th,
-                                                  check_ori, scale_factor, nlevels, match, nm))) return rc;
-    CSLAM_CUDA(cudaMemcpyAsync(match_cur, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nm, npairs * 4, cudaMemcpyDeviceToHost, t->stream));
+    StagedFrames s; const cslam_keypoint* kL; const uint8_t *valid, *dQ, *obs; const int32_t* nL; const float *Tcw, *dXw; int rc;
+    if ((rc = stage_frames(t, npairs, cur_stride, k_cur, d_cur, n_cur, cur_taken, face_w, face_h, s)) || (rc = a.upload(&Tcw, Tcw_cur, (size_t)npairs * 16)) ||
+        (rc = a.upload(&kL, k_last, nl)) || (rc = a.upload(&nL, n_last, npairs)) || (rc = a.upload(&valid, has_mp, nl)) || (rc = a.upload(&dXw, Xw, nl * 3)) ||
+        (rc = a.upload(&dQ, d_mp, nl * 32)) || (rc = a.upload(&obs, mp_obs, nl)) ||
+        (rc = cslam_search_by_projection_last_dev(t, npairs, s.k, s.d, s.n, cur_stride, s.cellStart, s.cellIdx, s.taken, Tcw, kL, nL, last_stride, valid, dXw, dQ, obs, face_w,
+                                                  face_h, cos_fov_th, th, check_ori, scale_factor, nlevels, s.match, s.nmatches))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match_cur, s.match, (size_t)npairs * cur_stride * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, s.nmatches, npairs * 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
 }
 
-extern "C" int cslam_search_by_projection_local(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride, const uint8_t* f_taken,
-                                                const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy, const int32_t* level, const float* view_cos,
-                                                const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio, float scale_factor, int nlevels,
-                                                int32_t* match_f, int32_t* nmatches) {
-    if (!t || nframes <= 0 || nframes > t->maxFrames || f_stride > t->maxFeat || mp_stride > t->maxFeat) { set_error("cslam_search_by_projection_local: sizes out of range"); return CSLAM_E_BADARG; }
-    CSLAM_CUDA(cudaSetDevice(t->device));
-    t->arena.reset();
-    const size_t nc = (size_t)nframes * f_stride, nm = (size_t)nframes * mp_stride;
-    DevArena& a = t->arena;
-    const cslam_keypoint* kF; const uint8_t *dF, *taken, *valid, *dQ, *obs; const int32_t *nF, *nQ, *lvl; const float *proj, *vcos; uint16_t *cs, *ci; int32_t *match, *nmOut; int rc;
-    if ((rc = a.upload(&kF, k_f, nc)) || (rc = a.upload(&dF, d_f, nc * 32)) || (rc = a.upload(&nF, n_f, nframes)) || (rc = a.upload(&taken, f_taken, nc)) ||
-        (rc = a.upload(&nQ, n_mp, nframes)) || (rc = a.upload(&valid, in_view, nm)) || (rc = a.upload(&proj, proj_xy, nm * 2)) || (rc = a.upload(&lvl, level, nm)) ||
-        (rc = a.upload(&vcos, view_cos, nm)) || (rc = a.upload(&dQ, d_mp, nm * 32)) || (rc = a.upload(&obs, mp_obs, nm)) || (rc = a.take(&cs, (size_t)nframes * (NCELLS + 1))) ||
-        (rc = a.take(&ci, nc)) || (rc = a.take(&match, nc)) || (rc = a.take(&nmOut, nframes)) ||
-        (rc = cslam_frame_index_dev(t, kF, nF, nframes, f_stride, face_w, face_h, nullptr, cs, ci)) ||
-        (rc = cslam_search_by_projection_local_dev(t, nframes, kF, dF, nF, f_stride, cs, ci, taken, nQ, mp_stride, valid, proj, lvl, vcos, dQ, obs, face_w, face_h, th, nnratio,
-                                                   scale_factor, nlevels, match, nmOut))) return rc;
-    CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
-    return cslam_tracker_sync(t);
-}
-
-// Local maps of up to CSLAM_LOCAL_MAP_MAX_POINTS MapPoints per frame, whatever the handle's max_features (frames stay <= max_features): the
-// arguments and outputs of cslam_search_by_projection_local, with -1 in every slot row past a frame's count. Every argument is checked before
-// anything is enqueued; the per-call scratch (LM_K + 1/2 words per MapPoint row) comes from the handle's arena.
-extern "C" int cslam_search_by_projection_local_large(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride,
-                                                      const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy,
-                                                      const int32_t* level, const float* view_cos, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h,
-                                                      float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f, int32_t* nmatches) {
-    static const char* fn = "cslam_search_by_projection_local_large";
-    if (!t || nframes <= 0 || nframes > t->maxFrames || f_stride <= 0 || f_stride > t->maxFeat || mp_stride <= 0 || mp_stride > CSLAM_LOCAL_MAP_MAX_POINTS ||
-        face_w <= 0 || face_w != face_h || nlevels < 1 || nlevels > 16 || !k_f || !d_f || !n_f || !f_taken || !n_mp || !in_view || !proj_xy || !level || !view_cos ||
-        !d_mp || !mp_obs || !match_f || !nmatches) {
+// cslam_search_by_projection_local and _local_large: local maps of up to mpMax MapPoints per frame. Every argument is checked before anything
+// is enqueued; match rows are -1 past a frame's count; the scratch (LM_K + 1/2 words per MapPoint row) comes from the handle's arena.
+static int local_host(const char* fn, int mpMax, cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride,
+                      const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy, const int32_t* level, const float* view_cos,
+                      const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f,
+                      int32_t* nmatches) {
+    if (!t || nframes <= 0 || nframes > t->maxFrames || f_stride <= 0 || f_stride > t->maxFeat || mp_stride <= 0 || mp_stride > mpMax || face_w <= 0 || face_w != face_h ||
+        nlevels < 1 || nlevels > 16 || !k_f || !d_f || !n_f || !f_taken || !n_mp || !in_view || !proj_xy || !level || !view_cos || !d_mp || !mp_obs || !match_f || !nmatches) {
         set_error("%s: bad argument (frames in [1, %d], f_stride in [1, %d], mp_stride in [1, %d], nlevels in [1, 16], square faces)", fn, t ? t->maxFrames : 0,
-                  t ? t->maxFeat : 0, CSLAM_LOCAL_MAP_MAX_POINTS);
+                  t ? t->maxFeat : 0, mpMax);
         return CSLAM_E_BADARG;
     }
     for (int f = 0; f < nframes; f++)   // the window radius reads the scale of the predicted level
@@ -792,26 +788,33 @@ extern "C" int cslam_search_by_projection_local_large(cslam_tracker* t, int nfra
         }
     CSLAM_CUDA(cudaSetDevice(t->device));
     t->arena.reset();
-    const size_t nc = (size_t)nframes * f_stride, nm = (size_t)nframes * mp_stride;
+    const size_t nm = (size_t)nframes * mp_stride;
     DevArena& a = t->arena;
-    const cslam_keypoint* kF; const uint8_t *dF, *taken, *valid, *dQ, *obs; const int32_t *nF, *nQ, *lvl; const float *proj, *vcos; uint16_t *cs, *ci, *lmCount;
-    uint32_t* lmList; int32_t *match, *nmOut; int rc;
-    if ((rc = a.upload(&kF, k_f, nc)) || (rc = a.upload(&dF, d_f, nc * 32)) || (rc = a.upload(&nF, n_f, nframes)) || (rc = a.upload(&taken, f_taken, nc)) ||
-        (rc = a.upload(&nQ, n_mp, nframes)) || (rc = a.upload(&valid, in_view, nm)) || (rc = a.upload(&proj, proj_xy, nm * 2)) || (rc = a.upload(&lvl, level, nm)) ||
-        (rc = a.upload(&vcos, view_cos, nm)) || (rc = a.upload(&dQ, d_mp, nm * 32)) || (rc = a.upload(&obs, mp_obs, nm)) || (rc = a.take(&cs, (size_t)nframes * (NCELLS + 1))) ||
-        (rc = a.take(&ci, nc)) || (rc = a.take(&lmList, nm * LM_K)) || (rc = a.take(&lmCount, nm)) || (rc = a.take(&match, nc)) || (rc = a.take(&nmOut, nframes)) ||
-        (rc = cslam_frame_index_dev(t, kF, nF, nframes, f_stride, face_w, face_h, nullptr, cs, ci))) return rc;
-    TrackArgs A; std::memset(&A, 0, sizeof(A));
-    A.kCur = kF; A.dCur = dF; A.nCur = nF; A.cellStart = cs; A.cellIdx = ci; A.curTaken = taken; A.curStride = f_stride;
-    A.nQ = nQ; A.qStride = mp_stride; A.qValid = valid; A.qDesc = dQ; A.qObs = obs; A.qProj = proj; A.qLevel = lvl; A.qViewCos = vcos;
-    A.mode = 1; A.W = face_w; A.H = face_h; A.th = th; A.nnratio = nnratio; fill_scales(A, scale_factor, nlevels);
-    A.match = match; A.nmatches = nmOut; A.errFlag = t->errFlag; A.lmList = lmList; A.lmCount = lmCount;
-    k_local_candidates<<<dim3(cdiv(mp_stride, TRK_WARPS), std::min(nframes, 65535)), TRK_WARPS * 32, 0, t->stream>>>(A, nframes); t->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    k_local_commit<<<nframes, TRK_WARPS * 32, 0, t->stream>>>(A); t->launches++;
-    CSLAM_CUDA(cudaGetLastError());
-    CSLAM_CUDA(cudaMemcpyAsync(match_f, match, nc * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, nmOut, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
+    StagedFrames s; const uint8_t *valid, *dQ, *obs; const int32_t *nQ, *lvl; const float *proj, *vcos; uint32_t* lmList; uint16_t* lmCount; int rc;
+    if ((rc = stage_frames(t, nframes, f_stride, k_f, d_f, n_f, f_taken, face_w, face_h, s)) || (rc = a.upload(&nQ, n_mp, nframes)) || (rc = a.upload(&valid, in_view, nm)) ||
+        (rc = a.upload(&proj, proj_xy, nm * 2)) || (rc = a.upload(&lvl, level, nm)) || (rc = a.upload(&vcos, view_cos, nm)) || (rc = a.upload(&dQ, d_mp, nm * 32)) ||
+        (rc = a.upload(&obs, mp_obs, nm)) || (rc = a.take(&lmList, nm * LM_K)) || (rc = a.take(&lmCount, nm))) return rc;
+    CSLAM_CUDA(cudaMemsetAsync(s.match, 0xff, (size_t)nframes * f_stride * 4, t->stream));   // the kernels write each frame's rows up to its count
+    if ((rc = local_search(t, nframes, s.k, s.d, s.n, f_stride, s.cellStart, s.cellIdx, s.taken, nQ, mp_stride, valid, proj, lvl, vcos, dQ, obs, face_w, face_h, th, nnratio,
+                           scale_factor, nlevels, s.match, s.nmatches, lmList, lmCount))) return rc;
+    CSLAM_CUDA(cudaMemcpyAsync(match_f, s.match, (size_t)nframes * f_stride * 4, cudaMemcpyDeviceToHost, t->stream)); CSLAM_CUDA(cudaMemcpyAsync(nmatches, s.nmatches, nframes * 4, cudaMemcpyDeviceToHost, t->stream));
     return cslam_tracker_sync(t);
+}
+
+extern "C" int cslam_search_by_projection_local(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride, const uint8_t* f_taken,
+                                                const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy, const int32_t* level, const float* view_cos,
+                                                const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio, float scale_factor, int nlevels,
+                                                int32_t* match_f, int32_t* nmatches) {
+    return local_host("cslam_search_by_projection_local", t ? t->maxFeat : 0, t, nframes, k_f, d_f, n_f, f_stride, f_taken, n_mp, mp_stride, in_view, proj_xy, level, view_cos,
+                      d_mp, mp_obs, face_w, face_h, th, nnratio, scale_factor, nlevels, match_f, nmatches);
+}
+
+extern "C" int cslam_search_by_projection_local_large(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride,
+                                                      const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy,
+                                                      const int32_t* level, const float* view_cos, const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h,
+                                                      float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f, int32_t* nmatches) {
+    return local_host("cslam_search_by_projection_local_large", CSLAM_LOCAL_MAP_MAX_POINTS, t, nframes, k_f, d_f, n_f, f_stride, f_taken, n_mp, mp_stride, in_view, proj_xy,
+                      level, view_cos, d_mp, mp_obs, face_w, face_h, th, nnratio, scale_factor, nlevels, match_f, nmatches);
 }
 
 // One pair of frames of up to CSLAM_BOW_FV_MAX_FEATURES key points each, whatever the handle's max_features. Every argument is checked before

@@ -66,13 +66,14 @@ class Tracker(Handle):
         return (int(nm[0]), match[0]) if single else (nm, match)
 
     def SearchByProjection_local(self, kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor=1.2, nlevels=8, nF=None, nMP=None):
+        """Local maps of up to max_features MapPoints per frame. Match rows past a frame's count are -1."""
         return self._local("cslam_search_by_projection_local", kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor, nlevels,
                            nF, nMP)
 
     def SearchByProjection_local_large(self, kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor=1.2, nlevels=8, nF=None,
                                        nMP=None):
         """SearchByProjection_local for local maps of up to CSLAM_LOCAL_MAP_MAX_POINTS MapPoints per frame, whatever max_features (frames stay
-        within it). Same arguments and results; match rows past a frame's count are -1."""
+        within it). Same arguments, kernels and results; match rows past a frame's count are -1, as there."""
         return self._local("cslam_search_by_projection_local_large", kF, dF, inView, projXY, level, viewCos, dMP, mpObs, fTaken, face_w, face_h, th, nnratio, scale_factor,
                            nlevels, nF, nMP)
 

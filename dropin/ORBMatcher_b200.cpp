@@ -95,9 +95,7 @@ int ORBMatcher::SearchByProjection(Frame& F, const std::vector<MapPoint*>& vpMap
     for (int i = 0; i < nF; i++) taken[i] = F.mvpMapPoints[i] && F.mvpMapPoints[i]->Observations() > 0;
     std::vector<int32_t> match(nF); int32_t n = 0, nf = nF, nm = nM;
     // Every size goes to the _large entry (Tracking::UpdateLocalPoints takes every point of every local key frame, past 4096 as the map grows).
-    // It is also the faster one below 4096: median host-call latency on an H100 80GB HBM3 (700 W), one frame of 4096 key points, face 650,
-    // th 5, two runs of tools/local_map_latency.py: 0.82-0.85 ms against 1.77-1.79 ms for cslam_search_by_projection_local at 1024
-    // MapPoints, 2.06-2.14 against 6.43-6.70 ms at 4096.
+    // It runs the kernels of cslam_search_by_projection_local without that entry's max_features bound on the map.
     if (cslam_search_by_projection_local_large(b200_tracker(), 1, reinterpret_cast<const cslam_keypoint*>(F.mvKeys.data()), dF.data(), &nf, nF, taken.data(), &nm, nM,
                                                inView.data(), proj.data(), lvl.data(), vcos.data(), dMP.data(), obs.data(), cam->GetCubeFaceWidth(),
                                                cam->GetCubeFaceHeight(), th, mfNNratio, F.mfScaleFactor, F.mnScaleLevels, match.data(), &n) != CSLAM_OK) b200_fatal();

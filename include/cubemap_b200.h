@@ -260,7 +260,12 @@ int cslam_search_by_projection_last_dev(cslam_tracker* t, int npairs, const csla
                                         const cslam_keypoint* k_last, const int32_t* n_last, int last_stride, const uint8_t* has_mp, const float* Xw, const uint8_t* d_mp,
                                         const uint8_t* mp_obs, int face_w, int face_h, float cos_fov_th, float th, int check_ori, float scale_factor, int nlevels,
                                         int32_t* match_cur, int32_t* nmatches);
-/* in_view: mbTrackInView && !isBad(); proj_xy / level / view_cos: mTrackProjX/Y, mnTrackScaleLevel, mTrackViewCos left by Frame::isInFrustum. */
+/* in_view: mbTrackInView && !isBad(); proj_xy / level / view_cos: mTrackProjX/Y, mnTrackScaleLevel, mTrackViewCos left by Frame::isInFrustum.
+ * match_f[f * f_stride + i]: the MapPoint assigned to slot i, -1 otherwise. nmatches: the function's return value. The host entry takes
+ * mp_stride <= max_features and the checks of cslam_search_by_projection_local_large (an in-view row's level in [0, nlevels), no NULL buffer:
+ * CSLAM_E_BADARG before anything runs, nothing written); its match rows are -1 past n_f[f]. The _dev entry writes nothing in a match row past
+ * n_f[f]; f_taken may be NULL (nothing taken); its scratch (34 bytes per (frame, MapPoint) row) comes from the handle's arena, which its
+ * first call may grow. */
 int cslam_search_by_projection_local(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride, const uint8_t* f_taken,
                                      const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy, const int32_t* level, const float* view_cos,
                                      const uint8_t* d_mp, const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio, float scale_factor, int nlevels,
@@ -271,11 +276,11 @@ int cslam_search_by_projection_local_dev(cslam_tracker* t, int nframes, const cs
                                          const uint8_t* mp_obs, int face_w, int face_h, float th, float nnratio, float scale_factor, int nlevels, int32_t* match_f,
                                          int32_t* nmatches);
 /* The same search for local maps of up to CSLAM_LOCAL_MAP_MAX_POINTS MapPoints per frame (Tracking::UpdateLocalPoints collects every MapPoint of
- * every local key frame, past 4096 once the map grows): arguments, layout and outputs of cslam_search_by_projection_local. mp_stride may be
- * anything in [1, CSLAM_LOCAL_MAP_MAX_POINTS] whatever the handle's max_features; f_stride <= max_features and nframes <= max_frames as there.
- * match_f[f * f_stride + i]: the MapPoint assigned to slot i (may be past 65535), -1 otherwise, also in every row past n_f[f]. An in-view row's
- * level must lie in [0, nlevels). Bad arguments: CSLAM_E_BADARG before anything runs, nothing written. A window of more than 256 candidates:
- * CSLAM_E_CAPACITY, as in cslam_search_by_projection_local. Host buffers, synchronous. */
+ * every local key frame, past 4096 once the map grows), on the same kernels: arguments, layout and outputs of cslam_search_by_projection_local.
+ * mp_stride may be anything in [1, CSLAM_LOCAL_MAP_MAX_POINTS] whatever the handle's max_features; f_stride <= max_features and nframes <=
+ * max_frames as there. match_f[f * f_stride + i]: the MapPoint assigned to slot i (may be past 65535), -1 otherwise, also in every row past n_f[f].
+ * An in-view row's level must lie in [0, nlevels). Bad arguments: CSLAM_E_BADARG before anything runs, nothing written. A window of more than 256
+ * candidates: CSLAM_E_CAPACITY, as in cslam_search_by_projection_local. Host buffers, synchronous. */
 #define CSLAM_LOCAL_MAP_MAX_POINTS (1 << 20)
 int cslam_search_by_projection_local_large(cslam_tracker* t, int nframes, const cslam_keypoint* k_f, const uint8_t* d_f, const int32_t* n_f, int f_stride,
                                            const uint8_t* f_taken, const int32_t* n_mp, int mp_stride, const uint8_t* in_view, const float* proj_xy,

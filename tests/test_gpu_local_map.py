@@ -1,7 +1,7 @@
 """cslam_search_by_projection_local_large (Tracker.SearchByProjection_local_large) against the oracle, exactly, on local maps past 4096
-MapPoints (tests/local_map_scenes.py): ragged batches up to CSLAM_LOCAL_MAP_MAX_POINTS, byte equality with cslam_search_by_projection_local up to
-4096, every bad argument, window capacity, and the drop-in ORBMatcher::SearchByProjection(F, vpMapPoints, th) on the reference's own Frame /
-MapPoint objects up to 65 537 MapPoints."""
+MapPoints (tests/local_map_scenes.py): ragged batches up to CSLAM_LOCAL_MAP_MAX_POINTS, cslam_search_by_projection_local against the oracle up to
+4096, every bad argument of both host entries, window capacity, and the drop-in ORBMatcher::SearchByProjection(F, vpMapPoints, th) on the
+reference's own Frame / MapPoint objects up to 65 537 MapPoints."""
 import ctypes as C
 import os
 
@@ -81,48 +81,57 @@ def test_largest_local_map(oracle, trk, W, th):
 
 
 @pytest.mark.parametrize("W,nlevels,th", [(450, 8, 5.0), (650, 12, 1.0), (650, 8, 5.0)])
-def test_equals_existing_entry_up_to_4096(trk, W, nlevels, th):
+def test_equals_existing_entry_up_to_4096(oracle, trk, W, nlevels, th):
     for counts in ([4096, 4000, 1, 0, 2048], [4096] * 3):
-        _, _, B = batch(counts, 4096, W, nlevels, 300 + W + len(counts))
+        frames, maps, B = batch(counts, 4096, W, nlevels, 300 + W + len(counts))
         B["nf"][:] = 4096
-        a = run_large(trk, B, W, th, nlevels)
-        b = trk.SearchByProjection_local(B["k"], B["d"], B["in_view"], B["proj"], B["level"], B["vcos"], B["dq"], B["obs"], B["taken"], W, W, th, NN, S.NLEVELS[nlevels],
-                                         nlevels, nF=B["nf"], nMP=B["nmp"])
-        assert a[0].tobytes() == b[0].tobytes() and a[1].tobytes() == b[1].tobytes()
-        assert a[0].max() > 1000
+        nm, m = trk.SearchByProjection_local(B["k"], B["d"], B["in_view"], B["proj"], B["level"], B["vcos"], B["dq"], B["obs"], B["taken"], W, W, th, NN,
+                                             S.NLEVELS[nlevels], nlevels, nF=B["nf"], nMP=B["nmp"])
+        check_against_oracle(oracle, frames, maps, B, nm, m, th, 4096)
+        assert nm.max() > 1000
 
 
-def _call(trk, B, nframes=None, f_stride=None, mp_stride=None, W=450, H=None, nlevels=8, null=None):
+def _call(trk, entry, B, nframes=None, f_stride=None, mp_stride=None, W=450, H=None, nlevels=8, null=None):
     P, fs = B["k"].shape
     ms = B["in_view"].shape[1]
     arrs = dict(k=B["k"], d=B["d"], nf=B["nf"], taken=B["taken"], nmp=B["nmp"], in_view=B["in_view"], proj=B["proj"], level=B["level"], vcos=B["vcos"], dq=B["dq"],
                 obs=B["obs"])
     ptrs = {key: (None if key == null else _p(v)) for key, v in arrs.items()}
     match = np.full((P, fs), 12345, np.int32); nm = np.full(P, 777, np.int32)
-    rc = lib().cslam_search_by_projection_local_large(trk._h, P if nframes is None else nframes, ptrs["k"], ptrs["d"], ptrs["nf"], fs if f_stride is None else f_stride,
-                                                      ptrs["taken"], ptrs["nmp"], ms if mp_stride is None else mp_stride, ptrs["in_view"], ptrs["proj"], ptrs["level"],
-                                                      ptrs["vcos"], ptrs["dq"], ptrs["obs"], W, W if H is None else H, C.c_float(5.0), C.c_float(NN), C.c_float(1.2), nlevels,
-                                                      None if null == "match" else _p(match), None if null == "nm" else _p(nm))
+    rc = getattr(lib(), entry)(trk._h, P if nframes is None else nframes, ptrs["k"], ptrs["d"], ptrs["nf"], fs if f_stride is None else f_stride, ptrs["taken"], ptrs["nmp"],
+                               ms if mp_stride is None else mp_stride, ptrs["in_view"], ptrs["proj"], ptrs["level"], ptrs["vcos"], ptrs["dq"], ptrs["obs"], W,
+                               W if H is None else H, C.c_float(5.0), C.c_float(NN), C.c_float(1.2), nlevels, None if null == "match" else _p(match),
+                               None if null == "nm" else _p(nm))
     return rc, match, nm
 
 
-def test_bad_arguments_write_nothing(trk):
-    _, _, B = batch([100, 5000], 5000, 450, 8, 11)
-    rc, m, nm = _call(trk, B)
+def _bad_arguments_write_nothing(trk, entry, mp_max, stride):
+    """Every bad argument of a host entry whose mp_stride bound is mp_max, on a batch of two frames with maps of 100 and `stride` MapPoints."""
+    _, _, B = batch([100, stride], stride, 450, 8, 11)
+    rc, m, nm = _call(trk, entry, B)
     assert rc == 0 and nm.max() > 0
-    cases = [dict(nframes=0), dict(nframes=9), dict(f_stride=0), dict(f_stride=4097), dict(mp_stride=0), dict(mp_stride=CSLAM_LOCAL_MAP_MAX_POINTS + 1), dict(W=450, H=451),
+    cases = [dict(nframes=0), dict(nframes=9), dict(f_stride=0), dict(f_stride=4097), dict(mp_stride=0), dict(mp_stride=mp_max + 1), dict(W=450, H=451),
              dict(W=0, H=0), dict(nlevels=0), dict(nlevels=17)] + [dict(null=key) for key in ("k", "d", "nf", "taken", "nmp", "in_view", "proj", "level", "vcos", "dq", "obs")]
     for c in cases:
-        rc, m, nm = _call(trk, B, **c)
+        rc, m, nm = _call(trk, entry, B, **c)
         assert rc == BADARG, c
         assert (m == 12345).all() and (nm == 777).all(), c
     for lv in (-1, 8):   # an in-view row's level outside [0, nlevels)
         B2 = dict(B); B2["level"] = B["level"].copy(); B2["in_view"] = B["in_view"].copy()
-        B2["level"][1, 4999] = lv; B2["in_view"][1, 4999] = 1
-        rc, m, nm = _call(trk, B2)
+        B2["level"][1, stride - 1] = lv; B2["in_view"][1, stride - 1] = 1
+        rc, m, nm = _call(trk, entry, B2)
         assert rc == BADARG and (m == 12345).all() and (nm == 777).all(), lv
-        B2["nmp"] = np.array([100, 4999], np.int32)   # the same row past the count is not read
-        assert _call(trk, B2)[0] == 0
+        B2["nmp"] = np.array([100, stride - 1], np.int32)   # the same row past the count is not read
+        assert _call(trk, entry, B2)[0] == 0
+
+
+def test_bad_arguments_write_nothing(trk):
+    _bad_arguments_write_nothing(trk, "cslam_search_by_projection_local_large", CSLAM_LOCAL_MAP_MAX_POINTS, 5000)
+
+
+def test_local_entry_bad_arguments_write_nothing(trk):
+    """cslam_search_by_projection_local takes the checks of _large, with mp_stride bounded by the handle's max_features (4096)."""
+    _bad_arguments_write_nothing(trk, "cslam_search_by_projection_local", 4096, 4000)
 
 
 def test_window_capacity(trk):

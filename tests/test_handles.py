@@ -88,7 +88,7 @@ def test_mapper_launch_counts():
 
 
 @pytest.mark.gpu
-def test_tracker_launch_counts():
+def test_tracker_launches_per_host_call():
     from cubemapslam_b200.tracker import Tracker
     s = synth.tracking_pair(0, n=1500, faceW=650)
     cth = np.float32(np.cos(np.radians(95.0)))
@@ -99,12 +99,12 @@ def test_tracker_launch_counts():
     t = Tracker(max_frames=2, max_features=4096)
     try:
         assert _launched(t, lambda: t.frame_index(s["kCur"], 650, 650)) == 1
-        # both searches index the current frame first
+        # both searches index the current frame first; the local-map search then runs in two launches (candidates, commit)
         assert _launched(t, lambda: t.SearchByProjection_last(s["kCur"], s["dCur"], s["TcwCur"], s["kLast"], s["hasMP"], s["Xw"], s["dLast"], s["mpObs"], s["curTaken"],
                                                               650, 650, cth, 15.0, True)) == 2
         assert _launched(t, lambda: t.SearchByProjection_local(s["kCur"], s["dCur"], np.ones(len(pick), np.uint8), proj, lvl, np.full(len(pick), 0.99, np.float32),
                                                                s["dLast"][s["src"][pick]], np.ones(len(pick), np.int32),
-                                                               (rng.random(len(s["kCur"])) < 0.05).astype(np.uint8), 650, 650, 3.0, 0.8)) == 2
+                                                               (rng.random(len(s["kCur"])) < 0.05).astype(np.uint8), 650, 650, 3.0, 0.8)) == 3
     finally:
         t.close()
 

@@ -1,6 +1,6 @@
-"""Host-call latency of the local-map SearchByProjection: cslam_search_by_projection_local_large at 1024 to 2^20 MapPoints, the existing
-cslam_search_by_projection_local at 1024 and 4096, and the reference's CPU body (through oracle/_ref/libdropin_local_map.so, which also builds
-its Frame / MapPoint objects outside the timed call) where that library exists. One frame of 4096 key points per call, face 650, th 5, as the
+"""Host-call latency of the local-map SearchByProjection: cslam_search_by_projection_local_large at 1024 to 2^20 MapPoints (the local entry
+runs the same kernels up to the handle's max_features), and the reference's CPU body (through oracle/_ref/libdropin_local_map.so, which also
+builds its Frame / MapPoint objects outside the timed call) where that library exists. One frame of 4096 key points per call, face 650, th 5, as the
 drop-in calls it; medians over --reps calls after a warm-up. Prints the card's name and power limit with the numbers, as one JSON line.
   python tools/local_map_latency.py [--reps 30]"""
 import argparse
@@ -42,8 +42,6 @@ def main():
         mp = S.local_map(fr, n, n)
         a = (fr["k"], fr["d"], mp["in_view"], mp["proj"], mp["level"], mp["vcos"], mp["dq"], mp["obs"], fr["taken"], W, W, th, nn)
         res["large_%d" % n] = median_ms(lambda: t.SearchByProjection_local_large(*a), args.reps)
-        if n <= 4096:
-            res["existing_%d" % n] = median_ms(lambda: t.SearchByProjection_local(*a), args.reps)
     t.close()
     lib = os.path.join(ROOT, "oracle", "_ref", "libdropin_local_map.so")
     if os.path.exists(lib):   # the reference's search alone, timed inside the library (its Frame / MapPoint objects are built untimed)
