@@ -328,16 +328,21 @@ __host__ __device__ inline uint32_t fdiv_magic(int d) { return ((1u << 20) + d -
 
 // Layout of one CTA: one tile column (CG cells wide) of FAST_R consecutive cell rows of one frame, walked tile by tile (a tile = CG cells of
 // one cell row, exactly the reference's per-cell ROIs). Phases of each tile:
-//  A0 compass pretest of every work item (4 pixels): an item goes to the tile's pass list (one shared atomic per warp) unless the compass
-//     bound (compass_x2) proves all 4 of its scores <= mt (mt = minTh clamped to 1..255, see below). On the warp path (`live` given) only
-//     the tile's live work items are tested: every other item's 7x7 windows hold one constant (DevLevels::live), so its scores are 0
+// The thresholds are mt = minTh and ti = max(iniTh, mt), each clamped to 1..255 (see below). A keypoint of cv::FAST at ti is exactly an NMS
+// survivor at mt with s > ti: a suppressor needs s_n >= s, and a neighbour with s_n <= ti < s suppresses nothing at either threshold.
+//  A0 compass pretest of every work item (4 pixels), at both thresholds from one bound (compass_x2): an item the bound cannot prove <= ti goes
+//     to the tile's pass list, one it proves <= ti but not <= mt to the deferred list (one shared atomic per warp each). On the warp path
+//     (`live` given) only the tile's live work items are tested: every other item's 7x7 windows hold one constant (DevLevels::live), so its
+//     scores are 0
 //  A  branch-free exact arc score of every pass-list item -> S (u16, (s - mt) << 8, 0 where s <= mt). An item left out scores 0, which the
-//     zeroed S already holds. Each warp appends the items it scored non-zero to the tile's nz list (one shared atomic per warp)
-//  B  3x3 NMS at minTh inside each cell, one work item (2 pair-words) per thread, over the nz list -> shared list; a keypoint at
-//     iniTh is exactly an NMS survivor with s > iniTh (a suppressor needs s_n >= s), so the per-cell 20->7 fallback is a filter on that list
-//  C  the selected entries (the per-cell fallback filter) appended to the strip's output buffer, one shared atomic per warp; the buffer is
-//     copied to the global candidate list (one global atomic) at the end of the strip, or at the end of a tile after which it could not
-//     hold another tile's survivors
+//     zeroed S already holds. Each warp appends the items it scored non-zero to the tile's nzHi list (some score > ti) or nzLo list
+//  B  round 1: 3x3 NMS at mt inside each cell, one work item (2 pair-words) per thread, over nzHi, keeping the survivors with s > ti: the
+//     keypoints at ti, exactly (the deferred items, still 0 in S, are <= ti). A cell none of them lies in falls back to mt (the reference's
+//     20->7 rule); if the tile has such cells (F), round 2 scores the deferred items with a pixel in F into S and, after a barrier, runs
+//     the NMS at mt over every non-zero item with a pixel in F, keeping every survivor in F. S already holds the pass-list items' scores
+//     at mt, so nothing is scored twice, and a cell whose pixels above ti all lose to equal neighbours (a plateau) falls back as it must
+//  C  every NMS survivor appended to the strip's output buffer, one shared atomic per warp; the buffer is copied to the global candidate
+//     list (one global atomic) at the end of the strip, or at the end of a tile after which it could not hold another tile's survivors
 static const int FAST_R = 8;            // cell rows per k_fast CTA
 static const int FAST_SW = FAST_TS / 2;   // pair-words per score row
 static const int FAST_OUT = CG * ((CELL_MAX + 1) / 2) * ((CELL_MAX + 1) / 2);   // candidates the strip's output buffer holds: >= any kmax
@@ -369,7 +374,7 @@ __host__ __device__ inline FastTileX fast_tile_x(const LevelGeom& g, int cx) {
 struct FastItem {
     uint32_t valid[2];    // column inside the detection area
     uint32_t cells;       // cell index within the tile of pixel j (tile column 4*wi + j) in bits 2j..2j+1
-    uint32_t pad;
+    uint32_t cellMask;    // bit c: some pixel of the item inside the detection area lies in cell c
     uint32_t left[2], right[2];   // has a left / right neighbour in its cell
 };
 // Everything k_fast needs that depends on the tile column alone; built once per level at create time (build_fast_cols)
@@ -381,10 +386,13 @@ struct FastCols {
 // Dynamic shared memory of a k_fast CTA (byte offsets), sized from the level's cell geometry; CELL_MAX bounds it (fast_smem_max)
 struct FastSmem {
     int items;                 // the tile column's FastCols::item table
-    int pass;                  // the current tile's items the compass bound could not prove corner-free (u16, encoded as the live list):
-                               // phase A's work list. Its own region, like the nz list
-    int nz;                    // the current tile's items phase A scored non-zero (u16, encoded as the live list): phase B's work list.
-                               // Its own region: warps append ahead of other warps' pass-list reads, and the other buffers hold the next tile
+    int pass;                  // listCap u16 entries, encoded as the live list: from the front the current tile's pass list (items the compass
+                               // bound cannot prove <= ti: phase A's work list), from the back its deferred list (provably <= ti, not <= mt:
+                               // scored in round 2 only). An item enters at most one of them. Its own region, like the nz list
+    int nz;                    // listCap u16 entries: from the front nzHi (items scored with a score > ti: round 1's work list), from the back
+                               // nzLo (scored non-zero, no score > ti; round 2 appends the deferred items it scores non-zero). Its own
+                               // region: warps append ahead of other warps' pass-list reads, and the other buffers hold the next tile
+    int listCap;               // entries of each list region: >= the items of a tile that phase A0 tests
     int tile, tileBytes;     // tile buffer b at tile + b * tileBytes: 16 bytes in front (phase A reads the word left of row 0 unguarded),
                                // then hCell + 6 rows of FAST_TS
     int s2, klist;             // score map (hCell + 2 rows of FAST_SW pair-words); NMS survivors, kmax entries
@@ -396,11 +404,11 @@ __host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
     m.tileBytes = 16 + (g.hCell + 6) * FAST_TS; m.liveBytes = 16 * ((g.liveCap + 14) / 8);
     m.kmax = CG * ((g.wCell + 1) / 2) * ((g.hCell + 1) / 2);   // NMS survivors of a cell are pairwise non-adjacent
     // items of a tile: nw <= (nx + 6) / 4 (fast_tile_x, nx <= CG * wCell) per detection row, hCell rows at most
-    const int nzCap = max(g.liveCap, ((CG * g.wCell + 6) >> 2) * g.hCell);
+    m.listCap = 8 * ((max(g.liveCap, ((CG * g.wCell + 6) >> 2) * g.hCell) + 7) / 8);
     m.items = 0;
     m.nz = m.items + (int)sizeof(FastItem) * (FAST_SW / 2);   // a constant offset: no register holds its address
-    m.pass = m.nz + 16 * ((nzCap + 7) / 8);
-    m.tile = m.pass + 16 * ((nzCap + 7) / 8);
+    m.pass = m.nz + 2 * m.listCap;
+    m.tile = m.pass + 2 * m.listCap;
     m.s2 = m.tile + 2 * m.tileBytes;
     m.live = m.s2 + (g.hCell + 2) * FAST_SW * 4;
     m.klist = m.live + 2 * m.liveBytes;
@@ -410,13 +418,14 @@ __host__ __device__ inline FastSmem fast_smem(const LevelGeom& g) {
 static_assert(FAST_TS % 16 == 0 && sizeof(FastItem) % 16 == 0, "k_fast shared-memory regions stay 16-byte aligned");
 
 // Neighbourhood maximum of pair-word `cur` over its 8 same-cell neighbours: a*, b*, c* = the pair-words left of, at and right of it in the
-// row above (0), its own row (1) and the row below (2); ml / mr mask the lanes without a left / right neighbour in their cell
+// row above (0), its own row (1) and the row below (2); ml / mr mask the lanes without a left / right neighbour in their cell. fl: a
+// floor in both lanes (free in the last max), so that a lane survives only if it is above the floor too
 __device__ __forceinline__ uint32_t nms_max(uint32_t a0, uint32_t b0, uint32_t c0, uint32_t a1, uint32_t cur, uint32_t c1, uint32_t a2, uint32_t b2,
-                                            uint32_t c2, uint32_t ml, uint32_t mr) {
+                                            uint32_t c2, uint32_t ml, uint32_t mr, uint32_t fl) {
     const uint32_t upL = __funnelshift_r(a0, b0, 16) & ml, upR = __funnelshift_r(b0, c0, 16) & mr;
     const uint32_t cuL = __funnelshift_r(a1, cur, 16) & ml, cuR = __funnelshift_r(cur, c1, 16) & mr;
     const uint32_t dnL = __funnelshift_r(a2, b2, 16) & ml, dnR = __funnelshift_r(b2, c2, 16) & mr;
-    return __vimax3_u16x2(__vimax3_u16x2(upL, b0, upR), __vimax3_u16x2(cuL, cuR, b2), __vmaxu2(dnL, dnR));
+    return __vimax3_u16x2(__vimax3_u16x2(upL, b0, upR), __vimax3_u16x2(cuL, cuR, b2), __vimax3_u16x2(dnL, dnR, fl));
 }
 
 __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img, LevelGeom g, int iniTh, int minTh, uint32_t* __restrict__ cand,
@@ -427,13 +436,15 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
     const FastSmem SM = fast_smem(g);
     // score map, one u16 per pixel as u16x2 pair-words: word 2*wi (+1) of row y+1 holds tile columns 4*wi..4*wi+1 (+2..+3)
     uint32_t* const S2 = reinterpret_cast<uint32_t*>(fsm + SM.s2);
-    uint32_t* const klist = reinterpret_cast<uint32_t*>(fsm + SM.klist);   // x | y<<8 | s<<16 | cell<<24
+    uint32_t* const klist = reinterpret_cast<uint32_t*>(fsm + SM.klist);   // x | y<<8 | s<<16
     const uint4* const items = reinterpret_cast<const uint4*>(fsm + SM.items);   // FastItem wi = items[2*wi], items[2*wi+1]
+    uint16_t* const passS = reinterpret_cast<uint16_t*>(fsm + SM.pass);   // pass list from the front, deferred list from the back
+    uint16_t* const nzS = reinterpret_cast<uint16_t*>(fsm + SM.nz);       // nzHi from the front, nzLo from the back
     __shared__ uint32_t rowLo[FAST_R], rowHi[FAST_R];   // live list of each strip row, [rowLo, rowHi)
     __shared__ int rowVisit[FAST_R];                    // the strip row's tile has work (not skipped, detection rows > 0)
     __shared__ uint32_t sout[FAST_OUT];   // the strip's selected candidates, packed as in cand
-    __shared__ int cnt20[CG];
-    __shared__ int nK, nPass, nNZ, nOut, flushN;
+    __shared__ uint32_t hit;              // bit c: cell c of the tile has a keypoint at ti (round 1)
+    __shared__ int nK, nPass, nDef, nHi, nLo, nOut, flushN;
     __shared__ uint32_t flushBase;
     const int frame = blockIdx.z, row0 = blockIdx.y * FAST_R, nr = min(FAST_R, g.nRowsEff - row0);
     const int tid = threadIdx.x, lane = tid & 31;
@@ -459,9 +470,14 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
     while (cur < nr && !rowVisit[cur]) cur++;
     if (cur == nr) return;
     // cv::FAST clamps its threshold to 0..255 and ranks corners by s - 1, with 0 for "no corner": at threshold 0 a corner with s = 1 ties
-    // with its non-corner neighbours and never survives NMS, exactly as if the threshold were 1
-    const int mt = min(max(minTh, 1), 255);
+    // with its non-corner neighbours and never survives NMS, exactly as if the threshold were 1. An iniTh at or below minTh gives ti = mt:
+    // every survivor at mt is then a keypoint at iniTh, as the fallback rule has it
+    const int mt = min(max(minTh, 1), 255), ti = max(min(max(iniTh, 1), 255), mt);
     const uint32_t T = (uint32_t)mt * 0x01000100u;
+    // ti in S's encoding, both lanes: a score is > ti iff its lane is > TH. Read from shared memory where it is used (after B1), which
+    // keeps it out of the registers of phases A and B
+    __shared__ uint32_t TH;
+    if (tid == 0) TH = (uint32_t)(ti - mt) * 0x01000100u;
     // strip row i's tile rows and live list (from the multiple of 8 at or below rowLo) into buffer b, by 16-byte copies: a0 and the level
     // pitch are multiples of 16. Thread tid copies 16-byte column tid % 16 of tile rows tid / 16, tid / 16 + 16, ... (a row has at most 16)
     auto stage = [&](int i, int b) {
@@ -495,13 +511,16 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         }
     };
     // Barriers of one tile (buffer b = tile parity in the strip):
-    //  top   S2 cleared, nK / nPass / nNZ / cnt20 reset: the previous tile's phases A, B and C are done with them (its end barrier), or it
-    //        ended at BP with nPass = 0 and read nothing else after B1
+    //  top   S2 cleared, nK / nPass / nDef / nHi / nLo / hit reset: the previous tile's phases A, B and C are done with them (its end
+    //        barrier), or it ended at BP with empty pass and deferred lists and read nothing else after B1
     //  wait  this thread's copies of the tile landed; B1 (__syncthreads_or) makes every thread's copies visible
-    //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phase A, before its B2
-    //  A0 (reads the live list of b; appends to the pass list, nPass) -> BP -> A (pass list, nPass; appends to the nz list, nNZ) -> B2 ->
-    //  B (S2, item table, nz list, nNZ) -> B3 -> C (klist, nK, cnt20; appends to the output buffer) -> end barrier
-    //  a tile whose pass list is empty has no corner: after BP it goes on to the next tile as the !any path does after B1
+    //  after B1: the next visited tile is staged into buffer b^1, which the previous tile last read in phase A or round 2, before its end
+    //  barrier
+    //  A0 (reads the live list of b; appends to the pass and deferred lists, nPass, nDef) -> BP -> A (pass list, nPass; appends to nzHi
+    //  and nzLo, nHi, nLo) -> B2 -> round 1 (S2, item table, nzHi, nHi; appends to klist, nK, hit) -> B3 -> only if the tile has a cell
+    //  in F (hit, block-uniform): round 2 scoring (deferred list, nDef; S2, appends to nzLo, nLo) -> B4 -> round 2 NMS (S2, nzHi, nzLo;
+    //  appends to klist, nK) -> B5 -> C (klist, nK; appends to the output buffer) -> end barrier
+    //  a tile whose pass and deferred lists are empty has no corner: after BP it goes on to the next tile as the !any path does after B1
     //  after the end barrier: flush when the buffer could not hold another tile's kmax entries, and at the end of the strip (one barrier
     //  more; the next appends follow the next tile's B1)
     for (int b = 0;; b ^= 1) {
@@ -518,8 +537,7 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
                 reinterpret_cast<uint4*>(S2 + r * FAST_SW)[q0 + i - r * nq] = make_uint4(0u, 0u, 0u, 0u);
             }
         }
-        if (tid < CG) cnt20[tid] = 0;
-        if (tid == 0) { nK = 0; nPass = 0; nNZ = 0; }
+        if (tid == 0) { nK = 0; nPass = 0; nDef = 0; nHi = 0; nLo = 0; hit = 0u; }
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         // caller canvases: an all-zero tile has no corners at any threshold (OR of the columns this thread staged)
         uint32_t acc = live ? 1u : 0u;
@@ -544,163 +562,192 @@ __global__ void __launch_bounds__(256, 4) k_fast(const uint8_t* __restrict__ img
         // of the word left of the centre row (m), and the centres bytes 0, 2 of the centre word.
         {
             const int w0 = X.w0;
-            const uint32_t T1 = T | 0x00ff00ffu;
-            auto passes = [&](int e) {   // e: the item, encoded as the live list
+            const uint32_t T1 = T | 0x00ff00ffu, T1i = (uint32_t)ti * 0x01000100u | 0x00ff00ffu;
+            // the bound of item e (encoded as the live list) at mt: T1 where it proves all 4 scores <= mt; above T1i where it cannot prove
+            // them <= ti (T1i >= T1, and a lane's bound exceeds t << 8 | 0xff exactly where its margin exceeds t)
+            auto bound = [&](int e) {
                 const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + (e >> 6) * FAST_TS + 4 * (w0 + (e & 63)));
                 const int RS = FAST_TS / 4;
                 const uint32_t* r3 = r0 + 3 * RS; const uint32_t* r6 = r0 + 6 * RS;
                 const uint32_t uc = r0[0], m = r3[-1], c = r3[0], p = r3[1], dc = r6[0];
                 const uint32_t V4 = __funnelshift_r(c, p, 24);
                 const uint32_t b02 = compass_x2(uc * 256u, V4 * 256u, dc * 256u, m, c * 256u, T1);
-                return compass_x2(uc, V4, dc, __funnelshift_r(m, c, 8), c, b02) != T1;
+                return compass_x2(uc, V4, dc, __funnelshift_r(m, c, 8), c, b02);
             };
-            // items that can score go to the pass list in the same encoding (ptxas aggregates the atomic: one ATOMS per warp)
-            uint16_t* const passS = reinterpret_cast<uint16_t*>(fsm + SM.pass);
+            // items that can score above ti go to the pass list, the others that can score above mt to the deferred list, in the same
+            // encoding (ptxas aggregates each atomic: one ATOMS per warp)
+            auto append = [&](int e) {
+                const uint32_t v = bound(e);
+                if (__vmaxu2(v, T1i) != T1i) passS[atomicAdd(&nPass, 1)] = (uint16_t)e;
+                else if (v != T1) passS[SM.listCap - 1 - atomicAdd(&nDef, 1)] = (uint16_t)e;
+            };
             if (live) {
-                for (uint32_t it = tid; it < nLive; it += 256) {
-                    const int e = liveS[it];
-                    if (passes(e)) passS[atomicAdd(&nPass, 1)] = (uint16_t)e;
-                }
+                for (uint32_t it = tid; it < nLive; it += 256) append(liveS[it]);
             } else {
                 const int nw = X.w1 - w0; const uint32_t mgItems = mg.x;
                 for (int it = tid; it < nw * ny; it += 256) {
-                    const int y = fdiv_small(it, mgItems), e = y << 6 | (it - y * nw);
-                    if (passes(e)) passS[atomicAdd(&nPass, 1)] = (uint16_t)e;
+                    const int y = fdiv_small(it, mgItems);
+                    append(y << 6 | (it - y * nw));
                 }
             }
         }
         __syncthreads();   // BP
         const int npass = nPass;
-        if (npass == 0) {   // no item can score: nothing reads S2, the lists, the counters or buffer b after BP
+        if (npass == 0 && nDef == 0) {   // no item can score: nothing reads S2, the lists, the counters or buffer b after BP
             if (next == nr) break;
             cur = next;
             continue;
         }
-        // ---- A
+        // Exact arc scores of item wi of detection row y into S2 (nothing is stored for an all-zero item: S2 already reads 0 there). Returns
+        // 0 for an all-zero item, 2 if some lane is above ti (> TH), else 1
+        auto score_item = [&](int y, int wi) {
+            const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
+            const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
+            const int RS = FAST_TS / 4;
+            // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
+            // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
+            // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle.
+            // arc_score_x2 reads only the high bytes, so where U[k] is no loaded word it is V[k] shifted left by 8 bits (V[k]'s low
+            // bytes are U's pixels): a multiply by 256 on the FMA pipe instead of a funnel shift on the integer pipe
+            uint32_t V[16], U[16], Cv, Cu;
+            {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
+                const uint32_t m = r0[-1], c = r0[0], p = r0[1];
+                V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
+                U[15] = V[15] * 256u; U[0] = V[15]; U[1] = c;
+            }
+            {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
+                const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
+                U[14] = V[14] * 256u; U[2] = V[2] * 256u;
+            }
+            {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
+                const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
+                U[13] = m; U[3] = V[3] * 256u;
+            }
+            {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
+                const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
+                U[12] = m; U[4] = V[4] * 256u; Cu = c * 256u;
+            }
+            {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
+                const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
+                U[11] = m; U[5] = V[5] * 256u;
+            }
+            {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
+                const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
+                U[10] = V[10] * 256u; U[6] = V[6] * 256u;
+            }
+            {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
+                const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
+                V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
+                U[9] = V[9] * 256u; U[8] = V[9]; U[7] = c;
+            }
+            const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
+            // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
+            // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset)
+            const uint32_t mx = __vmaxu2(s02, s13);
+            if (mx != 0u)
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
+                    make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
+            if (mx == 0u) return 0;
+            const uint32_t th = TH;
+            return __vmaxu2(mx, th) != th ? 2 : 1;
+        };
+        // ---- A: items scored non-zero go to nzHi or nzLo, in the same encoding. ptxas aggregates each atomic: one ATOMS per warp
+        // (tools/kfast_sass.py). The entry is read again after the score rather than held across it (register pressure)
         {
             const int w0 = X.w0;
-            auto score_item = [&](int y, int wi) {
-                const int to = y * FAST_TS + 4 * wi;   // byte offset of the item in tile row y, the row 3 above its centres
-                const uint32_t* r0 = reinterpret_cast<const uint32_t*>(tile + to);
-                const int RS = FAST_TS / 4;
-                // The word left of the item (m) feeds only centres 0..2 of item 0, which lie left of the detection area when w0 = 0 (xoff >= 3),
-                // so it is read unguarded. Read as u16x2, a word starting dx pixels right of the item holds ring pixel dx of centres 1 and 3 in the high bytes of its
-                // lanes (V), and the word one pixel further left holds those of centres 0 and 2 (U). ring k: (dx, dy) of the FAST-16 circle.
-                // arc_score_x2 reads only the high bytes, so where U[k] is no loaded word it is V[k] shifted left by 8 bits (V[k]'s low
-                // bytes are U's pixels): a multiply by 256 on the FMA pipe instead of a funnel shift on the integer pipe
-                uint32_t V[16], U[16], Cv, Cu;
-                {   // dy=-3: ring 15 (dx-1), 0 (dx 0), 1 (dx+1)
-                    const uint32_t m = r0[-1], c = r0[0], p = r0[1];
-                    V[15] = __funnelshift_r(m, c, 24); V[0] = c; V[1] = __funnelshift_r(c, p, 8);
-                    U[15] = V[15] * 256u; U[0] = V[15]; U[1] = c;
-                }
-                {   // dy=-2: ring 14 (dx-2), 2 (dx+2)
-                    const uint32_t* r = r0 + RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[14] = __funnelshift_r(m, c, 16); V[2] = __funnelshift_r(c, p, 16);
-                    U[14] = V[14] * 256u; U[2] = V[2] * 256u;
-                }
-                {   // dy=-1: ring 13 (dx-3), 3 (dx+3)
-                    const uint32_t* r = r0 + 2 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[13] = __funnelshift_r(m, c, 8); V[3] = __funnelshift_r(c, p, 24);
-                    U[13] = m; U[3] = V[3] * 256u;
-                }
-                {   // dy=0: ring 12 (dx-3), 4 (dx+3), centre
-                    const uint32_t* r = r0 + 3 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[12] = __funnelshift_r(m, c, 8); V[4] = __funnelshift_r(c, p, 24); Cv = c;
-                    U[12] = m; U[4] = V[4] * 256u; Cu = c * 256u;
-                }
-                {   // dy=+1: ring 11 (dx-3), 5 (dx+3)
-                    const uint32_t* r = r0 + 4 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[11] = __funnelshift_r(m, c, 8); V[5] = __funnelshift_r(c, p, 24);
-                    U[11] = m; U[5] = V[5] * 256u;
-                }
-                {   // dy=+2: ring 10 (dx-2), 6 (dx+2)
-                    const uint32_t* r = r0 + 5 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[10] = __funnelshift_r(m, c, 16); V[6] = __funnelshift_r(c, p, 16);
-                    U[10] = V[10] * 256u; U[6] = V[6] * 256u;
-                }
-                {   // dy=+3: ring 9 (dx-1), 8 (dx 0), 7 (dx+1)
-                    const uint32_t* r = r0 + 6 * RS; const uint32_t m = r[-1], c = r[0], p = r[1];
-                    V[9] = __funnelshift_r(m, c, 24); V[8] = c; V[7] = __funnelshift_r(c, p, 8);
-                    U[9] = V[9] * 256u; U[8] = V[9]; U[7] = c;
-                }
-                const uint32_t s13 = arc_score_x2(V, Cv, T), s02 = arc_score_x2(U, Cu, T);
-                // back to pair-word order (pixels 0,1) (2,3). Lanes outside the detection area keep what they scored: phase B masks them
-                // (S2 row y+1 holds tile row y's 4 pixels of an item in 8 bytes at twice the tile offset). An all-zero item is not stored:
-                // S2 already reads 0 there
-                const bool nz = (s02 | s13) != 0u;
-                if (nz)
-                    *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(S2) + 4 * FAST_SW + 2 * to) =
-                        make_uint2(__byte_perm(s02, s13, 0x5410), __byte_perm(s02, s13, 0x7632));
-                return nz;
-            };
-            // items scored non-zero go to the tile's nz list, in the same encoding. ptxas aggregates the atomic: one ATOMS per warp
-            // (tools/kfast_sass.py). The entry is read again after the score rather than held across it (register pressure)
-            const uint16_t* const passS = reinterpret_cast<const uint16_t*>(fsm + SM.pass);
-            uint16_t* const nzS = reinterpret_cast<uint16_t*>(fsm + SM.nz);
             for (int it = tid; it < npass; it += 256) {
                 const int e = passS[it];
-                if (score_item(e >> 6, w0 + (e & 63))) nzS[atomicAdd(&nNZ, 1)] = passS[it];
+                const int k = score_item(e >> 6, w0 + (e & 63));
+                if (k == 2) nzS[atomicAdd(&nHi, 1)] = passS[it];
+                else if (k == 1) nzS[SM.listCap - 1 - atomicAdd(&nLo, 1)] = passS[it];
             }
         }
         __syncthreads();   // B2
-        // ---- B: NMS at minTh in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > minTh). A pair-word can be
-        // non-zero only inside an item phase A scored non-zero, so B walks the tile's nz list; one thread reads the item's 3 x 4 pair-word
-        // neighbourhood once.
+        // ---- B: NMS at mt in u16x2 lanes: keep s iff every same-cell neighbour is < s (all stored scores are > mt). A pair-word can be
+        // non-zero only inside an item phase A (or round 2) scored non-zero, so B walks the nz lists; one thread reads the item's 3 x 4
+        // pair-word neighbourhood once.
         // Lanes outside the detection area hold scores of pixels outside it: the current pair-words are masked to the valid lanes, and a valid
-        // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows)
-        {
-            const int w0 = X.w0, xoff = X.xoff;
-            auto nms_item = [&](int y, int wi) {
-                const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
-                const uint4 hd = items[2 * wi];
-                uint2 cu = *reinterpret_cast<const uint2*>(r1);
-                cu.x &= hd.x; cu.y &= hd.y;
-                if ((cu.x | cu.y) == 0) return;
-                const uint32_t* r0 = r1 - FAST_SW; const uint32_t* r2 = r1 + FAST_SW;
-                const uint2 up = *reinterpret_cast<const uint2*>(r0), dn = *reinterpret_cast<const uint2*>(r2);
-                const uint32_t uL = wi > 0 ? r0[-1] : 0u, cL = wi > 0 ? r1[-1] : 0u, dL = wi > 0 ? r2[-1] : 0u;
-                const uint32_t uR = r0[2], cR = r1[2], dR = r2[2];
-                const uint4 lr = items[2 * wi + 1];
-                const uint32_t M0 = nms_max(uL, up.x, up.y, cL, cu.x, cu.y, dL, dn.x, dn.y, lr.x, lr.z);
-                const uint32_t M1 = nms_max(up.x, up.y, uR, cu.x, cu.y, cR, dn.x, dn.y, dR, lr.y, lr.w);
-                // survivors: the lanes where c > m. Every lane holds a multiple of 256 (the stored scores' low bytes are 0), so max(c, m) - m
-                // never borrows and its high byte is non-zero exactly there; byte j of `keep` is that byte of pixel j
-                uint32_t keep = __byte_perm(__vmaxu2(cu.x, M0) - M0, __vmaxu2(cu.y, M1) - M1, 0x7531);
-                while (keep) {
-                    const int j = (__ffs(keep) - 1) >> 3;
-                    keep &= ~(0xffu << (8 * j));
-                    const uint32_t sv = ((j < 2 ? cu.x : cu.y) >> (16 * (j & 1))) & 0xffff;
-                    const int x = 4 * wi + j - xoff, cell = (hd.z >> (2 * j)) & 3, s = (int)(sv >> 8) + mt;
-                    const int pos = atomicAdd(&nK, 1);
-                    if (pos >= SM.kmax) *errFlag = CSLAM_E_CAPACITY;
-                    else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)s << 16) | ((uint32_t)cell << 24);
-                    if (s > iniTh) atomicAdd(&cnt20[cell], 1);
-                }
-            };
-            const uint16_t* const nzS = reinterpret_cast<const uint16_t*>(fsm + SM.nz);
-            const int nnz = nNZ;
-            for (int it = tid; it < nnz; it += 256) { const int e = nzS[it]; nms_item(e >> 6, w0 + (e & 63)); }
+        // lane's neighbours are valid or masked by the left / right masks (the rows above and below are the same columns, or the zeroed rows).
+        // Round 1 (fb = false) keeps the survivors above ti (the floor TH) and marks their cells in `hit`; round 2 (fb = true) skips the items
+        // without a pixel in the cells of fm and keeps every survivor in those cells
+        auto nms_item = [&](int y, int wi, bool fb, uint32_t fm) {
+            const uint4 hd = items[2 * wi];
+            if (fb && !(hd.w & fm)) return;
+            const uint32_t* r1 = S2 + (y + 1) * FAST_SW + 2 * wi;
+            uint2 cu = *reinterpret_cast<const uint2*>(r1);
+            cu.x &= hd.x; cu.y &= hd.y;
+            if ((cu.x | cu.y) == 0) return;
+            const uint32_t* r0 = r1 - FAST_SW; const uint32_t* r2 = r1 + FAST_SW;
+            const uint2 up = *reinterpret_cast<const uint2*>(r0), dn = *reinterpret_cast<const uint2*>(r2);
+            const uint32_t uL = wi > 0 ? r0[-1] : 0u, cL = wi > 0 ? r1[-1] : 0u, dL = wi > 0 ? r2[-1] : 0u;
+            const uint32_t uR = r0[2], cR = r1[2], dR = r2[2];
+            const uint4 lr = items[2 * wi + 1];
+            const uint32_t fl = fb ? 0u : TH;
+            const uint32_t M0 = nms_max(uL, up.x, up.y, cL, cu.x, cu.y, dL, dn.x, dn.y, lr.x, lr.z, fl);
+            const uint32_t M1 = nms_max(up.x, up.y, uR, cu.x, cu.y, cR, dn.x, dn.y, dR, lr.y, lr.w, fl);
+            // survivors: the lanes where c > m. Every lane holds a multiple of 256 (the stored scores' low bytes are 0), so max(c, m) - m
+            // never borrows and its high byte is non-zero exactly there; byte j of `keep` is that byte of pixel j
+            uint32_t keep = __byte_perm(__vmaxu2(cu.x, M0) - M0, __vmaxu2(cu.y, M1) - M1, 0x7531);
+            const int xoff = X.xoff;
+            while (keep) {
+                const int j = (__ffs(keep) - 1) >> 3;
+                keep &= ~(0xffu << (8 * j));
+                const int cell = (hd.z >> (2 * j)) & 3;
+                if (fb && !((fm >> cell) & 1u)) continue;
+                const uint32_t sv = ((j < 2 ? cu.x : cu.y) >> (16 * (j & 1))) & 0xffff;
+                const int x = 4 * wi + j - xoff, s = (int)(sv >> 8) + mt;
+                const int pos = atomicAdd(&nK, 1);
+                if (pos >= SM.kmax) *errFlag = CSLAM_E_CAPACITY;
+                else klist[pos] = (uint32_t)x | ((uint32_t)y << 8) | ((uint32_t)s << 16);
+                if (!fb) atomicOr(&hit, 1u << cell);
+            }
+        };
+        {   // round 1
+            const int w0 = X.w0, nh = nHi;
+            for (int it = tid; it < nh; it += 256) { const int e = nzS[it]; nms_item(e >> 6, w0 + (e & 63), false, 0u); }
         }
-        __syncthreads();
-        // ---- C: each warp filters its stride of klist and appends with one shared atomic; the buffer has room for nk <= kmax entries
+        __syncthreads();   // B3
+        // F: the tile's cells without a keypoint at ti (block-uniform: hit is final after B3 and nothing writes it before the end barrier)
+        const uint32_t fm = ~hit & ((1u << min(CG, g.nColsEff - (int)blockIdx.x * CG)) - 1u);
+        if (fm) {
+            const int w0 = X.w0;
+            {   // round 2 scoring: the deferred items with a pixel in F, appended to nzLo when non-zero
+                const int nd = nDef;
+                for (int it = tid; it < nd; it += 256) {
+                    const int e = passS[SM.listCap - 1 - it], wi = w0 + (e & 63);
+                    if ((items[2 * wi].w & fm) && score_item(e >> 6, wi)) nzS[SM.listCap - 1 - atomicAdd(&nLo, 1)] = passS[SM.listCap - 1 - it];
+                }
+            }
+            __syncthreads();   // B4
+            {   // round 2 NMS over nzHi and nzLo (at [listCap - nl, listCap)), in F only
+                const int nh = nHi, nl = nLo;
+                for (int it = tid; it < nh + nl; it += 256) {
+                    const int e = nzS[it < nh ? it : SM.listCap - nl + (it - nh)];
+                    nms_item(e >> 6, w0 + (e & 63), true, fm);
+                }
+            }
+            __syncthreads();   // B5
+        }
+        // ---- C: each warp appends its stride of klist with one shared atomic; the buffer has room for nk <= kmax entries
         const int nk = min(nK, SM.kmax);
 #pragma unroll 1
         for (int i = tid - lane; i < nk; i += 256) {   // warp-uniform bounds
-            uint32_t v = 0; bool sel = false;
-            if (i + lane < nk) {
+            uint32_t v = 0; const bool sel = i + lane < nk;
+            if (sel) {
                 const uint32_t e = klist[i + lane];
-                const int sv = (e >> 16) & 0xff, cell = e >> 24;
-                sel = cnt20[cell] > 0 ? sv > iniTh : true;
                 const uint32_t x = X.tx0 + 3 + (e & 0xff) - g.minB, y = iniY + 3 + ((e >> 8) & 0xff) - g.minB;
-                v = x | (y << 12) | ((uint32_t)(sv - 1) << 24);
+                v = x | (y << 12) | ((((e >> 16) & 0xff) - 1) << 24);
             }
             const unsigned ball = __ballot_sync(0xffffffffu, sel);
-            if (ball == 0) continue;
             int pos = 0;
             if (lane == 0) pos = atomicAdd(&nOut, __popc(ball));
             pos = __shfl_sync(0xffffffffu, pos, 0);
-            if (sel) sout[pos + __popc(ball & ((1u << lane) - 1))] = v;
+            if (sel) sout[pos + lane] = v;
         }
         __syncthreads();   // end barrier
         if (next == nr) break;
@@ -1500,6 +1547,7 @@ static std::vector<FastCols> build_fast_cols(const LevelGeom& g) {
                 if (xl != 0) it.left[j >> 1] |= lane;
                 if (xl != g.wCell - 1 && x != t.nx - 1) it.right[j >> 1] |= lane;
                 it.cells |= (uint32_t)cell << (2 * j);
+                it.cellMask |= 1u << cell;
             }
     }
     return cols;

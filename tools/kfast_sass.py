@@ -16,6 +16,9 @@ object:
   phase_a0                             each compass-pretest loop (a loop without a barrier whose body issues fewer than 64 VIMNMX3 / VIMNMX, a
                                        shared-memory atomic and a u16 store: the pass-list append), with `live` and `append` as for phase_a
   phase_b                              each NMS loop (a loop with a shared-memory atomic, VIMNMX3 and no barrier)
+
+k_fast has two phase_a0 loops (live list, caller canvases), two phase_a loops (the pass list, then round 2's deferred items) and two
+phase_b loops (round 1 over nzHi, round 2 over the fallback cells).
   compaction                           the other loops with a shared-memory atomic and no barrier (NMS survivors, phase C)
   each loop                            [start, end] byte offsets, the body's instruction count and its opcode histogram
 
